@@ -3,6 +3,7 @@ samples => 128-sample fine pass, scene + object branch, voxel embedding) through
 `render_rays()`, plus the fused-MLP tensor-core roofline.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision bf16|fp32] [--no-extras]
+                  [--dump-outputs DIR]
 
 One process per GPU (torchrun for N > 1).  Headline (`value`, `e2e`, `roofline`): a step = one full frame (307 200 rays)
 per rank, rendered in 65 536-ray chunks; N > 1: every rank renders its own frame and the (rgb, depth) tiles are
@@ -13,8 +14,11 @@ The same JSON line carries, unless --no-extras:
   "strong"  BASELINE configs[4] sharding: ONE frame tile-sharded over the N ranks, gather inside the timed region
   "edit"    BASELINE configs[4] path: render_rays_multi with ray sets [0, 4, 4], chunk 4096 (edit_scannet_0113.yaml shape)
   "parity"  the GPU render of the cpu_baseline sample against the reference / oracle output of the same rays
-  "gpu_torch_baseline"  the unmodified reference (PyTorch) running on the same B200 (fp32 and TF32)
+  "gpu_torch_baseline"  the unmodified reference (PyTorch) running on the same GPU (fp32 and TF32)
 Prints ONE JSON line (rank 0).  See DESIGN.md §5 for the definitions.
+--dump-outputs DIR writes what the last timed headline step returned (rank 0's frame: rgb_fine (H*W, 3) and depth_fine
+(H*W,), float32) as DIR/<name>.npy.  The scene and rays are generated from fixed seeds, so two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -52,7 +56,8 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return json.load(f), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16; a data-sheet figure, not a measurement
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "datasheet"
 
 
 class ClockSampler:
@@ -224,9 +229,8 @@ def reference_renderer(sc, device="cpu"):
 
 
 def pick_cpu_threads(fn):
-    """torch's CPU matmuls on these small (32768 x 256) chunks get slower when oversubscribed (128 threads on
-    the B200 host: 101 rays/s vs 468 rays/s at 16, profiles/r01_cpu_threads.md), so "all the host threads it
-    can use" is found by timing a small probe at a few thread counts and keeping the fastest."""
+    """torch's CPU matmuls on these small (32768 x 256) chunks can get slower when oversubscribed, so "all the host
+    threads it can use" is found by timing a small probe at a few thread counts and keeping the fastest."""
     cores = os.cpu_count() or 1
     best, best_t = cores, None
     for t in sorted({cores, max(1, cores // 2), max(1, cores // 4), 32, 16}, reverse=True):
@@ -302,7 +306,7 @@ def psnr(a, b):
 
 
 def gpu_torch_baseline(sc, dev):
-    """The reference as its users run it: unmodified PyTorch code on the same B200 (cuBLAS SGEMM, then TF32)."""
+    """The reference as its users run it: unmodified PyTorch code on the same GPU (cuBLAS SGEMM, then TF32)."""
     try:
         kind, render = reference_renderer(sc, dev)
         if kind != "reference":
@@ -626,8 +630,11 @@ def run_ours(args, rank, world, local_rank):
                 rgbd[i:i + CHUNK, 3] = r[keys[1]]
         return rgbd
 
+    last = {}
+
     def step_device():          # weak scaling: every rank renders its own frame, no collective on the data path
-        return render(rays_dev, codes_dev)
+        last["rgbd"] = render(rays_dev, codes_dev)
+        return last["rgbd"]
 
     def step_e2e():
         r = rays_host.to(dev, non_blocking=True)
@@ -646,6 +653,11 @@ def run_ours(args, rank, world, local_rank):
         ms = timer.timed(step_device, args.steps)
     launches = _lib.launch_count(dev) - launches0
     clocks = cs.summary()
+    if args.dump_outputs and rank == 0:
+        rgbd = last["rgbd"].float().cpu().numpy()
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "rgb_fine.npy"), np.ascontiguousarray(rgbd[:, :3]))
+        np.save(os.path.join(args.dump_outputs, "depth_fine.npy"), np.ascontiguousarray(rgbd[:, 3]))
     step_e2e()
     ms_e2e = timer.timed(step_e2e, args.steps)
 
@@ -660,11 +672,7 @@ def run_ours(args, rank, world, local_rank):
     fine_ms = statistics.mean(fine)
     flops = CHUNK * (N_SAMPLES + N_IMPORTANCE) * FLOP_PER_SAMPLE
     achieved = flops / (fine_ms * 1e-3) / 1e12
-    peak = peaks["bf16_tflops_sustained"] if args.precision == "bf16" else 75.0
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "field_tc_traffic.json")
-    if os.path.exists(tpath):
-        traffic = json.load(open(tpath)).get("dram_bytes_per_launch")
+    peak = peaks["bf16_tflops_sustained"] if args.precision == "bf16" else 67.0   # H100 SXM data sheet, FP32 non-tensor
 
     extras = {}
     if not args.no_extras:
@@ -697,19 +705,18 @@ def run_ours(args, rank, world, local_rank):
         "vs_baseline": None, "dtype": args.precision, "data": "synthetic",
         "config": {"workload": WORKLOAD, "rays_per_step_per_gpu": N_RAYS, "chunk_rays": CHUNK,
                    "parallelism": f"ray-sharded dp{world}" if world > 1 else "single GPU",
-                   "l2": "no explicit flush: each step streams ~3 GB of intermediates (>> 126 MB L2)",
+                   "l2": "no explicit flush: each step streams ~3 GB of intermediates (>> 50 MB L2)",
                    "tflops_algorithmic_whole_step": N_RAYS * world * FLOP_PER_RAY * args.steps / (ms * 1e-3) / 1e12},
         "clocks": clocks,
         "e2e": {"value": e2e, "unit": "rays/s", "h2d_bytes_per_step": N_RAYS * (8 * 4 + 8),
                 "d2h_bytes_per_step": N_RAYS * 4 * 4},
         "gpu_launches": launches,
-        "roofline": {"bound": "tensor", "kernel": "field_tc2_kernel (two-tile, voxel) fine pass (65536 rays x 128 samples)",
+        "roofline": {"bound": "tensor", "kernel": "field_tc_kernel (wgmma, voxel) fine pass (65536 rays x 128 samples)",
                      "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                      "peak_source": f"{peaks_kind} bf16_tflops_sustained (kernel timed inside the step)",
                      "flops_per_launch": flops, "ms_per_launch": fine_ms,
                      "ms_per_launch_coarse": statistics.mean(coarse) if coarse else None,
-                     "field_kernel_share_of_step": field_ms_total / (ms / args.steps),
-                     "traffic": traffic},
+                     "field_kernel_share_of_step": field_ms_total / (ms / args.steps)},
     }
     line.update(extras)
     if world == 1 and not args.no_cpu:
@@ -749,6 +756,8 @@ def main():
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline / parity legs (development runs)")
     ap.add_argument("--no-extras", action="store_true", help="headline only: skip train / strong / edit / gpu baseline")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (rgb_fine, depth_fine) as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

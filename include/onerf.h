@@ -1,5 +1,5 @@
 /*
- * onerf.h — C ABI of libonerf_sm100.so: the B200-native (sm_100a) per-ray render path of
+ * onerf.h — C ABI of libonerf_sm90.so: the H100-native (sm_90a) per-ray render path of
  * zju3dv/object_nerf (stratified + PDF sampling, positional / sparse-voxel encoding, the two-branch
  * scene+object MLP, sigma->alpha front-to-back compositing, single-scene and multi-object variants).
  *
@@ -38,7 +38,7 @@ typedef enum onerf_status {
 /* arithmetic of the fused encode+MLP ("field") kernel */
 typedef enum onerf_precision {
   ONERF_PREC_FP32 = 0, /* FFMA, fp32 throughout: verification / gradient-check mode */
-  ONERF_PREC_BF16 = 1  /* tcgen05 tensor cores: bf16 operands, fp32 accumulate in TMEM (product default) */
+  ONERF_PREC_BF16 = 1  /* wgmma tensor cores: bf16 operands, fp32 accumulate in registers (product default) */
 } onerf_precision;
 
 typedef struct onerf_ctx onerf_ctx;
@@ -65,7 +65,7 @@ int64_t onerf_ctx_launch_count(const onerf_ctx* ctx);
 
 size_t onerf_packed_weights_bytes(int use_voxel);
 /* Re-lay the 20 (W,b) pairs into the kernels' formats (fp32 K-major for the FFMA path; bf16, K-major,
- * swizzled stage images in program order for the tcgen05 path).  Re-run whenever parameters change. */
+ * swizzled stage images in program order for the tensor-core path).  Re-run whenever parameters change. */
 int onerf_pack_weights(onerf_ctx* ctx, int use_voxel, const float* const* W_host_ptrs,
                        const float* const* b_host_ptrs, void* packed, size_t packed_bytes, void* stream);
 
@@ -345,8 +345,8 @@ int onerf_total_loss(onerf_ctx* ctx, const onerf_loss_args* args, void* stream);
  * onerf_render_rays_fwd with train_ws set runs the bf16 forward and keeps the backward operands;
  * onerf_render_rays_bwd turns the upstream gradients of the rendered maps into gradients of the 2 x 20 nn.Linear
  * tensors, the per-ray object codes and the voxel feature table:
- *   compositing backward -> head gradients -> input-gradient chain (tcgen05, transposed weight images, operand resident
- *   in TMEM) -> weight gradients (tcgen05, sample-axis reduction) -> encoding gradient (tcgen05 + scatter-add) ->
+ *   compositing backward -> head gradients -> input-gradient chain (wgmma, transposed weight images, operand resident
+ *   in registers) -> weight gradients (wgmma, sample-axis reduction) -> encoding gradient (wgmma + scatter-add) ->
  *   per-ray-constant columns (direction encoding, object code) -> reference [out,in] layout.
  * No gradient flows to rays or depths (the importance samples are detached in the reference, models/rendering.py:307).
  * ------------------------------------------------------------------------------------------- */

@@ -1,4 +1,4 @@
-"""object_nerf_b200 — B200-native (sm_100a) per-ray render path of zju3dv/object_nerf behind the
+"""object_nerf_b200 — H100-native (sm_90a) per-ray render path of zju3dv/object_nerf behind the
 reference's own call surface.  See DESIGN.md and INTEGRATION.md."""
 from .rendering import render_rays, inference_model, query_sigma  # noqa: F401
 from .nerf_model import ObjectNeRF  # noqa: F401

@@ -1,6 +1,6 @@
-"""ctypes binding of libonerf_sm100.so (the C ABI declared in include/onerf.h).
+"""ctypes binding of libonerf_sm90.so (the C ABI declared in include/onerf.h).
 
-There is no fallback: if the shared library is missing or the device is not sm_100 every entry point
+There is no fallback: if the shared library is missing or the device is not sm_90 every entry point
 raises.  PyTorch is used only for device memory and streams.
 """
 from __future__ import annotations
@@ -13,7 +13,7 @@ import threading
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("ONERF_LIB_PATH") or os.path.join(_HERE, "libonerf_sm100.so")   # override: A/B experiments
+LIB_PATH = os.environ.get("ONERF_LIB_PATH") or os.path.join(_HERE, "libonerf_sm90.so")   # override: A/B experiments
 CSRC = os.path.join(_HERE, "csrc")
 
 PREC_FP32, PREC_BF16 = 0, 1
@@ -126,13 +126,13 @@ class RenderBwdArgs(C.Structure):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile the CUDA sources for sm_100a into libonerf_sm100.so (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA sources for sm_90a into libonerf_sm90.so (nvcc cross-compiles without a GPU)."""
     r = subprocess.run(["make", "-C", CSRC, "-j8"], capture_output=True, text=True)
     if verbose or r.returncode != 0:
         print(r.stdout[-4000:])
         print(r.stderr[-4000:])
     if r.returncode != 0:
-        raise RuntimeError("building libonerf_sm100.so failed")
+        raise RuntimeError("building libonerf_sm90.so failed")
     return LIB_PATH
 
 
@@ -205,14 +205,14 @@ def load() -> C.CDLL:
         lib.onerf_render_multi_workspace_bytes.restype = C.c_size_t
         lib.onerf_render_multi_fwd.argtypes = [_p, C.POINTER(RenderMultiArgs), _p]
         if lib.onerf_abi_version() != ABI_VERSION:
-            raise RuntimeError("libonerf_sm100.so ABI version mismatch")
+            raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib
         return lib
 
 
 def check(rc: int):
     if rc != 0:
-        raise RuntimeError(f"libonerf_sm100 error {rc}: {load().onerf_last_error().decode()}")
+        raise RuntimeError(f"libonerf_sm90 error {rc}: {load().onerf_last_error().decode()}")
 
 
 def ptr(t):
@@ -229,7 +229,7 @@ _ctx = {}
 def ctx(device: torch.device):
     """One library context per (process, device)."""
     if device.type != "cuda":
-        raise RuntimeError("object_nerf_b200 runs on CUDA (sm_100a) devices only; got tensor on " + str(device))
+        raise RuntimeError("object_nerf_b200 runs on CUDA (sm_90a) devices only; got tensor on " + str(device))
     idx = device.index if device.index is not None else torch.cuda.current_device()
     if idx not in _ctx:
         h = _p()

@@ -3,9 +3,9 @@
 models/code_library.py; SURVEY.md §8 row a14).
 
 Two arithmetics, selected by `precision`:
-  bf16 (default)  RenderRaysTcFn: ONE C call forward (onerf_render_rays_fwd with a training workspace: the tcgen05 forward
+  bf16 (default)  RenderRaysTcFn: ONE C call forward (onerf_render_rays_fwd with a training workspace: the tensor-core forward
                   keeps every layer's activations as bf16 operand tiles) and ONE C call backward (onerf_render_rays_bwd:
-                  tcgen05 input-gradient chain, weight-gradient and encoding-gradient GEMMs).  Voxel model only.
+                  wgmma input-gradient chain, weight-gradient and encoding-gradient GEMMs).  Voxel model only.
   fp32            RenderRaysFn below: the verification path (FFMA forward re-run with fp32 activation dump, fp32 GEMMs).
 
 Gradients are produced for exactly what the reference trains: the 2 x 40 nn.Linear tensors of the coarse and fine

@@ -24,8 +24,8 @@ extern "C" int onerf_ctx_create(int device, onerf_ctx** out) {
   ONERF_CHECK_ARG(device >= 0 && device < count, "no such CUDA device");
   cudaDeviceProp prop;
   ONERF_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    onerf_set_error("onerf_ctx_create: device %d is sm_%d%d; this library is built for sm_100a only (no fallback)",
+  if (prop.major != 9 || prop.minor != 0) {
+    onerf_set_error("onerf_ctx_create: device %d is sm_%d%d; this library is built for sm_90a only (no fallback)",
                     device, prop.major, prop.minor);
     return ONERF_ERR_UNSUPPORTED;
   }

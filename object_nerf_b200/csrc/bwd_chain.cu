@@ -1,11 +1,11 @@
-// Input-gradient chain of the two-branch MLP on tcgen05 tensor cores (SURVEY.md §8 row a14): for every sample tile,
+// Input-gradient chain of the two-branch MLP on wgmma tensor cores (SURVEY.md §8 row a14): for every sample tile,
 //   dZ_dir = (dL/d rgb_pre . W_rgb) * leaky'(H_dir)                                    (CUDA cores, 3-wide head)
-//   dZ_l-1 = (dZ_l . W_l[:, hidden block]  [+ dL/d sigma . w_sigma]) * leaky'(H_l-1)    (tcgen05, fp32 accumulate)
+//   dZ_l-1 = (dZ_l . W_l[:, hidden block]  [+ dL/d sigma . w_sigma]) * leaky'(H_l-1)    (wgmma, fp32 accumulate)
 // walking the layers of models/nerf_model.py:97-152 backwards, scene branch then object branch.  It is the forward
-// machinery (tc_chain.cuh: TMA weight ring, TS-form MMAs with the operand resident in TMEM, half-layer overlap) run on
-// the TRANSPOSED weight images (layout.h: bimg_off); the LeakyReLU derivative comes from the 1-bit sign masks the training
-// forward left behind.  Every dZ_l is also written to the training workspace as bf16 atoms: the weight-gradient GEMM
-// (bwd_wgrad.cu), the encoding gradient (bwd_dx.cu) and the bias / per-ray sums (bwd_small.cu) read them from there.
+// machinery (tc_chain.cuh: bulk-copy weight ring, register-resident operand chain) run on the TRANSPOSED weight images
+// (layout.h: bimg_off); the LeakyReLU derivative comes from the 1-bit sign masks the training forward left behind.
+// Every dZ_l is also written to the training workspace as bf16 atoms: the weight-gradient GEMM (bwd_wgrad.cu), the
+// encoding gradient (bwd_dx.cu) and the bias / per-ray sums (bwd_small.cu) read them from there.
 #include "field_common.cuh"
 #include "tc_chain.cuh"
 
@@ -24,15 +24,77 @@ struct ChainParams {
   const float4* dA_obj;       // (B) or null
   int64_t total;              // samples
   int want_object;
-  int last_scene_layer;       // index of the scene branch's last chain layer
-  TcLayer layers[MAX_LAYERS];
+  WLayer layers[MAX_LAYERS];
   int n_layers;
 };
 
-__device__ __forceinline__ void st_global_chunks4(uint8_t* base, int chunk0, int swz, const uint32_t* pk) {
+struct Rows {
+  int row[2];
+  float4 dAs[2], dAo[2];
+  const uint32_t* mrow;       // &masks[tile][0][0]
+  int64_t tile;
+};
+
+// store the packed fragment (N columns, rows R.row[0..1]) into dZ slot `slot` of the tile
+template <int N>
+__device__ __forceinline__ void store_dz(const ChainParams& P, const Rows& R, int slot, const uint32_t* pk) {
+  const int q = threadIdx.x & 3;
 #pragma unroll
-  for (int j = 0; j < 4; ++j)
-    *reinterpret_cast<uint4*>(base + (((chunk0 + j) ^ swz) << 4)) = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
+  for (int r = 0; r < 2; ++r) {
+    const int row = R.row[r];
+    uint8_t* base = P.ws + P.TL.dz_off[slot] + ((size_t)R.tile * P.TL.dz_atoms[slot]) * ATOM_BYTES + (size_t)row * 128 + q * 4;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+      *reinterpret_cast<uint32_t*>(base + (size_t)(j >> 3) * ATOM_BYTES + (((j & 7) ^ (row & 7)) << 4)) = pk[2 * j + r];
+  }
+}
+
+// dZ of a direction layer from the 3-wide rgb head: N = 128 (scene, mask words 64..67) or 64 (object, 84..87)
+template <int N>
+__device__ __forceinline__ void dir_dz(const Rows& R, const float* rgb_w, int branch, uint32_t* pk) {
+  constexpr int CPW = N >= 128 ? 32 : 16;
+  const int word0 = branch ? 84 : 64, q = threadIdx.x & 3;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const float4 d = branch ? R.dAo[r] : R.dAs[r];
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const int c = 8 * j + 2 * q;
+      const uint32_t m = R.mrow[(word0 + c / CPW) * 128 + R.row[r]];
+      float v0 = d.x * rgb_w[c] + d.y * rgb_w[N + c] + d.z * rgb_w[2 * N + c];
+      float v1 = d.x * rgb_w[c + 1] + d.y * rgb_w[N + c + 1] + d.z * rgb_w[2 * N + c + 1];
+      v0 *= ((m >> (c % CPW)) & 1u) ? 1.0f : 0.01f;
+      v1 *= ((m >> ((c + 1) % CPW)) & 1u) ? 1.0f : 0.01f;
+      pk[2 * j + r] = pack_bf16(v0, v1);
+    }
+  }
+}
+
+// chain epilogue: v = acc [+ dsigma . w_sigma]  [* leaky'(mask of activation slot `act`)], bf16 pairs
+template <int N, int EPI>
+__device__ __forceinline__ void chain_epi(const float (&acc)[N / 2], uint32_t* pk, const Rows& R, int branch, int act,
+                                          const float* wsig) {
+  const int q = threadIdx.x & 3;
+  const int word0 = EPI == BE_PLAIN ? 0 : onerf_mask_word0(act);
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const float dsig = branch ? R.dAo[r].w : R.dAs[r].w;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const int c = 8 * j + 2 * q;
+      float v0 = acc[4 * j + 2 * r], v1 = acc[4 * j + 2 * r + 1];
+      if (EPI == BE_MASK_SIG) {
+        v0 = fmaf(dsig, wsig[c], v0);
+        v1 = fmaf(dsig, wsig[c + 1], v1);
+      }
+      if (EPI != BE_PLAIN) {
+        const uint32_t m = R.mrow[(word0 + (c >> 5)) * 128 + R.row[r]];
+        v0 *= ((m >> (c & 31)) & 1u) ? 1.0f : 0.01f;
+        v1 *= ((m >> ((c + 1) & 31)) & 1u) ? 1.0f : 0.01f;
+      }
+      pk[2 * j + r] = pack_bf16(v0, v1);
+    }
+  }
 }
 
 __global__ void __launch_bounds__(NUM_THREADS, 1) bwd_chain_kernel(const __grid_constant__ ChainParams P) {
@@ -42,20 +104,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) bwd_chain_kernel(const __grid_
   const uint32_t sB = sbase;
   const uint32_t sHead = sB + NSTAGE * STAGE_BYTES;                  // 960 floats: rgb_w 384 | sigma_w 256 | orgb_w 192 | osigma_w 128
   const uint32_t sBar = sHead + 960 * 4;
-  TcBars bar;
-  bar.full = sBar;
-  bar.empty = sBar + 8 * NSTAGE;
-  bar.x_ready = sBar + 16 * NSTAGE;
-  bar.acc_ready = bar.x_ready + 8;
-  bar.epi_done = bar.acc_ready + 16;
-  const uint32_t tmem_slot = bar.epi_done + 16;
   uint8_t* gen_base = smem_raw + (sbase - smem_u32(smem_raw));
   float* head = reinterpret_cast<float*>(gen_base + (sHead - sbase));
-  volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(gen_base + (tmem_slot - sbase));
   const float* Pf = reinterpret_cast<const float*>(P.packed);
+  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u};
 
-  if (threadIdx.x == 0) tc_init_bars(bar);
-  if (warp == MMA_WARP) tmem_alloc(tmem_slot, 512);
+  if (threadIdx.x == 0) ring_init_bars(ring.full, ring.empty);
   for (int i = threadIdx.x; i < 960; i += NUM_THREADS) {
     float v;
     if (i < 384) v = __ldg(Pf + P.L.rgb_w + i);
@@ -64,127 +118,73 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) bwd_chain_kernel(const __grid_
     else v = __ldg(Pf + P.L.osigma_w + (i - 832));
     head[i] = v;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_gen;
   const int64_t n_tiles = (P.total + TM - 1) / TM;
 
-  if (warp == PRODUCER_WARP) {
-    tc_producer_loop(P.layers, P.n_layers, P.packed, sB, bar, n_tiles);
-  } else if (warp == MMA_WARP) {
-    tc_mma_loop<false>(P.layers, P.n_layers, 0u, sB, bar, tmem_base, n_tiles, nullptr, nullptr, 0);
-  } else {
-    // =============================== head gradient + epilogue warps ===============================
-    const int q = warp & 3, cq = warp >> 2;          // TMEM lane quarter (rows), column quarter
-    const int row = q * 32 + lane, swz = row & 7;
-    const uint32_t lane_taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-    uint32_t acc_phase0 = 0, acc_phase1 = 0;
-    const float* rgb_w = head, *sigma_w = head + 384, *orgb_w = head + 640, *osigma_w = head + 832;
-    uint32_t* masks = reinterpret_cast<uint32_t*>(P.ws + P.TL.mask_off);
-    // nothing to drain before the very first layer
-    if (lane == 0) {
-      mbar_arrive(bar.epi_done);
-      if (P.layers[0].prev_two) mbar_arrive(bar.epi_done + 8);
-    }
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      const int64_t e = tile * TM + row;
-      const bool live = e < P.total;
-      const float4 dAs = live ? __ldg(P.dA_scene + e) : make_float4(0.f, 0.f, 0.f, 0.f);
-      const float4 dAo = (live && P.want_object) ? __ldg(P.dA_obj + e) : make_float4(0.f, 0.f, 0.f, 0.f);
-      const uint32_t* mrow = masks + (size_t)tile * ONERF_MASK_WORDS * 128 + row;
-      // ---- scene dir layer: dZ_dir (128 columns, 32 per thread) from the rgb head ----
-      {
-        const int n = cq * 32;
-        const uint32_t m = mrow[(64 + cq) * 128];
-        uint32_t pk[16];
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          float v0 = dAs.x * rgb_w[n + j] + dAs.y * rgb_w[128 + n + j] + dAs.z * rgb_w[256 + n + j];
-          float v1 = dAs.x * rgb_w[n + j + 1] + dAs.y * rgb_w[128 + n + j + 1] + dAs.z * rgb_w[256 + n + j + 1];
-          v0 *= ((m >> j) & 1u) ? 1.0f : 0.01f;
-          v1 *= ((m >> (j + 1)) & 1u) ? 1.0f : 0.01f;
-          pk[j >> 1] = pack_bf16(v0, v1);
-        }
-        tmem_st16(lane_taddr + (uint32_t)(P.layers[0].h_in_col + (n >> 1)), pk);
-        uint8_t* dst = P.ws + P.TL.dz_off[9] + ((size_t)tile * P.TL.dz_atoms[9] + (n >> 6)) * ATOM_BYTES + (size_t)row * 128;
-        st_global_chunks4(dst, (n & 63) >> 3, swz, pk);
-        tmem_st_wait();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar.x_ready);
+  if (warp >= PRODUCER_WARP) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == PRODUCER_WARP)
+      tc_producer_loop(P.layers, P.n_layers, P.packed, ring, n_tiles);
+    return;
+  }
+  setmaxnreg_inc<CONSUMER_REGS>();
 
-      for (int l = 0; l < P.n_layers; ++l) {
-        const TcLayer& Ly = P.layers[l];
-        const int HW = Ly.N >> (Ly.nhalf - 1);       // 128 for every chain layer
-        const float dsig = Ly.branch ? dAo.w : dAs.w;
-        const float* wsig = Ly.branch ? osigma_w : sigma_w;
-        const bool last_of_branch = (l == P.last_scene_layer) || (l == P.n_layers - 1);
+  const float* rgb_w = head, *sigma_w = head + 384, *orgb_w = head + 640, *osigma_w = head + 832;
+  const int wg = warp >> 2;
+  Rows R;
+  R.row[0] = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  R.row[1] = R.row[0] + 8;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    R.tile = tile;
+    R.mrow = reinterpret_cast<const uint32_t*>(P.ws + P.TL.mask_off) + (size_t)tile * ONERF_MASK_WORDS * 128;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int64_t e = tile * TM + R.row[r];
+      const bool live = e < P.total;
+      R.dAs[r] = live ? __ldg(P.dA_scene + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+      R.dAo[r] = (live && P.want_object) ? __ldg(P.dA_obj + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    {
+      // ---- scene: dZ_dir (128) -> dZ_final -> dZ_7 (+ sigma head) -> ... -> dZ_0 ----
+      uint32_t a[32];
+      dir_dz<128>(R, rgb_w, 0, a);
+      store_dz<128>(P, R, 9, a);
+      float acc[128];
+      uint32_t h[64];
+      mma_layer<256, 0, 4>(acc, a, 0u, ring);
+      chain_epi<256, BE_PLAIN>(acc, h, R, 0, 9, nullptr);
+      store_dz<256>(P, R, 8, h);
+      mma_layer<256, 0, 8>(acc, h, 0u, ring);
+      chain_epi<256, BE_MASK_SIG>(acc, h, R, 0, 8, sigma_w);
+      store_dz<256>(P, R, 7, h);
 #pragma unroll 1
-        for (int h = 0; h < Ly.nhalf; ++h) {
-          const int n = h * HW + cq * 32;            // first output column of this thread in this half
-          const uint32_t acc_addr = lane_taddr + (uint32_t)(h * TM_ACC1 + cq * 32);
-          uint32_t mword = 0xffffffffu;
-          if (Ly.epi != BE_PLAIN) mword = mrow[(Ly.mask_word0 + h * 4 + cq) * 128];   // issued before the wait
-          if (h == 0) { mbar_wait(bar.acc_ready, acc_phase0); acc_phase0 ^= 1; }
-          else { mbar_wait(bar.acc_ready + 8, acc_phase1); acc_phase1 ^= 1; }
-          tc_fence_after();
-          uint32_t v[32];
-          tmem_ld32(acc_addr, v);
-          tmem_ld_wait();
-          uint32_t pk[16];
-#pragma unroll
-          for (int j = 0; j < 32; j += 2) {
-            float v0 = __uint_as_float(v[j]), v1 = __uint_as_float(v[j + 1]);
-            if (Ly.epi == BE_MASK_SIG) {
-              v0 = fmaf(dsig, wsig[n + j], v0);
-              v1 = fmaf(dsig, wsig[n + j + 1], v1);
-            }
-            v0 *= ((mword >> j) & 1u) ? 1.0f : 0.01f;
-            v1 *= ((mword >> (j + 1)) & 1u) ? 1.0f : 0.01f;
-            pk[j >> 1] = pack_bf16(v0, v1);
-          }
-          if (!last_of_branch) tmem_st16(lane_taddr + (uint32_t)(Ly.h_out_col + (n >> 1)), pk);
-          {
-            const int sl = Ly.act_slot;   // dZ slot
-            uint8_t* dst = P.ws + P.TL.dz_off[sl] + ((size_t)tile * P.TL.dz_atoms[sl] + (n >> 6)) * ATOM_BYTES + (size_t)row * 128;
-            st_global_chunks4(dst, (n & 63) >> 3, swz, pk);
-          }
-          if (l == P.last_scene_layer && h == 0 && P.want_object) {
-            // ---- object dir layer: dZ_odir (64 columns, 16 per thread) from the object rgb head, written where the
-            //      first object chain layer reads its operand ----
-            const int no = cq * 16;
-            const uint32_t mo = mrow[(84 + cq) * 128];
-            uint32_t po[8];
-#pragma unroll
-            for (int j = 0; j < 16; j += 2) {
-              float v0 = dAo.x * orgb_w[no + j] + dAo.y * orgb_w[64 + no + j] + dAo.z * orgb_w[128 + no + j];
-              float v1 = dAo.x * orgb_w[no + j + 1] + dAo.y * orgb_w[64 + no + j + 1] + dAo.z * orgb_w[128 + no + j + 1];
-              v0 *= ((mo >> j) & 1u) ? 1.0f : 0.01f;
-              v1 *= ((mo >> (j + 1)) & 1u) ? 1.0f : 0.01f;
-              po[j >> 1] = pack_bf16(v0, v1);
-            }
-            tmem_st8(lane_taddr + (uint32_t)(P.layers[l + 1].h_in_col + (no >> 1)), po);
-            uint8_t* dst = P.ws + P.TL.dz_off[15] + ((size_t)tile * P.TL.dz_atoms[15]) * ATOM_BYTES + (size_t)row * 128;
-            const int c0 = no >> 3;
-            *reinterpret_cast<uint4*>(dst + (((c0) ^ swz) << 4)) = make_uint4(po[0], po[1], po[2], po[3]);
-            *reinterpret_cast<uint4*>(dst + (((c0 + 1) ^ swz) << 4)) = make_uint4(po[4], po[5], po[6], po[7]);
-          }
-          tmem_st_wait();
-          // accumulator half h drained, output of this half written
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar.epi_done + 8 * h);
-        }
+      for (int l = 7; l >= 1; --l) {
+        mma_layer<256, 0, 8>(acc, h, 0u, ring);
+        chain_epi<256, BE_MASK>(acc, h, R, 0, l, nullptr);
+        store_dz<256>(P, R, l - 1, h);
+      }
+    }
+    if (P.want_object) {
+      // ---- object: dZ_odir (64) -> dZ_ofinal -> dZ_o3 (+ sigma head) -> ... -> dZ_o0 ----
+      uint32_t a[16];
+      dir_dz<64>(R, orgb_w, 1, a);
+      store_dz<64>(P, R, 15, a);
+      float acc[64];
+      uint32_t h[32];
+      mma_layer<128, 0, 2>(acc, a, 0u, ring);
+      chain_epi<128, BE_PLAIN>(acc, h, R, 1, 15, nullptr);
+      store_dz<128>(P, R, 14, h);
+      mma_layer<128, 0, 4>(acc, h, 0u, ring);
+      chain_epi<128, BE_MASK_SIG>(acc, h, R, 1, 14, osigma_w);
+      store_dz<128>(P, R, 13, h);
+#pragma unroll 1
+      for (int l = 3; l >= 1; --l) {
+        mma_layer<128, 0, 4>(acc, h, 0u, ring);
+        chain_epi<128, BE_MASK>(acc, h, R, 1, 10 + l, nullptr);
+        store_dz<128>(P, R, 10 + l - 1, h);
       }
     }
   }
-
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace
@@ -203,27 +203,20 @@ int onerf_launch_bwd_chain(onerf_ctx* ctx, int use_voxel, int want_object, const
   P.total = n_samples;
   P.want_object = want_object;
   int n = 0;
-  // chain layer: operand = dZ of GEMM `g` (its N outputs = K of this layer), result = dZ slot `dz_out` (hid_n wide),
-  // masked by the sign mask of the activation that dZ slot belongs to (activation slot dz_out + 1)
-  auto add = [&](int g, int epi, int branch, int dz_out, bool first_of_branch) {
-    const int act = dz_out + 1;
-    tc_add_layer(P.layers, n, L.g[g].hid_n, 0, L.g[g].N / 32, epi, branch, 0, L.g[g].bimg_off, 0, 128, dz_out,
-                 epi == BE_PLAIN ? -1 : onerf_mask_word0(act), false, first_of_branch);
-  };
-  add(G_SDIR, BE_PLAIN, 0, 8, true);       // dZ_dir (128) -> dZ_final (no activation on the final layer)
-  add(G_SFIN, BE_MASK_SIG, 0, 7, false);   // -> dZ_7 (+ sigma head)
-  for (int l = 7; l >= 1; --l) add(G_S0 + l, BE_MASK, 0, l - 1, false);
-  P.last_scene_layer = n - 1;
+  // chain layer of GEMM g: operand = dZ of g (its N outputs = K of this layer), result = the hid_n inputs of g
+  auto add = [&](int g) { P.layers[n++] = WLayer{L.g[g].bimg_off, L.g[g].hid_n, L.g[g].N / 32}; };
+  add(G_SDIR);
+  add(G_SFIN);
+  for (int l = 7; l >= 1; --l) add(G_S0 + l);
   if (want_object) {
-    add(G_ODIR, BE_PLAIN, 1, 14, true);    // dZ_odir (64) -> dZ_ofinal
-    add(G_OFIN, BE_MASK_SIG, 1, 13, false);
-    for (int l = 3; l >= 1; --l) add(G_O0 + l, BE_MASK, 1, 10 + l - 1, false);
+    add(G_ODIR);
+    add(G_OFIN);
+    for (int l = 3; l >= 1; --l) add(G_O0 + l);
   }
   P.n_layers = n;
-  tc_finish_program(P.layers, n);
   const int64_t tiles = (n_samples + TM - 1) / TM;
   const int blocks = (int)(tiles < ctx->num_sms ? tiles : ctx->num_sms);
-  const size_t smem = 1024 + NSTAGE * STAGE_BYTES + 960 * 4 + 512;
+  const size_t smem = 1024 + NSTAGE * STAGE_BYTES + 960 * 4 + 16 * NSTAGE;
   ONERF_CUDA(cudaFuncSetAttribute(bwd_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   bwd_chain_kernel<<<blocks, NUM_THREADS, smem, stream>>>(P);
   ONERF_LAUNCH_CHECK(ctx);

@@ -1,19 +1,21 @@
-// Weight-gradient GEMMs of the two-branch MLP on tcgen05 tensor cores (SURVEY.md §8 row a14; what autograd does for
+// Weight-gradient GEMMs of the two-branch MLP on wgmma tensor cores (SURVEY.md §8 row a14; what autograd does for
 // every nn.Linear of models/nerf_model.py:97-152:  dW_l += dZ_l^T . In_l, reduction over ALL samples).
 //
 // Operands are the bf16 "atoms" the training forward and the input-gradient chain leave in the training workspace
 // (layout.h: [128 samples x 64 columns] SWIZZLE_128B images).  For this GEMM the reduction (K) dimension is the
-// SAMPLE axis, so both operands are MN-major UMMA operands: the very same atom image that the chain consumed K-major.
+// SAMPLE axis, so both operands are MN-major (transposed) wgmma operands: the very same atom image that the chain
+// consumed K-major.
 //   D[M = outputs of layer l  x  N = inputs of layer l] += A[M x K] . B[N x K]^T,  K = samples
 //   A: dZ atoms (64 output columns each), B: activation atoms (64 input columns each)
-// One persistent CTA per SM.  The (layer, column block) work items are laid end to end, each weighted by the bytes it
-// streams per 64-sample stage (the kernel is HBM-bound: 128 FLOP per byte), and the byte axis is cut into gridDim.x
-// equal pieces: a CTA owns one contiguous piece = a few (item, stage range) segments.  Per segment the accumulators
-// live in TMEM ([128 x 256] fp32 per 128 outputs) and are flushed once with vector reductions (REDG.ADD.F32x4) into
-// the kernel-layout gradient buffer (layout.h: GradLayout).
-//   warp 4: producer (cp.async.bulk, 3-stage ring of 64-sample stages)   warp 5: tcgen05.mma issuer (owns TMEM)
-//   warps 0-3: accumulator drain; while the ring streams they also form the bias gradients db_l = sum_s dZ_l from the
-//              dZ tiles that are passing through shared memory anyway (first column block of every layer)
+// One persistent CTA per SM.  The (layer, 128-output block, input column block) work items are laid end to end, each
+// weighted by the bytes it streams per 64-sample stage (the kernel is HBM-bound), and the byte axis is cut into
+// gridDim.x equal pieces: a CTA owns one contiguous piece = a few (item, stage range) segments.  Per segment each of the
+// two consumer warpgroups accumulates 64 outputs x up to 256 inputs in registers and flushes them once with vector
+// reductions (red.global.add.v2.f32) into the kernel-layout gradient buffer (layout.h: GradLayout).
+//   warp 8: producer (cp.async.bulk, 4-stage ring of 64-sample stages)
+//   warpgroups 0 / 1: wgmma on dZ atom 0 / 1 of the item; while the ring streams, the first warp of each also forms the
+//   bias gradients db_l = sum_s dZ_l from the dZ tiles that are passing through shared memory anyway (first column
+//   block of every layer)
 #include "common.cuh"
 #include "layout.h"
 #include "tc_common.cuh"
@@ -22,23 +24,23 @@ namespace {
 
 using namespace tc;
 
-constexpr int WG_STAGES = 3;
+constexpr int WG_STAGES = 4;
 constexpr int HALF_ATOM = 8192;                 // 64 samples x 128 B
-constexpr int WG_STAGE_BYTES = 8 * HALF_ATOM;   // up to 4 A half-atoms + 4 B half-atoms
-constexpr int WG_THREADS = 192;
-constexpr int WG_MAX_ITEMS = 24;
+constexpr int WG_STAGE_BYTES = 6 * HALF_ATOM;   // 2 A half-atoms + up to 4 B half-atoms
+constexpr int WG_THREADS = 288;
+constexpr int WG_MAX_ITEMS = 40;
 
 struct WgItem {
   int64_t a_off;      // byte offset of the A slot (dZ) in the workspace
   int64_t b_off;      // byte offset of the B slot (activations)
   int a_atoms_slot;   // atoms per tile of the A slot
   int b_atoms_slot;
-  int a_atom0, a_atoms;   // M block: atoms a_atom0 .. + a_atoms (2 = one accumulator, 4 = two)
+  int a_atom0;        // M block: atoms a_atom0, a_atom0 + 1 (128 outputs)
   int b_atom0, b_atoms;   // N block: 1..4 atoms
   int64_t out_off;    // float offset of D[0][0] in the gradient buffer
   int out_ld;
-  int m_valid, n_valid;
-  int cost;           // a_atoms + b_atoms (8 KB units per stage)
+  int m_valid, n_valid;   // outputs of the layer, valid input columns of the block
+  int cost;           // 2 + b_atoms (8 KB units per stage)
   int64_t db_off;     // float offset of the layer's bias gradient, or -1: this item does not form it
 };
 
@@ -50,20 +52,8 @@ struct WgParams {
   WgItem items[WG_MAX_ITEMS];
 };
 
-// MN-major SWIZZLE_128B shared-memory descriptor (cute::UMMA::SmemDescriptor, make_umma_desc<Major::MN>):
-//   canonical layout ((8,n),(8,k)) : ((1,LBO),(8,SBO)) in 16-byte units: 128 B of MN per K row, 8 K rows per 1024-byte
-//   group (SBO), 64-wide MN blocks LBO apart.
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-// instruction descriptor: D fp32, A/B bf16, both MN-major, M = 128
-__device__ __forceinline__ uint32_t make_idesc_mn(int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
-__device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+__device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 
 // segment s of this CTA: item index and stage range; returns false when there is no further segment
@@ -98,152 +88,118 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sStage = sbase;
   const uint32_t sBar = sStage + WG_STAGES * WG_STAGE_BYTES;
-  const uint32_t bar_full = sBar, bar_empty = sBar + 8 * WG_STAGES, bar_acc_ready = sBar + 16 * WG_STAGES,
-                 bar_acc_free = bar_acc_ready + 8, tmem_slot = bar_acc_free + 8;
-  volatile uint32_t* tmem_slot_gen =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (sbase - smem_u32(smem_raw)) + (tmem_slot - sbase));
+  const uint32_t bar_full = sBar, bar_empty = sBar + 8 * WG_STAGES;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < WG_STAGES; ++s) {
       mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, 1 + 4);   // tcgen05.commit + the four drain warps (they read the dZ tiles)
+      mbar_init(bar_empty + 8 * s, 8);   // one arrival per consumer warp
     }
-    mbar_init(bar_acc_ready, 1);
-    mbar_init(bar_acc_free, 4);
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_gen;
 
   // this CTA's piece of the byte axis
   int64_t total = 0;
   for (int i = 0; i < P.n_items; ++i) total += (int64_t)P.items[i].cost * P.n_stages;
   const int64_t lo = total * blockIdx.x / gridDim.x, hi = total * (blockIdx.x + 1) / gridDim.x;
+  int item = 0;
+  int64_t item_start = 0;
+  Segment seg;
+  uint32_t stage = 0, phase = 0;
 
-  if (warp == 4) {
+  if (warp == 8) {
     // =============================== producer ===============================
-    uint32_t stage = 0, phase = 0;
-    int item = 0;
-    int64_t item_start = 0;
-    Segment seg;
     while (next_segment(P, lo, hi, item, item_start, seg)) {
       const WgItem& it = P.items[seg.item];
       for (int s = seg.s0; s < seg.s1; ++s) {
         const int tile = s >> 1, half = s & 1;
         mbar_wait(bar_empty + 8 * stage, phase ^ 1);
         if (elect_one()) {
-          mbar_expect_tx(bar_full + 8 * stage, (uint32_t)(it.a_atoms + it.b_atoms) * HALF_ATOM);
+          mbar_expect_tx(bar_full + 8 * stage, (uint32_t)(2 + it.b_atoms) * HALF_ATOM);
           const uint32_t dst = sStage + stage * WG_STAGE_BYTES;
           const uint8_t* a = P.ws + it.a_off + ((size_t)tile * it.a_atoms_slot + it.a_atom0) * ATOM_BYTES + (size_t)half * HALF_ATOM;
-          for (int i = 0; i < it.a_atoms; ++i)
+          for (int i = 0; i < 2; ++i)
             tma_bulk_g2s(dst + i * HALF_ATOM, a + (size_t)i * ATOM_BYTES, HALF_ATOM, bar_full + 8 * stage);
           const uint8_t* b = P.ws + it.b_off + ((size_t)tile * it.b_atoms_slot + it.b_atom0) * ATOM_BYTES + (size_t)half * HALF_ATOM;
           for (int i = 0; i < it.b_atoms; ++i)
-            tma_bulk_g2s(dst + (4 + i) * HALF_ATOM, b + (size_t)i * ATOM_BYTES, HALF_ATOM, bar_full + 8 * stage);
+            tma_bulk_g2s(dst + (2 + i) * HALF_ATOM, b + (size_t)i * ATOM_BYTES, HALF_ATOM, bar_full + 8 * stage);
         }
         __syncwarp();
         if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 5) {
-    // =============================== MMA issuer ===============================
-    uint32_t stage = 0, phase = 0, free_phase = 0;
-    int item = 0, nseg = 0;
-    int64_t item_start = 0;
-    Segment seg;
-    while (next_segment(P, lo, hi, item, item_start, seg)) {
-      const WgItem& it = P.items[seg.item];
-      const uint32_t idesc = make_idesc_mn(it.b_atoms * 64);
-      if (nseg > 0) {   // the previous segment's accumulators have been drained
-        mbar_wait(bar_acc_free, free_phase);
-        free_phase ^= 1;
-        tc_fence_after();
-      }
-      ++nseg;
-      for (int s = seg.s0; s < seg.s1; ++s) {
-        mbar_wait(bar_full + 8 * stage, phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sa = sStage + stage * WG_STAGE_BYTES, sb = sa + 4 * HALF_ATOM;
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            const uint64_t bdesc = make_desc_mn(sb + k16 * 2048, HALF_ATOM, 1024);
-            for (int mh = 0; mh < (it.a_atoms >> 1); ++mh) {
-              const uint64_t adesc = make_desc_mn(sa + mh * 2 * HALF_ATOM + k16 * 2048, HALF_ATOM, 1024);
-              umma_bf16(tmem_base + (uint32_t)(mh * 256), adesc, bdesc, idesc, (s > seg.s0 || k16 > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(bar_empty + 8 * stage);
-          if (s == seg.s1 - 1) umma_commit(bar_acc_ready);
-        }
-        __syncwarp();
-        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else {
-    // =============================== bias gradients + accumulator drain ===============================
-    uint32_t ready_phase = 0, stage = 0, phase = 0;
-    int item = 0;
-    int64_t item_start = 0;
-    Segment seg;
-    const int m = warp * 32 + lane;
-    const uint32_t lane_taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    while (next_segment(P, lo, hi, item, item_start, seg)) {
-      const WgItem& it = P.items[seg.item];
-      // thread t owns dZ columns 64 (t / 32) + 2 (t % 32), + 1 of the M block: word (t % 32) of every row of atom t / 32
-      const bool cs = it.db_off >= 0 && warp < it.a_atoms;
-      float c0 = 0.0f, c1 = 0.0f;
-      for (int s = seg.s0; s < seg.s1; ++s) {
-        mbar_wait(bar_full + 8 * stage, phase);
-        if (cs) {
-          const uint32_t base = sStage + stage * WG_STAGE_BYTES + (uint32_t)warp * HALF_ATOM + (uint32_t)(lane & 3) * 4u;
-#pragma unroll 8
-          for (int r = 0; r < 64; ++r) {
-            uint32_t w;
-            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(base + (uint32_t)r * 128u + ((((uint32_t)lane >> 2) ^ ((uint32_t)r & 7u)) << 4)));
-            c0 += __uint_as_float(w << 16);
-            c1 += __uint_as_float(w & 0xffff0000u);
-          }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_empty + 8 * stage);
-        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (cs && warp * 64 + 2 * lane < it.m_valid) {
-        atomicAdd(P.grad + it.db_off + warp * 64 + 2 * lane, c0);
-        atomicAdd(P.grad + it.db_off + warp * 64 + 2 * lane + 1, c1);
-      }
-      mbar_wait(bar_acc_ready, ready_phase);
-      ready_phase ^= 1;
-      tc_fence_after();
-      for (int mh = 0; mh < (it.a_atoms >> 1); ++mh) {
-        const int row = mh * 128 + m;
-        float* out = P.grad + it.out_off + (int64_t)row * it.out_ld;
-        for (int c0_ = 0; c0_ < it.b_atoms * 64; c0_ += 32) {
-          uint32_t v[32];
-          tmem_ld32(lane_taddr + (uint32_t)(mh * 256 + c0_), v);
-          tmem_ld_wait();
-          if (row < it.m_valid) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              if (c0_ + j < it.n_valid)
-                red_add_v4(out + c0_ + j, __uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                           __uint_as_float(v[j + 3]));
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_acc_free);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, 512);
+  // =============================== consumers: wgmma + bias gradients + flush ===============================
+  const int wg = warp >> 2, wi = warp & 3, q = lane & 3;
+  while (next_segment(P, lo, hi, item, item_start, seg)) {
+    const WgItem& it = P.items[seg.item];
+    const int nb = it.b_atoms;
+    // the first warp of a warpgroup owns dZ columns 2 lane, 2 lane + 1 of its atom: word `lane` of every sample row
+    const bool cs = it.db_off >= 0 && wi == 0;
+    float c0 = 0.0f, c1 = 0.0f;
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.0f;
+    uint32_t prev = 0;
+    for (int s = seg.s0; s < seg.s1; ++s) {
+      mbar_wait(bar_full + 8 * stage, phase);
+      const uint32_t sa = sStage + stage * WG_STAGE_BYTES + (uint32_t)wg * HALF_ATOM, sb = sStage + stage * WG_STAGE_BYTES + 2 * HALF_ATOM;
+      wgmma_fence();
+#pragma unroll
+      for (int k16 = 0; k16 < 4; ++k16) {
+        const uint64_t ad = desc_mn_sw128(sa + (uint32_t)k16 * 2048u, HALF_ATOM);
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          if (i < nb) wgmma_ss_n64<1, 1>(acc + 32 * i, ad, desc_mn_sw128(sb + (uint32_t)i * HALF_ATOM + (uint32_t)k16 * 2048u, HALF_ATOM));
+      }
+      wgmma_commit();
+      if (cs) {
+        const uint32_t base = sa + (uint32_t)(lane & 3) * 4u;
+#pragma unroll 8
+        for (int r = 0; r < 64; ++r) {
+          uint32_t w;
+          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(base + (uint32_t)r * 128u + ((((uint32_t)lane >> 2) ^ ((uint32_t)r & 7u)) << 4)));
+          c0 += bf16_lo(w);
+          c1 += bf16_hi(w);
+        }
+      }
+      if (s > seg.s0) {   // the previous stage's MMAs have completed
+        wgmma_wait<1>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+      }
+      prev = stage;
+      if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+    fence_regs<128>(acc);
+    const int m0 = (it.a_atom0 + wg) * 64;
+    if (cs && m0 + 2 * lane < it.m_valid) {
+      atomicAdd(P.grad + it.db_off + m0 + 2 * lane, c0);
+      atomicAdd(P.grad + it.db_off + m0 + 2 * lane + 1, c1);
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int m = m0 + wi * 16 + (lane >> 2) + 8 * r;
+      if (m >= it.m_valid) continue;
+      float* out = P.grad + it.out_off + (int64_t)m * it.out_ld;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        if (i < nb) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int c = 64 * i + 8 * j + 2 * q;
+            if (c < it.n_valid) red_add_v2(out + c, acc[32 * i + 4 * j + 2 * r], acc[32 * i + 4 * j + 2 * r + 1]);
+          }
+        }
+      }
+    }
+  }
 }
 
 }  // namespace
@@ -263,21 +219,24 @@ int onerf_launch_wgrad(onerf_ctx* ctx, int use_voxel, int want_object, const voi
   const int gemm_of[ONERF_DZ_SLOTS] = {G_S0, G_S1, G_S2, G_S3, G_S4, G_S5, G_S6, G_S7, G_SFIN, G_SDIR,
                                        G_O0, G_O1, G_O2, G_O3, G_OFIN, G_ODIR};
   int n = 0;
-  bool db_done[ONERF_DZ_SLOTS] = {};
-  // input blocks of a layer: (activation slot, first atom, atoms, first kernel-K column, valid columns)
+  bool db_done[ONERF_DZ_SLOTS][2] = {};
+  // input blocks of a layer: (activation slot, first atom, atoms, first kernel-K column, valid columns); one item per
+  // 128 outputs
   auto add = [&](int dz, int act, int b_atom0, int b_atoms, int col0, int n_valid) {
     const int g = gemm_of[dz];
     const int out_n = L.g[g].N;                 // 256 / 128 / 64
-    WgItem& it = P.items[n++];
-    it.a_off = T.dz_off[dz]; it.a_atoms_slot = T.dz_atoms[dz];
-    it.b_off = T.act_off[act]; it.b_atoms_slot = T.act_atoms[act];
-    it.a_atom0 = 0; it.a_atoms = out_n >= 256 ? 4 : 2;   // the 64-wide object dir layer reads one atom past its slot
-    it.b_atom0 = b_atom0; it.b_atoms = b_atoms;
-    it.out_off = G.w_off[g] + col0; it.out_ld = L.g[g].K;
-    it.m_valid = out_n; it.n_valid = n_valid;
-    it.cost = it.a_atoms + it.b_atoms;
-    it.db_off = db_done[dz] ? -1 : G.b_off[g];   // the first column block of a layer also forms its bias gradient
-    db_done[dz] = true;
+    for (int mb = 0; mb < (out_n + 127) / 128; ++mb) {
+      WgItem& it = P.items[n++];
+      it.a_off = T.dz_off[dz]; it.a_atoms_slot = T.dz_atoms[dz];
+      it.b_off = T.act_off[act]; it.b_atoms_slot = T.act_atoms[act];
+      it.a_atom0 = 2 * mb;   // the 64-wide object dir layer reads one atom past its slot
+      it.b_atom0 = b_atom0; it.b_atoms = b_atoms;
+      it.out_off = G.w_off[g] + col0; it.out_ld = L.g[g].K;
+      it.m_valid = out_n; it.n_valid = n_valid;
+      it.cost = 2 + it.b_atoms;
+      it.db_off = db_done[dz][mb] ? -1 : G.b_off[g];   // the first column block of a layer also forms its bias gradient
+      db_done[dz][mb] = true;
+    }
   };
   const int xa = use_voxel ? 4 : 1;             // leading X atoms (256 / 64 columns)
   auto x_blocks = [&](int dz, int kx) {         // X[0, kx)

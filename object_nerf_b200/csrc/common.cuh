@@ -1,4 +1,4 @@
-// Shared helpers for libonerf_sm100.so (sm_100a only).
+// Shared helpers for libonerf_sm90.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,4 +1,4 @@
-// Parameters shared by the field kernels (FFMA and tcgen05) and their launchers.
+// Parameters shared by the field kernels (FFMA and wgmma) and their launchers.
 #pragma once
 #include "common.cuh"
 #include "layout.h"

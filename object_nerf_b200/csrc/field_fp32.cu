@@ -2,7 +2,7 @@
 // with the tensor-core path, and the stand-alone encode entry point.
 //
 // This is the verification / gradient-check arithmetic (ONERF_PREC_FP32): same fusion and data flow as
-// the tcgen05 kernel in field_tc.cu, fp32 end to end, accurate sinf/cosf.  A CTA owns 32 consecutive
+// the wgmma kernel in field_tc.cu, fp32 end to end, accurate sinf/cosf.  A CTA owns 32 consecutive
 // samples; activations live in shared memory as [k][32 samples]; each layer is a register-tiled
 // 32 x N GEMM (thread = 4 samples x N/32 outputs) streaming W^T rows from L1/L2.
 //

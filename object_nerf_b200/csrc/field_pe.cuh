@@ -1,5 +1,5 @@
-// Positional encoding of one sample row into UMMA K-major SWIZZLE_128B shared-memory atoms (the A operand "X" of the
-// X-fed layers), shared by the fused forward kernels (field_tc.cu, field_tc2.cu).
+// Positional encoding of one sample row into K-major SWIZZLE_128B shared-memory atoms (the A operand "X" of the
+// X-fed layers) of the fused forward kernel (field_tc.cu).
 // Reference: models/embedding_helper.py:57-74 (Embedding.forward), :403-409 (channel split + PE of the voxel features).
 #pragma once
 #include "tc_common.cuh"
@@ -71,35 +71,6 @@ __device__ __forceinline__ void pe_xyz_to_chunks(uint32_t xbase, int row, int ch
 #pragma unroll
   for (int q = 0; q < 8; ++q)
     st_chunk(a_chunk_addr(xbase, row, chunk0 + q), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-}
-
-// ---- training dump (field_tc.cu, field_tc2.cu): bf16 activation atoms and LeakyReLU sign masks, layout.h: TrainLayout ----
-// where one thread's output of one layer half goes in the training dump
-struct DumpDst {
-  uint8_t* row;      // byte address of (tile, atom 0, this row) of the layer's activation slot; null = no dump
-  uint32_t* mask;    // &masks[tile][word 0 of the layer][this row], stride 128 words per mask word; null = no mask
-  int swz;           // row & 7
-};
-// store NP packed bf16 pairs (columns n .. n + 2 NP - 1 of the layer) and their sign bits
-template <int NP>
-__device__ __forceinline__ void dump_packed(const DumpDst& d, int n, int word, const uint32_t* pk) {
-  if (d.row == nullptr) return;
-  uint8_t* base = d.row + (size_t)(n >> 6) * ATOM_BYTES;
-  const int chunk0 = (n & 63) >> 3;
-#pragma unroll
-  for (int j = 0; j < NP / 4; ++j)
-    *reinterpret_cast<uint4*>(base + (((chunk0 + j) ^ d.swz) << 4)) = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-  if (d.mask) {
-    // bit 2 j / 2 j + 1 = 1 where the low / high bf16 of pk[j] is non-negative.  Four values at a time: the two sign-carrying
-    // bytes of two words gathered by one PRMT, their top bits squeezed into a nibble by one multiply.
-    uint32_t m = 0;
-#pragma unroll
-    for (int k = 0; k < NP / 2; ++k) {
-      const uint32_t y = (__byte_perm(pk[2 * k], pk[2 * k + 1], 0x7531) >> 7) & 0x01010101u;
-      m |= ((((y * 0x01020408u) >> 24) & 15u) ^ 15u) << (4 * k);
-    }
-    d.mask[word * 128] = m;
-  }
 }
 
 

@@ -1,43 +1,26 @@
-// tcgen05 (5th-gen tensor core) implementation of the fused encode + two-branch MLP for sm_100a.
+// wgmma (Hopper tensor core) implementation of the fused encode + two-branch MLP for sm_90a.
 //
-// One persistent CTA per SM; a CTA owns one M = 128 tile of consecutive samples at a time.
-//   warps 0-15 (512 thr)  encode the tile into shared memory (X, bf16, UMMA K-major SWIZZLE_128B atoms) and run
-//                         every layer's epilogue: TMEM accumulator -> registers (tcgen05.ld) -> bias / per-ray
-//                         constant -> LeakyReLU -> bf16x2 -> back into TMEM (tcgen05.st) as the NEXT layer's A
-//                         operand.  Hidden activations never touch shared or global memory.  Heads (sigma,
-//                         rgb) are CUDA-core dot products on the fp32 values.
-//   warp 16    (1 lane)   streams the weights global -> shared with cp.async.bulk (TMA): one (N/2 x 32) bf16
-//                         half K-slab per stage (pre-swizzled SWIZZLE_64B stage images written by pack.cu),
-//                         NSTAGE-deep mbarrier ring running ahead across layers and tiles.
-//   warp 17    (1 lane)   issues tcgen05.mma (M=128, K=16, bf16 x bf16 -> fp32 in TMEM): A from shared memory
-//                         (X slabs) or from TMEM (hidden slabs), B from the weight ring; owns the TMEM allocation.
-// Overlap: the N = 256 layers are computed as two halves of 128 outputs.  While the epilogue warps drain half 0, the
-// tensor pipe computes half 1; the next layer's half 0 starts on the K range produced by the first epilogue half as
-// soon as that is written, and waits for the second only for the remaining K slabs.  Layers with N <= 128 (dir and
-// object layers) use one accumulator and full-width MMAs: narrow MMAs are bound by the issue rate of the single
-// MMA thread (~45-65 cycles per instruction whatever N), so two N = 64 halves would cost twice the issue time and
-// twice the barrier hand-offs for the same tensor work (measured: 700 -> 763 TFLOP/s, profiles/r01_experiments.md).
-// TMEM map (512 columns): [0,256) accumulator halves at 0 / 128, [256,384) and [384,512) activation ping-pong
-// (bf16 pairs packed in 32-bit columns: K = 2c, 2c+1 in column c).
+// One persistent CTA per SM; a CTA owns one 128-sample tile at a time (tc_chain.cuh).
+//   warpgroups 0 / 1 (256 thr)  encode rows [0, 64) / [64, 128) of the tile into shared memory (X, bf16, K-major
+//                               SWIZZLE_128B atoms) and run every layer on them: wgmma M = 64 with the accumulator in
+//                               registers, then the epilogue (bias / per-ray constant -> LeakyReLU -> bf16 pairs) leaves
+//                               the output in registers as the NEXT layer's A operand.  Hidden activations never touch
+//                               shared or global memory.  Heads (sigma, rgb) are CUDA-core dot products on the fp32
+//                               values, reduced over the four lanes that share a row.
+//   warpgroup 2                 its first warp streams the weights global -> shared with cp.async.bulk (pre-swizzled
+//                               SWIZZLE_64B stage images written by pack.cu) through an mbarrier ring running ahead across
+//                               layers and tiles; the warpgroup hands most of its registers to warpgroups 0 / 1.
 // Skip / dir / code concatenations never materialise: a skip layer takes K-slabs from both X and H, and the
 // per-ray-constant terms arrive through ray_const (see layout.h).
 //
 // Reference semantics: models/rendering.py:85-137, models/nerf_model.py:97-152,
 // models/embedding_helper.py:325-411, render_tools/multi_rendering.py:16-93.
 #include <cuda_bf16.h>
-#include <cstdlib>
 
 #include "encode.cuh"
 #include "field_common.cuh"
 #include "tc_chain.cuh"
 #include "field_pe.cuh"
-
-// In-kernel clock64() timeline (tools/timeline.py): compiled in only with -DONERF_TIMELINE (make TIMELINE=1).
-#ifdef ONERF_TIMELINE
-#define ONERF_TL_ON true
-#else
-#define ONERF_TL_ON false
-#endif
 
 namespace {
 
@@ -49,37 +32,26 @@ enum Epi { EPI_HIDDEN = 0, EPI_HIDDEN_RC = 1, EPI_HIDDEN_SIGMA = 2, EPI_FINAL = 
 
 struct TcParams {
   FieldParams f;
-  long long* timeline;   // debug: per-event clock64() of block 0, second tile (null = off); see tools/timeline.py
-  TcLayer layers[MAX_LAYERS];
+  WLayer layers[MAX_LAYERS];   // producer program (same order as the consumers' layer sequence)
   int n_layers;
-  int x_atoms;     // 6 (voxel) or 1 (plain)
   // training forward (DUMP): every layer's output activations (bf16 atoms), the encoded input X and the LeakyReLU sign
   // masks are left in the training workspace for the tensor-core backward (layout.h: TrainLayout)
   uint8_t* dump;
   TrainLayout TL;
 };
 
-// ------------------------------------------------------------------------------------------------
-// epilogue of one layer half for one thread: NC accumulator columns of its row
-// ------------------------------------------------------------------------------------------------
-template <int NC>
-__device__ __forceinline__ void tmem_ld_cols(uint32_t taddr, uint32_t* v) {
-  if constexpr (NC == 32) { tmem_ld16(taddr, v); tmem_ld16(taddr + 16, v + 16); }
-  else if constexpr (NC == 16) { tmem_ld16(taddr, v); }
-  else {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr)
-                 : "memory");
-  }
-}
-template <int NP>
-__device__ __forceinline__ void tmem_st_cols(uint32_t taddr, const uint32_t* v) {
-  if constexpr (NP == 16) tmem_st16(taddr, v);
-  else if constexpr (NP == 8) tmem_st8(taddr, v);
-  else asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-                    "r"(v[2]), "r"(v[3]) : "memory");
-}
+struct RowMeta {
+  int ray, si, mute, live;   // mute bit 0: scene sigma muted, bit 1: object sigma muted
+};
+
+// the two rows of one thread in the accumulator fragment (tc_common.cuh)
+struct Rows {
+  int row[2];       // tile rows
+  int live[2];
+  int ray[2], si[2], mute[2];
+  const float* rc[2];
+  int64_t tile;
+};
 
 __device__ __forceinline__ uint32_t leaky_bf16x2(uint32_t x) {
   __nv_bfloat162 v = *reinterpret_cast<__nv_bfloat162*>(&x);
@@ -88,98 +60,108 @@ __device__ __forceinline__ uint32_t leaky_bf16x2(uint32_t x) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-// Hidden / final layer: t = acc + bias in fp32, one rounding to bf16, LeakyReLU on packed bf16 pairs,
-// result written to TMEM as the next layer's A operand.  BIAS_GLOBAL: per-ray constant from global memory.
-template <int NC, bool ACT, bool BIAS_GLOBAL>
-__device__ __forceinline__ void epi_hidden(uint32_t acc_addr, const float* bias, uint32_t out_addr, const DumpDst& dd, int n, int word) {
-  uint32_t v[NC];
-  tmem_ld_cols<NC>(acc_addr, v);
-  tmem_ld_wait();
-  uint32_t pk[NC / 2];
+// store the packed output of one layer and (mask_word0 >= 0) its sign masks in the training dump
+template <int N>
+__device__ __forceinline__ void dump_layer(const TcParams& P, const Rows& R, int slot, int mask_word0, const uint32_t* pk) {
+  const int q = threadIdx.x & 3;
 #pragma unroll
-  for (int j4 = 0; j4 < NC / 4; ++j4) {
-    float4 b;
-    if (BIAS_GLOBAL) b = __ldg(reinterpret_cast<const float4*>(bias) + j4);
-    else b = *(reinterpret_cast<const float4*>(bias) + j4);
-    uint32_t p0 = pack_bf16(__uint_as_float(v[4 * j4 + 0]) + b.x, __uint_as_float(v[4 * j4 + 1]) + b.y);
-    uint32_t p1 = pack_bf16(__uint_as_float(v[4 * j4 + 2]) + b.z, __uint_as_float(v[4 * j4 + 3]) + b.w);
-    if (ACT) { p0 = leaky_bf16x2(p0); p1 = leaky_bf16x2(p1); }
-    pk[2 * j4] = p0;
-    pk[2 * j4 + 1] = p1;
-  }
-  tmem_st_cols<NC / 2>(out_addr, pk);
-  dump_packed<NC / 2>(dd, n, word, pk);
-  tmem_st_wait();
-}
-
-// Last hidden layer of a branch: like epi_hidden, plus the sigma head as an fp32 dot product on the
-// un-rounded activations (reference: sigma = Linear(h), models/nerf_model.py:108,140).
-template <int NC>
-__device__ __forceinline__ float epi_hidden_sigma(uint32_t acc_addr, const float* bias, const float* headw, uint32_t out_addr,
-                                                  const DumpDst& dd, int n, int word) {
-  uint32_t v[NC];
-  tmem_ld_cols<NC>(acc_addr, v);
-  tmem_ld_wait();
-  uint32_t pk[NC / 2];
-  float part = 0.0f;
+  for (int r = 0; r < 2; ++r) {
+    const int row = R.row[r];
+    uint8_t* base = P.dump + P.TL.act_off[slot] + ((size_t)R.tile * P.TL.act_atoms[slot]) * ATOM_BYTES + (size_t)row * 128 + q * 4;
 #pragma unroll
-  for (int j4 = 0; j4 < NC / 4; ++j4) {
-    const float4 b = *(reinterpret_cast<const float4*>(bias) + j4);
-    const float4 w = __ldg(reinterpret_cast<const float4*>(headw) + j4);
-    float t0 = __uint_as_float(v[4 * j4 + 0]) + b.x, t1 = __uint_as_float(v[4 * j4 + 1]) + b.y;
-    float t2 = __uint_as_float(v[4 * j4 + 2]) + b.z, t3 = __uint_as_float(v[4 * j4 + 3]) + b.w;
-    t0 = fmaxf(t0, t0 * kLeaky); t1 = fmaxf(t1, t1 * kLeaky); t2 = fmaxf(t2, t2 * kLeaky); t3 = fmaxf(t3, t3 * kLeaky);
-    part = fmaf(t0, w.x, part); part = fmaf(t1, w.y, part); part = fmaf(t2, w.z, part); part = fmaf(t3, w.w, part);
-    pk[2 * j4] = pack_bf16(t0, t1);
-    pk[2 * j4 + 1] = pack_bf16(t2, t3);
+    for (int j = 0; j < N / 8; ++j)
+      *reinterpret_cast<uint32_t*>(base + (size_t)(j >> 3) * ATOM_BYTES + (((j & 7) ^ (row & 7)) << 4)) = pk[2 * j + r];
   }
-  tmem_st_cols<NC / 2>(out_addr, pk);
-  dump_packed<NC / 2>(dd, n, word, pk);
-  tmem_st_wait();
-  return part;
-}
-
-// Direction layer: LeakyReLU(acc + per-ray constant) feeds the 3-wide rgb head directly (fp32 dots).
-template <int NC>
-__device__ __forceinline__ void epi_dir(uint32_t acc_addr, const float* rcbias, const float* headw, int head_ld,
-                                        float& p0, float& p1, float& p2, const DumpDst& dd, int n, int word) {
-  uint32_t v[NC];
-  tmem_ld_cols<NC>(acc_addr, v);
-  tmem_ld_wait();
-  uint32_t pk[NC / 2];
+  if (mask_word0 < 0) return;
+  // bit b of mask word w = the bf16 at column w * CPW + b is non-negative (CPW = 32, or 16 for the 64-wide layer)
+  constexpr int CPW = N >= 128 ? 32 : 16, NW = N / CPW, BPW = CPW / 8;
+  uint32_t* mrow = reinterpret_cast<uint32_t*>(P.dump + P.TL.mask_off) + ((size_t)R.tile * ONERF_MASK_WORDS + mask_word0) * 128;
 #pragma unroll
-  for (int j4 = 0; j4 < NC / 4; ++j4) {
-    const float4 b = __ldg(reinterpret_cast<const float4*>(rcbias) + j4);
-    const float4 w0 = __ldg(reinterpret_cast<const float4*>(headw) + j4);
-    const float4 w1 = __ldg(reinterpret_cast<const float4*>(headw + head_ld) + j4);
-    const float4 w2 = __ldg(reinterpret_cast<const float4*>(headw + 2 * head_ld) + j4);
-    float t0 = __uint_as_float(v[4 * j4 + 0]) + b.x, t1 = __uint_as_float(v[4 * j4 + 1]) + b.y;
-    float t2 = __uint_as_float(v[4 * j4 + 2]) + b.z, t3 = __uint_as_float(v[4 * j4 + 3]) + b.w;
-    t0 = fmaxf(t0, t0 * kLeaky); t1 = fmaxf(t1, t1 * kLeaky); t2 = fmaxf(t2, t2 * kLeaky); t3 = fmaxf(t3, t3 * kLeaky);
-    p0 = fmaf(t0, w0.x, p0); p0 = fmaf(t1, w0.y, p0); p0 = fmaf(t2, w0.z, p0); p0 = fmaf(t3, w0.w, p0);
-    p1 = fmaf(t0, w1.x, p1); p1 = fmaf(t1, w1.y, p1); p1 = fmaf(t2, w1.z, p1); p1 = fmaf(t3, w1.w, p1);
-    p2 = fmaf(t0, w2.x, p2); p2 = fmaf(t1, w2.y, p2); p2 = fmaf(t2, w2.z, p2); p2 = fmaf(t3, w2.w, p2);
-    pk[2 * j4] = pack_bf16(t0, t1);
-    pk[2 * j4 + 1] = pack_bf16(t2, t3);
-  }
-  if constexpr (NC >= 8) dump_packed<NC / 2>(dd, n, word, pk);   // training: the dir activations feed the rgb head's wgrad
-}
-
-// dispatch on the (warp-uniform) layer width; NC = N / 8 columns per thread per layer half
-template <int NC>
-__device__ __forceinline__ void epilogue_half(const TcLayer& Ly, uint32_t acc_addr, uint32_t out_addr, const float* bias_smem,
-                                              const float* rc, const float* headw, int n, float& part0, float& part1,
-                                              float& part2, const DumpDst& dd, int word) {
-  if constexpr (NC >= 16) {
-    switch (Ly.epi) {
-      case EPI_HIDDEN: epi_hidden<NC, true, false>(acc_addr, bias_smem + n, out_addr, dd, n, word); break;
-      case EPI_HIDDEN_RC: epi_hidden<NC, true, true>(acc_addr, rc + Ly.rc_base + n, out_addr, dd, n, word); break;
-      case EPI_FINAL: epi_hidden<NC, false, false>(acc_addr, bias_smem + n, out_addr, dd, n, word); break;
-      case EPI_HIDDEN_SIGMA: part0 += epi_hidden_sigma<NC>(acc_addr, bias_smem + n, headw + n, out_addr, dd, n, word); break;
-      default: epi_dir<NC>(acc_addr, rc + Ly.rc_base + n, headw + n, Ly.N, part0, part1, part2, dd, n, word); break;
+  for (int w = 0; w < NW; ++w) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      uint32_t m = 0;
+#pragma unroll
+      for (int jj = 0; jj < BPW; ++jj) {
+        const uint32_t v = pk[2 * (w * BPW + jj) + r];
+        const uint32_t bits = (((v >> 15) & 1u) ^ 1u) | ((((v >> 31) & 1u) ^ 1u) << 1);
+        m |= bits << (8 * jj + 2 * q);
+      }
+      m |= __shfl_xor_sync(0xffffffffu, m, 1);
+      m |= __shfl_xor_sync(0xffffffffu, m, 2);
+      if (q == 0) mrow[w * 128 + R.row[r]] = m;
     }
-  } else {
-    epi_dir<NC>(acc_addr, rc + Ly.rc_base + n, headw + n, Ly.N, part0, part1, part2, dd, n, word);  // only the N = 64 dir layer
+  }
+}
+
+// Epilogue of one layer for one thread: t = acc + bias (fp32), then
+//   HIDDEN / HIDDEN_RC / FINAL: one rounding to bf16, LeakyReLU on packed bf16 pairs (not for FINAL);
+//   HIDDEN_SIGMA: LeakyReLU in fp32, sigma head dot product on the un-rounded values (models/nerf_model.py:108,140);
+//   DIR: LeakyReLU in fp32 feeding the 3-wide rgb head (fp32 dots).
+// part[r] accumulates the row's head partial sums (sigma, r, g, b) over this thread's columns.
+template <int N, int EPI>
+__device__ __forceinline__ void epilogue(const float (&acc)[N / 2], uint32_t* pk, const float* bias, const Rows& R,
+                                         int rc_base, const float* headw, float (&part)[2][4]) {
+  const int q = threadIdx.x & 3;
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const int c = 8 * j + 2 * q;
+    float2 b[2];
+    if (EPI == EPI_HIDDEN_RC || EPI == EPI_DIR) {
+      b[0] = __ldg(reinterpret_cast<const float2*>(R.rc[0] + rc_base + c));
+      b[1] = __ldg(reinterpret_cast<const float2*>(R.rc[1] + rc_base + c));
+    } else {
+      b[0] = b[1] = *reinterpret_cast<const float2*>(bias + c);
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      float t0 = acc[4 * j + 2 * r] + b[r].x, t1 = acc[4 * j + 2 * r + 1] + b[r].y;
+      uint32_t p;
+      if (EPI == EPI_HIDDEN || EPI == EPI_HIDDEN_RC) {
+        p = leaky_bf16x2(pack_bf16(t0, t1));
+      } else if (EPI == EPI_FINAL) {
+        p = pack_bf16(t0, t1);
+      } else {
+        t0 = fmaxf(t0, t0 * kLeaky);
+        t1 = fmaxf(t1, t1 * kLeaky);
+        if (EPI == EPI_HIDDEN_SIGMA) {
+          const float2 w = __ldg(reinterpret_cast<const float2*>(headw + c));
+          part[r][0] = fmaf(t1, w.y, fmaf(t0, w.x, part[r][0]));
+        } else {
+#pragma unroll
+          for (int k = 0; k < 3; ++k) {
+            const float2 w = __ldg(reinterpret_cast<const float2*>(headw + k * N + c));
+            part[r][1 + k] = fmaf(t1, w.y, fmaf(t0, w.x, part[r][1 + k]));
+          }
+        }
+        p = pack_bf16(t0, t1);
+      }
+      pk[2 * j + r] = p;
+    }
+  }
+}
+
+// finish the heads of one branch: sum the four lanes of each row, add the head biases, write (rgb, sigma)
+__device__ __forceinline__ void write_heads(const FieldParams& p, const Rows& R, int branch, float (&part)[2][4]) {
+  const float* Pf = reinterpret_cast<const float*>(p.packed);
+  const float* hb = Pf + (branch ? p.L.orgb_b : p.L.rgb_b);
+  const float sb = __ldg(Pf + (branch ? p.L.osigma_b : p.L.sigma_b));
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      part[r][k] += __shfl_xor_sync(0xffffffffu, part[r][k], 1);
+      part[r][k] += __shfl_xor_sync(0xffffffffu, part[r][k], 2);
+    }
+    if ((threadIdx.x & 3) == 0 && R.live[r]) {
+      float sg = part[r][0] + sb;
+      const float cr = 1.0f / (1.0f + __expf(-(part[r][1] + __ldg(hb + 0))));
+      const float cg = 1.0f / (1.0f + __expf(-(part[r][2] + __ldg(hb + 1))));
+      const float cb = 1.0f / (1.0f + __expf(-(part[r][3] + __ldg(hb + 2))));
+      if (R.mute[r] & (branch ? 2 : 1)) sg = -1e5f;
+      float* outp = branch ? p.obj_out : p.scene_out;
+      reinterpret_cast<float4*>(outp)[(int64_t)R.ray[r] * p.out_stride + R.si[r]] = make_float4(cr, cg, cb, sg);
+    }
   }
 }
 
@@ -189,66 +171,52 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
   const FieldParams& p = P.f;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int X_ATOMS = VOXEL ? 6 : 1;
+  constexpr int XS = VOXEL ? 9 : 2, XO = VOXEL ? 12 : 2;   // K slabs of X read by the scene / object branch (KX, KO)
 
   // ---- shared memory carve-up (base is 1024-byte aligned: required by the 128B swizzle) ----
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sX = sbase;
   const uint32_t sB = sX + X_ATOMS * ATOM_BYTES;
-  const uint32_t sBias = sB + NSTAGE * STAGE_BYTES;                 // [MAX_LAYERS][256] floats
-  const uint32_t sScratch = sBias + MAX_LAYERS * 256 * 4;           // [128][4][4] floats
-  const uint32_t sBar = sScratch + TM * 4 * 4 * 4;
-  TcBars bar;
-  bar.full = sBar;                                                  // NSTAGE x 8 B
-  bar.empty = sBar + 8 * NSTAGE;
-  bar.x_ready = sBar + 16 * NSTAGE;                                 // compute -> MMA, once per tile
-  bar.acc_ready = bar.x_ready + 8;                                  // [2] MMA -> compute, per layer half
-  bar.epi_done = bar.acc_ready + 16;                                // [2] compute -> MMA, per layer half
-  const uint32_t bar_x_ready = bar.x_ready, bar_acc_ready = bar.acc_ready, bar_epi_done = bar.epi_done;
-  const uint32_t tmem_slot = bar.epi_done + 16;
+  const uint32_t sBias = sB + NSTAGE * STAGE_BYTES;                 // [G_COUNT][256] floats
+  const uint32_t sMeta = sBias + G_COUNT * 256 * 4;                 // [128] RowMeta
+  const uint32_t sBar = sMeta + TM * sizeof(RowMeta);
   uint8_t* gen_base = smem_raw + (sbase - smem_u32(smem_raw));
   float* bias_tab = reinterpret_cast<float*>(gen_base + (sBias - sbase));
-  float* scratch = reinterpret_cast<float*>(gen_base + (sScratch - sbase));
-  volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(gen_base + (tmem_slot - sbase));
+  RowMeta* meta = reinterpret_cast<RowMeta*>(gen_base + (sMeta - sbase));
   const float* Pf = reinterpret_cast<const float*>(p.packed);
+  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u};
 
-  if (threadIdx.x == 0) tc_init_bars(bar);
-  if (warp == MMA_WARP) tmem_alloc(tmem_slot, 512);
-  // per-column biases of every layer -> shared memory (layers with a per-ray constant read ray_const instead)
-  for (int i = threadIdx.x; i < P.n_layers * 256; i += NUM_THREADS) {
-    const int l = i >> 8, c = i & 255;
-    bias_tab[i] = (c < P.layers[l].N) ? __ldg(Pf + P.layers[l].bias_off + c) : 0.0f;
+  if (threadIdx.x == 0) ring_init_bars(ring.full, ring.empty);
+  // per-column biases of every GEMM -> shared memory (layers with a per-ray constant read ray_const instead)
+  for (int i = threadIdx.x; i < G_COUNT * 256; i += NUM_THREADS) {
+    const int g = i >> 8, c = i & 255;
+    bias_tab[i] = (c < p.L.g[g].N) ? __ldg(Pf + p.L.g[g].bias_off + c) : 0.0f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_gen;
 
   const int64_t total = (int64_t)p.n_rays * p.S;
   const int64_t n_tiles = (total + TM - 1) / TM;
-  const uint8_t* blob = reinterpret_cast<const uint8_t*>(p.packed);
 
-  if (warp == PRODUCER_WARP) {
-    tc_producer_loop(P.layers, P.n_layers, blob, sB, bar, n_tiles);
-  } else if (warp == MMA_WARP) {
-    tc_mma_loop<ONERF_TL_ON>(P.layers, P.n_layers, sX, sB, bar, tmem_base, n_tiles, P.timeline,
-                             DUMP ? P.dump + P.TL.act_off[0] : nullptr, X_ATOMS);
-    if (DUMP) {   // the last tile's bulk store must have left shared memory before the CTA exits
-      if (elect_one()) bulk_wait_group0();
-      __syncwarp();
-    }
-  } else {
-    // =============================== encode + epilogue warps ===============================
-    const int q = warp & 3, cq = warp >> 2;          // TMEM lane quarter (rows), column quarter
-    const int row = q * 32 + lane;
-    const uint32_t lane_taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-    uint32_t acc_phase0 = 0, acc_phase1 = 0;
-    // nothing to drain before the very first layer
-    if (lane == 0) {
-      mbar_arrive(bar_epi_done);
-      if (P.layers[0].prev_two) mbar_arrive(bar_epi_done + 8);
-    }
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      if (ONERF_TL_ON && P.timeline && blockIdx.x == 0 && tile == (int64_t)gridDim.x && threadIdx.x == 0) P.timeline[201] = clock64();
+  if (warp >= PRODUCER_WARP) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == PRODUCER_WARP)
+      tc_producer_loop(P.layers, P.n_layers, reinterpret_cast<const uint8_t*>(p.packed), ring, n_tiles);
+    return;
+  }
+  setmaxnreg_inc<CONSUMER_REGS>();
+
+  // =============================== encode + MMA + epilogue warpgroups ===============================
+  const int wg = warp >> 2, tid = threadIdx.x & 127;
+  const uint32_t sXw = sX + (uint32_t)wg * 64u * 128u;
+  Rows R;
+  R.row[0] = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  R.row[1] = R.row[0] + 8;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    R.tile = tile;
+    // ---- encode this warpgroup's 64 rows of X: (row, column quarter) jobs ----
+#pragma unroll 1
+    for (int job = tid; job < 256; job += 128) {
+      const int row = wg * 64 + (job & 63), cq = job >> 6;
       const int64_t e = tile * TM + row;
       const bool live = e < total;
       const int ray = live ? (int)(e / p.S) : 0;
@@ -263,14 +231,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
         x = __ldg(qq); y = __ldg(qq + 1); z = __ldg(qq + 2);
       }
       if (!live) { x = 0.f; y = 0.f; z = 0.f; }
-      int mute = 0;  // bit 0: scene sigma muted, bit 1: object sigma muted
       if (cq == 0) {
+        int mute = 0;
         if (live && p.mute_zero_rays && __ldg(p.z + (int64_t)ray * p.z_stride + (p.S - 1)) == 0.0f) mute = 3;
         if (live && mute == 0 && p.n_boxes > 0 && point_in_boxes(p.boxes, p.n_boxes, x, y, z)) mute = 1;
+        meta[row] = RowMeta{ray, si, mute, live ? 1 : 0};
       }
-      const float* rc = p.ray_const + (int64_t)ray * ONERF_RAY_CONST_FLOATS;
-
-      // ---- encode this thread's quarter of the row of X ----
       if (VOXEL) {
         const GridView g = load_grid_view(p.grid);
         float f[8];
@@ -290,132 +256,105 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
       } else {
         if (cq == 0) pe_xyz_to_chunks(sX, row, 0, x, y, z);
       }
-      fence_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_x_ready);
-      if (ONERF_TL_ON && P.timeline && blockIdx.x == 0 && tile == (int64_t)gridDim.x && threadIdx.x == 0) P.timeline[200] = clock64();
-
-      float sigma_part = 0.0f;
-      for (int l = 0; l < P.n_layers; ++l) {
-        const TcLayer& Ly = P.layers[l];
-        const int HW = Ly.N >> (Ly.nhalf - 1);               // accumulator width of one layer half
-        const int NC = HW >> 2;                        // columns this thread handles per layer half (32/16/8)
-        const float* headw = nullptr;
-        if (Ly.epi == EPI_HIDDEN_SIGMA) headw = Pf + (Ly.branch ? p.L.osigma_w : p.L.sigma_w);
-        if (Ly.epi == EPI_DIR) headw = Pf + (Ly.branch ? p.L.orgb_w : p.L.rgb_w);
-        float part0 = 0.0f, part1 = 0.0f, part2 = 0.0f;
+    }
+    fence_async_smem();
+    wg_sync(wg);
+    if (DUMP) {   // this warpgroup's rows of the X atoms, byte for byte
 #pragma unroll 1
-        for (int h = 0; h < Ly.nhalf; ++h) {
-          const int n = h * HW + cq * NC;              // first output column of this thread in this half
-          const uint32_t acc_addr = lane_taddr + (uint32_t)(h * TM_ACC1 + cq * NC);
-          const uint32_t out_addr = lane_taddr + (uint32_t)(Ly.h_out_col + (n >> 1));
-          if (h == 0) { mbar_wait(bar_acc_ready, acc_phase0); acc_phase0 ^= 1; }
-          else { mbar_wait(bar_acc_ready + 8, acc_phase1); acc_phase1 ^= 1; }
-          tc_fence_after();
-          if (ONERF_TL_ON && P.timeline && blockIdx.x == 0 && tile == (int64_t)gridDim.x && threadIdx.x == 0) P.timeline[(l * 2 + h) * 4 + 2] = clock64();
-          DumpDst dd;
-          dd.row = nullptr; dd.mask = nullptr; dd.swz = row & 7;
-          if (DUMP && Ly.act_slot >= 0) {
-            dd.row = P.dump + P.TL.act_off[Ly.act_slot] + ((size_t)tile * P.TL.act_atoms[Ly.act_slot]) * ATOM_BYTES + (size_t)row * 128;
-            if (Ly.mask_word0 >= 0)
-              dd.mask = reinterpret_cast<uint32_t*>(P.dump + P.TL.mask_off) + ((size_t)tile * ONERF_MASK_WORDS + Ly.mask_word0) * 128 + row;
-          }
-          const int word = h * 4 + cq;
-          if (NC == 32) epilogue_half<32>(Ly, acc_addr, out_addr, bias_tab + l * 256, rc, headw, n, part0, part1, part2, dd, word);
-          else if (NC == 16) epilogue_half<16>(Ly, acc_addr, out_addr, bias_tab + l * 256, rc, headw, n, part0, part1, part2, dd, word);
-          else epilogue_half<8>(Ly, acc_addr, out_addr, bias_tab + l * 256, rc, headw, n, part0, part1, part2, dd, word);
-          // accumulator half h drained, output activations of this half written
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_epi_done + 8 * h);
-          if (ONERF_TL_ON && P.timeline && blockIdx.x == 0 && tile == (int64_t)gridDim.x && threadIdx.x == 0) P.timeline[(l * 2 + h) * 4 + 3] = clock64();
-        }
-        if (Ly.epi == EPI_HIDDEN_SIGMA) sigma_part = part0;
-        if (Ly.epi == EPI_DIR) {
-          // combine the four column quarters of this row through shared memory, finish the heads, write out
-          float* sc = scratch + (row * 4 + cq) * 4;
-          sc[0] = sigma_part; sc[1] = part0; sc[2] = part1; sc[3] = part2;
-          asm volatile("bar.sync 1, %0;" ::"n"(NUM_COMPUTE) : "memory");
-          if (cq == 0 && live) {
-            const float4 a1 = *reinterpret_cast<const float4*>(scratch + (row * 4 + 1) * 4);
-            const float4 a2 = *reinterpret_cast<const float4*>(scratch + (row * 4 + 2) * 4);
-            const float4 a3 = *reinterpret_cast<const float4*>(scratch + (row * 4 + 3) * 4);
-            const float* hb = Pf + (Ly.branch ? p.L.orgb_b : p.L.rgb_b);
-            float sg = sigma_part + a1.x + a2.x + a3.x + __ldg(Pf + (Ly.branch ? p.L.osigma_b : p.L.sigma_b));
-            const float r = 1.0f / (1.0f + __expf(-(part0 + a1.y + a2.y + a3.y + __ldg(hb + 0))));
-            const float gch = 1.0f / (1.0f + __expf(-(part1 + a1.z + a2.z + a3.z + __ldg(hb + 1))));
-            const float b = 1.0f / (1.0f + __expf(-(part2 + a1.w + a2.w + a3.w + __ldg(hb + 2))));
-            if (mute & (Ly.branch ? 2 : 1)) sg = -1e5f;
-            float* outp = Ly.branch ? p.obj_out : p.scene_out;
-            reinterpret_cast<float4*>(outp)[(int64_t)ray * p.out_stride + si] = make_float4(r, gch, b, sg);
-          }
-          asm volatile("bar.sync 1, %0;" ::"n"(NUM_COMPUTE) : "memory");  // scratch reusable
-        }
+      for (int a = 0; a < X_ATOMS; ++a) {
+        const uint4* src = reinterpret_cast<const uint4*>(gen_base + (size_t)a * ATOM_BYTES + (size_t)wg * 8192);
+        uint4* dst = reinterpret_cast<uint4*>(P.dump + P.TL.act_off[0] + ((size_t)tile * X_ATOMS + a) * ATOM_BYTES + (size_t)wg * 8192);
+        for (int i = tid; i < 512; i += 128) dst[i] = src[i];
       }
     }
-  }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const RowMeta m = meta[R.row[r]];
+      R.live[r] = m.live; R.ray[r] = m.ray; R.si[r] = m.si; R.mute[r] = m.mute;
+      R.rc[r] = p.ray_const + (int64_t)m.ray * ONERF_RAY_CONST_FLOATS;
+    }
 
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) tmem_dealloc(tmem_base, 512);
+    if (p.want_scene) {
+      float acc[128];
+      uint32_t h[64];
+      float part[2][4] = {};
+      const float* sw = Pf + p.L.sigma_w;
+      mma_layer<256, XS, 0>(acc, h, sXw, ring);
+      epilogue<256, EPI_HIDDEN>(acc, h, bias_tab + G_S0 * 256, R, 0, nullptr, part);
+      if (DUMP) dump_layer<256>(P, R, 1, onerf_mask_word0(1), h);
+#pragma unroll 1
+      for (int l = 1; l < 4; ++l) {
+        mma_layer<256, 0, 8>(acc, h, sXw, ring);
+        epilogue<256, EPI_HIDDEN>(acc, h, bias_tab + (G_S0 + l) * 256, R, 0, nullptr, part);
+        if (DUMP) dump_layer<256>(P, R, 1 + l, onerf_mask_word0(1 + l), h);
+      }
+      mma_layer<256, XS, 8>(acc, h, sXw, ring);   // skip layer: [X | h3]
+      epilogue<256, EPI_HIDDEN>(acc, h, bias_tab + G_S4 * 256, R, 0, nullptr, part);
+      if (DUMP) dump_layer<256>(P, R, 5, onerf_mask_word0(5), h);
+#pragma unroll 1
+      for (int l = 5; l < 7; ++l) {
+        mma_layer<256, 0, 8>(acc, h, sXw, ring);
+        epilogue<256, EPI_HIDDEN>(acc, h, bias_tab + (G_S0 + l) * 256, R, 0, nullptr, part);
+        if (DUMP) dump_layer<256>(P, R, 1 + l, onerf_mask_word0(1 + l), h);
+      }
+      mma_layer<256, 0, 8>(acc, h, sXw, ring);
+      epilogue<256, EPI_HIDDEN_SIGMA>(acc, h, bias_tab + G_S7 * 256, R, 0, sw, part);
+      if (DUMP) dump_layer<256>(P, R, 8, onerf_mask_word0(8), h);
+      mma_layer<256, 0, 8>(acc, h, sXw, ring);
+      epilogue<256, EPI_FINAL>(acc, h, bias_tab + G_SFIN * 256, R, 0, nullptr, part);
+      if (DUMP) dump_layer<256>(P, R, 9, -1, h);
+      float accd[64];
+      uint32_t hd[32];
+      mma_layer<128, 0, 8>(accd, h, sXw, ring);
+      epilogue<128, EPI_DIR>(accd, hd, nullptr, R, RC_SDIR, Pf + p.L.rgb_w, part);
+      if (DUMP) dump_layer<128>(P, R, 10, onerf_mask_word0(10), hd);
+      write_heads(p, R, 0, part);
+    }
+    if (p.want_object) {
+      float acc[64];
+      uint32_t h[32];
+      float part[2][4] = {};
+      mma_layer<128, XO, 0>(acc, h, sXw, ring);
+      epilogue<128, EPI_HIDDEN_RC>(acc, h, nullptr, R, RC_OL0, nullptr, part);
+      if (DUMP) dump_layer<128>(P, R, 11, onerf_mask_word0(11), h);
+      mma_layer<128, 0, 4>(acc, h, sXw, ring);
+      epilogue<128, EPI_HIDDEN>(acc, h, bias_tab + G_O1 * 256, R, 0, nullptr, part);
+      if (DUMP) dump_layer<128>(P, R, 12, onerf_mask_word0(12), h);
+      mma_layer<128, XO, 4>(acc, h, sXw, ring);   // [X | h1], object code through ray_const
+      epilogue<128, EPI_HIDDEN_RC>(acc, h, nullptr, R, RC_OL2, nullptr, part);
+      if (DUMP) dump_layer<128>(P, R, 13, onerf_mask_word0(13), h);
+      mma_layer<128, 0, 4>(acc, h, sXw, ring);
+      epilogue<128, EPI_HIDDEN_SIGMA>(acc, h, bias_tab + G_O3 * 256, R, 0, Pf + p.L.osigma_w, part);
+      if (DUMP) dump_layer<128>(P, R, 14, onerf_mask_word0(14), h);
+      mma_layer<128, 0, 4>(acc, h, sXw, ring);
+      epilogue<128, EPI_FINAL>(acc, h, bias_tab + G_OFIN * 256, R, 0, nullptr, part);
+      if (DUMP) dump_layer<128>(P, R, 15, -1, h);
+      float accd[32];
+      uint32_t hd[16];
+      mma_layer<64, 0, 4>(accd, h, sXw, ring);
+      epilogue<64, EPI_DIR>(accd, hd, nullptr, R, RC_ODIR, Pf + p.L.orgb_w, part);
+      if (DUMP) dump_layer<64>(P, R, 16, onerf_mask_word0(16), hd);
+      write_heads(p, R, 1, part);
+    }
+    // the next tile's encode overwrites X and the row metadata: both warpgroups' reads of them are done
+    wg_sync(wg);
+  }
 }
 
 }  // namespace
 
-static long long* g_timeline = nullptr;
-extern "C" void onerf_debug_timeline(void* dev_buf) { g_timeline = reinterpret_cast<long long*>(dev_buf); }
-
-int onerf_launch_field_bf16_two_tile(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t stream);   // field_tc2.cu
-static int g_force_one_tile = -1;   // -1: take ONERF_TC_ONE_TILE from the environment at the first launch
-extern "C" void onerf_debug_force_one_tile(int on) { g_force_one_tile = on ? 1 : 0; }
-
 int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t stream) {
   const PackLayout& L = fp.L;
-  // The voxel model's forward runs on the two-tile kernel (field_tc2.cu): inference, and the training forward (activation
-  // dump) when both branches are evaluated.  This one-tile kernel serves the plain-PE model and single-branch training
-  // dumps; ONERF_TC_ONE_TILE=1 / onerf_debug_force_one_tile(1) force it everywhere (A/B runs, bitwise dump comparison).
-  if (g_force_one_tile < 0) { const char* v = getenv("ONERF_TC_ONE_TILE"); g_force_one_tile = (v && v[0] == '1') ? 1 : 0; }
-  if (L.use_voxel && !g_force_one_tile && (!fp.train_ws || (fp.want_scene && fp.want_object)))
-    return onerf_launch_field_bf16_two_tile(ctx, fp, stream);
   TcParams P;
   memset(&P, 0, sizeof(P));
   P.f = fp;
-  P.timeline = g_timeline;
-  const int xs = L.KX / 32, xo = L.KO / 32;
-  // Layers with N <= 128 use ONE accumulator and full-width MMAs: half as many tcgen05.mma issues and barrier
-  // hand-offs as two N = 64 halves (the MMA issue rate, not the tensor pipe, bounds narrow layers).
-  // ONERF_TC_SPLIT_ALL=1 restores two halves everywhere (A/B measurements; not with a training dump).
-  static const int split_all = [] { const char* v = getenv("ONERF_TC_SPLIT_ALL"); return (v && v[0] == '1') ? 1 : 0; }();
-  const int single_max_n = (split_all && !fp.train_ws) ? 0 : 128;
   int n = 0;
-  auto add = [&](int gemm, int nx, int nh, int epi, int branch, int rc_base, int act_slot) {
-    tc_add_layer(P.layers, n, L.g[gemm].N, nx, nh, epi, branch, rc_base, L.g[gemm].img_off, L.g[gemm].bias_off, single_max_n,
-                 act_slot, onerf_mask_word0(act_slot));
-  };
-  if (fp.want_scene) {
-    add(G_S0, xs, 0, EPI_HIDDEN, 0, 0, 1);
-    add(G_S1, 0, 8, EPI_HIDDEN, 0, 0, 2);
-    add(G_S2, 0, 8, EPI_HIDDEN, 0, 0, 3);
-    add(G_S3, 0, 8, EPI_HIDDEN, 0, 0, 4);
-    add(G_S4, xs, 8, EPI_HIDDEN, 0, 0, 5);
-    add(G_S5, 0, 8, EPI_HIDDEN, 0, 0, 6);
-    add(G_S6, 0, 8, EPI_HIDDEN, 0, 0, 7);
-    add(G_S7, 0, 8, EPI_HIDDEN_SIGMA, 0, 0, 8);
-    add(G_SFIN, 0, 8, EPI_FINAL, 0, 0, 9);
-    add(G_SDIR, 0, 8, EPI_DIR, 0, RC_SDIR, 10);
-  }
-  if (fp.want_object) {
-    add(G_O0, xo, 0, EPI_HIDDEN_RC, 1, RC_OL0, 11);
-    add(G_O1, 0, 4, EPI_HIDDEN, 1, 0, 12);
-    add(G_O2, xo, 4, EPI_HIDDEN_RC, 1, RC_OL2, 13);
-    add(G_O3, 0, 4, EPI_HIDDEN_SIGMA, 1, 0, 14);
-    add(G_OFIN, 0, 4, EPI_FINAL, 1, 0, 15);
-    add(G_ODIR, 0, 4, EPI_DIR, 1, RC_ODIR, 16);
-  }
+  auto add = [&](int g) { P.layers[n++] = WLayer{L.g[g].img_off, L.g[g].N, L.g[g].K / 32}; };
+  if (fp.want_scene)
+    for (int g = G_S0; g <= G_SDIR; ++g) add(g);
+  if (fp.want_object)
+    for (int g = G_O0; g <= G_ODIR; ++g) add(g);
   P.n_layers = n;
-  tc_finish_program(P.layers, n);
-  P.x_atoms = L.use_voxel ? 6 : 1;
   const int64_t total = (int64_t)fp.n_rays * fp.S;
   const int64_t tiles = (total + TM - 1) / TM;
   if (fp.train_ws) {
@@ -423,8 +362,9 @@ int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t 
     P.TL = onerf_make_train_layout(L.use_voxel, total);
   }
   const int blocks = (int)(tiles < ctx->num_sms ? tiles : ctx->num_sms);
-  const size_t smem = 1024 + (size_t)P.x_atoms * ATOM_BYTES + NSTAGE * STAGE_BYTES + MAX_LAYERS * 256 * 4 +
-                      TM * 4 * 4 * 4 + 512;
+  const int x_atoms = L.use_voxel ? 6 : 1;
+  const size_t smem = 1024 + (size_t)x_atoms * ATOM_BYTES + NSTAGE * STAGE_BYTES + G_COUNT * 256 * 4 + TM * sizeof(RowMeta) +
+                      16 * NSTAGE;
   auto launch = [&](auto kernel) -> int {
     ONERF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<blocks, NUM_THREADS, smem, stream>>>(P);

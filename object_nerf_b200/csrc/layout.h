@@ -3,8 +3,8 @@
 // One ObjectNeRF (reference models/nerf_model.py:18-95) is re-laid into one blob:
 //   [fp32 section]  every GEMM layer as W^T [K][N] (K-major, kernel-K order), head vectors, biases and
 //                   the per-ray-constant ("hoisted") column blocks
-//   [bf16 section]  the tcgen05 stage images: per GEMM layer, per 32-wide K slab, an N x 32 bf16 tile
-//                   in the UMMA K-major SWIZZLE_64B shared-memory layout, in program order
+//   [bf16 section]  the tensor-core stage images: per GEMM layer, per 32-wide K slab, an N x 32 bf16 tile
+//                   in the K-major SWIZZLE_64B shared-memory layout, in program order
 //
 // Kernel-K order ("X layout").  The encoded input of a sample is kept as one vector X:
 //   voxel model:  X[0..271)   = scene input  [PE6(scene voxel ftr 16) | PE10(xyz)]  (reference order)
@@ -118,7 +118,7 @@ static inline PackLayout onerf_make_layout(int use_voxel) {
 
 // ---------------------------------------------------------------------------------------------------
 // Training dump ("atoms"): what the bf16 forward leaves behind for the tensor-core backward.
-// An atom is a [128 samples x 64 columns] bf16 block in the UMMA SWIZZLE_128B shared-memory layout
+// An atom is a [128 samples x 64 columns] bf16 block in the SWIZZLE_128B shared-memory layout
 // (row r at r*128 B, 16-byte chunk c of the row stored at chunk position c ^ (r & 7)); 16 KB.  The same image
 // serves as a K-major operand (K = columns: input-gradient GEMMs) and as an MN-major operand (K = samples:
 // weight-gradient GEMMs), so one bulk copy brings a ready-to-use tile into shared memory.
@@ -143,6 +143,9 @@ struct TrainLayout {
   int64_t total_bytes;
 };
 
+#ifdef __CUDACC__
+__host__ __device__
+#endif
 static inline int onerf_mask_word0(int act_slot) {   // first mask word of the layer whose output is `act_slot`
   if (act_slot >= 1 && act_slot <= 8) return (act_slot - 1) * 8;
   if (act_slot == 10) return 64;

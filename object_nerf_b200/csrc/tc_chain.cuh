@@ -1,244 +1,119 @@
-// Layer-program machinery shared by the fused forward (field_tc.cu) and the input-gradient chain (bwd_tc.cu):
-// a persistent CTA walks a static list of GEMM "layers" per 128-row tile,
-//   warp PRODUCER_WARP streams the layers' weight stage images into a shared-memory ring with cp.async.bulk,
-//   warp MMA_WARP issues tcgen05.mma (A from shared-memory X slabs and / or from TMEM-resident activations),
-//   the 16 compute warps (kernel specific) run the epilogues and hand activations back through TMEM.
-// Barrier protocol (all CTA-local mbarriers):
-//   full[s] / empty[s]   ring stage filled by TMA / released by tcgen05.commit
-//   x_ready              compute -> MMA, once per tile: the tile's first-layer operand is in place
-//   acc_ready[h]         MMA -> compute: accumulator half h of the current layer is complete
-//   epi_done[h]          compute -> MMA: accumulator half h drained and the matching half of the output written
+// Layer-chain machinery shared by the fused forward (field_tc.cu) and the input-gradient chain (bwd_chain.cu):
+// a persistent CTA walks a static list of GEMM "layers" per 128-row tile.
+//   warp PRODUCER_WARP streams the layers' weight stage images into a shared-memory ring with cp.async.bulk;
+//   warpgroups 0 and 1 own rows [0, 64) and [64, 128) of the tile and issue wgmma (M = 64) on them: A from shared-memory
+//   X atoms (K-major SWIZZLE_128B) or from registers (the previous layer's packed output), B from the ring (K-major
+//   SWIZZLE_64B stage images, layout.h).  Accumulators and hidden activations never leave the registers.
+// Barrier protocol (CTA-local mbarriers):
+//   full[s]   producer -> consumers: ring stage s filled (transaction bytes)
+//   empty[s]  consumers -> producer: the MMAs that read stage s have completed (one arrival per consumer warp)
+// The producer and the consumers walk the same stage sequence: per layer, its 32-wide K slabs in order, 256 / N slabs
+// (16 KB) per stage.
 #pragma once
 #include "tc_common.cuh"
 
 namespace tc {
 
-constexpr int NSTAGE = 3;           // weight ring depth
-constexpr int SLAB_BYTES = 8192;    // 128 rows x 64 B: one half K-slab (32 of K) of an N = 256 layer
-constexpr int STAGE_SLABS = 4;      // a ring stage carries up to 4 consecutive K-slabs (128 of K) of one layer half
-constexpr int STAGE_BYTES = STAGE_SLABS * SLAB_BYTES;
-constexpr int MAX_GROUPS = 6;
-constexpr int TM_ACC1 = 128;        // TMEM column of accumulator half 1
-constexpr int TM_HA = 256, TM_HB = 384;
-constexpr int NUM_COMPUTE = 512;    // 16 encode/epilogue warps: 4 per TMEM lane quarter
-constexpr int PRODUCER_WARP = 16, MMA_WARP = 17;
-constexpr int NUM_THREADS = 576;
+constexpr int NSTAGE = 6;            // weight ring depth
+constexpr int STAGE_BYTES = 16384;   // 32 K-slab rows of N = 256, or 2 / 4 slabs of N = 128 / 64
+constexpr int NUM_WG = 2;
+constexpr int NUM_CONSUMER = NUM_WG * 128;
+constexpr int PRODUCER_WARP = NUM_CONSUMER / 32;   // first warp of the third warpgroup; its other three warps exit
+constexpr int NUM_THREADS = NUM_CONSUMER + 128;
+// Register split: a 64 x 256 fp32 accumulator plus the 256-wide register A operand need more than the 168 registers a
+// 384-thread CTA gets per thread, so the producer warpgroup hands registers to the two consumer warpgroups
+// (40 x 128 + 232 x 256 = 64 512 <= 65 536).
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 constexpr int MAX_LAYERS = 16;
 
-struct TcLayer {
-  int N;           // outputs (UMMA N)
-  int nslab_x;     // leading K slabs (32 wide) taken from X
-  int nslab_h;     // following K slabs taken from H
-  int epi;         // kernel-specific epilogue kind
-  int branch;      // 0 scene, 1 object
-  int rc_base;     // ray_const offset for *_RC / DIR epilogues
-  int h_in_col;    // TMEM column of the input activations (K pairs), if nslab_h > 0
-  int h_out_col;   // TMEM column the epilogue writes the output activations to
-  int64_t img_off;   // byte offset of this layer's stage images in the packed blob
-  int64_t bias_off;  // float offset of the bias vector
-  // K-slab groups (one ring stage each), identical for both halves of the layer:
-  //   bits [0,5) first slab (index inside X or H), [5,8) slab count (1..4), bit 8: from H, bit 9: needs the
-  //   second epilogue half of the previous layer (high-K half of the input activations)
-  int ngroups;
-  int groups[MAX_GROUPS];
-  int nhalf;       // 2: the N outputs are computed as two halves (accumulators 0 / 1); 1: one N <= 128 accumulator
-  int prev_two;    // the previous layer (cyclically) has two halves, i.e. posts a second epilogue-done arrival
-  int act_slot;    // training dump: activation slot of the layer's output (forward) / dZ slot (backward); -1 none
-  int mask_word0;  // training dump: first sign-mask word of the layer (-1: layer without activation)
+struct WLayer {
+  int64_t img_off;   // byte offset of the layer's stage images in the packed blob (nslab images of N * 64 bytes)
+  int N;             // outputs: 256, 128 or 64
+  int nslab;         // 32-wide K slabs
 };
 
-struct TcBars {
-  uint32_t full, empty, x_ready, acc_ready, epi_done;   // shared-memory addresses; [s] / [h] at + 8 * index
+struct Ring {
+  uint32_t sB, full, empty;
+  uint32_t stage, phase;
 };
 
-__device__ __forceinline__ void tc_init_bars(const TcBars& b) {
+__device__ __forceinline__ void ring_init_bars(uint32_t full, uint32_t empty) {
   for (int s = 0; s < NSTAGE; ++s) {
-    mbar_init(b.full + 8 * s, 1);
-    mbar_init(b.empty + 8 * s, 1);
-  }
-  // compute -> MMA barriers take ONE arrive per warp (after __syncwarp): 512 serialized shared-memory
-  // atomics per phase would cost more than the epilogue math
-  mbar_init(b.x_ready, NUM_COMPUTE / 32);
-  for (int h = 0; h < 2; ++h) {
-    mbar_init(b.acc_ready + 8 * h, 1);
-    mbar_init(b.epi_done + 8 * h, NUM_COMPUTE / 32);
+    mbar_init(full + 8 * s, 1);
+    mbar_init(empty + 8 * s, NUM_CONSUMER / 32);
   }
   fence_barrier_init();
 }
 
-// =============================== weight producer (TMA bulk copies) ===============================
-// The whole warp runs the (uniform) loop; one elected lane talks to the barriers / TMA.
-__device__ __forceinline__ void tc_producer_loop(const TcLayer* layers, int n_layers, const uint8_t* blob, uint32_t sB,
-                                                 const TcBars& bar, int64_t n_tiles) {
-  uint32_t stage = 0, phase = 0;
+// =============================== weight producer (bulk copies) ===============================
+// The whole warp runs the (uniform) loop; one elected lane talks to the barriers.
+__device__ __forceinline__ void tc_producer_loop(const WLayer* layers, int n_layers, const uint8_t* blob, Ring r,
+                                                 int64_t n_tiles) {
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     for (int l = 0; l < n_layers; ++l) {
-      const TcLayer& Ly = layers[l];
-      const uint32_t slab_bytes = (uint32_t)Ly.N * 64u, half_bytes = slab_bytes >> (Ly.nhalf - 1);
-      const uint8_t* src = blob + Ly.img_off;
-      for (int h = 0; h < Ly.nhalf; ++h) {
-        for (int gi = 0; gi < Ly.ngroups; ++gi) {
-          const int grp = Ly.groups[gi];
-          const int first = grp & 31, cnt = (grp >> 5) & 7;
-          const int gslab = ((grp >> 8) & 1) ? Ly.nslab_x + first : first;   // slab index inside the layer
-          mbar_wait(bar.empty + 8 * stage, phase ^ 1);
-          if (elect_one()) {
-            mbar_expect_tx(bar.full + 8 * stage, (uint32_t)cnt * half_bytes);
-            for (int i2 = 0; i2 < cnt; ++i2)
-              tma_bulk_g2s(sB + stage * STAGE_BYTES + (uint32_t)i2 * half_bytes,
-                           src + (size_t)(gslab + i2) * slab_bytes + (size_t)h * half_bytes, half_bytes,
-                           bar.full + 8 * stage);
-          }
-          __syncwarp();
-          if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+      const WLayer& Ly = layers[l];
+      const int spp = 256 / Ly.N;
+      const uint32_t slab_bytes = (uint32_t)Ly.N * 64u;
+      for (int s0 = 0; s0 < Ly.nslab; s0 += spp) {
+        const int cnt = (Ly.nslab - s0 < spp) ? Ly.nslab - s0 : spp;
+        mbar_wait(r.empty + 8 * r.stage, r.phase ^ 1);
+        if (elect_one()) {
+          mbar_expect_tx(r.full + 8 * r.stage, (uint32_t)cnt * slab_bytes);
+          tma_bulk_g2s(r.sB + r.stage * STAGE_BYTES, blob + Ly.img_off + (size_t)s0 * slab_bytes, (uint32_t)cnt * slab_bytes,
+                       r.full + 8 * r.stage);
         }
-      }
-    }
-  }
-}
-
-// =============================== MMA issuer ===============================
-// Warp-uniform control flow (barrier waits by all lanes), tcgen05.mma / commit by one elected lane.
-// x_dump != null (training forward): the tile's X atoms are copied shared -> global (bulk store) once they are
-// complete; the copy is drained before the tile's last layer is issued, i.e. before X can be overwritten.
-template <bool TIMELINE>
-__device__ __forceinline__ void tc_mma_loop(const TcLayer* layers, int n_layers, uint32_t sX, uint32_t sB, const TcBars& bar,
-                                            uint32_t tmem_base, int64_t n_tiles, long long* timeline, uint8_t* x_dump,
-                                            int x_atoms) {
-  const int lane = threadIdx.x & 31;
-  uint32_t stage = 0, phase = 0, x_phase = 0, ed_phase0 = 0, ed_phase1 = 0;
-  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    for (int l = 0; l < n_layers; ++l) {
-      const TcLayer& Ly = layers[l];
-      const uint32_t idesc = make_idesc(Ly.N >> (Ly.nhalf - 1));
-      const uint32_t half_bytes = ((uint32_t)Ly.N * 64u) >> (Ly.nhalf - 1);
-      if (l == 0) {  // this tile's first operand is in place
-        mbar_wait(bar.x_ready, x_phase);
-        x_phase ^= 1;
-        if (x_dump) {
-          if (elect_one()) {
-            bulk_s2g(x_dump + (size_t)tile * x_atoms * ATOM_BYTES, sX, (uint32_t)x_atoms * ATOM_BYTES);
-            bulk_commit_group();
-          }
-          __syncwarp();
-        }
-      }
-      if (x_dump && l == n_layers - 1) {
-        if (elect_one()) bulk_wait_group_read0();
         __syncwarp();
-      }
-      // accumulator half 0 drained and the low-K half of the input activations written (previous layer,
-      // or the previous tile's last layer)
-      mbar_wait(bar.epi_done, ed_phase0);
-      ed_phase0 ^= 1;
-      tc_fence_after();
-      bool waited1 = !Ly.prev_two;   // a second epilogue-done arrival exists only after a two-half layer
-      for (int h = 0; h < Ly.nhalf; ++h) {
-        if (h == 1 && !waited1) {
-          mbar_wait(bar.epi_done + 8, ed_phase1);
-          ed_phase1 ^= 1;
-          tc_fence_after();
-          waited1 = true;
-        }
-        const uint32_t d_tmem = tmem_base + (uint32_t)(h * TM_ACC1);
-        if (TIMELINE && timeline && blockIdx.x == 0 && tile == (int64_t)gridDim.x && lane == 0) timeline[(l * 2 + h) * 4 + 0] = clock64();
-        for (int gi = 0; gi < Ly.ngroups; ++gi) {
-          const int grp = Ly.groups[gi];
-          const int first = grp & 31, cnt = (grp >> 5) & 7;
-          const bool from_h = (grp >> 8) & 1;
-          // Descriptor words are formed BEFORE the barrier waits (the empty asm pins them there): whatever sits between
-          // a satisfied wait and the first tcgen05.mma is pure latency on the layer-to-layer dependency chain.
-          // High words are constants; the low words advance by (bytes >> 4) per K step.
-          const uint32_t b_lo0 = (((sB + stage * STAGE_BYTES) >> 4) & 0x3FFFu) | 0x10000u;
-          const uint32_t hb16 = half_bytes >> 4;
-          // X slabs: `first` is a multiple of 4, i.e. atom aligned; slab i2 sits at atom (i2 >> 1), half (i2 & 1)
-          const uint32_t a0 = from_h ? tmem_base + (uint32_t)(Ly.h_in_col + first * 16)
-                                     : ((((sX + (uint32_t)(first >> 1) * ATOM_BYTES) >> 4) & 0x3FFFu) | 0x10000u);
-          const uint32_t accum0 = (gi > 0) ? 1u : 0u;
-          asm volatile("" ::"r"(b_lo0), "r"(hb16), "r"(a0), "r"(accum0), "r"(d_tmem), "r"(idesc));
-          if (((grp >> 9) & 1) && !waited1) {   // high-K half of the input activations
-            mbar_wait(bar.epi_done + 8, ed_phase1);
-            ed_phase1 ^= 1;
-            tc_fence_after();
-            waited1 = true;
-          }
-          mbar_wait(bar.full + 8 * stage, phase);
-          tc_fence_after();
-          if (elect_one()) {
-            uint32_t accum = accum0;
-            if (!from_h) {
-#pragma unroll
-              for (int i2 = 0; i2 < STAGE_SLABS; ++i2) {
-                if (i2 < cnt) {
-                  const uint32_t a_lo = a0 + (uint32_t)(i2 >> 1) * (ATOM_BYTES >> 4) + (uint32_t)(i2 & 1) * 4u;
-                  const uint32_t b_lo = b_lo0 + (uint32_t)i2 * hb16;
-                  umma_bf16(d_tmem, make_desc_hl(a_lo, DESC_HI_SW128), make_desc_hl(b_lo, DESC_HI_SW64), idesc, accum);
-                  umma_bf16(d_tmem, make_desc_hl(a_lo + 2u, DESC_HI_SW128), make_desc_hl(b_lo + 2u, DESC_HI_SW64), idesc, 1u);
-                  accum = 1u;
-                }
-              }
-            } else {
-#pragma unroll
-              for (int i2 = 0; i2 < STAGE_SLABS; ++i2) {
-                if (i2 < cnt) {
-                  const uint32_t b_lo = b_lo0 + (uint32_t)i2 * hb16;
-                  umma_bf16_ts(d_tmem, a0 + (uint32_t)i2 * 16u, make_desc_hl(b_lo, DESC_HI_SW64), idesc, accum);
-                  umma_bf16_ts(d_tmem, a0 + (uint32_t)i2 * 16u + 8u, make_desc_hl(b_lo + 2u, DESC_HI_SW64), idesc, 1u);
-                  accum = 1u;
-                }
-              }
-            }
-            umma_commit(bar.empty + 8 * stage);
-            if (gi == Ly.ngroups - 1) umma_commit(bar.acc_ready + 8 * h);
-          }
-          if (TIMELINE && gi == Ly.ngroups - 1 && timeline && blockIdx.x == 0 && tile == (int64_t)gridDim.x && lane == 0)
-            timeline[(l * 2 + h) * 4 + 1] = clock64();
-          __syncwarp();
-          if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-        }
-      }
-      if (!waited1) {   // one-half layer without high-K input after a two-half layer: keep the barrier phase in step
-        mbar_wait(bar.epi_done + 8, ed_phase1);
-        ed_phase1 ^= 1;
+        if (++r.stage == NSTAGE) { r.stage = 0; r.phase ^= 1; }
       }
     }
   }
 }
 
-// Host side: append one layer to a program.  in_two: the input activations were written in two halves.
-inline void tc_add_layer(TcLayer* layers, int& n, int N, int nx, int nh, int epi, int branch, int rc_base, int64_t img_off,
-                         int64_t bias_off, int single_max_n, int act_slot, int mask_word0, bool in_two_override = false,
-                         bool use_override = false) {
-  TcLayer& t = layers[n];
-  t.N = N; t.nslab_x = nx; t.nslab_h = nh; t.epi = epi; t.branch = branch; t.rc_base = rc_base;
-  t.h_in_col = (n & 1) ? TM_HB : TM_HA;     // layer n reads what layer n-1 wrote
-  t.h_out_col = (n & 1) ? TM_HA : TM_HB;
-  t.img_off = img_off; t.bias_off = bias_off;
-  t.nhalf = (t.N <= single_max_n) ? 1 : 2;
-  t.act_slot = act_slot; t.mask_word0 = mask_word0;
-  bool in_two = n > 0 && layers[n - 1].nhalf == 2;   // the input activations were written in two halves
-  if (use_override) in_two = in_two_override;
-  // K-slab groups: X slabs in runs of 4, then the low-K and high-K halves of H in runs of 4
-  int ng = 0;
-  auto emit = [&](int first, int count, int from_h, int needs_hi) {
-    for (int o = 0; o < count; o += STAGE_SLABS) {
-      const int c = (count - o < STAGE_SLABS) ? count - o : STAGE_SLABS;
-      t.groups[ng++] = (first + o) | (c << 5) | (from_h << 8) | (needs_hi << 9);
-    }
-  };
-  emit(0, nx, 0, 0);
-  if (in_two) {
-    emit(0, nh / 2, 1, 0);
-    emit(nh / 2, nh - nh / 2, 1, 1);
-  } else {
-    emit(0, nh, 1, 0);
-  }
-  t.ngroups = ng;
-  ++n;
+__device__ __forceinline__ void ring_release(const Ring& r, uint32_t stage) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(r.empty + 8 * stage);
 }
 
-inline void tc_finish_program(TcLayer* layers, int n) {
-  for (int i = 0; i < n; ++i) layers[i].prev_two = layers[(i + n - 1) % n].nhalf == 2;
+// =============================== one layer of one warpgroup ===============================
+// acc[64 x N] = X[:, 0 : 32 NX] . W_x^T  +  H[:, 0 : 32 NH] . W_h^T, with X in shared memory (sXw: this warpgroup's
+// first row of the X atoms) and H in registers (hin: 2 NH m64k16 A fragments).  Returns with every MMA complete and
+// every stage of the layer released.
+template <int N, int NX, int NH>
+__device__ __forceinline__ void mma_layer(float (&acc)[N / 2], const uint32_t* hin, uint32_t sXw, Ring& r) {
+  constexpr int SPP = 256 / N, NS = NX + NH, NB = N / 64;
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.0f;
+  uint32_t prev = 0;
+#pragma unroll
+  for (int s = 0; s < NS; ++s) {
+    if (s % SPP == 0) mbar_wait(r.full + 8 * r.stage, r.phase);
+    const uint32_t b0 = r.sB + r.stage * STAGE_BYTES + (uint32_t)(s % SPP) * (uint32_t)N * 64u;
+    wgmma_fence();
+#pragma unroll
+    for (int k16 = 0; k16 < 2; ++k16) {
+#pragma unroll
+      for (int nb = 0; nb < NB; ++nb) {
+        const uint64_t bd = desc_k_sw64(b0 + (uint32_t)nb * 4096u + (uint32_t)k16 * 32u);
+        if (s < NX)
+          wgmma_ss_n64<0, 0>(acc + nb * 32, desc_k_sw128(sXw + (uint32_t)(s >> 1) * ATOM_BYTES + (uint32_t)(s & 1) * 64u +
+                                                         (uint32_t)k16 * 32u), bd);
+        else
+          wgmma_rs_n64(acc + nb * 32, hin + ((s - NX) * 2 + k16) * 4, bd);
+      }
+    }
+    if (s % SPP == SPP - 1 || s == NS - 1) {
+      wgmma_commit();
+      if (s >= SPP) {   // the previous stage's MMAs have completed: hand it back to the producer
+        wgmma_wait<1>();
+        ring_release(r, prev);
+      }
+      prev = r.stage;
+      if (++r.stage == NSTAGE) { r.stage = 0; r.phase ^= 1; }
+    }
+  }
+  wgmma_wait<0>();
+  ring_release(r, prev);
+  fence_regs<N / 2>(acc);
 }
 
 }  // namespace tc

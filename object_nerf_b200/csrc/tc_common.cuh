@@ -1,5 +1,5 @@
-// tcgen05 / TMEM / mbarrier / bulk-copy PTX wrappers and UMMA descriptor helpers shared by the tensor-core kernels
-// (field_tc.cu: fused forward; bwd_tc.cu: backward chain, weight-gradient and input-gradient GEMMs).  sm_100a only.
+// wgmma / mbarrier / bulk-copy PTX wrappers and shared-memory descriptor helpers shared by the tensor-core kernels
+// (field_tc.cu: fused forward; bwd_chain.cu, bwd_wgrad.cu, bwd_dx.cu: backward).  sm_90a.
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
@@ -7,7 +7,7 @@
 
 namespace tc {
 
-constexpr int TM = 128;             // samples per tile (UMMA M)
+constexpr int TM = 128;             // samples per tile (two warpgroups of 64 rows)
 constexpr int ATOM_BYTES = 16384;   // 128 rows x 128 B (64 bf16 of K): one SWIZZLE_128B atom
 
 // ------------------------------------------------------------------------------------------------
@@ -24,9 +24,8 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// try_wait is a hardware sleep that ends when the phase completes or after a time limit.  The default limit is a few
-// hundred cycles: twenty waiting warps re-issuing the probe loop took a third of all issued instructions in the
-// two-tile kernel (profiles/r02_two_tile.md).  The hint (ns) stretches the limit; the wake-up on completion stays prompt.
+// try_wait is a hardware sleep that ends when the phase completes or after a time limit; the hint (ns) stretches the
+// limit so that waiting warps do not spin on the probe loop.  The wake-up on completion stays prompt.
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -51,24 +50,14 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-// make generic-proxy shared-memory writes visible to the async proxy (TMA / tcgen05 operand reads)
+// make generic-proxy shared-memory writes visible to the async proxy (bulk copies / wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-
-// shared -> global bulk copy (bulk async-group completion)
-__device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -80,102 +69,85 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t slot_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// per-thread register budget of the executing warpgroup (all its warps execute it)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// named barrier over the 128 threads of one warpgroup (ids 1 + warpgroup; 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+
+// ------------------------------------------------------------------------------------------------
+// wgmma (warpgroup MMA, M = 64 rows per warpgroup, K = 16 per instruction, bf16 x bf16 -> fp32 in registers)
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+template <int NR>
+__device__ __forceinline__ void fence_regs(float* d) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem desc] . B[smem desc]^T, bf16 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+#define ONERF_WG_D32                                                                                                   \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, " \
+  "%25, %26, %27, %28, %29, %30, %31}"
+#define ONERF_WG_OUT32(d)                                                                                              \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),          \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),           \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),          \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+
+// D[64 x 64] += A[64 x 16] (registers: the m64k16 A fragment, bf16 pairs) . B (shared memory, K-major)
+__device__ __forceinline__ void wgmma_rs_n64(float* d, const uint32_t* a, uint64_t desc_b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ONERF_WG_D32 ", {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+      : ONERF_WG_OUT32(d)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
 }
-// same with A taken from TMEM (bf16 pairs per column)
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 64] += A (shared memory) . B (shared memory); TA / TB: operand is MN-major (transposed)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss_n64(float* d, uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ONERF_WG_D32 ", %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : ONERF_WG_OUT32(d)
+      : "l"(desc_a), "l"(desc_b), "r"(1), "n"(TA), "n"(TB));
 }
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+// Shared-memory matrix descriptor (sm_90 GMMA):
+//   [0,14) start address >> 4, [16,30) leading byte offset >> 4, [32,46) stride byte offset >> 4,
+//   [62,64) layout type (1 = SWIZZLE_128B, 2 = SWIZZLE_64B)
+// K-major SWIZZLE_128B (X / dZ atoms): 8-row groups 1024 B apart.  K-major SWIZZLE_64B (weight stage images): 512 B.
+// MN-major SWIZZLE_128B (atoms read with K = samples): 64-wide MN blocks LBO apart, 8-row K groups 1024 B apart.
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
+  return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | ((uint64_t)layout << 62);
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr),
-               "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory matrix descriptor, K-major (cute::UMMA::SmemDescriptor):
-//   [0,14) start address >> 4, [16,30) leading byte offset >> 4, [32,46) stride byte offset >> 4 (8-row group pitch),
-//   [46,48) version = 1, [61,64) layout type (2 = SWIZZLE_128B, 4 = SWIZZLE_64B)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type) {
-  return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)layout_type << 61);
-}
-// same, from a precomputed high word and a low word ((addr >> 4) & 0x3FFF) | (1 << 16)
-constexpr uint32_t DESC_HI_SW128 = (1024u >> 4) | (1u << 14) | (2u << 29);
-constexpr uint32_t DESC_HI_SW64 = (512u >> 4) | (1u << 14) | (4u << 29);
-__device__ __forceinline__ uint64_t make_desc_hl(uint32_t lo, uint32_t hi) {
-  uint64_t d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
-  return d;
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D fp32, A/B bf16, both K-major, M = 128
-__device__ __forceinline__ uint32_t make_idesc(int N) {  // N = columns of ONE mma (a layer half)
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-}
+__device__ __forceinline__ uint64_t desc_k_sw128(uint32_t saddr) { return make_desc(saddr, 16, 1024, 1); }
+__device__ __forceinline__ uint64_t desc_k_sw64(uint32_t saddr) { return make_desc(saddr, 16, 512, 2); }
+__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes) { return make_desc(saddr, lbo_bytes, 1024, 1); }
 
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&t);
 }
-
+__device__ __forceinline__ float bf16_lo(uint32_t w) { return __uint_as_float(w << 16); }
+__device__ __forceinline__ float bf16_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
 
 // 16-byte chunk `chunk` (8 bf16 of K) of row `row` in a buffer made of SWIZZLE_128B atoms (64 K per atom, 128 rows)
 __device__ __forceinline__ uint32_t atom_chunk_off(int row, int chunk) {
   return (uint32_t)(chunk >> 3) * ATOM_BYTES + (uint32_t)row * 128u + (uint32_t)(((chunk & 7) ^ (row & 7)) << 4);
 }
+
+// Register fragment of a warpgroup's m64nN accumulator: thread (warp w of the group, lane l) holds rows
+// 16 w + l / 4 (entries 4 j, 4 j + 1) and 16 w + l / 4 + 8 (entries 4 j + 2, 4 j + 3), columns 8 j + 2 (l % 4) + {0, 1}.
+// Packed to bf16 pairs as pk[2 j] (first row) / pk[2 j + 1] (second row), 16 columns (pk[4 c .. 4 c + 3]) are exactly the
+// m64k16 A fragment of the next MMA: the output of one layer is the register operand of the next.
 
 }  // namespace tc

@@ -3,7 +3,7 @@
     import object_nerf_b200.dropin as dropin
     dropin.install()            # before `import train` / `from render_tools.editable_renderer import ...`
 
-After install(), these module names resolve to the B200 implementations (same public names, signatures and
+After install(), these module names resolve to the H100 implementations (same public names, signatures and
 result keys as the reference files they shadow):
 
     models.rendering              -> object_nerf_b200.rendering         (render_rays, sample_pdf, inference_model)

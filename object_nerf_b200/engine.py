@@ -22,7 +22,7 @@ PROFILE_EVENTS = None
 
 
 def default_precision() -> str:
-    """bf16 = tcgen05 tensor-core path (product default); fp32 = FFMA verification arithmetic."""
+    """bf16 = wgmma tensor-core path (product default); fp32 = FFMA verification arithmetic."""
     return os.environ.get("ONERF_PRECISION", "bf16")
 
 
@@ -85,7 +85,7 @@ def check_architecture(model, use_voxel: bool):
     got = [tuple(w.shape) for w, _ in lin]
     if got != want:
         raise RuntimeError(
-            "unsupported ObjectNeRF architecture for the sm_100a kernels (built for D=8, W=256, skips=[4], "
+            "unsupported ObjectNeRF architecture for the sm_90a kernels (built for D=8, W=256, skips=[4], "
             f"inst_D=4, inst_W=128, inst_skips=[2]); layer shapes {got}")
     return lin
 

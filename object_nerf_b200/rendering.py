@@ -198,7 +198,7 @@ def render_rays(models: Dict[str, Any], embeddings: Dict[str, Any], rays: torch.
             params += [w, b]
     precision = cfg["precision"] or engine.default_precision()
     if precision == "bf16" and has_table:
-        fn = backward.RenderRaysTcFn      # tcgen05 forward + backward
+        fn = backward.RenderRaysTcFn      # tensor-core forward + backward
     else:
         # verification arithmetic (and the plain-PE model): fp32 forward AND backward, one function end to end
         cfg["precision"] = "fp32"

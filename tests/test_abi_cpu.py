@@ -27,7 +27,7 @@ def test_exports_every_declared_symbol(lib):
     names = declared_functions()
     assert len(names) >= 13
     for n in names:
-        assert hasattr(lib, n), f"libonerf_sm100.so does not export {n}"
+        assert hasattr(lib, n), f"libonerf_sm90.so does not export {n}"
     from object_nerf_b200 import _lib
     assert sorted(_lib.EXPORTS) == names
 

@@ -1,6 +1,6 @@
 """The drop-in claim, demonstrated: the reference's UNMODIFIED entry points (byte-compiled into oracle/_ref by
 oracle/build_ref.py; test-only shims for pytorch_lightning / omegaconf / kornia / open3d, SURVEY.md §8c) run once on the
-reference's own hot path (CPU: the ground truth) and once over object_nerf_b200.dropin (sm_100a kernels), on a synthetic
+reference's own hot path (CPU: the ground truth) and once over object_nerf_b200.dropin (sm_90a kernels), on a synthetic
 ScanNet-style scene written to disk:
   * train.ObjectNeRFSystem.training_step (train.py:147-180) -> loss and gradients
   * render_tools.editable_renderer.EditableRenderer.render_edit (:203-294) as test/demo_editable_render.py:45-103

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Every CUDA stage and the full reference call
+"""GPU parity tests (pytest -m gpu).  Every CUDA stage and the full reference call
 surface are compared with (a) the CPU oracle on the same seeded inputs and (b) the committed golden
 fixtures produced by the real reference (tests/golden/, tools/make_golden.py).
 

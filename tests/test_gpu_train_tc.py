@@ -41,7 +41,7 @@ def _lib():
 
 
 def test_wgrad_kernel_matches_torch_matmul():
-    """dW_l = dZ_l^T In_l over all samples with MN-major tcgen05 operands, on random bf16 operand tiles."""
+    """dW_l = dZ_l^T In_l over all samples with MN-major wgmma operands, on random bf16 operand tiles."""
     L = _lib()
     lib = L.load()
     n_samples = 128 * 37          # 37 tiles: 74 stages, not a multiple of anything convenient
@@ -149,51 +149,6 @@ def test_training_forward_dump_matches_fp32_activations():
         clear = acts[slot].abs() > 2e-2
         agree = ((bits == 1) == want)[clear].float().mean().item()
         assert agree > 0.999, (slot, agree)
-
-
-@pytest.mark.parametrize("n_rays", [96, 97])
-def test_two_tile_training_dump_is_bitwise_the_one_tile_dump(n_rays):
-    """The training forward runs on the two-tile kernel; its workspace (X atoms, 16 activation slots, sign masks) must be
-    what the one-tile kernel writes, bit for bit, on the rows that exist (97 rays x 64 samples = 48.5 tiles: an odd tile
-    count and a partial last tile)."""
-    from object_nerf_b200 import engine
-    L = _lib()
-    inp = _small_scene(n_rays=n_rays)
-    S = 64
-    model, emb, rays, z, packed, grid, codes, n = _run_field(inp, S, "bf16")
-    B = n * S
-    T = helpers.train_layout(True, B)
-    lib = L.load()
-    out = {}
-    try:
-        for one_tile in (1, 0):
-            lib.onerf_debug_force_one_tile(one_tile)
-            ws = helpers.aligned_u8(T["total"], DEV, fill=0)
-            a = L.FieldArgs()
-            scene = torch.empty(n, S, 4, device=DEV)
-            obj = torch.empty(n, S, 4, device=DEV)
-            rc = torch.empty(n, 448, device=DEV)
-            a.rays, a.z, a.z_stride, a.codes = rays.data_ptr(), z.data_ptr(), S, codes.data_ptr()
-            a.n_rays, a.n_samples = n, S
-            a.grid = C.pointer(grid.c)
-            a.packed = packed.data_ptr()
-            a.want_scene, a.want_object, a.precision = 1, 1, L.PREC_BF16
-            a.scene_out, a.obj_out, a.out_stride, a.ray_const = scene.data_ptr(), obj.data_ptr(), S, rc.data_ptr()
-            a.train_ws = ws.data_ptr()
-            L.check(lib.onerf_field_fwd(L.ctx(torch.device(DEV)), C.byref(a), L.stream()))
-            torch.cuda.synchronize()
-            widths = [384] + [256] * 8 + [256, 128] + [128] * 4 + [128, 64]
-            acts = [helpers.from_atoms(ws, T["act_off"][slot], T["n_tiles"], T["act_atoms"][slot])[:B, :widths[slot]].clone()
-                    for slot in range(17)]
-            masks = helpers.read_masks(ws, T).reshape(T["n_tiles"], -1, 128).permute(0, 2, 1).reshape(T["n_tiles"] * 128, -1)[:B].clone()
-            out[one_tile] = (scene, obj, acts, masks)
-    finally:
-        lib.onerf_debug_force_one_tile(0)
-    assert torch.equal(out[0][0], out[1][0]) and torch.equal(out[0][1], out[1][1])
-    for slot in range(17):
-        assert torch.equal(out[0][2][slot], out[1][2][slot]), slot
-    assert torch.equal(out[0][3], out[1][3])
-    assert out[0][2][0].abs().max().item() > 0.5 and out[0][2][8].abs().max().item() > 0     # something was written
 
 
 def _torch_chain(acts_bf, w, dA_s, dA_o):

@@ -12,9 +12,6 @@ import torch.multiprocessing as mp
 
 from tests import cases
 
-REF = "/root/reference"
-
-
 def test_dropin_aliases_and_surface():
     from object_nerf_b200 import dropin
     saved = {k: sys.modules.get(k) for k in list(dropin.ALIASES) + ["models", "render_tools"]}
@@ -49,6 +46,18 @@ REF_SIGS = {
                           "use_disp", "perturb", "noise_std", "N_importance", "chunk", "white_back",
                           "background_skip_bbox"],
 }
+# the reference's literal default values of those parameters (same source lines)
+REF_DEFAULTS = {
+    "render_rays": {"N_samples": 64, "use_disp": False, "perturb": 0, "noise_std": 1, "N_importance": 0,
+                    "white_back": False, "forward_instance": True, "embedding_instance": None, "frustum_bound_th": 0,
+                    "pass_through_mask": None, "rays_in_bbox": False},
+    "inference_model": {"is_eval": False, "use_zero_as_last_delta": False, "forward_instance": True,
+                        "embedding_instance": None, "frustum_bound_th": 0, "pass_through_mask": None,
+                        "rays_in_bbox": False},
+    "sample_pdf": {"det": False, "eps": 1e-05},
+    "render_rays_multi": {"N_samples": 64, "use_disp": False, "perturb": 0, "noise_std": 0, "N_importance": 0,
+                          "white_back": False, "background_skip_bbox": None},
+}
 
 
 def test_signatures_match_reference():
@@ -58,22 +67,10 @@ def test_signatures_match_reference():
     for name, want in REF_SIGS.items():
         params = list(inspect.signature(ours[name]).parameters)
         assert params[: len(want)] == want, (name, params)
-    if os.path.isdir(REF):  # build container: compare defaults against the real reference source
-        import ast
-        src = {"rendering": open(f"{REF}/models/rendering.py").read(),
-               "multi": open(f"{REF}/render_tools/multi_rendering.py").read()}
-        for key, text in src.items():
-            for node in ast.walk(ast.parse(text)):
-                if isinstance(node, ast.FunctionDef) and node.name in REF_SIGS:
-                    ref_args = [a.arg for a in node.args.args]
-                    assert ref_args == REF_SIGS[node.name], (node.name, ref_args)
-                    ref_defaults = [ast.literal_eval(d) if isinstance(d, ast.Constant) else None for d in node.args.defaults]
-                    sig = inspect.signature(ours[node.name])
-                    our_defaults = [p.default for p in list(sig.parameters.values())[: len(ref_args)]
-                                    if p.default is not inspect.Parameter.empty]
-                    for rd, od in zip(ref_defaults, our_defaults):
-                        if rd is not None:
-                            assert rd == od, (node.name, rd, od)
+    for name, defaults in REF_DEFAULTS.items():
+        params = inspect.signature(ours[name]).parameters
+        for arg, want in defaults.items():
+            assert params[arg].default == want, (name, arg, params[arg].default, want)
 
 
 def test_state_dict_keys_match_reference_names():
