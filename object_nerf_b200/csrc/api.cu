@@ -35,12 +35,24 @@ extern "C" int onerf_ctx_create(int device, onerf_ctx** out) {
   c->num_sms = prop.multiProcessorCount;
   c->launches = 0;
   c->pack_tables = nullptr;
+  void* diag = nullptr;
+  const cudaError_t e = cudaHostAlloc(&diag, 16, cudaHostAllocMapped);
+  if (e != cudaSuccess) {
+    delete c;
+    onerf_set_error("onerf_ctx_create: cudaHostAlloc failed: %s", cudaGetErrorString(e));
+    return ONERF_ERR_CUDA;
+  }
+  memset(diag, 0, 16);
+  c->tc_diag = static_cast<uint32_t*>(diag);
   *out = c;
   return ONERF_OK;
 }
 
 extern "C" int onerf_ctx_destroy(onerf_ctx* ctx) {
-  if (ctx) onerf_free_pack_tables(ctx);
+  if (ctx) {
+    onerf_free_pack_tables(ctx);
+    if (ctx->tc_diag) cudaFreeHost(ctx->tc_diag);
+  }
   delete ctx;
   return ONERF_OK;
 }

@@ -26,6 +26,7 @@ struct ChainParams {
   int want_object;
   WLayer layers[MAX_LAYERS];
   int n_layers;
+  uint32_t* diag;             // mbarrier timeout record (onerf_ctx)
 };
 
 struct Rows {
@@ -107,7 +108,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) bwd_chain_kernel(const __grid_
   uint8_t* gen_base = smem_raw + (sbase - smem_u32(smem_raw));
   float* head = reinterpret_cast<float*>(gen_base + (sHead - sbase));
   const float* Pf = reinterpret_cast<const float*>(P.packed);
-  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u};
+  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u, P.diag};
 
   if (threadIdx.x == 0) ring_init_bars(ring.full, ring.empty);
   for (int i = threadIdx.x; i < 960; i += NUM_THREADS) {
@@ -144,6 +145,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) bwd_chain_kernel(const __grid_
       R.dAs[r] = live ? __ldg(P.dA_scene + e) : make_float4(0.f, 0.f, 0.f, 0.f);
       R.dAo[r] = (live && P.want_object) ? __ldg(P.dA_obj + e) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
+    // m64n64k16 MMAs: with full-width ones the chain's register demand (dZ fragments, per-row head gradients) does not
+    // fit the consumer budget and ptxas spills several KB per thread.
     {
       // ---- scene: dZ_dir (128) -> dZ_final -> dZ_7 (+ sigma head) -> ... -> dZ_0 ----
       uint32_t a[32];
@@ -151,15 +154,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) bwd_chain_kernel(const __grid_
       store_dz<128>(P, R, 9, a);
       float acc[128];
       uint32_t h[64];
-      mma_layer<256, 0, 4>(acc, a, 0u, ring);
+      mma_layer<256, 0, 4, 64>(acc, a, 0u, ring);
       chain_epi<256, BE_PLAIN>(acc, h, R, 0, 9, nullptr);
       store_dz<256>(P, R, 8, h);
-      mma_layer<256, 0, 8>(acc, h, 0u, ring);
+      mma_layer<256, 0, 8, 64>(acc, h, 0u, ring);
       chain_epi<256, BE_MASK_SIG>(acc, h, R, 0, 8, sigma_w);
       store_dz<256>(P, R, 7, h);
 #pragma unroll 1
       for (int l = 7; l >= 1; --l) {
-        mma_layer<256, 0, 8>(acc, h, 0u, ring);
+        mma_layer<256, 0, 8, 64>(acc, h, 0u, ring);
         chain_epi<256, BE_MASK>(acc, h, R, 0, l, nullptr);
         store_dz<256>(P, R, l - 1, h);
       }
@@ -171,15 +174,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) bwd_chain_kernel(const __grid_
       store_dz<64>(P, R, 15, a);
       float acc[64];
       uint32_t h[32];
-      mma_layer<128, 0, 2>(acc, a, 0u, ring);
+      mma_layer<128, 0, 2, 64>(acc, a, 0u, ring);
       chain_epi<128, BE_PLAIN>(acc, h, R, 1, 15, nullptr);
       store_dz<128>(P, R, 14, h);
-      mma_layer<128, 0, 4>(acc, h, 0u, ring);
+      mma_layer<128, 0, 4, 64>(acc, h, 0u, ring);
       chain_epi<128, BE_MASK_SIG>(acc, h, R, 1, 14, osigma_w);
       store_dz<128>(P, R, 13, h);
 #pragma unroll 1
       for (int l = 3; l >= 1; --l) {
-        mma_layer<128, 0, 4>(acc, h, 0u, ring);
+        mma_layer<128, 0, 4, 64>(acc, h, 0u, ring);
         chain_epi<128, BE_MASK>(acc, h, R, 1, 10 + l, nullptr);
         store_dz<128>(P, R, 10 + l - 1, h);
       }
@@ -202,6 +205,7 @@ int onerf_launch_bwd_chain(onerf_ctx* ctx, int use_voxel, int want_object, const
   P.dA_obj = reinterpret_cast<const float4*>(dA_obj);
   P.total = n_samples;
   P.want_object = want_object;
+  P.diag = ctx->tc_diag;
   int n = 0;
   // chain layer of GEMM g: operand = dZ of g (its N outputs = K of this layer), result = the hid_n inputs of g
   auto add = [&](int g) { P.layers[n++] = WLayer{L.g[g].bimg_off, L.g[g].hid_n, L.g[g].N / 32}; };

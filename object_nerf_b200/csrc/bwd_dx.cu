@@ -37,6 +37,7 @@ struct DxParams {
   onerf_grid grid;
   float* table_grad;      // (n_rows, 24)
   int want_object;
+  uint32_t* diag;         // mbarrier timeout record (onerf_ctx)
 };
 
 __device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
@@ -123,7 +124,7 @@ __global__ void __launch_bounds__(DX_THREADS, 1) bwd_dx_kernel(const __grid_cons
       for (int pass = 0; pass < (P.want_object ? 2 : 1); ++pass) {
         const uint32_t rows_off = pass ? 256u * 64u : 0u, rows_bytes = pass ? 128u * 64u : 256u * 64u;
         for (int qa = pass ? 8 : 0; qa < (pass ? 12 : n_src); ++qa) {
-          mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+          mbar_wait(bar_empty + 8 * stage, phase ^ 1, P.diag);
           if (elect_one()) {
             mbar_expect_tx(bar_full + 8 * stage, ATOM_BYTES + 2 * rows_bytes);
             const uint32_t dst = sStage + stage * DX_STAGE_BYTES;
@@ -154,7 +155,7 @@ __global__ void __launch_bounds__(DX_THREADS, 1) bwd_dx_kernel(const __grid_cons
     for (int i = 0; i < 128; ++i) acc[i] = 0.0f;
     uint32_t prev = 0;
     for (int qa = qa0; qa < qa1; ++qa) {
-      mbar_wait(bar_full + 8 * stage, phase);
+      mbar_wait(bar_full + 8 * stage, phase, P.diag);
       const uint32_t sa = sStage + stage * DX_STAGE_BYTES + (uint32_t)wg * 8192u, sb = sStage + stage * DX_STAGE_BYTES + ATOM_BYTES;
       wgmma_fence();
 #pragma unroll
@@ -217,6 +218,7 @@ int onerf_launch_bwd_dx(onerf_ctx* ctx, int want_object, const void* packed, con
                         cudaStream_t stream) {
   DxParams P;
   memset(&P, 0, sizeof(P));
+  P.diag = ctx->tc_diag;
   const PackLayout L = onerf_make_layout(1);
   P.packed = reinterpret_cast<const uint8_t*>(packed);
   P.ximg_off = L.ximg_off;

@@ -49,6 +49,7 @@ struct WgParams {
   float* grad;
   int n_stages;       // 64-sample stages = 2 * tiles
   int n_items;
+  uint32_t* diag;     // mbarrier timeout record (onerf_ctx)
   WgItem items[WG_MAX_ITEMS];
 };
 
@@ -114,7 +115,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
       const WgItem& it = P.items[seg.item];
       for (int s = seg.s0; s < seg.s1; ++s) {
         const int tile = s >> 1, half = s & 1;
-        mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+        mbar_wait(bar_empty + 8 * stage, phase ^ 1, P.diag);
         if (elect_one()) {
           mbar_expect_tx(bar_full + 8 * stage, (uint32_t)(2 + it.b_atoms) * HALF_ATOM);
           const uint32_t dst = sStage + stage * WG_STAGE_BYTES;
@@ -145,7 +146,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_const
     for (int i = 0; i < 128; ++i) acc[i] = 0.0f;
     uint32_t prev = 0;
     for (int s = seg.s0; s < seg.s1; ++s) {
-      mbar_wait(bar_full + 8 * stage, phase);
+      mbar_wait(bar_full + 8 * stage, phase, P.diag);
       const uint32_t sa = sStage + stage * WG_STAGE_BYTES + (uint32_t)wg * HALF_ATOM, sb = sStage + stage * WG_STAGE_BYTES + 2 * HALF_ATOM;
       wgmma_fence();
 #pragma unroll
@@ -212,6 +213,7 @@ int onerf_launch_wgrad(onerf_ctx* ctx, int use_voxel, int want_object, const voi
   const TrainLayout T = onerf_make_train_layout(use_voxel, n_samples);
   WgParams P;
   memset(&P, 0, sizeof(P));
+  P.diag = ctx->tc_diag;
   P.ws = reinterpret_cast<const uint8_t*>(ws);
   P.grad = grad;
   P.n_stages = 2 * T.n_tiles;

@@ -11,6 +11,10 @@ struct onerf_ctx {
   int num_sms;
   int64_t launches;
   void* pack_tables;   // pack.cu: per-layout job tables in device memory (created on first use)
+  // Mapped host memory the tensor-core kernels' bounded mbarrier wait (tc_common.cuh: mbar_wait) writes
+  // {1, block, barrier, parity} to before it traps.  Host memory stays readable after the trap has ended the CUDA
+  // context, so the next launch check can say which wait timed out.
+  uint32_t* tc_diag;
 };
 void onerf_free_pack_tables(onerf_ctx* ctx);
 
@@ -45,7 +49,12 @@ void onerf_set_error(const char* fmt, ...);
   do {                                                                            \
     cudaError_t e_ = cudaGetLastError();                                          \
     if (e_ != cudaSuccess) {                                                      \
-      onerf_set_error("%s: kernel launch failed: %s", __func__, cudaGetErrorString(e_)); \
+      const uint32_t* d_ = (ctx)->tc_diag;                                        \
+      if (d_ && d_[0])                                                            \
+        onerf_set_error("%s: kernel launch failed: %s (an earlier kernel timed out in an mbarrier wait: block %u, " \
+                        "barrier 0x%x, parity %u)", __func__, cudaGetErrorString(e_), d_[1], d_[2], d_[3]); \
+      else                                                                        \
+        onerf_set_error("%s: kernel launch failed: %s", __func__, cudaGetErrorString(e_)); \
       return ONERF_ERR_CUDA;                                                      \
     }                                                                             \
     (ctx)->launches++;                                                            \

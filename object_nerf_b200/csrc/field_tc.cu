@@ -38,6 +38,7 @@ struct TcParams {
   // masks are left in the training workspace for the tensor-core backward (layout.h: TrainLayout)
   uint8_t* dump;
   TrainLayout TL;
+  uint32_t* diag;   // mbarrier timeout record (onerf_ctx)
 };
 
 struct RowMeta {
@@ -184,7 +185,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
   float* bias_tab = reinterpret_cast<float*>(gen_base + (sBias - sbase));
   RowMeta* meta = reinterpret_cast<RowMeta*>(gen_base + (sMeta - sbase));
   const float* Pf = reinterpret_cast<const float*>(p.packed);
-  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u};
+  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u, P.diag};
 
   if (threadIdx.x == 0) ring_init_bars(ring.full, ring.empty);
   // per-column biases of every GEMM -> shared memory (layers with a per-ray constant read ray_const instead)
@@ -355,6 +356,7 @@ int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t 
   if (fp.want_object)
     for (int g = G_O0; g <= G_ODIR; ++g) add(g);
   P.n_layers = n;
+  P.diag = ctx->tc_diag;
   const int64_t total = (int64_t)fp.n_rays * fp.S;
   const int64_t tiles = (total + TM - 1) / TM;
   if (fp.train_ws) {

@@ -35,6 +35,7 @@ struct WLayer {
 struct Ring {
   uint32_t sB, full, empty;
   uint32_t stage, phase;
+  uint32_t* diag;   // timeout record of mbar_wait (onerf_ctx)
 };
 
 __device__ __forceinline__ void ring_init_bars(uint32_t full, uint32_t empty) {
@@ -56,7 +57,7 @@ __device__ __forceinline__ void tc_producer_loop(const WLayer* layers, int n_lay
       const uint32_t slab_bytes = (uint32_t)Ly.N * 64u;
       for (int s0 = 0; s0 < Ly.nslab; s0 += spp) {
         const int cnt = (Ly.nslab - s0 < spp) ? Ly.nslab - s0 : spp;
-        mbar_wait(r.empty + 8 * r.stage, r.phase ^ 1);
+        mbar_wait(r.empty + 8 * r.stage, r.phase ^ 1, r.diag);
         if (elect_one()) {
           mbar_expect_tx(r.full + 8 * r.stage, (uint32_t)cnt * slab_bytes);
           tma_bulk_g2s(r.sB + r.stage * STAGE_BYTES, blob + Ly.img_off + (size_t)s0 * slab_bytes, (uint32_t)cnt * slab_bytes,
@@ -69,36 +70,44 @@ __device__ __forceinline__ void tc_producer_loop(const WLayer* layers, int n_lay
   }
 }
 
+// One arrival per consumer warp, from lane 0.  The lane test is a predicate inside the asm statement, not a branch:
+// a divergent path between two wgmmas makes ptxas serialise every wgmma of the kernel.  wgmma.wait_group is
+// warp-synchronous, so when lane 0 arrives the whole warp has seen its MMAs complete.
 __device__ __forceinline__ void ring_release(const Ring& r, uint32_t stage) {
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) mbar_arrive(r.empty + 8 * stage);
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(
+          r.empty + 8 * stage),
+      "r"(threadIdx.x & 31)
+      : "memory");
 }
 
 // =============================== one layer of one warpgroup ===============================
 // acc[64 x N] = X[:, 0 : 32 NX] . W_x^T  +  H[:, 0 : 32 NH] . W_h^T, with X in shared memory (sXw: this warpgroup's
 // first row of the X atoms) and H in registers (hin: 2 NH m64k16 A fragments).  Returns with every MMA complete and
-// every stage of the layer released.
-template <int N, int NX, int NH>
+// every stage of the layer released.  Each stage's MMAs form one commit group; the wait for the previous group leaves
+// this one in flight.  W is the MMA width: N / W m64nWk16 MMAs per k16 step (W = N: one MMA, since a stage image
+// spans all N rows of B with one descriptor).
+template <int N, int NX, int NH, int W = N>
 __device__ __forceinline__ void mma_layer(float (&acc)[N / 2], const uint32_t* hin, uint32_t sXw, Ring& r) {
-  constexpr int SPP = 256 / N, NS = NX + NH, NB = N / 64;
+  constexpr int SPP = 256 / N, NS = NX + NH;
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] = 0.0f;
   uint32_t prev = 0;
 #pragma unroll
   for (int s = 0; s < NS; ++s) {
-    if (s % SPP == 0) mbar_wait(r.full + 8 * r.stage, r.phase);
+    if (s % SPP == 0) mbar_wait(r.full + 8 * r.stage, r.phase, r.diag);
     const uint32_t b0 = r.sB + r.stage * STAGE_BYTES + (uint32_t)(s % SPP) * (uint32_t)N * 64u;
     wgmma_fence();
 #pragma unroll
     for (int k16 = 0; k16 < 2; ++k16) {
 #pragma unroll
-      for (int nb = 0; nb < NB; ++nb) {
-        const uint64_t bd = desc_k_sw64(b0 + (uint32_t)nb * 4096u + (uint32_t)k16 * 32u);
+      for (int nb = 0; nb < N / W; ++nb) {
+        const uint64_t bd = desc_k_sw64(b0 + (uint32_t)nb * (uint32_t)W * 64u + (uint32_t)k16 * 32u);
         if (s < NX)
-          wgmma_ss_n64<0, 0>(acc + nb * 32, desc_k_sw128(sXw + (uint32_t)(s >> 1) * ATOM_BYTES + (uint32_t)(s & 1) * 64u +
-                                                         (uint32_t)k16 * 32u), bd);
+          wgmma_ss<W>(acc + nb * (W / 2),
+                      desc_k_sw128(sXw + (uint32_t)(s >> 1) * ATOM_BYTES + (uint32_t)(s & 1) * 64u + (uint32_t)k16 * 32u), bd);
         else
-          wgmma_rs_n64(acc + nb * 32, hin + ((s - NX) * 2 + k16) * 4, bd);
+          wgmma_rs<W>(acc + nb * (W / 2), hin + ((s - NX) * 2 + k16) * 4, bd);
       }
     }
     if (s % SPP == SPP - 1 || s == NS - 1) {

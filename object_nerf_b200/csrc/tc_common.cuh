@@ -3,7 +3,6 @@
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
-#include <stdio.h>
 
 namespace tc {
 
@@ -24,30 +23,38 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// try_wait is a hardware sleep that ends when the phase completes or after a time limit; the hint (ns) stretches the
+// try_wait is a hardware sleep that ends when the phase completes or after a time limit; the hint (20 us) stretches the
 // limit so that waiting warps do not spin on the probe loop.  The wake-up on completion stays prompt.
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
+// Bounded wait: a protocol bug must become an error, not a hung GPU.  The probe loop, the clock bound and the trap are
+// one asm statement with no call and no branch visible to the compiler, so consumers can wait while wgmma groups are in
+// flight (a function call or a divergent branch between wgmmas makes ptxas serialise them).  On timeout the thread
+// records (1, block, barrier, parity) in `diag` (mapped host memory owned by onerf_ctx, reported by the next launch
+// check on the host) and traps.
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, uint32_t* diag) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity), "r"(20000u)
+      "{\n\t.reg .pred p;\n\t.reg .u64 t0, t1;\n\t.reg .u32 b;\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n\t"
+      "@p bra DONE;\n\t"
+      "mov.u64 t0, %%clock64;\n"
+      "WAIT:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n\t"
+      "@p bra DONE;\n\t"
+      "mov.u64 t1, %%clock64;\n\t"
+      "sub.u64 t1, t1, t0;\n\t"
+      "setp.lt.u64 p, t1, %4;\n\t"
+      "@p bra WAIT;\n\t"
+      "mov.u32 b, %%ctaid.x;\n\t"
+      "st.volatile.u32 [%3 + 4], b;\n\t"
+      "st.volatile.u32 [%3 + 8], %0;\n\t"
+      "st.volatile.u32 [%3 + 12], %1;\n\t"
+      "membar.sys;\n\t"
+      "st.volatile.u32 [%3], 1;\n\t"
+      "membar.sys;\n\t"
+      "trap;\n"
+      "DONE:\n\t}"
+      :
+      : "r"(bar), "r"(parity), "r"(20000u), "l"(diag), "n"(4000000000ll)
       : "memory");
-  return ok != 0;
-}
-// Bounded wait: a protocol bug must become an error, not a hung GPU.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000ll) {
-      printf("onerf tc: mbarrier timeout (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x,
-             bar, parity);
-      __trap();
-    }
-  }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 // make generic-proxy shared-memory writes visible to the async proxy (bulk copies / wgmma operand reads)
@@ -97,10 +104,27 @@ __device__ __forceinline__ void fence_regs(float* d) {
   "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, " \
   "%25, %26, %27, %28, %29, %30, %31}"
 #define ONERF_WG_OUT32(d)                                                                                              \
-  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),          \
-      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),           \
-      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),          \
-      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+  "+f"((d)[0]), "+f"((d)[1]), "+f"((d)[2]), "+f"((d)[3]), "+f"((d)[4]), "+f"((d)[5]), "+f"((d)[6]), "+f"((d)[7]),      \
+      "+f"((d)[8]), "+f"((d)[9]), "+f"((d)[10]), "+f"((d)[11]), "+f"((d)[12]), "+f"((d)[13]), "+f"((d)[14]),           \
+      "+f"((d)[15]), "+f"((d)[16]), "+f"((d)[17]), "+f"((d)[18]), "+f"((d)[19]), "+f"((d)[20]), "+f"((d)[21]),         \
+      "+f"((d)[22]), "+f"((d)[23]), "+f"((d)[24]), "+f"((d)[25]), "+f"((d)[26]), "+f"((d)[27]), "+f"((d)[28]),         \
+      "+f"((d)[29]), "+f"((d)[30]), "+f"((d)[31])
+#define ONERF_WG_OUT64(d) ONERF_WG_OUT32(d), ONERF_WG_OUT32((d) + 32)
+#define ONERF_WG_OUT128(d) ONERF_WG_OUT64(d), ONERF_WG_OUT64((d) + 64)
+#define ONERF_WG_D64 "{" \
+  "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, " \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, " \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63" "}"
+#define ONERF_WG_D128 "{" \
+  "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, " \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, " \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, " \
+  "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, " \
+  "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, " \
+  "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, " \
+  "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127" "}"
 
 // D[64 x 64] += A[64 x 16] (registers: the m64k16 A fragment, bf16 pairs) . B (shared memory, K-major)
 __device__ __forceinline__ void wgmma_rs_n64(float* d, const uint32_t* a, uint64_t desc_b) {
@@ -118,6 +142,47 @@ __device__ __forceinline__ void wgmma_ss_n64(float* d, uint64_t desc_a, uint64_t
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ONERF_WG_D32 ", %32, %33, p, 1, 1, %35, %36;\n\t}"
       : ONERF_WG_OUT32(d)
       : "l"(desc_a), "l"(desc_b), "r"(1), "n"(TA), "n"(TB));
+}
+
+// Full-width shapes of the layer chain (tc_chain.cuh): D[64 x N] += A . B, N = 64, 128 or 256, both operands K-major,
+// A from registers (rs) or shared memory (ss).  One instruction covers all N columns of a k16 step.
+template <int N>
+__device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t desc_b) {
+  if constexpr (N == 64) {
+    wgmma_rs_n64(d, a, desc_b);
+  } else if constexpr (N == 128) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " ONERF_WG_D64 ", {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+        : ONERF_WG_OUT64(d)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+  } else {
+    static_assert(N == 256, "wgmma_rs: N is 64, 128 or 256");
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " ONERF_WG_D128 ", {%128, %129, %130, %131}, %132, p, 1, 1, 0;\n\t}"
+        : ONERF_WG_OUT128(d)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+  }
+}
+template <int N>
+__device__ __forceinline__ void wgmma_ss(float* d, uint64_t desc_a, uint64_t desc_b) {
+  if constexpr (N == 64) {
+    wgmma_ss_n64<0, 0>(d, desc_a, desc_b);
+  } else if constexpr (N == 128) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " ONERF_WG_D64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : ONERF_WG_OUT64(d)
+        : "l"(desc_a), "l"(desc_b), "r"(1));
+  } else {
+    static_assert(N == 256, "wgmma_ss: N is 64, 128 or 256");
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " ONERF_WG_D128 ", %128, %129, p, 1, 1, 0, 0;\n\t}"
+        : ONERF_WG_OUT128(d)
+        : "l"(desc_a), "l"(desc_b), "r"(1));
+  }
 }
 
 // Shared-memory matrix descriptor (sm_90 GMMA):
