@@ -141,8 +141,8 @@ typedef struct onerf_field_args {
    * activations of the forward: [0] X (384 voxel / 64 plain), [1..8] scene hidden 1..8 (256), [9] scene final (256),
    * [10] scene dir (128), [11..14] object hidden 1..4 (128), [15] object final (128), [16] object dir (64). */
   float* const* activations;
-  /* training forward (ONERF_PREC_BF16, voxel model, dense z / outputs): if non-NULL, a workspace of
-   * onerf_field_train_bytes(n_rays * n_samples) bytes receiving what the tensor-core backward needs: every layer's
+  /* training forward (ONERF_PREC_BF16, either model, dense z / outputs): if non-NULL, a workspace of
+   * onerf_field_train_bytes(grid != NULL, n_rays * n_samples) bytes receiving what the tensor-core backward needs: every layer's
    * output activations and the encoded input as bf16 tiles in the tensor cores' operand layout, and 1-bit LeakyReLU
    * masks (object_nerf_b200/csrc/layout.h: TrainLayout). */
   void* train_ws;
@@ -214,8 +214,9 @@ typedef struct onerf_render_args {
   onerf_render_maps fine;       /* written iff n_importance > 0 */
   void* workspace;              /* >= onerf_render_rays_workspace_bytes(...) bytes, 256-byte aligned */
   size_t workspace_bytes;
-  /* training: if non-NULL (ONERF_PREC_BF16, voxel model), >= onerf_train_workspace_bytes(...) bytes, 1024-byte aligned;
-   * the forward then keeps both passes' per-sample fields and the backward operands there for onerf_render_rays_bwd. */
+  /* training: if non-NULL (ONERF_PREC_BF16, either model), >= onerf_train_workspace_bytes(grid != NULL, ...) bytes,
+   * 1024-byte aligned; the forward then keeps both passes' per-sample fields and the backward operands there for
+   * onerf_render_rays_bwd.  With ONERF_PREC_FP32 a training workspace is ONERF_ERR_UNSUPPORTED. */
   void* train_ws;
   size_t train_ws_bytes;
 } onerf_render_args;
@@ -344,7 +345,8 @@ int onerf_total_loss(onerf_ctx* ctx, const onerf_loss_args* args, void* stream);
  * through models/rendering.py, models/nerf_model.py:97-152, models/embedding_helper.py:354-409, models/code_library.py).
  * onerf_render_rays_fwd with train_ws set runs the bf16 forward and keeps the backward operands;
  * onerf_render_rays_bwd turns the upstream gradients of the rendered maps into gradients of the 2 x 20 nn.Linear
- * tensors, the per-ray object codes and the voxel feature table:
+ * tensors, the per-ray object codes and (voxel model) the voxel feature table, for either model (fwd->grid NULL = plain
+ * PE model, whose encoding has no trainable parameters):
  *   compositing backward -> head gradients -> input-gradient chain (wgmma, transposed weight images, operand resident
  *   in registers) -> weight gradients (wgmma, sample-axis reduction) -> encoding gradient (wgmma + scatter-add) ->
  *   per-ray-constant columns (direction encoding, object code) -> reference [out,in] layout.
@@ -371,7 +373,8 @@ typedef struct onerf_render_bwd_args {
   float* const* dW_fine;
   float* const* db_fine;
   float* d_codes;                /* (N,64); required iff forward_instance */
-  float* table_grad;             /* (n_rows,24) gradient of grid->table */
+  float* table_grad;             /* (n_rows,24) gradient of grid->table, or NULL; must be NULL for the plain PE model
+                                    (ONERF_ERR_BAD_ARG otherwise) */
 } onerf_render_bwd_args;
 
 int onerf_render_rays_bwd(onerf_ctx* ctx, const onerf_render_args* fwd, const onerf_render_bwd_args* bwd, void* stream);

@@ -5,7 +5,8 @@ models/code_library.py; SURVEY.md §8 row a14).
 Two arithmetics, selected by `precision`:
   bf16 (default)  RenderRaysTcFn: ONE C call forward (onerf_render_rays_fwd with a training workspace: the tensor-core forward
                   keeps every layer's activations as bf16 operand tiles) and ONE C call backward (onerf_render_rays_bwd:
-                  wgmma input-gradient chain, weight-gradient and encoding-gradient GEMMs).  Voxel model only.
+                  wgmma input-gradient chain, weight-gradient and encoding-gradient GEMMs).  Voxel and plain-PE model;
+                  the plain model has no voxel table and so no encoding gradient.
   fp32            RenderRaysFn below: the verification path (FFMA forward re-run with fp32 activation dump, fp32 GEMMs).
 
 Gradients are produced for exactly what the reference trains: the 2 x 40 nn.Linear tensors of the coarse and fine
@@ -309,7 +310,7 @@ class _Lease:
 
 class RenderRaysTcFn(torch.autograd.Function):
     """Differentiable render_rays on the tensor cores.  Inputs after `cfg`: rays, codes, then the flat list of trainable
-    tensors ([voxel table] + coarse 40 + fine 40), as assembled by rendering.render_rays."""
+    tensors ([voxel table, voxel model only] + coarse 40 + fine 40), as assembled by rendering.render_rays."""
 
     @staticmethod
     def forward(ctx, cfg, rays, codes, *params):
@@ -320,14 +321,15 @@ class RenderRaysTcFn(torch.autograd.Function):
         ns, ni = cfg["N_samples"], cfg["N_importance"]
         fi = cfg["forward_instance"]
         rand = cfg["rand"]
+        use_voxel = cfg["has_table"]
         f = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
-        grid = engine.GridBuffers.from_module(emb)
+        grid = engine.GridBuffers.from_module(emb) if use_voxel else None
         keep = [rays, grid]
         a = _lib.RenderArgs()
         packed, lins = {}, {}
         for typ in cfg["model_order"]:
             lins[typ] = engine.model_linears(cfg["models"][typ])
-            packed[typ] = engine.packed_for(cfg["models"][typ], True, fresh=True)
+            packed[typ] = engine.packed_for(cfg["models"][typ], use_voxel, fresh=True)
         maps = {}
         for typ, s in (("coarse", ns), ("fine", ns + ni)):
             if typ == "fine" and ni == 0:
@@ -341,7 +343,7 @@ class RenderRaysTcFn(torch.autograd.Function):
                 setattr(cm, k, v.data_ptr())
         ws_bytes = lib.onerf_render_rays_workspace_bytes(n, ns, ni)
         workspace = torch.empty(max(ws_bytes, 256), dtype=torch.uint8, device=dev)
-        tws_bytes = lib.onerf_train_workspace_bytes(1, n, ns, ni)
+        tws_bytes = lib.onerf_train_workspace_bytes(int(use_voxel), n, ns, ni)
         lease = _Lease(_pool.take(tws_bytes, dev))
         codes_c = engine._f32(codes.detach()) if (codes is not None and fi) else None
         mask = cfg["pass_through_mask"]
@@ -351,7 +353,7 @@ class RenderRaysTcFn(torch.autograd.Function):
         keep += [codes_c, mask, opt, workspace, packed]
         a.rays, a.codes = rays.data_ptr(), _lib.ptr(codes_c)
         a.n_rays, a.n_samples, a.n_importance = n, ns, ni
-        a.grid = C.pointer(grid.c)
+        a.grid = C.pointer(grid.c) if use_voxel else None
         a.packed_coarse = packed["coarse"].data_ptr()
         a.packed_fine = packed["fine"].data_ptr() if ni > 0 else None
         a.precision = _lib.PREC_BF16
@@ -413,8 +415,9 @@ class RenderRaysTcFn(torch.autograd.Function):
             setattr(b, "dW_" + typ, dWp)
             setattr(b, "db_" + typ, dbp)
         d_codes = torch.zeros(a.n_rays, 64, dtype=torch.float32, device=dev) if ctx.has_codes else None
-        table = cfg["embeddings"]["xyz"].embedding_space_ftr.weight
-        table_grad = torch.zeros_like(table, dtype=torch.float32) if cfg["has_table"] else None
+        table_grad = None
+        if cfg["has_table"]:
+            table_grad = torch.zeros_like(cfg["embeddings"]["xyz"].embedding_space_ftr.weight, dtype=torch.float32)
         b.d_codes, b.table_grad = _lib.ptr(d_codes), _lib.ptr(table_grad)
         with torch.cuda.device(dev):
             _lib.check(lib.onerf_render_rays_bwd(_lib.ctx(dev), C.byref(a), C.byref(b), _lib.stream()))

@@ -187,9 +187,9 @@ extern "C" int onerf_render_rays_fwd(onerf_ctx* ctx, const onerf_render_args* a,
   float *scene_c = scene, *obj_c = obj, *scene_f = scene, *obj_f = obj;
   void *tl_c = nullptr, *tl_f = nullptr;
   if (a->train_ws) {
-    ONERF_UNSUPPORTED(!a->grid || a->precision != ONERF_PREC_BF16, "training workspace: bf16 voxel model only");
+    ONERF_UNSUPPORTED(a->precision != ONERF_PREC_BF16, "training workspace: bf16 only");
     ONERF_CHECK_ARG((reinterpret_cast<uintptr_t>(a->train_ws) & 1023u) == 0, "train_ws must be 1024-byte aligned");
-    const TrainWs W = onerf_make_train_ws(1, a->n_rays, a->n_samples, a->n_importance);
+    const TrainWs W = onerf_make_train_ws(onerf_train_use_voxel(a), a->n_rays, a->n_samples, a->n_importance);
     if (a->train_ws_bytes < (size_t)W.total) {
       onerf_set_error("onerf_render_rays_fwd: training workspace too small (%zu < %lld)", a->train_ws_bytes, (long long)W.total);
       return ONERF_ERR_WORKSPACE;

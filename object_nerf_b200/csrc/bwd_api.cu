@@ -60,10 +60,10 @@ extern "C" int onerf_bwd_dx(onerf_ctx* ctx, int want_object, const void* packed,
 }
 
 // ---- backward of one pass ----
-static int bwd_pass(onerf_ctx* ctx, const onerf_render_args* f, const onerf_render_bwd_args* b, const TrainWs& W, bool fine,
-                    char* ws, const float* pe, void* stream_) {
+static int bwd_pass(onerf_ctx* ctx, const onerf_render_args* f, const onerf_render_bwd_args* b, const TrainWs& W, int use_voxel,
+                    bool fine, char* ws, const float* pe, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  const int use_voxel = 1, fi = f->forward_instance ? 1 : 0;
+  const int fi = f->forward_instance ? 1 : 0;
   const int S = fine ? f->n_samples + f->n_importance : f->n_samples;
   const int R = f->n_rays;
   const int64_t B = (int64_t)R * S;
@@ -109,11 +109,12 @@ static int bwd_pass(onerf_ctx* ctx, const onerf_render_args* f, const onerf_rend
   TRY(onerf_launch_bwd_colsums(ctx, use_voxel, fi, tl, B, dA_s, fi ? dA_o : nullptr, gk, stream));
   TRY(onerf_launch_wgrad(ctx, use_voxel, fi, tl, B, gk, stream));
   TRY(onerf_unpack_grads(ctx, use_voxel, gk, dW, db, stream_));
-  // 5. encoding -> voxel table
+  // 5. encoding -> voxel table (voxel model only: the plain model has nothing trainable in front of X)
   if (b->table_grad) TRY(onerf_launch_bwd_dx(ctx, fi, packed, tl, B, f->rays, m.z_vals, S, f->grid, b->table_grad, stream));
   // 6. per-ray-constant columns: direction encoding into the two dir layers, object code into object layers 1 and 3
   TRY(onerf_launch_bwd_raysums(ctx, use_voxel, fi, tl, R, S, rs, stream));
-  const int xin = 271, ovx = 104, oin = xin + ovx + ONERF_NCODE;
+  // reference input widths: scene input [voxel PE | xyz PE] or [xyz PE], object voxel block, object input [.. | code]
+  const int xin = use_voxel ? 271 : 63, ovx = use_voxel ? 104 : 0, oin = xin + ovx + ONERF_NCODE;
   TRY(onerf_gemm(ctx, rs + RC_SDIR, ONERF_RAY_CONST_FLOATS, 1, pe, 27, dW[10] + 256, 256 + 27, 128, 27, R, 1, stream_));
   if (fi) {
     TRY(onerf_gemm(ctx, rs + RC_ODIR, ONERF_RAY_CONST_FLOATS, 1, pe, 27, dW[18] + 128, 128 + 27, 64, 27, R, 1, stream_));
@@ -131,11 +132,13 @@ static int bwd_pass(onerf_ctx* ctx, const onerf_render_args* f, const onerf_rend
 extern "C" int onerf_render_rays_bwd(onerf_ctx* ctx, const onerf_render_args* f, const onerf_render_bwd_args* b, void* stream) {
   ONERF_CHECK_ARG(ctx && f && b, "null argument");
   ONERF_CHECK_ARG(f->train_ws, "the forward was not run with a training workspace");
-  ONERF_UNSUPPORTED(!f->grid || f->precision != ONERF_PREC_BF16, "the tensor-core backward is built for the bf16 voxel model");
+  ONERF_UNSUPPORTED(f->precision != ONERF_PREC_BF16, "the tensor-core backward is built for bf16");
   ONERF_CHECK_ARG(b->W_coarse && b->dW_coarse && b->db_coarse, "null coarse gradient arguments");
   ONERF_CHECK_ARG(f->n_importance == 0 || (b->W_fine && b->dW_fine && b->db_fine), "null fine gradient arguments");
+  const int use_voxel = onerf_train_use_voxel(f);
+  ONERF_CHECK_ARG(use_voxel || !b->table_grad, "table_grad given for the plain-PE model, which has no voxel table");
   ONERF_CHECK_ARG(!b->table_grad || onerf_aligned16(b->table_grad), "table_grad misaligned");
-  const TrainWs W = onerf_make_train_ws(1, f->n_rays, f->n_samples, f->n_importance);
+  const TrainWs W = onerf_make_train_ws(use_voxel, f->n_rays, f->n_samples, f->n_importance);
   if (f->train_ws_bytes < (size_t)W.total) {
     onerf_set_error("onerf_render_rays_bwd: training workspace too small (%zu < %lld)", f->train_ws_bytes, (long long)W.total);
     return ONERF_ERR_WORKSPACE;
@@ -146,8 +149,8 @@ extern "C" int onerf_render_rays_bwd(onerf_ctx* ctx, const onerf_render_args* f,
   int rc = onerf_dir_encode(ctx, f->rays, f->n_rays, pe, stream);
   if (rc != ONERF_OK) return rc;
   if (f->n_importance > 0) {
-    rc = bwd_pass(ctx, f, b, W, true, ws, pe, stream);
+    rc = bwd_pass(ctx, f, b, W, use_voxel, true, ws, pe, stream);
     if (rc != ONERF_OK) return rc;
   }
-  return bwd_pass(ctx, f, b, W, false, ws, pe, stream);
+  return bwd_pass(ctx, f, b, W, use_voxel, false, ws, pe, stream);
 }

@@ -1,6 +1,11 @@
 // Layout of the training workspace of onerf_render_rays_fwd / onerf_render_rays_bwd (one caller-owned blob).
 #pragma once
+#include "../../include/onerf.h"
 #include "layout.h"
+
+// The model a training call trains: voxel when it carries a grid, plain PE otherwise.  The forward and the backward
+// both derive the workspace layout from it.
+static inline int onerf_train_use_voxel(const onerf_render_args* a) { return a->grid ? 1 : 0; }
 
 struct TrainWs {
   int64_t tl_coarse, tl_fine;                   // field training workspaces (layout.h: TrainLayout) of the two passes

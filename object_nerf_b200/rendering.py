@@ -197,10 +197,10 @@ def render_rays(models: Dict[str, Any], embeddings: Dict[str, Any], rays: torch.
         for w, b in engine.model_linears(models[typ]):
             params += [w, b]
     precision = cfg["precision"] or engine.default_precision()
-    if precision == "bf16" and has_table:
-        fn = backward.RenderRaysTcFn      # tensor-core forward + backward
+    if precision == "bf16":
+        fn = backward.RenderRaysTcFn      # tensor-core forward + backward, voxel and plain-PE model alike
     else:
-        # verification arithmetic (and the plain-PE model): fp32 forward AND backward, one function end to end
+        # verification arithmetic, selected explicitly: fp32 forward AND backward, one function end to end
         cfg["precision"] = "fp32"
         cfg["fresh_pack"] = True          # training: never trust a cached blob (optimizers may write through .data)
         fn = backward.RenderRaysFn

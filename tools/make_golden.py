@@ -1,10 +1,12 @@
 """Generate tests/golden/*.npz by running the REAL reference (/root/reference, CPU) on the
 deterministic synthetic scenes of tests/synth.py.  Run in the build container only:
 
-    python tools/make_golden.py
+    python tools/make_golden.py                    # every fixture
+    python tools/make_golden.py grad_case_plain    # only the named generators (see GENERATORS)
 
 The fixtures hold reference OUTPUTS (and the case parameters); inputs are regenerated from seeds by
-tests/cases.py, which is shared by this script, the CPU oracle tests and the GPU parity tests.
+tests/cases.py (tests/grad_plain.py for the plain-PE training step), which is shared by this script, the CPU oracle
+tests and the GPU parity tests.
 The reference draws RNG inside the path (models/rendering.py:40,156,187,276); to pin those branches
 the torch.rand* entry points are patched for the duration of a reference call so that it consumes
 the pre-drawn buffers of synth.random_buffers in call order.
@@ -29,7 +31,7 @@ from models.embedding_helper import Embedding, EmbeddingVoxel  # noqa: E402
 from render_tools.multi_rendering import render_rays_multi as ref_render_rays_multi  # noqa: E402
 from utils.bbox_utils import BBoxRayHelper  # noqa: E402
 
-from tests import cases, synth  # noqa: E402
+from tests import cases, grad_plain, synth  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 
@@ -190,13 +192,22 @@ def gen_multi_cases():
 def gen_grad_case():
     """Training step through the REAL reference: render_rays (train mode, injected RNG) -> reference TotalLoss ->
     backward.  The fixture keeps the loss and, per parameter tensor, its L2 norm, sum and sampled entries."""
+    _gen_grad(cases.GRAD_CASE, cases.build_grad_case(), "grad_train_step")
+
+
+def gen_grad_case_plain():
+    """The same training step on the plain positional-encoding model (Embedding(3, 10) as the xyz embedding): the
+    fixture has the keys of grad_train_step minus voxel|*."""
+    _gen_grad(grad_plain.GRAD_CASE_PLAIN, grad_plain.build_grad_case_plain(), "grad_train_step_plain")
+
+
+def _gen_grad(c, inp, name):
     from models.losses import TotalLoss
     from models.code_library import CodeLibrary
-    c = cases.GRAD_CASE
-    inp = cases.build_grad_case()
-    models = {"coarse": ref_model(inp["weights"]["coarse"], True).train(),
-              "fine": ref_model(inp["weights"]["fine"], True).train()}
-    emb = ref_voxel_embedding(inp["grid"])
+    use_voxel = c["use_voxel"]
+    models = {"coarse": ref_model(inp["weights"]["coarse"], use_voxel).train(),
+              "fine": ref_model(inp["weights"]["fine"], use_voxel).train()}
+    emb = ref_voxel_embedding(inp["grid"]) if use_voxel else Embedding(3, 10)
     lib = CodeLibrary(R.default_model_config())
     with torch.no_grad():
         lib.embedding_instance.weight.copy_(inp["code_table"])
@@ -215,16 +226,20 @@ def gen_grad_case():
     loss.backward()
     fix = {"loss": loss.detach()}
     named = [(f"{typ}.{k}", p) for typ, m in models.items() for k, p in m.named_parameters()]
-    named += [("codes", lib.embedding_instance.weight), ("voxel", emb.embedding_space_ftr.weight)]
-    for name, p in named:
+    named += [("codes", lib.embedding_instance.weight)]
+    if use_voxel:
+        named += [("voxel", emb.embedding_space_ftr.weight)]
+    for pname, p in named:
         g = p.grad.reshape(-1)
-        fix[name + "|norm"] = g.norm()
-        fix[name + "|sum"] = g.sum()
-        fix[name + "|samples"] = g[cases.sample_indices(name, g.numel())]
-    nz = torch.nonzero(emb.embedding_space_ftr.weight.grad.abs().sum(1)).view(-1)
-    fix["voxel|nonzero_rows"] = nz
-    save("grad_train_step", **fix)
-    print("loss", loss.item(), "voxel rows touched", nz.numel())
+        fix[pname + "|norm"] = g.norm()
+        fix[pname + "|sum"] = g.sum()
+        fix[pname + "|samples"] = g[cases.sample_indices(pname, g.numel())]
+    if use_voxel:
+        nz = torch.nonzero(emb.embedding_space_ftr.weight.grad.abs().sum(1)).view(-1)
+        fix["voxel|nonzero_rows"] = nz
+        print("voxel rows touched", nz.numel())
+    save(name, **fix)
+    print(name, "loss", loss.item())
 
 
 def gen_gridbuild():
@@ -330,13 +345,24 @@ def gen_maint_cases():
     print("pruning:", n_occu, "->", int(torch.nonzero(emb.voxel_occupancy).shape[0]))
 
 
+GENERATORS = ("ray_cases", "maint_cases", "loss_cases", "gridbuild", "grad_case", "grad_case_plain", "stage_cases",
+              "render_cases", "multi_cases")
+
 if __name__ == "__main__":
     torch.set_num_threads(8)
+    if len(sys.argv) > 1:      # python tools/make_golden.py grad_case_plain ...: only the named generators
+        unknown = [a for a in sys.argv[1:] if a not in GENERATORS]
+        if unknown:
+            sys.exit(f"unknown generator(s) {unknown}; choose from {list(GENERATORS)}")
+        for a in sys.argv[1:]:
+            globals()["gen_" + a]()
+        sys.exit(0)
     gen_ray_cases()
     gen_maint_cases()
     gen_loss_cases()
     gen_gridbuild()
     gen_grad_case()
+    gen_grad_case_plain()
     gen_stage_cases()
     gen_render_cases()
     gen_multi_cases()
