@@ -39,14 +39,16 @@ __device__ __forceinline__ void pe8_to_chunks(uint32_t xbase, int row, int chunk
 }
 
 // PE10(xyz): 63 values in reference order + one zero -> 8 chunks starting at chunk0.  Values are packed to
-// bf16 pairs as they are produced (the stream position is a compile-time constant after unrolling).
+// bf16 pairs as they are produced and each chunk is stored once complete (the stream position is a compile-time
+// constant after unrolling), so few registers stay live: the encoder warps run at the producer's register budget.
 __device__ __forceinline__ void pe_xyz_to_chunks(uint32_t xbase, int row, int chunk0, float x, float y, float z) {
-  uint32_t pk[32];
+  uint32_t pk[4];
   float pend = 0.0f;
   int pos = 0;
   auto emit = [&](float val) {
     if ((pos & 1) == 0) pend = val;
-    else pk[pos >> 1] = pack_bf16(pend, val);
+    else pk[(pos >> 1) & 3] = pack_bf16(pend, val);
+    if ((pos & 7) == 7) st_chunk(a_chunk_addr(xbase, row, chunk0 + (pos >> 3)), pk[0], pk[1], pk[2], pk[3]);
     ++pos;
   };
   emit(x); emit(y); emit(z);
@@ -68,9 +70,6 @@ __device__ __forceinline__ void pe_xyz_to_chunks(uint32_t xbase, int row, int ch
     }
   }
   emit(0.0f);
-#pragma unroll
-  for (int q = 0; q < 8; ++q)
-    st_chunk(a_chunk_addr(xbase, row, chunk0 + q), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
 }
 
 

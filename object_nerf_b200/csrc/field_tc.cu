@@ -1,15 +1,16 @@
 // wgmma (Hopper tensor core) implementation of the fused encode + two-branch MLP for sm_90a.
 //
 // One persistent CTA per SM; a CTA owns one 128-sample tile at a time (tc_chain.cuh).
-//   warpgroups 0 / 1 (256 thr)  encode rows [0, 64) / [64, 128) of the tile into shared memory (X, bf16, K-major
-//                               SWIZZLE_128B atoms) and run every layer on them: wgmma M = 64 with the accumulator in
-//                               registers, then the epilogue (bias / per-ray constant -> LeakyReLU -> bf16 pairs) leaves
-//                               the output in registers as the NEXT layer's A operand.  Hidden activations never touch
-//                               shared or global memory.  Heads (sigma, rgb) are CUDA-core dot products on the fp32
-//                               values, reduced over the four lanes that share a row.
+//   warpgroups 0 / 1 (256 thr)  run every layer on rows [0, 64) / [64, 128) of the tile, object branch first: wgmma
+//                               M = 64 with the accumulator in registers, then the epilogue (bias / per-ray constant ->
+//                               LeakyReLU -> bf16 pairs) leaves the output in registers as the NEXT layer's A operand.
+//                               Hidden activations never touch shared or global memory.  Heads (sigma, rgb) are CUDA-core
+//                               dot products on the fp32 values, reduced over the four lanes that share a row.
 //   warpgroup 2                 its first warp streams the weights global -> shared with cp.async.bulk (pre-swizzled
 //                               SWIZZLE_64B stage images written by pack.cu) through an mbarrier ring running ahead across
-//                               layers and tiles; the warpgroup hands most of its registers to warpgroups 0 / 1.
+//                               layers and tiles; its other three warps (encoder_loop) encode the next tile into shared
+//                               memory (X, bf16, K-major SWIZZLE_128B atoms) while the consumers run the layers after the
+//                               last X-fed one.  The warpgroup hands most of its registers to warpgroups 0 / 1.
 // Skip / dir / code concatenations never materialise: a skip layer takes K-slabs from both X and H, and the
 // per-ray-constant terms arrive through ray_const (see layout.h).
 //
@@ -39,6 +40,9 @@ struct TcParams {
   uint8_t* dump;
   TrainLayout TL;
   uint32_t* diag;   // mbarrier timeout record (onerf_ctx)
+#ifdef ONERF_FIELD_TIMELINE
+  uint64_t* tl;     // phase stamps (below)
+#endif
 };
 
 struct RowMeta {
@@ -52,7 +56,33 @@ struct Rows {
   int ray[2], si[2], mute[2];
   const float* rc[2];
   int64_t tile;
+#ifdef ONERF_FIELD_TIMELINE
+  uint64_t* tl;     // this warpgroup's stamp record of this tile, or null
+#endif
 };
+
+#ifdef ONERF_FIELD_TIMELINE
+// Phase timeline, built only by tools/field_timeline.py: lane 0 of each warpgroup stores clock64 stamps of the first
+// TL_TILES tiles of CTAs [0, TL_CTAS) at tl[((cta * 3 + warpgroup) * TL_TILES + k) * TL_SLOTS + slot] (slot meanings in
+// the tool).  The store is predicated inside one asm statement, so no branch lands between two wgmmas.
+constexpr int TL_CTAS = 8, TL_TILES = 16, TL_SLOTS = 80;
+uint64_t* g_timeline = nullptr;
+__device__ __forceinline__ void tl_put(uint64_t* tl, int slot, uint64_t v) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u64 p, %0, 0;\n\t@p st.global.u64 [%1], %2;\n\t}" ::"l"(tl), "l"(tl + slot),
+               "l"(v)
+               : "memory");
+}
+__device__ __forceinline__ uint64_t* tl_record(const TcParams& P, int64_t tile, int wg, bool lead) {
+  const int64_t k = (tile - blockIdx.x) / gridDim.x;
+  if (!P.tl || !lead || blockIdx.x >= TL_CTAS || k >= TL_TILES) return nullptr;
+  return P.tl + (((int64_t)blockIdx.x * 3 + wg) * TL_TILES + k) * TL_SLOTS;
+}
+#define TL_AT(tl, slot) tl_put((tl), (slot), clock64())
+#define TL_PUT(tl, slot, v) tl_put((tl), (slot), (v))
+#else
+#define TL_AT(tl, slot)
+#define TL_PUT(tl, slot, v)
+#endif
 
 __device__ __forceinline__ uint32_t leaky_bf16x2(uint32_t x) {
   __nv_bfloat162 v = *reinterpret_cast<__nv_bfloat162*>(&x);
@@ -166,58 +196,83 @@ __device__ __forceinline__ void write_heads(const FieldParams& p, const Rows& R,
   }
 }
 
-template <bool VOXEL, bool DUMP>
-__global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_constant__ TcParams P) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
+// consumers -> encoders: lane 0 of each consumer warp arrives on x_free when `on` (a predicate, not a branch)
+__device__ __forceinline__ void x_release(uint32_t x_free, bool on) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, %1, 1;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(x_free),
+      "r"((uint32_t)on & (uint32_t)((threadIdx.x & 31) == 0))
+      : "memory");
+}
+
+// One layer of one warpgroup: MMAs, epilogue, and in the training forward the dump of its output to activation slot
+// `slot` (= GEMM index + 1) with its sign masks (mask_word0 >= 0).  An X-fed layer with free_x set hands X to the
+// encoder warps once its MMAs have completed.
+template <int N, int NX, int NH, int EPI, bool DUMP>
+__device__ __forceinline__ void run_layer(const TcParams& P, const Rows& R, Ring& ring, uint32_t sXw, float (&acc)[N / 2],
+                                          const uint32_t* hin, uint32_t* hout, const float* bias, int rc_base,
+                                          const float* headw, float (&part)[2][4], int slot, int mask_word0,
+                                          uint32_t x_free = 0, bool free_x = false) {
+  TL_AT(R.tl, 3 * slot);
+  mma_layer<N, NX, NH>(acc, hin, sXw, ring);
+  if constexpr (NX > 0) x_release(x_free, free_x);
+  TL_AT(R.tl, 3 * slot + 1);
+#ifdef ONERF_FIELD_TIMELINE
+  TL_PUT(R.tl, 55 + slot, ring.full_wait);
+  ring.full_wait = 0;
+#endif
+  epilogue<N, EPI>(acc, hout, bias, R, rc_base, headw, part);
+  if (DUMP) dump_layer<N>(P, R, slot, mask_word0, hout);
+  TL_AT(R.tl, 3 * slot + 2);
+}
+
+// =============================== encoder warps (warps 1-3 of the producer warpgroup) ===============================
+// They write X (bf16, K-major SWIZZLE_128B atoms) and the row metadata of tile t + gridDim.x while the consumers still
+// run tile t: (row, column quarter) jobs, each gathering before it waits for X to be free, so the first job's loads
+// overlap the consumers' last X-fed layer.  Hand-off through two CTA-local mbarriers:
+//   x_full  encoders -> consumers: X and meta[] of the tile are written (one arrival per encoder thread, after
+//           fence.proxy.async so that wgmma sees the stores)
+//   x_free  consumers -> encoders: the last X-fed layer's MMAs have completed and meta[] has been read (one arrival
+//           per consumer warp)
+// Channel order and arithmetic are those of the in-line encode they replace, so X is bit for bit the same.
+constexpr int NUM_ENCODER = 3 * 32;
+
+__device__ __forceinline__ void prefetch_l2(const void* ptr) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
+}
+
+// L2 prefetch of the 128-byte lines [bytes0, bytes0 + nbytes) of rows [r0, r1] (row pitch `pitch` bytes) of `base`
+__device__ __forceinline__ void prefetch_rows(const void* base, int64_t pitch, int64_t bytes0, int nbytes, int r0,
+                                              int r1, int et) {
+  const int lines = (nbytes + 127) >> 7;
+  for (int i = et; i < (r1 - r0 + 1) * lines; i += NUM_ENCODER)
+    prefetch_l2(reinterpret_cast<const char*>(base) + (r0 + i / lines) * pitch + bytes0 + (int64_t)(i % lines) * 128);
+}
+
+template <bool VOXEL>
+__device__ __forceinline__ void encoder_loop(const TcParams& P, uint32_t sX, RowMeta* meta, uint32_t x_full,
+                                             uint32_t x_free, int64_t n_tiles, int64_t total) {
   const FieldParams& p = P.f;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int X_ATOMS = VOXEL ? 6 : 1;
-  constexpr int XS = VOXEL ? 9 : 2, XO = VOXEL ? 12 : 2;   // K slabs of X read by the scene / object branch (KX, KO)
-
-  // ---- shared memory carve-up (base is 1024-byte aligned: required by the 128B swizzle) ----
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sX = sbase;
-  const uint32_t sB = sX + X_ATOMS * ATOM_BYTES;
-  const uint32_t sBias = sB + NSTAGE * STAGE_BYTES;                 // [G_COUNT][256] floats
-  const uint32_t sMeta = sBias + G_COUNT * 256 * 4;                 // [128] RowMeta
-  const uint32_t sBar = sMeta + TM * sizeof(RowMeta);
-  uint8_t* gen_base = smem_raw + (sbase - smem_u32(smem_raw));
-  float* bias_tab = reinterpret_cast<float*>(gen_base + (sBias - sbase));
-  RowMeta* meta = reinterpret_cast<RowMeta*>(gen_base + (sMeta - sbase));
-  const float* Pf = reinterpret_cast<const float*>(p.packed);
-  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u, P.diag};
-
-  if (threadIdx.x == 0) ring_init_bars(ring.full, ring.empty);
-  // per-column biases of every GEMM -> shared memory (layers with a per-ray constant read ray_const instead)
-  for (int i = threadIdx.x; i < G_COUNT * 256; i += NUM_THREADS) {
-    const int g = i >> 8, c = i & 255;
-    bias_tab[i] = (c < p.L.g[g].N) ? __ldg(Pf + p.L.g[g].bias_off + c) : 0.0f;
-  }
-  __syncthreads();
-
-  const int64_t total = (int64_t)p.n_rays * p.S;
-  const int64_t n_tiles = (total + TM - 1) / TM;
-
-  if (warp >= PRODUCER_WARP) {
-    setmaxnreg_dec<PRODUCER_REGS>();
-    if (warp == PRODUCER_WARP)
-      tc_producer_loop(P.layers, P.n_layers, reinterpret_cast<const uint8_t*>(p.packed), ring, n_tiles);
-    return;
-  }
-  setmaxnreg_inc<CONSUMER_REGS>();
-
-  // =============================== encode + MMA + epilogue warpgroups ===============================
-  const int wg = warp >> 2, tid = threadIdx.x & 127;
-  const uint32_t sXw = sX + (uint32_t)wg * 64u * 128u;
-  Rows R;
-  R.row[0] = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  R.row[1] = R.row[0] + 8;
-  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    R.tile = tile;
-    // ---- encode this warpgroup's 64 rows of X: (row, column quarter) jobs ----
+  const int et = threadIdx.x - NUM_CONSUMER - 32;
+  constexpr int JOBS = VOXEL ? 4 * TM : TM;
+  uint32_t it = 0;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+#ifdef ONERF_FIELD_TIMELINE
+    uint64_t* tl = tl_record(P, tile, 2, et == 0);
+#endif
+    TL_AT(tl, 0);
+    {  // rows the consumers' per-ray-constant epilogues read for this tile, and the next tile's rays and depths
+      const int64_t e0 = tile * TM, e1 = min(e0 + TM, total) - 1;
+      prefetch_rows(p.ray_const, ONERF_RAY_CONST_FLOATS * 4, 0, ONERF_RAY_CONST_FLOATS * 4, (int)(e0 / p.S),
+                    (int)(e1 / p.S), et);
+      const int64_t n0 = e0 + (int64_t)gridDim.x * TM, n1 = min(n0 + TM, total) - 1;
+      if (n0 < total) {
+        prefetch_rows(p.rays, 32, 0, 32, (int)(n0 / p.S), (int)(n1 / p.S), et);
+        prefetch_rows(p.z, p.z_stride * 4, 0, p.S * 4, (int)(n0 / p.S), (int)(n1 / p.S), et);
+      }
+    }
 #pragma unroll 1
-    for (int job = tid; job < 256; job += 128) {
-      const int row = wg * 64 + (job & 63), cq = job >> 6;
+    for (int job = et; job < JOBS; job += NUM_ENCODER) {
+      const int row = job & (TM - 1), cq = job / TM;
       const int64_t e = tile * TM + row;
       const bool live = e < total;
       const int ray = live ? (int)(e / p.S) : 0;
@@ -236,30 +291,97 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
         int mute = 0;
         if (live && p.mute_zero_rays && __ldg(p.z + (int64_t)ray * p.z_stride + (p.S - 1)) == 0.0f) mute = 3;
         if (live && mute == 0 && p.n_boxes > 0 && point_in_boxes(p.boxes, p.n_boxes, x, y, z)) mute = 1;
+        mbar_wait(x_free, (it & 1) ^ 1, P.diag);
         meta[row] = RowMeta{ray, si, mute, live ? 1 : 0};
       }
-      if (VOXEL) {
+      if (VOXEL && cq < 3) {
         const GridView g = load_grid_view(p.grid);
         float f[8];
-        if (cq == 0) {
-          voxel_trilinear<0, 8, false>(g, x, y, z, f);
-          pe8_to_chunks(sX, row, 0, 2, f);        // scene channels 0-7 : chunks 0, 2, 4, ...
-        } else if (cq == 1) {
-          voxel_trilinear<8, 8, false>(g, x, y, z, f);
-          pe8_to_chunks(sX, row, 1, 2, f);        // scene channels 8-15: chunks 1, 3, 5, ...
-        } else if (cq == 2) {
-          voxel_trilinear<16, 8, false>(g, x, y, z, f);
-          pe8_to_chunks(sX, row, 34, 1, f);       // object voxel block starts at column 272 = chunk 34
-        } else {
-          pe_xyz_to_chunks(sX, row, 26, x, y, z); // columns 208..271
-          st_chunk(a_chunk_addr(sX, row, 47), 0u, 0u, 0u, 0u);  // columns 376..383
-        }
-      } else {
-        if (cq == 0) pe_xyz_to_chunks(sX, row, 0, x, y, z);
+        // scene channels 0-7: chunks 0, 2, 4, ...; 8-15: chunks 1, 3, 5, ...; object channels: chunk 34 (column 272) on
+        if (cq == 0) voxel_trilinear<0, 8, false>(g, x, y, z, f);
+        else if (cq == 1) voxel_trilinear<8, 8, false>(g, x, y, z, f);
+        else voxel_trilinear<16, 8, false>(g, x, y, z, f);
+        mbar_wait(x_free, (it & 1) ^ 1, P.diag);
+        pe8_to_chunks(sX, row, cq < 2 ? cq : 34, cq < 2 ? 2 : 1, f);
+      } else if (cq == (VOXEL ? 3 : 0)) {
+        mbar_wait(x_free, (it & 1) ^ 1, P.diag);
+        pe_xyz_to_chunks(sX, row, VOXEL ? 26 : 0, x, y, z);                   // columns 208..271 (voxel model)
+        if (VOXEL) st_chunk(a_chunk_addr(sX, row, 47), 0u, 0u, 0u, 0u);       // columns 376..383
       }
     }
+    mbar_wait(x_free, (it & 1) ^ 1, P.diag);   // (a no-op after the first job: keeps one arrival per phase)
+    TL_AT(tl, 1);
     fence_async_smem();
-    wg_sync(wg);
+    mbar_arrive(x_full);
+    TL_AT(tl, 2);
+  }
+}
+
+template <bool VOXEL, bool DUMP>
+__global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_constant__ TcParams P) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const FieldParams& p = P.f;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  constexpr int X_ATOMS = VOXEL ? 6 : 1;
+  constexpr int XS = VOXEL ? 9 : 2, XO = VOXEL ? 12 : 2;   // K slabs of X read by the scene / object branch (KX, KO)
+
+  // ---- shared memory carve-up (base is 1024-byte aligned: required by the 128B swizzle) ----
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t sX = sbase;
+  const uint32_t sB = sX + X_ATOMS * ATOM_BYTES;
+  const uint32_t sBias = sB + NSTAGE * STAGE_BYTES;                 // [G_COUNT][256] floats
+  const uint32_t sMeta = sBias + G_COUNT * 256 * 4;                 // [128] RowMeta
+  const uint32_t sBar = sMeta + TM * sizeof(RowMeta);               // ring full[], empty[], then x_full, x_free
+  const uint32_t x_full = sBar + 16 * NSTAGE, x_free = x_full + 8;
+  uint8_t* gen_base = smem_raw + (sbase - smem_u32(smem_raw));
+  float* bias_tab = reinterpret_cast<float*>(gen_base + (sBias - sbase));
+  RowMeta* meta = reinterpret_cast<RowMeta*>(gen_base + (sMeta - sbase));
+  const float* Pf = reinterpret_cast<const float*>(p.packed);
+  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u, P.diag};
+
+  if (threadIdx.x == 0) {
+    mbar_init(x_full, NUM_ENCODER);
+    mbar_init(x_free, NUM_CONSUMER / 32);
+    ring_init_bars(ring.full, ring.empty);   // (its fence covers the two above)
+  }
+  // per-column biases of every GEMM -> shared memory (layers with a per-ray constant read ray_const instead)
+  for (int i = threadIdx.x; i < G_COUNT * 256; i += NUM_THREADS) {
+    const int g = i >> 8, c = i & 255;
+    bias_tab[i] = (c < p.L.g[g].N) ? __ldg(Pf + p.L.g[g].bias_off + c) : 0.0f;
+  }
+  __syncthreads();
+
+  const int64_t total = (int64_t)p.n_rays * p.S;
+  const int64_t n_tiles = (total + TM - 1) / TM;
+
+  if (warp >= PRODUCER_WARP) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == PRODUCER_WARP)
+      tc_producer_loop(P.layers, P.n_layers, reinterpret_cast<const uint8_t*>(p.packed), ring, n_tiles);
+    else
+      encoder_loop<VOXEL>(P, sX, meta, x_full, x_free, n_tiles, total);
+    return;
+  }
+  setmaxnreg_inc<CONSUMER_REGS>();
+
+  // =============================== MMA + epilogue warpgroups ===============================
+  // Object branch first, then scene: the last X-fed layer is then the scene skip layer S4 (O2 in an object-only
+  // launch), and the encoders write the next tile's X during the layers after it.
+  const int wg = warp >> 2, tid = threadIdx.x & 127;
+  const uint32_t sXw = sX + (uint32_t)wg * 64u * 128u;
+  const bool free_after_o2 = !p.want_scene;
+  Rows R;
+  R.row[0] = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  R.row[1] = R.row[0] + 8;
+  uint32_t it = 0;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+    R.tile = tile;
+#ifdef ONERF_FIELD_TIMELINE
+    R.tl = tl_record(P, tile, wg, tid == 0);
+#endif
+    TL_AT(R.tl, 0);
+    mbar_wait(x_full, it & 1, P.diag);
+    TL_AT(R.tl, 1);
     if (DUMP) {   // this warpgroup's rows of the X atoms, byte for byte
 #pragma unroll 1
       for (int a = 0; a < X_ATOMS; ++a) {
@@ -268,77 +390,64 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
         for (int i = tid; i < 512; i += 128) dst[i] = src[i];
       }
     }
+    // the row metadata is read before this warp releases X (x_free covers meta[] too)
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const RowMeta m = meta[R.row[r]];
       R.live[r] = m.live; R.ray[r] = m.ray; R.si[r] = m.si; R.mute[r] = m.mute;
       R.rc[r] = p.ray_const + (int64_t)m.ray * ONERF_RAY_CONST_FLOATS;
     }
+    TL_AT(R.tl, 2);
 
+    if (p.want_object) {
+      float acc[64];
+      uint32_t h[32];
+      float part[2][4] = {};
+      run_layer<128, XO, 0, EPI_HIDDEN_RC, DUMP>(P, R, ring, sXw, acc, h, h, nullptr, RC_OL0, nullptr, part, 11,
+                                                 onerf_mask_word0(11), x_free, false);
+      run_layer<128, 0, 4, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_O1 * 256, 0, nullptr, part, 12,
+                                             onerf_mask_word0(12));
+      // [X | h1], object code through ray_const
+      run_layer<128, XO, 4, EPI_HIDDEN_RC, DUMP>(P, R, ring, sXw, acc, h, h, nullptr, RC_OL2, nullptr, part, 13,
+                                                 onerf_mask_word0(13), x_free, free_after_o2);
+      run_layer<128, 0, 4, EPI_HIDDEN_SIGMA, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_O3 * 256, 0,
+                                                   Pf + p.L.osigma_w, part, 14, onerf_mask_word0(14));
+      run_layer<128, 0, 4, EPI_FINAL, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_OFIN * 256, 0, nullptr, part, 15, -1);
+      float accd[32];
+      uint32_t hd[16];
+      run_layer<64, 0, 4, EPI_DIR, DUMP>(P, R, ring, sXw, accd, h, hd, nullptr, RC_ODIR, Pf + p.L.orgb_w, part, 16,
+                                         onerf_mask_word0(16));
+      write_heads(p, R, 1, part);
+    }
     if (p.want_scene) {
       float acc[128];
       uint32_t h[64];
       float part[2][4] = {};
       const float* sw = Pf + p.L.sigma_w;
-      mma_layer<256, XS, 0>(acc, h, sXw, ring);
-      epilogue<256, EPI_HIDDEN>(acc, h, bias_tab + G_S0 * 256, R, 0, nullptr, part);
-      if (DUMP) dump_layer<256>(P, R, 1, onerf_mask_word0(1), h);
+      run_layer<256, XS, 0, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_S0 * 256, 0, nullptr, part, 1,
+                                              onerf_mask_word0(1), x_free, false);
 #pragma unroll 1
-      for (int l = 1; l < 4; ++l) {
-        mma_layer<256, 0, 8>(acc, h, sXw, ring);
-        epilogue<256, EPI_HIDDEN>(acc, h, bias_tab + (G_S0 + l) * 256, R, 0, nullptr, part);
-        if (DUMP) dump_layer<256>(P, R, 1 + l, onerf_mask_word0(1 + l), h);
-      }
-      mma_layer<256, XS, 8>(acc, h, sXw, ring);   // skip layer: [X | h3]
-      epilogue<256, EPI_HIDDEN>(acc, h, bias_tab + G_S4 * 256, R, 0, nullptr, part);
-      if (DUMP) dump_layer<256>(P, R, 5, onerf_mask_word0(5), h);
+      for (int l = 1; l < 4; ++l)
+        run_layer<256, 0, 8, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + (G_S0 + l) * 256, 0, nullptr, part,
+                                               1 + l, onerf_mask_word0(1 + l));
+      // skip layer [X | h3]: the last reader of X
+      run_layer<256, XS, 8, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_S4 * 256, 0, nullptr, part, 5,
+                                              onerf_mask_word0(5), x_free, true);
 #pragma unroll 1
-      for (int l = 5; l < 7; ++l) {
-        mma_layer<256, 0, 8>(acc, h, sXw, ring);
-        epilogue<256, EPI_HIDDEN>(acc, h, bias_tab + (G_S0 + l) * 256, R, 0, nullptr, part);
-        if (DUMP) dump_layer<256>(P, R, 1 + l, onerf_mask_word0(1 + l), h);
-      }
-      mma_layer<256, 0, 8>(acc, h, sXw, ring);
-      epilogue<256, EPI_HIDDEN_SIGMA>(acc, h, bias_tab + G_S7 * 256, R, 0, sw, part);
-      if (DUMP) dump_layer<256>(P, R, 8, onerf_mask_word0(8), h);
-      mma_layer<256, 0, 8>(acc, h, sXw, ring);
-      epilogue<256, EPI_FINAL>(acc, h, bias_tab + G_SFIN * 256, R, 0, nullptr, part);
-      if (DUMP) dump_layer<256>(P, R, 9, -1, h);
+      for (int l = 5; l < 7; ++l)
+        run_layer<256, 0, 8, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + (G_S0 + l) * 256, 0, nullptr, part,
+                                               1 + l, onerf_mask_word0(1 + l));
+      run_layer<256, 0, 8, EPI_HIDDEN_SIGMA, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_S7 * 256, 0, sw, part, 8,
+                                                   onerf_mask_word0(8));
+      run_layer<256, 0, 8, EPI_FINAL, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_SFIN * 256, 0, nullptr, part, 9, -1);
       float accd[64];
       uint32_t hd[32];
-      mma_layer<128, 0, 8>(accd, h, sXw, ring);
-      epilogue<128, EPI_DIR>(accd, hd, nullptr, R, RC_SDIR, Pf + p.L.rgb_w, part);
-      if (DUMP) dump_layer<128>(P, R, 10, onerf_mask_word0(10), hd);
+      run_layer<128, 0, 8, EPI_DIR, DUMP>(P, R, ring, sXw, accd, h, hd, nullptr, RC_SDIR, Pf + p.L.rgb_w, part, 10,
+                                          onerf_mask_word0(10));
       write_heads(p, R, 0, part);
     }
-    if (p.want_object) {
-      float acc[64];
-      uint32_t h[32];
-      float part[2][4] = {};
-      mma_layer<128, XO, 0>(acc, h, sXw, ring);
-      epilogue<128, EPI_HIDDEN_RC>(acc, h, nullptr, R, RC_OL0, nullptr, part);
-      if (DUMP) dump_layer<128>(P, R, 11, onerf_mask_word0(11), h);
-      mma_layer<128, 0, 4>(acc, h, sXw, ring);
-      epilogue<128, EPI_HIDDEN>(acc, h, bias_tab + G_O1 * 256, R, 0, nullptr, part);
-      if (DUMP) dump_layer<128>(P, R, 12, onerf_mask_word0(12), h);
-      mma_layer<128, XO, 4>(acc, h, sXw, ring);   // [X | h1], object code through ray_const
-      epilogue<128, EPI_HIDDEN_RC>(acc, h, nullptr, R, RC_OL2, nullptr, part);
-      if (DUMP) dump_layer<128>(P, R, 13, onerf_mask_word0(13), h);
-      mma_layer<128, 0, 4>(acc, h, sXw, ring);
-      epilogue<128, EPI_HIDDEN_SIGMA>(acc, h, bias_tab + G_O3 * 256, R, 0, Pf + p.L.osigma_w, part);
-      if (DUMP) dump_layer<128>(P, R, 14, onerf_mask_word0(14), h);
-      mma_layer<128, 0, 4>(acc, h, sXw, ring);
-      epilogue<128, EPI_FINAL>(acc, h, bias_tab + G_OFIN * 256, R, 0, nullptr, part);
-      if (DUMP) dump_layer<128>(P, R, 15, -1, h);
-      float accd[32];
-      uint32_t hd[16];
-      mma_layer<64, 0, 4>(accd, h, sXw, ring);
-      epilogue<64, EPI_DIR>(accd, hd, nullptr, R, RC_ODIR, Pf + p.L.orgb_w, part);
-      if (DUMP) dump_layer<64>(P, R, 16, onerf_mask_word0(16), hd);
-      write_heads(p, R, 1, part);
-    }
-    // the next tile's encode overwrites X and the row metadata: both warpgroups' reads of them are done
-    wg_sync(wg);
+    TL_AT(R.tl, 51);
+    TL_AT(R.tl, 52);
   }
 }
 
@@ -351,12 +460,15 @@ int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t 
   P.f = fp;
   int n = 0;
   auto add = [&](int g) { P.layers[n++] = WLayer{L.g[g].img_off, L.g[g].N, L.g[g].K / 32}; };
-  if (fp.want_scene)
-    for (int g = G_S0; g <= G_SDIR; ++g) add(g);
   if (fp.want_object)
     for (int g = G_O0; g <= G_ODIR; ++g) add(g);
+  if (fp.want_scene)
+    for (int g = G_S0; g <= G_SDIR; ++g) add(g);
   P.n_layers = n;
   P.diag = ctx->tc_diag;
+#ifdef ONERF_FIELD_TIMELINE
+  P.tl = g_timeline;
+#endif
   const int64_t total = (int64_t)fp.n_rays * fp.S;
   const int64_t tiles = (total + TM - 1) / TM;
   if (fp.train_ws) {
@@ -366,7 +478,7 @@ int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t 
   const int blocks = (int)(tiles < ctx->num_sms ? tiles : ctx->num_sms);
   const int x_atoms = L.use_voxel ? 6 : 1;
   const size_t smem = 1024 + (size_t)x_atoms * ATOM_BYTES + NSTAGE * STAGE_BYTES + G_COUNT * 256 * 4 + TM * sizeof(RowMeta) +
-                      16 * NSTAGE;
+                      16 * NSTAGE + 16;
   auto launch = [&](auto kernel) -> int {
     ONERF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<blocks, NUM_THREADS, smem, stream>>>(P);
@@ -376,3 +488,8 @@ int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t 
   if (L.use_voxel) return fp.train_ws ? launch(field_tc_kernel<true, true>) : launch(field_tc_kernel<true, false>);
   return fp.train_ws ? launch(field_tc_kernel<false, true>) : launch(field_tc_kernel<false, false>);
 }
+
+#ifdef ONERF_FIELD_TIMELINE
+// device buffer of TL_CTAS * 3 * TL_TILES * TL_SLOTS uint64 stamps that later field launches fill; null = off
+extern "C" void onerf_field_timeline(void* buf) { g_timeline = static_cast<uint64_t*>(buf); }
+#endif

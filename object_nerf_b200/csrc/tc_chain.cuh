@@ -18,7 +18,8 @@ constexpr int NSTAGE = 6;            // weight ring depth
 constexpr int STAGE_BYTES = 16384;   // 32 K-slab rows of N = 256, or 2 / 4 slabs of N = 128 / 64
 constexpr int NUM_WG = 2;
 constexpr int NUM_CONSUMER = NUM_WG * 128;
-constexpr int PRODUCER_WARP = NUM_CONSUMER / 32;   // first warp of the third warpgroup; its other three warps exit
+// first warp of the third warpgroup; its other three warps encode X in the forward (field_tc.cu) and exit in bwd_chain
+constexpr int PRODUCER_WARP = NUM_CONSUMER / 32;
 constexpr int NUM_THREADS = NUM_CONSUMER + 128;
 // Register split: a 64 x 256 fp32 accumulator plus the 256-wide register A operand need more than the 168 registers a
 // 384-thread CTA gets per thread, so the producer warpgroup hands registers to the two consumer warpgroups
@@ -36,6 +37,9 @@ struct Ring {
   uint32_t sB, full, empty;
   uint32_t stage, phase;
   uint32_t* diag;   // timeout record of mbar_wait (onerf_ctx)
+#ifdef ONERF_FIELD_TIMELINE
+  uint64_t full_wait = 0;   // cycles spent waiting on full barriers since the last reset (tools/field_timeline.py)
+#endif
 };
 
 __device__ __forceinline__ void ring_init_bars(uint32_t full, uint32_t empty) {
@@ -86,16 +90,23 @@ __device__ __forceinline__ void ring_release(const Ring& r, uint32_t stage) {
 // first row of the X atoms) and H in registers (hin: 2 NH m64k16 A fragments).  Returns with every MMA complete and
 // every stage of the layer released.  Each stage's MMAs form one commit group; the wait for the previous group leaves
 // this one in flight.  W is the MMA width: N / W m64nWk16 MMAs per k16 step (W = N: one MMA, since a stage image
-// spans all N rows of B with one descriptor).
+// spans all N rows of B with one descriptor).  The first k16 MMA of each output block runs with scale-d = 0 and so
+// starts the sum: acc needs no zeroing.
 template <int N, int NX, int NH, int W = N>
 __device__ __forceinline__ void mma_layer(float (&acc)[N / 2], const uint32_t* hin, uint32_t sXw, Ring& r) {
   constexpr int SPP = 256 / N, NS = NX + NH;
-#pragma unroll
-  for (int i = 0; i < N / 2; ++i) acc[i] = 0.0f;
   uint32_t prev = 0;
 #pragma unroll
   for (int s = 0; s < NS; ++s) {
-    if (s % SPP == 0) mbar_wait(r.full + 8 * r.stage, r.phase, r.diag);
+    if (s % SPP == 0) {
+#ifdef ONERF_FIELD_TIMELINE
+      const uint64_t t0 = clock64();
+#endif
+      mbar_wait(r.full + 8 * r.stage, r.phase, r.diag);
+#ifdef ONERF_FIELD_TIMELINE
+      r.full_wait += clock64() - t0;
+#endif
+    }
     const uint32_t b0 = r.sB + r.stage * STAGE_BYTES + (uint32_t)(s % SPP) * (uint32_t)N * 64u;
     wgmma_fence();
 #pragma unroll
@@ -103,11 +114,13 @@ __device__ __forceinline__ void mma_layer(float (&acc)[N / 2], const uint32_t* h
 #pragma unroll
       for (int nb = 0; nb < N / W; ++nb) {
         const uint64_t bd = desc_k_sw64(b0 + (uint32_t)nb * (uint32_t)W * 64u + (uint32_t)k16 * 32u);
+        const int scale_d = (s == 0 && k16 == 0) ? 0 : 1;
         if (s < NX)
           wgmma_ss<W>(acc + nb * (W / 2),
-                      desc_k_sw128(sXw + (uint32_t)(s >> 1) * ATOM_BYTES + (uint32_t)(s & 1) * 64u + (uint32_t)k16 * 32u), bd);
+                      desc_k_sw128(sXw + (uint32_t)(s >> 1) * ATOM_BYTES + (uint32_t)(s & 1) * 64u + (uint32_t)k16 * 32u), bd,
+                      scale_d);
         else
-          wgmma_rs<W>(acc + nb * (W / 2), hin + ((s - NX) * 2 + k16) * 4, bd);
+          wgmma_rs<W>(acc + nb * (W / 2), hin + ((s - NX) * 2 + k16) * 4, bd, scale_d);
       }
     }
     if (s % SPP == SPP - 1 || s == NS - 1) {

@@ -82,9 +82,6 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 template <int N>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
-// named barrier over the 128 threads of one warpgroup (ids 1 + warpgroup; 0 is __syncthreads)
-__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
-
 // ------------------------------------------------------------------------------------------------
 // wgmma (warpgroup MMA, M = 64 rows per warpgroup, K = 16 per instruction, bf16 x bf16 -> fp32 in registers)
 // ------------------------------------------------------------------------------------------------
@@ -127,61 +124,62 @@ __device__ __forceinline__ void fence_regs(float* d) {
   "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127" "}"
 
 // D[64 x 64] += A[64 x 16] (registers: the m64k16 A fragment, bf16 pairs) . B (shared memory, K-major)
-__device__ __forceinline__ void wgmma_rs_n64(float* d, const uint32_t* a, uint64_t desc_b) {
+__device__ __forceinline__ void wgmma_rs_n64(float* d, const uint32_t* a, uint64_t desc_b, int scale_d = 1) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ONERF_WG_D32 ", {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
       : ONERF_WG_OUT32(d)
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
 }
 // D[64 x 64] += A (shared memory) . B (shared memory); TA / TB: operand is MN-major (transposed)
 template <int TA, int TB>
-__device__ __forceinline__ void wgmma_ss_n64(float* d, uint64_t desc_a, uint64_t desc_b) {
+__device__ __forceinline__ void wgmma_ss_n64(float* d, uint64_t desc_a, uint64_t desc_b, int scale_d = 1) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ONERF_WG_D32 ", %32, %33, p, 1, 1, %35, %36;\n\t}"
       : ONERF_WG_OUT32(d)
-      : "l"(desc_a), "l"(desc_b), "r"(1), "n"(TA), "n"(TB));
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
 // Full-width shapes of the layer chain (tc_chain.cuh): D[64 x N] += A . B, N = 64, 128 or 256, both operands K-major,
-// A from registers (rs) or shared memory (ss).  One instruction covers all N columns of a k16 step.
+// A from registers (rs) or shared memory (ss).  One instruction covers all N columns of a k16 step.  scale_d = 0 makes
+// the MMA write D = A . B without reading the accumulator (the first MMA of a sum).
 template <int N>
-__device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t desc_b) {
+__device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t desc_b, int scale_d = 1) {
   if constexpr (N == 64) {
-    wgmma_rs_n64(d, a, desc_b);
+    wgmma_rs_n64(d, a, desc_b, scale_d);
   } else if constexpr (N == 128) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " ONERF_WG_D64 ", {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
         : ONERF_WG_OUT64(d)
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
   } else {
     static_assert(N == 256, "wgmma_rs: N is 64, 128 or 256");
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " ONERF_WG_D128 ", {%128, %129, %130, %131}, %132, p, 1, 1, 0;\n\t}"
         : ONERF_WG_OUT128(d)
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
   }
 }
 template <int N>
-__device__ __forceinline__ void wgmma_ss(float* d, uint64_t desc_a, uint64_t desc_b) {
+__device__ __forceinline__ void wgmma_ss(float* d, uint64_t desc_a, uint64_t desc_b, int scale_d = 1) {
   if constexpr (N == 64) {
-    wgmma_ss_n64<0, 0>(d, desc_a, desc_b);
+    wgmma_ss_n64<0, 0>(d, desc_a, desc_b, scale_d);
   } else if constexpr (N == 128) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " ONERF_WG_D64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
         : ONERF_WG_OUT64(d)
-        : "l"(desc_a), "l"(desc_b), "r"(1));
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));
   } else {
     static_assert(N == 256, "wgmma_ss: N is 64, 128 or 256");
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " ONERF_WG_D128 ", %128, %129, p, 1, 1, 0, 0;\n\t}"
         : ONERF_WG_OUT128(d)
-        : "l"(desc_a), "l"(desc_b), "r"(1));
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));
   }
 }
 
