@@ -34,6 +34,8 @@ EXPORTS = [
     "onerf_unpack_grads", "onerf_bwd_chain", "onerf_bwd_wgrad", "onerf_bwd_colsums", "onerf_bwd_raysums", "onerf_bwd_dx",
     "onerf_code_gather", "onerf_code_scatter_add", "onerf_render_multi_workspace_bytes", "onerf_render_multi_fwd",
 ]
+# additions to ABI version 2 declared in include/onerf_ext.h
+EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_ws", "onerf_composite_multi_merge"]
 
 _p = C.c_void_p
 
@@ -204,6 +206,10 @@ def load() -> C.CDLL:
         lib.onerf_render_multi_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
         lib.onerf_render_multi_workspace_bytes.restype = C.c_size_t
         lib.onerf_render_multi_fwd.argtypes = [_p, C.POINTER(RenderMultiArgs), _p]
+        lib.onerf_composite_multi_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+        lib.onerf_composite_multi_workspace_bytes.restype = C.c_size_t
+        for name in ("onerf_composite_multi_ws", "onerf_composite_multi_merge"):
+            getattr(lib, name).argtypes = lib.onerf_composite_multi.argtypes[:-1] + [_p, C.c_size_t, _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

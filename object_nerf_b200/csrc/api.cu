@@ -4,6 +4,7 @@
 
 #include "field_common.cuh"
 #include "train_ws.h"
+#include "../../include/onerf_ext.h"
 
 static thread_local char g_err[512] = "";
 
@@ -59,7 +60,8 @@ extern "C" int onerf_ctx_destroy(onerf_ctx* ctx) {
 
 extern "C" int64_t onerf_ctx_launch_count(const onerf_ctx* ctx) { return ctx ? ctx->launches : 0; }
 
-extern "C" int onerf_field_fwd(onerf_ctx* ctx, const onerf_field_args* a, void* stream_) {
+// n_live: optional device-side count of the rays to evaluate (field_common.cuh: FieldParams::n_live)
+static int field_fwd(onerf_ctx* ctx, const onerf_field_args* a, const int* n_live, void* stream_) {
   ONERF_CHECK_ARG(ctx && a, "null argument");
   ONERF_CHECK_ARG(a->rays && a->z && a->packed && a->ray_const, "null buffer");
   ONERF_CHECK_ARG(a->n_rays >= 0 && a->n_samples >= 1, "bad shape");
@@ -90,6 +92,7 @@ extern "C" int onerf_field_fwd(onerf_ctx* ctx, const onerf_field_args* a, void* 
   p.boxes = a->boxes; p.n_boxes = a->n_boxes;
   p.scene_out = a->scene_out; p.obj_out = a->obj_out; p.out_stride = a->out_stride;
   p.ray_const = a->ray_const;
+  p.n_live = n_live;
   if (a->activations) {
     ONERF_UNSUPPORTED(a->precision != ONERF_PREC_FP32, "activation dump is built for ONERF_PREC_FP32 only");
     ONERF_UNSUPPORTED(a->z_stride != a->n_samples || a->out_stride != a->n_samples, "activation dump needs dense z / outputs");
@@ -112,6 +115,10 @@ extern "C" int onerf_field_fwd(onerf_ctx* ctx, const onerf_field_args* a, void* 
   if (a->precision == ONERF_PREC_BF16) return onerf_launch_field_bf16(ctx, p, stream);
   onerf_set_error("onerf_field_fwd: unknown precision %d", a->precision);
   return ONERF_ERR_BAD_ARG;
+}
+
+extern "C" int onerf_field_fwd(onerf_ctx* ctx, const onerf_field_args* a, void* stream) {
+  return field_fwd(ctx, a, nullptr, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -216,40 +223,83 @@ extern "C" int onerf_render_rays_fwd(onerf_ctx* ctx, const onerf_render_args* a,
 // render_rays_multi() forward as one call (render_tools/multi_rendering.py:160-325): per ray set coarse depths and a
 // one-branch field evaluation (scene branch + removed-object boxes for id 0, object branch with the id's code row
 // otherwise, zero-length rays muted), joint stable depth sort + compositing, per-set importance resampling, fine pass.
-// Same kernels, order and arguments as object_nerf_b200/multi_rendering.py::render_rays_multi (staged route).
+// Same kernels, order and arguments as object_nerf_b200/multi_rendering.py::render_rays_multi (staged route), except that
+// object sets evaluate only the rays that hit their box (multi_fields); the outputs are bit-identical.
 // ------------------------------------------------------------------------------------------------
+struct MultiWs {
+  float *ray_const, *z_all, *z_fine, *field_all, *w_unsorted;
+  int *live, *slot, *count;                // box culling of one object set (reused set after set)
+  float *rays_c, *z_c, *field_c;
+  void* sort;                              // onerf_composite_multi_ws scratch
+  size_t sort_bytes;
+  size_t total;
+};
+
+static MultiWs multi_ws_layout(char* base, int n_rays, int n_obj, int n_samples, int n_importance) {
+  const size_t sf = (size_t)n_samples + (size_t)n_importance, no = (size_t)n_obj, n = (size_t)n_rays;
+  MultiWs w;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { void* p = base + off; off += align256(bytes); return p; };
+  w.ray_const = (float*)take(n * ONERF_RAY_CONST_FLOATS * sizeof(float));   // per-ray hoisted terms (one set at a time)
+  w.z_all = (float*)take(no * n * n_samples * sizeof(float));               // coarse depths of every set
+  w.z_fine = (float*)take(no * n * sf * sizeof(float));                     // fine depths
+  w.field_all = (float*)take(no * n * sf * 4 * sizeof(float));              // fields (rgb, sigma) of every set
+  w.w_unsorted = (float*)take(no * n * n_samples * sizeof(float));          // per-set coarse weights in sample order
+  w.live = (int*)take(n * sizeof(int));
+  w.slot = (int*)take(n * sizeof(int));
+  w.count = (int*)take(sizeof(int));
+  w.rays_c = (float*)take(n * 8 * sizeof(float));
+  w.z_c = (float*)take(n * sf * sizeof(float));
+  w.field_c = (float*)take(n * sf * 4 * sizeof(float));
+  w.sort_bytes = onerf_composite_multi_workspace_bytes(n_rays, n_obj, (int)sf);
+  w.sort = take(w.sort_bytes);
+  w.total = off;
+  return w;
+}
+
 extern "C" size_t onerf_render_multi_workspace_bytes(int n_rays, int n_obj, int n_samples, int n_importance) {
   if (n_rays < 0 || n_obj < 1 || n_samples < 1 || n_importance < 0) return 0;
-  const size_t sf = (size_t)n_samples + (size_t)n_importance, no = (size_t)n_obj, n = (size_t)n_rays;
-  return align256(n * ONERF_RAY_CONST_FLOATS * sizeof(float)) +          // per-ray hoisted terms (one set at a time)
-         align256(no * n * n_samples * sizeof(float)) +                  // coarse depths of every set
-         align256(no * n * sf * sizeof(float)) +                         // fine depths
-         align256(no * n * sf * 4 * sizeof(float)) +                     // fields (rgb, sigma) of every set
-         align256(no * n * n_samples * sizeof(float));                   // per-set coarse weights in sample order
+  return multi_ws_layout(nullptr, n_rays, n_obj, n_samples, n_importance).total;
 }
 
 static int multi_fields(onerf_ctx* ctx, const onerf_render_multi_args* a, const void* packed, const float* z_all, int S,
-                        float* field_all, float* ray_const, void* stream) {
+                        const MultiWs& w, void* stream) {
+  const int N = a->n_rays;
   for (int i = 0; i < a->n_obj; ++i) {
     const int id = a->obj_ids_host[i];
+    const float* z = z_all + (size_t)i * N * S;
+    float* out = w.field_all + (size_t)i * N * S * 4;
     onerf_field_args f;
     memset(&f, 0, sizeof(f));
     f.rays = a->rays_list_host[i];
-    f.z = z_all + (size_t)i * a->n_rays * S;
+    f.z = z;
     f.z_stride = S;
     f.code_row = id > 0 ? a->code_table + (size_t)id * ONERF_NCODE : nullptr;
-    f.n_rays = a->n_rays; f.n_samples = S;
+    f.n_rays = N; f.n_samples = S;
     f.grid = a->grid; f.packed = packed;
     f.want_scene = id > 0 ? 0 : 1; f.want_object = id > 0 ? 1 : 0;
     f.precision = a->precision;
     f.mute_zero_rays = 1;
     if (id == 0) { f.boxes = a->boxes; f.n_boxes = a->n_boxes; }
-    float* out = field_all + (size_t)i * a->n_rays * S * 4;
     f.scene_out = id > 0 ? nullptr : out;
-    f.obj_out = id > 0 ? out : nullptr;
+    f.obj_out = id > 0 ? w.field_c : nullptr;
     f.out_stride = S;
-    f.ray_const = ray_const;
-    int rc = onerf_field_fwd(ctx, &f, stream);
+    f.ray_const = w.ray_const;
+    int rc;
+    if (id == 0) {   // the scene set is evaluated on every ray
+      f.scene_out = out;
+      rc = field_fwd(ctx, &f, nullptr, stream);
+      if (rc != ONERF_OK) return rc;
+      continue;
+    }
+    // object set: only the rays that hit the box (the others would be muted), then scatter back with the muted value
+    rc = onerf_cull_rays(ctx, f.rays, z, N, S, w.live, w.slot, w.count, w.rays_c, w.z_c, (cudaStream_t)stream);
+    if (rc != ONERF_OK) return rc;
+    f.rays = w.rays_c;
+    f.z = w.z_c;
+    rc = field_fwd(ctx, &f, w.count, stream);
+    if (rc != ONERF_OK) return rc;
+    rc = onerf_uncull_field(ctx, w.field_c, w.slot, N, S, out, (cudaStream_t)stream);
     if (rc != ONERF_OK) return rc;
   }
   return ONERF_OK;
@@ -259,7 +309,8 @@ extern "C" int onerf_render_multi_fwd(onerf_ctx* ctx, const onerf_render_multi_a
   ONERF_CHECK_ARG(ctx && a, "null argument");
   ONERF_CHECK_ARG(a->rays_list_host && a->obj_ids_host && a->packed_coarse && a->grid && a->code_table, "null input");
   ONERF_CHECK_ARG(a->n_rays >= 0 && a->n_obj >= 1 && a->n_samples >= 2 && a->n_importance >= 0, "bad shape");
-  ONERF_UNSUPPORTED((size_t)a->n_obj * (a->n_samples + a->n_importance) > 4096, "n_obj * samples > 4096");
+  ONERF_UNSUPPORTED((int64_t)a->n_obj * (a->n_samples + a->n_importance) > INT32_MAX, "n_obj * samples >= 2^31");
+  ONERF_UNSUPPORTED(a->n_samples + a->n_importance > 2048, "more than 2048 samples per ray set");
   ONERF_CHECK_ARG(a->n_importance == 0 || a->packed_fine, "n_importance > 0 needs packed_fine");
   ONERF_CHECK_ARG(a->n_boxes == 0 || a->boxes, "n_boxes > 0 with null boxes");
   for (int i = 0; i < a->n_obj; ++i) {
@@ -278,31 +329,26 @@ extern "C" int onerf_render_multi_fwd(onerf_ctx* ctx, const onerf_render_multi_a
   }
   if (a->n_rays == 0) return ONERF_OK;
   const int S = a->n_samples, SF = a->n_samples + a->n_importance, N = a->n_rays, NO = a->n_obj;
-  char* ws = reinterpret_cast<char*>(a->workspace);
-  auto take = [&](size_t bytes) { float* p = reinterpret_cast<float*>(ws); ws += align256(bytes); return p; };
-  float* ray_const = take((size_t)N * ONERF_RAY_CONST_FLOATS * sizeof(float));
-  float* z_all = take((size_t)NO * N * S * sizeof(float));
-  float* z_fine = take((size_t)NO * N * SF * sizeof(float));
-  float* field_all = take((size_t)NO * N * SF * 4 * sizeof(float));
-  float* w_unsorted = take((size_t)NO * N * S * sizeof(float));
+  const MultiWs w = multi_ws_layout(reinterpret_cast<char*>(a->workspace), N, NO, S, a->n_importance);
   int rc;
   for (int i = 0; i < NO; ++i) {   // multi_rendering.py:196-213: coarse depths are never jittered on this path
-    rc = onerf_sample_coarse(ctx, a->rays_list_host[i], N, S, a->use_disp, 0.0f, nullptr, 0, z_all + (size_t)i * N * S, stream);
+    rc = onerf_sample_coarse(ctx, a->rays_list_host[i], N, S, a->use_disp, 0.0f, nullptr, 0, w.z_all + (size_t)i * N * S, stream);
     if (rc != ONERF_OK) return rc;
   }
-  rc = multi_fields(ctx, a, a->packed_coarse, z_all, S, field_all, ray_const, stream);
+  rc = multi_fields(ctx, a, a->packed_coarse, w.z_all, S, w, stream);
   if (rc != ONERF_OK) return rc;
-  rc = onerf_composite_multi(ctx, z_all, field_all, N, NO, S, a->white_back, c.z_vals, c.weights, c.obj_ids,
-                             a->n_importance > 0 ? w_unsorted : nullptr, c.opacity, c.rgb, c.depth, stream);
+  rc = onerf_composite_multi_ws(ctx, w.z_all, w.field_all, N, NO, S, a->white_back, c.z_vals, c.weights, c.obj_ids,
+                                a->n_importance > 0 ? w.w_unsorted : nullptr, c.opacity, c.rgb, c.depth, w.sort, w.sort_bytes,
+                                stream);
   if (rc != ONERF_OK || a->n_importance == 0) return rc;
   const int det = a->perturb == 0.0f ? 1 : 0;
   for (int i = 0; i < NO; ++i) {
-    rc = onerf_sample_pdf_merge(ctx, z_all + (size_t)i * N * S, w_unsorted + (size_t)i * N * S, N, S, a->n_importance, det, nullptr,
-                                det ? 0 : a->seed + (uint64_t)i, z_fine + (size_t)i * N * SF, stream);
+    rc = onerf_sample_pdf_merge(ctx, w.z_all + (size_t)i * N * S, w.w_unsorted + (size_t)i * N * S, N, S, a->n_importance, det,
+                                nullptr, det ? 0 : a->seed + (uint64_t)i, w.z_fine + (size_t)i * N * SF, stream);
     if (rc != ONERF_OK) return rc;
   }
-  rc = multi_fields(ctx, a, a->packed_fine, z_fine, SF, field_all, ray_const, stream);
+  rc = multi_fields(ctx, a, a->packed_fine, w.z_fine, SF, w, stream);
   if (rc != ONERF_OK) return rc;
-  return onerf_composite_multi(ctx, z_fine, field_all, N, NO, SF, a->white_back, a->fine.z_vals, a->fine.weights, nullptr, nullptr,
-                               a->fine.opacity, a->fine.rgb, a->fine.depth, stream);
+  return onerf_composite_multi_ws(ctx, w.z_fine, w.field_all, N, NO, SF, a->white_back, a->fine.z_vals, a->fine.weights, nullptr,
+                                  nullptr, a->fine.opacity, a->fine.rgb, a->fine.depth, w.sort, w.sort_bytes, stream);
 }

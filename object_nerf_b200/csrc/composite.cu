@@ -3,7 +3,10 @@
 // float4 access), multiplicative warp scan for the exclusive transmittance product.
 //
 // Reference behaviour: models/rendering.py:139-229; render_tools/multi_rendering.py:96-157.
+#include <algorithm>
+
 #include "common.cuh"
+#include "../../include/onerf_ext.h"
 
 namespace {
 
@@ -213,6 +216,163 @@ composite_multi_kernel(const float* __restrict__ z_all, const float4* __restrict
 #undef SRC_OFF
 }
 
+// ---------------------------------------------------------------------------------------------
+// multi-object, any T: per-set sort, rank by binary search, composite in rank order.  Gives the same order as the
+// bitonic kernel (a stable sort of the concatenation by float_order_key) without holding T keys in shared memory.
+// Scratch (caller workspace), ray-major: skey[r][obj][p] = p-th smallest key of set obj of ray r, sidx[r][obj][p] = its
+// sample index in the set.  The rank kernel leaves the concatenated index of sorted position i in weights[r][i] (as
+// bits) and its depth in z_sorted[r][i]; the composite kernel reads both and overwrites weights[r][i] with the weight.
+// ---------------------------------------------------------------------------------------------
+constexpr int kMergeMaxS = 2048;   // per-set list sorted in shared memory; sidx is 16-bit
+
+// One warp per (ray, set).  A set that is already ascending in key order (the usual case: unjittered coarse depths with
+// near <= far, merged fine depths, all-zero muted rays) is copied; any other set is bitonic-sorted by (key, s).
+__global__ void __launch_bounds__(128)
+merge_sort_sets_kernel(const float* __restrict__ z_all, int n_rays, int n_obj, int S, int P,
+                       uint32_t* __restrict__ skey, uint16_t* __restrict__ sidx) {
+  extern __shared__ unsigned long long keys_all[];
+  const int warps_per_block = blockDim.x >> 5;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  unsigned long long* keys = keys_all + (size_t)warp * P;
+  const int64_t n_lists = (int64_t)n_rays * n_obj;
+  for (int64_t l = (int64_t)blockIdx.x * warps_per_block + warp; l < n_lists; l += (int64_t)gridDim.x * warps_per_block) {
+    const int r = (int)(l / n_obj), obj = (int)(l % n_obj);
+    const float* z = z_all + ((int64_t)obj * n_rays + r) * S;
+    uint32_t* ko = skey + l * S;
+    uint16_t* io = sidx + l * S;
+    bool ascending = true;
+    for (int s = lane; s + 1 < S; s += 32)
+      ascending = ascending && (float_order_key(__ldg(z + s)) <= float_order_key(__ldg(z + s + 1)));
+    if (__all_sync(0xffffffffu, ascending)) {
+      for (int s = lane; s < S; s += 32) {
+        ko[s] = float_order_key(__ldg(z + s));
+        io[s] = (uint16_t)s;
+      }
+      continue;
+    }
+    for (int i = lane; i < P; i += 32)
+      keys[i] = (i < S) ? (((unsigned long long)float_order_key(__ldg(z + i)) << 32) | (unsigned)i) : 0xffffffffffffffffull;
+    __syncwarp();
+    for (int k2 = 2; k2 <= P; k2 <<= 1) {
+      for (int j = k2 >> 1; j > 0; j >>= 1) {
+        for (int t = lane; t < (P >> 1); t += 32) {
+          const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
+          const int m = i | j;
+          const bool up = ((i & k2) == 0);
+          const unsigned long long a = keys[i], b = keys[m];
+          if ((a > b) == up) { keys[i] = b; keys[m] = a; }
+        }
+        __syncwarp();
+      }
+    }
+    for (int s = lane; s < S; s += 32) {
+      ko[s] = (uint32_t)(keys[s] >> 32);
+      io[s] = (uint16_t)(keys[s] & 0xffffu);
+    }
+    __syncwarp();
+  }
+}
+
+// number of entries of the ascending list k[0, n) that are < key (strict) or <= key
+__device__ __forceinline__ int count_below(const uint32_t* __restrict__ k, int n, uint32_t key, bool strict) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    const uint32_t v = __ldg(k + mid);
+    if (strict ? (v < key) : (v <= key)) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// One warp per (ray, set).  Sample p of sorted set obj goes to rank p + #(keys <= its key in sets before obj) +
+// #(keys < its key in sets after obj): ties resolve in concatenated-index order, as the stable sort does.
+__global__ void __launch_bounds__(128)
+merge_rank_kernel(const float* __restrict__ z_all, int n_rays, int n_obj, int S, const uint32_t* __restrict__ skey,
+                  const uint16_t* __restrict__ sidx, float* __restrict__ z_sorted, float* __restrict__ order) {
+  const int warps_per_block = blockDim.x >> 5;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t n_lists = (int64_t)n_rays * n_obj;
+  const int64_t T = (int64_t)n_obj * S;
+  for (int64_t l = (int64_t)blockIdx.x * warps_per_block + warp; l < n_lists; l += (int64_t)gridDim.x * warps_per_block) {
+    const int r = (int)(l / n_obj), obj = (int)(l % n_obj);
+    const uint32_t* kr = skey + (int64_t)r * T;
+    for (int p = lane; p < S; p += 32) {
+      const uint32_t key = __ldg(kr + (int64_t)obj * S + p);
+      const int s = __ldg(sidx + l * S + p);
+      int rank = p;
+      for (int q = 0; q < n_obj; ++q)
+        if (q != obj) rank += count_below(kr + (int64_t)q * S, S, key, q > obj);
+      const int64_t o = (int64_t)r * T + rank;
+      z_sorted[o] = __ldg(z_all + ((int64_t)obj * n_rays + r) * S + s);
+      order[o] = __uint_as_float((uint32_t)(obj * S + s));
+    }
+  }
+}
+
+// One warp per ray: composite_multi_kernel's compositing loop (same arithmetic, same 32-wide scan blocks) over the
+// order the rank kernel left in weights[] / z_sorted[].
+__global__ void __launch_bounds__(128)
+merge_composite_kernel(const float4* __restrict__ field_all, int n_rays, int n_obj, int S,
+                       int white_back, const float* __restrict__ z_sorted, float* __restrict__ weights,
+                       float* __restrict__ obj_ids, float* __restrict__ weights_unsorted, float* __restrict__ opacity,
+                       float* __restrict__ rgb, float* __restrict__ depth) {
+  const int warps_per_block = blockDim.x >> 5;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int T = n_obj * S;
+  for (int r = blockIdx.x * warps_per_block + warp; r < n_rays; r += gridDim.x * warps_per_block) {
+    const int64_t obj_stride = (int64_t)n_rays * S;
+    const float4* fld = field_all + (int64_t)r * S;
+    const float* zs = z_sorted + (int64_t)r * T;
+    float* wr = weights + (int64_t)r * T;
+#define SRC_OFF(c) ((int64_t)((c) / S) * obj_stride + ((c) % S))
+    Acc acc = {0.f, 0.f, 0.f, 0.f, 0.f};
+    float carry = 1.0f;
+    for (int base = 0; base < T; base += 32) {
+      const int i = base + lane;
+      float alpha = 0.0f, zi = 0.0f;
+      float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
+      int src = 0;
+      if (i < T) {
+        src = (int)__float_as_uint(wr[i]);
+        zi = zs[i];
+        const float zn = (i + 1 < T) ? zs[i + 1] : zi;
+        const float delta = (i + 1 < T) ? __fsub_rn(zn, zi) : 0.0f;  // multi_rendering.py:125-128
+        f = __ldg(fld + SRC_OFF(src));
+        alpha = alpha_from(f.w, delta);
+      }
+      const float t = (i < T) ? __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f) : 1.0f;
+      const float incl = warp_scan_mul(t, lane);
+      float excl = __shfl_up_sync(0xffffffffu, incl, 1);
+      if (lane == 0) excl = 1.0f;
+      const float w = alpha * (carry * excl);
+      carry *= __shfl_sync(0xffffffffu, incl, 31);
+      if (i < T) {
+        wr[i] = w;
+        if (obj_ids) obj_ids[(int64_t)r * T + i] = (float)(src / S);
+        if (weights_unsorted) weights_unsorted[(int64_t)r * S + SRC_OFF(src)] = w;
+        acc.opacity += w;
+        acc.r += w * f.x;
+        acc.g += w * f.y;
+        acc.b += w * f.z;
+        acc.depth += w * zi;
+      }
+    }
+    acc.opacity = warp_sum(acc.opacity);
+    acc.r = warp_sum(acc.r);
+    acc.g = warp_sum(acc.g);
+    acc.b = warp_sum(acc.b);
+    acc.depth = warp_sum(acc.depth);
+    if (lane == 0) {
+      opacity[r] = acc.opacity;
+      depth[r] = acc.depth;
+      rgb[r * 3 + 0] = white_back ? __fadd_rn(__fadd_rn(acc.r, 1.0f), -acc.opacity) : acc.r;
+      rgb[r * 3 + 1] = white_back ? __fadd_rn(__fadd_rn(acc.g, 1.0f), -acc.opacity) : acc.g;
+      rgb[r * 3 + 2] = white_back ? __fadd_rn(__fadd_rn(acc.b, 1.0f), -acc.opacity) : acc.b;
+    }
+#undef SRC_OFF
+  }
+}
+
 }  // namespace
 
 extern "C" int onerf_composite(onerf_ctx* ctx, const onerf_composite_args* a, void* stream) {
@@ -231,27 +391,105 @@ extern "C" int onerf_composite(onerf_ctx* ctx, const onerf_composite_args* a, vo
   return ONERF_OK;
 }
 
+// workspace of the rank-merge path: sorted keys (uint32) and in-set indices (uint16) of every sample
+static size_t merge_ws_bytes(int64_t n_rays, int64_t T) { return ((n_rays * T * 4 + 255) & ~(int64_t)255) + n_rays * T * 2; }
+
+extern "C" size_t onerf_composite_multi_workspace_bytes(int n_rays, int n_obj, int n_samples) {
+  if (n_rays < 0 || n_obj < 1 || n_samples < 1) return 0;
+  return merge_ws_bytes(n_rays, (int64_t)n_obj * n_samples);
+}
+
+// path: 0 = bitonic kernel (T <= 4096, no workspace), 1 = rank merge (any T up to the int32 / per-set bounds)
+static int composite_multi_run(onerf_ctx* ctx, int path, const float* z_all, const float* field_all, int n_rays, int n_obj,
+                               int n_samples, int white_back, float* z_sorted, float* weights, float* obj_ids,
+                               float* weights_unsorted, float* opacity, float* rgb, float* depth, void* workspace,
+                               size_t workspace_bytes, cudaStream_t stream) {
+  const int T = n_obj * n_samples;
+  if (n_rays == 0) return ONERF_OK;
+  const int warps = 4;
+  if (path == 0) {
+    int P = 2;
+    while (P < T) P <<= 1;
+    const size_t smem = (size_t)warps * P * sizeof(unsigned long long);
+    ONERF_CUDA(cudaFuncSetAttribute(composite_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int blocks = (n_rays + warps - 1) / warps;
+    const int cap = ctx->num_sms * 8;
+    if (blocks > cap) blocks = cap;
+    composite_multi_kernel<<<blocks, warps * 32, smem, stream>>>(
+        z_all, reinterpret_cast<const float4*>(field_all), n_rays, n_obj, n_samples, P, white_back, z_sorted,
+        weights, obj_ids, weights_unsorted, opacity, rgb, depth);
+    ONERF_LAUNCH_CHECK(ctx);
+    return ONERF_OK;
+  }
+  uint32_t* skey = static_cast<uint32_t*>(workspace);
+  uint16_t* sidx = reinterpret_cast<uint16_t*>(static_cast<char*>(workspace) + (((int64_t)n_rays * T * 4 + 255) & ~(int64_t)255));
+  int P = 2;
+  while (P < n_samples) P <<= 1;
+  const size_t smem = (size_t)warps * P * sizeof(unsigned long long);
+  ONERF_CUDA(cudaFuncSetAttribute(merge_sort_sets_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int64_t lists = (int64_t)n_rays * n_obj;
+  const int64_t cap = (int64_t)ctx->num_sms * 16;
+  const int list_blocks = (int)std::min((lists + warps - 1) / warps, cap);
+  merge_sort_sets_kernel<<<list_blocks, warps * 32, smem, stream>>>(z_all, n_rays, n_obj, n_samples, P, skey, sidx);
+  ONERF_LAUNCH_CHECK(ctx);
+  merge_rank_kernel<<<list_blocks, warps * 32, 0, stream>>>(z_all, n_rays, n_obj, n_samples, skey, sidx, z_sorted, weights);
+  ONERF_LAUNCH_CHECK(ctx);
+  const int ray_blocks = (int)std::min<int64_t>((n_rays + warps - 1) / warps, (int64_t)ctx->num_sms * 8);
+  merge_composite_kernel<<<ray_blocks, warps * 32, 0, stream>>>(
+      reinterpret_cast<const float4*>(field_all), n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
+      weights_unsorted, opacity, rgb, depth);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
+#define MULTI_ARGS_OK()                                                                                                 \
+  ONERF_CHECK_ARG(ctx && z_all && field_all && z_sorted && weights && opacity && rgb && depth, "null argument");        \
+  ONERF_CHECK_ARG(n_rays >= 0 && n_obj >= 1 && n_samples >= 1, "bad shape");                                            \
+  ONERF_CHECK_ARG(onerf_aligned16(field_all), "field buffer must be 16-byte aligned")
+
 extern "C" int onerf_composite_multi(onerf_ctx* ctx, const float* z_all, const float* field_all, int n_rays,
                                      int n_obj, int n_samples, int white_back, float* z_sorted,
                                      float* weights, float* obj_ids, float* weights_unsorted, float* opacity,
                                      float* rgb, float* depth, void* stream) {
-  ONERF_CHECK_ARG(ctx && z_all && field_all && z_sorted && weights && opacity && rgb && depth, "null argument");
-  ONERF_CHECK_ARG(n_rays >= 0 && n_obj >= 1 && n_samples >= 1, "bad shape");
-  ONERF_CHECK_ARG(onerf_aligned16(field_all), "field buffer must be 16-byte aligned");
-  const int T = n_obj * n_samples;
-  ONERF_UNSUPPORTED(T > 4096, "n_obj * n_samples > 4096");
-  if (n_rays == 0) return ONERF_OK;
-  int P = 2;
-  while (P < T) P <<= 1;
-  const int warps = 4;
-  const size_t smem = (size_t)warps * P * sizeof(unsigned long long);
-  ONERF_CUDA(cudaFuncSetAttribute(composite_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int blocks = (n_rays + warps - 1) / warps;
-  const int cap = ctx->num_sms * 8;
-  if (blocks > cap) blocks = cap;
-  composite_multi_kernel<<<blocks, warps * 32, smem, (cudaStream_t)stream>>>(
-      z_all, reinterpret_cast<const float4*>(field_all), n_rays, n_obj, n_samples, P, white_back, z_sorted,
-      weights, obj_ids, weights_unsorted, opacity, rgb, depth);
-  ONERF_LAUNCH_CHECK(ctx);
-  return ONERF_OK;
+  MULTI_ARGS_OK();
+  ONERF_UNSUPPORTED((int64_t)n_obj * n_samples > 4096, "n_obj * n_samples > 4096 (onerf_composite_multi_ws has no such limit)");
+  return composite_multi_run(ctx, 0, z_all, field_all, n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
+                             weights_unsorted, opacity, rgb, depth, nullptr, 0, (cudaStream_t)stream);
+}
+
+static int composite_multi_ws(onerf_ctx* ctx, int force_merge, const float* z_all, const float* field_all, int n_rays,
+                              int n_obj, int n_samples, int white_back, float* z_sorted, float* weights, float* obj_ids,
+                              float* weights_unsorted, float* opacity, float* rgb, float* depth, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+  MULTI_ARGS_OK();
+  const int64_t T = (int64_t)n_obj * n_samples;
+  const int path = (force_merge || T > 4096) ? 1 : 0;
+  if (path == 1) {
+    ONERF_UNSUPPORTED(T > INT32_MAX, "n_obj * n_samples >= 2^31");
+    ONERF_UNSUPPORTED(n_samples > kMergeMaxS, "more than 2048 samples per ray set");
+    const size_t need = onerf_composite_multi_workspace_bytes(n_rays, n_obj, n_samples);
+    ONERF_CHECK_ARG(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
+    if (workspace_bytes < need) {
+      onerf_set_error("%s: workspace too small (%zu < %zu)", __func__, workspace_bytes, need);
+      return ONERF_ERR_WORKSPACE;
+    }
+  }
+  return composite_multi_run(ctx, path, z_all, field_all, n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
+                             weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int onerf_composite_multi_ws(onerf_ctx* ctx, const float* z_all, const float* field_all, int n_rays, int n_obj,
+                                        int n_samples, int white_back, float* z_sorted, float* weights, float* obj_ids,
+                                        float* weights_unsorted, float* opacity, float* rgb, float* depth, void* workspace,
+                                        size_t workspace_bytes, void* stream) {
+  return composite_multi_ws(ctx, 0, z_all, field_all, n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
+                            weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, stream);
+}
+
+extern "C" int onerf_composite_multi_merge(onerf_ctx* ctx, const float* z_all, const float* field_all, int n_rays, int n_obj,
+                                           int n_samples, int white_back, float* z_sorted, float* weights, float* obj_ids,
+                                           float* weights_unsorted, float* opacity, float* rgb, float* depth, void* workspace,
+                                           size_t workspace_bytes, void* stream) {
+  return composite_multi_ws(ctx, 1, z_all, field_all, n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
+                            weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, stream);
 }

@@ -31,7 +31,15 @@ struct FieldParams {
   // training forward of the tensor-core kernel: bf16 activation atoms, X atoms and LeakyReLU sign masks of every tile
   // go to this workspace (layout.h: onerf_make_train_layout(use_voxel, n_rays * S)); null = inference
   void* train_ws;
+  // optional device-side ray count (<= n_rays): only rays [0, *n_live) are evaluated.  Set by the editing path for object
+  // ray sets compacted on the device to the rays that hit the object's box (api.cu: multi_fields).
+  const int* n_live;
 };
+
+// rays a field launch evaluates: n_rays, or the device-side count when there is one (read once at kernel start)
+__device__ __forceinline__ int field_rays(const FieldParams& p) {
+  return p.n_live ? min(*p.n_live, p.n_rays) : p.n_rays;
+}
 
 // removed-object mask: inside any box <=> lo <= A p + t <= hi (inclusive), utils/bbox_utils.py:158-207
 __device__ __forceinline__ bool point_in_boxes(const float* __restrict__ boxes, int n_boxes, float x, float y, float z) {
@@ -56,3 +64,11 @@ __device__ __forceinline__ bool point_in_boxes(const float* __restrict__ boxes, 
 int onerf_launch_ray_const(onerf_ctx* ctx, const FieldParams& p, cudaStream_t stream);
 int onerf_launch_field_fp32(onerf_ctx* ctx, const FieldParams& p, cudaStream_t stream);
 int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& p, cudaStream_t stream);
+
+// box culling of an (N,8) ray set with depths z (N,S) (cull.cu): live[0, *count) = rays whose last depth is not 0, in ray
+// order, slot[r] = position of ray r in that list or -1; rays_c / z_c = the listed rays' rows.  uncull writes the field
+// rows of the listed rays from field_c (count,S,4) to out (N,S,4) and (0, 0, 0, -1e5) to the others.
+int onerf_cull_rays(onerf_ctx* ctx, const float* rays, const float* z, int n_rays, int S, int* live, int* slot, int* count,
+                    float* rays_c, float* z_c, cudaStream_t stream);
+int onerf_uncull_field(onerf_ctx* ctx, const float* field_c, const int* slot, int n_rays, int S, float* out,
+                       cudaStream_t stream);

@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(256) field_fp32_kernel(FieldParams p) {
   __shared__ int s_ray[TS];
   __shared__ float s_mute[TS];     // 1 -> scene sigma forced to -1e5 (box / zero ray); 2 bit -> object too
   const float* Pf = reinterpret_cast<const float*>(p.packed);
-  const int64_t total = (int64_t)p.n_rays * p.S;
+  const int64_t total = (int64_t)field_rays(p) * p.S;
 
   for (int64_t tile = blockIdx.x; tile * TS < total; tile += gridDim.x) {
     const int64_t e0 = tile * TS;
@@ -266,10 +266,12 @@ __global__ void __launch_bounds__(128) ray_const_kernel(FieldParams p) {
   __shared__ float s_code[8][ONERF_NCODE];
   const PackLayout& L = p.L;
   const float* Pf = reinterpret_cast<const float*>(p.packed);
+  const int n_rays = field_rays(p);
   const int r0 = blockIdx.x * 8;
+  if (r0 >= n_rays) return;
   for (int t = threadIdx.x; t < 8 * 3; t += blockDim.x) {
     const int lr = t / 3, c = t % 3;
-    const int ray = min(r0 + lr, p.n_rays - 1);
+    const int ray = min(r0 + lr, n_rays - 1);
     const float d = __ldg(p.rays + (int64_t)ray * 8 + 3 + c);
     s_dir[lr][c] = d;
     for (int k = 0; k < 4; ++k) {
@@ -280,7 +282,7 @@ __global__ void __launch_bounds__(128) ray_const_kernel(FieldParams p) {
   }
   for (int t = threadIdx.x; t < 8 * ONERF_NCODE; t += blockDim.x) {
     const int lr = t / ONERF_NCODE, c = t % ONERF_NCODE;
-    const int ray = min(r0 + lr, p.n_rays - 1);
+    const int ray = min(r0 + lr, n_rays - 1);
     float v = 0.0f;
     if (p.want_object) v = p.codes ? __ldg(p.codes + (int64_t)ray * ONERF_NCODE + c) : __ldg(p.code_row + c);
     s_code[lr][c] = v;
@@ -318,7 +320,7 @@ __global__ void __launch_bounds__(128) ray_const_kernel(FieldParams p) {
 #pragma unroll
   for (int r = 0; r < 8; ++r) {
     const int ray = r0 + r;
-    if (ray >= p.n_rays) break;
+    if (ray >= n_rays) break;
     float* o = p.ray_const + (int64_t)ray * ONERF_RAY_CONST_FLOATS;
     o[RC_SDIR + n] = a_sdir[r];
     if (n < 64) o[RC_ODIR + n] = a_odir[r];

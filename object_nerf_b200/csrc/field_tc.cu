@@ -351,7 +351,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
   }
   __syncthreads();
 
-  const int64_t total = (int64_t)p.n_rays * p.S;
+  const int64_t total = (int64_t)field_rays(p) * p.S;
   const int64_t n_tiles = (total + TM - 1) / TM;
 
   if (warp >= PRODUCER_WARP) {

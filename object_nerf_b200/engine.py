@@ -321,19 +321,26 @@ def composite(z, scene, obj, noise_std=0.0, white_back=False, is_eval=False, zer
 
 
 @_on_device
-def composite_multi(z_all, field_all, white_back=False, want_ids=False, want_unsorted=False):
-    """z_all (n_obj, N, S), field_all (n_obj, N, S, 4) -> sorted-order outputs (N, n_obj*S)."""
+def composite_multi(z_all, field_all, white_back=False, want_ids=False, want_unsorted=False, merge=False):
+    """z_all (n_obj, N, S), field_all (n_obj, N, S, 4) -> sorted-order outputs (N, n_obj*S).  Any n_obj * S: the bitonic
+    kernel up to 4096 samples per ray, the rank-merge path above (or always, with merge=True)."""
     n_obj, n, s = z_all.shape
     t = n_obj * s
     dev = z_all.device
+    lib = _lib.load()
     f = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
     out = {"z_vals": f(n, t), "weights": f(n, t), "opacity": f(n), "rgb": f(n, 3), "depth": f(n)}
     ids = f(n, t) if want_ids else None
     unsorted = f(n_obj, n, s) if want_unsorted else None
-    _lib.check(_lib.load().onerf_composite_multi(
+    ws = None
+    if merge or t > 4096:
+        ws = torch.empty(max(lib.onerf_composite_multi_workspace_bytes(n, n_obj, s), 256), dtype=torch.uint8, device=dev)
+    entry = lib.onerf_composite_multi_merge if merge else lib.onerf_composite_multi_ws
+    _lib.check(entry(
         _lib.ctx(dev), z_all.data_ptr(), field_all.data_ptr(), n, n_obj, s, int(bool(white_back)),
         out["z_vals"].data_ptr(), out["weights"].data_ptr(), _lib.ptr(ids), _lib.ptr(unsorted),
-        out["opacity"].data_ptr(), out["rgb"].data_ptr(), out["depth"].data_ptr(), _lib.stream()))
+        out["opacity"].data_ptr(), out["rgb"].data_ptr(), out["depth"].data_ptr(), _lib.ptr(ws),
+        ws.numel() if ws is not None else 0, _lib.stream()))
     if want_ids:
         out["obj_ids"] = ids
     if want_unsorted:

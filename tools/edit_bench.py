@@ -1,0 +1,146 @@
+"""Frame time of render_rays_multi (the editing path) with many ray sets.
+
+For each frame size and ray-set list, renders the whole frame in chunks of 4 096 rays (64 + 64 samples per set, bf16,
+synthetic scene of bench.py) and prints one JSON line per configuration: ms per frame (CUDA events, median of --reps
+frames after one warm-up frame) and the fraction of object rows the field kernel evaluated (the rays that hit the set's
+box; before box culling every object row was evaluated).  Object set k gets an axis-aligned box of half-size 0.12 around
+a point at depth 1 on a random pixel's ray; near / far come from the slab test, misses get near = far = 0 as in
+EditableRenderer.  The scene set carries two removed-object boxes.  A configuration the library refuses prints its error.
+
+  python tools/edit_bench.py                      # 320x240 and 640x480: [0,4,4] with bench.py's random near / far
+                                                  # (30 % misses), and [0] + [4] * k with boxes, k in 2 8 24 40
+  python tools/edit_bench.py --bench-leg          # only bench.py's edit leg configuration (640x480, [0,4,4], 30 % misses)
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import statistics
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+CHUNK = 4096
+
+
+class Box:   # the attributes of BBoxRayHelper that the removed-object mask reads (as bench.py's edit leg)
+    def __init__(self, b):
+        self.scale_factor = 2.0
+        self.pose_avg = np.eye(4)
+        self.axis_align_mat = np.eye(4)
+        self.axis_align_mat[:3, 3] = [0.05 * b, -0.1, 0.0]
+        lo = np.array([-0.5, -0.4, -0.3]) + 0.1 * b
+        self.bbox_bounds = np.array([lo, lo + 0.6])
+
+
+def scene(dev):
+    from object_nerf_b200 import Embedding, synthetic as S
+    wc = S.make_weights(0, True, sigma_gain=8.0, sigma_bias=1.0, rgb_gain=24.0)
+    wf = S.make_weights(1000, True, sigma_gain=8.0, sigma_bias=1.0, rgb_gain=24.0)
+    grid = S.make_grid(seed=5, shape=(42, 42, 22), occupancy=0.6, voxel_size=0.05, n_rows=800000)
+    models = {"coarse": S.make_model(wc, True, dev), "fine": S.make_model(wf, True, dev)}
+    emb = {"xyz": S.GridModule(grid).to(dev), "dir": Embedding(3, 4)}
+    return models, emb, S.make_code_library(S.make_codes(2)).to(dev)
+
+
+def box_sets(rays, k, rng):
+    """k object ray sets, each with near / far from the slab test against its own box"""
+    o, d = rays[:, 0:3], rays[:, 3:6]
+    sets, hit_frac = [], []
+    for _ in range(k):
+        p = int(rng.integers(rays.shape[0]))
+        c = o[p] + d[p] * 1.0
+        lo, hi = c - 0.12, c + 0.12
+        inv = 1.0 / torch.where(d.abs() < 1e-9, torch.full_like(d, 1e-9), d)
+        t1, t2 = (lo - o) * inv, (hi - o) * inv
+        tmin = torch.minimum(t1, t2).amax(1).clamp(min=0)
+        tmax = torch.maximum(t1, t2).amin(1)
+        hit = tmax > tmin
+        r = rays.clone()
+        r[:, 6] = torch.where(hit, tmin, torch.zeros_like(tmin))
+        r[:, 7] = torch.where(hit, tmax, torch.zeros_like(tmax))
+        sets.append(r)
+        hit_frac.append(hit.float().mean().item())
+    return sets, hit_frac
+
+
+def bench_sets(rays, rng):
+    """bench.py's edit leg: two object sets with random near / far and 30 % misses"""
+    n = rays.shape[0]
+    sets, hit_frac = [], []
+    for _ in range(2):
+        r = rays.clone()
+        near = torch.from_numpy(rng.uniform(0.4, 1.2, size=n).astype(np.float32)).to(rays.device)
+        far = near + torch.from_numpy(rng.uniform(0.2, 0.9, size=n).astype(np.float32)).to(rays.device)
+        miss = torch.from_numpy(rng.random(n) < 0.3).to(rays.device)
+        near[miss], far[miss] = 0, 0
+        r[:, 6], r[:, 7] = near, far
+        sets.append(r)
+        hit_frac.append(1.0 - miss.float().mean().item())
+    return sets, hit_frac
+
+
+def time_frame(models, emb, lib, sets, ids, reps):
+    from object_nerf_b200.multi_rendering import render_rays_multi
+    boxes = {"4": Box(0), "6": Box(1)}
+    n = sets[0].shape[0]
+
+    def frame():
+        with torch.no_grad():
+            for i in range(0, n, CHUNK):
+                render_rays_multi(models, emb, lib, [s[i:i + CHUNK] for s in sets], ids, N_samples=64, N_importance=64,
+                                  chunk=CHUNK, white_back=False, background_skip_bbox=boxes, precision="bf16")
+
+    frame()
+    torch.cuda.synchronize()
+    ms = []
+    for _ in range(reps):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        frame()
+        b.record()
+        torch.cuda.synchronize()
+        ms.append(a.elapsed_time(b))
+    return statistics.median(ms)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--sizes", default="320x240,640x480")
+    ap.add_argument("--counts", default="2,8,24,40", help="k of the set lists [0] + [4] * k")
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--bench-leg", action="store_true")
+    args = ap.parse_args()
+    from object_nerf_b200 import synthetic as S
+    dev = torch.device("cuda:0")
+    models, emb, lib = scene(dev)
+    gpu = torch.cuda.get_device_name(dev)
+    if args.bench_leg:
+        rays = S.pinhole_rays(480, 640).to(dev)
+        sets, hf = bench_sets(rays, np.random.default_rng(7))
+        ms = time_frame(models, emb, lib, [rays] + sets, [0, 4, 4], args.reps)
+        print(json.dumps({"config": "bench edit leg", "size": "640x480", "ids": [0, 4, 4], "ms_per_frame": ms,
+                          "object_rows_evaluated": statistics.mean(hf), "gpu": gpu}))
+        return
+    for size in args.sizes.split(","):
+        w, h = (int(x) for x in size.split("x"))
+        rays = S.pinhole_rays(h, w).to(dev)
+        lists = [("[0,4,4]", 2)] + [(f"[0]+[4]*{k}", int(k)) for k in args.counts.split(",")]
+        for name, k in lists:
+            rng = np.random.default_rng(100 + k)
+            sets, hf = bench_sets(rays, rng) if name == "[0,4,4]" else box_sets(rays, k, rng)
+            row = {"size": size, "ids": name, "n_sets": k + 1, "object_rows_evaluated": statistics.mean(hf), "gpu": gpu}
+            try:
+                row["ms_per_frame"] = time_frame(models, emb, lib, [rays] + sets, [0] + [4] * k, args.reps)
+            except RuntimeError as ex:
+                row["error"] = str(ex)[:160]
+            print(json.dumps(row), flush=True)
+
+
+if __name__ == "__main__":
+    main()
