@@ -69,8 +69,9 @@ class _Ops:
 
 
 def composite_backward(z, scene, obj, depth_scene, grads, noise_std, white_back, is_eval, zero_last_delta,
-                       frustum_bound_th, pass_through_mask, noise_scene, noise_obj):
-    """grads: dict with optional rgb, depth, opacity, rgb_instance, depth_instance, opacity_instance (N,..) tensors."""
+                       frustum_bound_th, pass_through_mask, noise_scene, noise_obj, seed=0):
+    """grads: dict with optional rgb, depth, opacity, rgb_instance, depth_instance, opacity_instance (N,..) tensors.
+    With noise_std > 0 and no noise buffer the noise is re-drawn from `seed`, as the forward (engine.composite) drew it."""
     n, s = z.shape
     dev = z.device
     dscene = torch.empty(n, s, 4, dtype=torch.float32, device=dev)
@@ -79,7 +80,7 @@ def composite_backward(z, scene, obj, depth_scene, grads, noise_std, white_back,
     a.z, a.scene, a.obj = z.data_ptr(), scene.data_ptr(), _lib.ptr(obj)
     a.n_rays, a.n_samples = n, s
     a.noise_std = float(noise_std)
-    a.noise_scene, a.noise_obj, a.seed = _lib.ptr(noise_scene), _lib.ptr(noise_obj), 0
+    a.noise_scene, a.noise_obj, a.seed = _lib.ptr(noise_scene), _lib.ptr(noise_obj), seed
     a.white_back, a.is_eval = int(bool(white_back)), int(bool(is_eval))
     a.zero_last_delta, a.rays_in_bbox = int(bool(zero_last_delta)), 0
     a.frustum_bound_th = float(frustum_bound_th)

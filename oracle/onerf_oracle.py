@@ -233,7 +233,10 @@ def alpha_weights(sigma, z, last_delta, noise=None, noise_std=0.0, zero_mask=Non
     """sigma (N,S), z (N,S) -> alpha (N,S), weights (N,S).  models/rendering.py:139-162.
     zero_mask: positions whose alpha is forced to 0 (occlusion mask, :202)."""
     deltas = z[:, 1:] - z[:, :-1]
-    deltas = torch.cat([deltas, torch.full_like(deltas[:, :1], last_delta)], -1)
+    # An extension of the reference, not a port: models/rendering.py shapes the last delta from deltas[:, :1], which is
+    # empty for one sample per ray and breaks there.  Shaped from z it is the same for S >= 2, and a lone sample gets
+    # last_delta, as the library's kernels give it.
+    deltas = torch.cat([deltas, torch.full_like(z[:, :1], last_delta)], -1)
     s = sigma if noise is None else sigma + noise * noise_std
     alpha = 1 - torch.exp(-deltas * torch.relu(s))
     if zero_mask is not None:
