@@ -59,8 +59,9 @@ def _grad_offsets(use_voxel):
     return Kd, w_off, b_off, heads, off
 
 
-def _train_forward(rays, z, packed, grid, codes, use_voxel, want_object, fill=0):
-    """onerf_field_fwd with a training workspace -> (ws, layout)."""
+def _train_forward(rays, z, packed, grid, codes, use_voxel, want_object, fill=0, outputs=False):
+    """onerf_field_fwd with a training workspace -> (ws, layout), and with outputs=True also the scene / object field
+    outputs and the ray_const buffer."""
     L = _lib()
     n, S = z.shape
     T = helpers.train_layout(bool(use_voxel), n * S)
@@ -77,6 +78,8 @@ def _train_forward(rays, z, packed, grid, codes, use_voxel, want_object, fill=0)
     a.scene_out, a.obj_out, a.out_stride, a.ray_const = scene.data_ptr(), obj.data_ptr() if want_object else None, S, rc.data_ptr()
     a.train_ws = ws.data_ptr()
     L.check(L.load().onerf_field_fwd(_ctx(), C.byref(a), L.stream()))
+    if outputs:
+        return ws, T, scene, obj if want_object else None, rc
     return ws, T
 
 
