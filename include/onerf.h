@@ -214,9 +214,10 @@ typedef struct onerf_render_args {
   onerf_render_maps fine;       /* written iff n_importance > 0 */
   void* workspace;              /* >= onerf_render_rays_workspace_bytes(...) bytes, 256-byte aligned */
   size_t workspace_bytes;
-  /* training: if non-NULL (ONERF_PREC_BF16, either model), >= onerf_train_workspace_bytes(grid != NULL, ...) bytes,
-   * 1024-byte aligned; the forward then keeps both passes' per-sample fields and the backward operands there for
-   * onerf_render_rays_bwd.  With ONERF_PREC_FP32 a training workspace is ONERF_ERR_UNSUPPORTED. */
+  /* training: if non-NULL (either model, either precision), >= onerf_train_workspace_bytes_prec(precision, grid != NULL,
+   * ...) bytes (include/onerf_ext.h; onerf_train_workspace_bytes for ONERF_PREC_BF16), 1024-byte aligned; the forward
+   * then keeps both passes' per-sample fields there for onerf_render_rays_bwd, and with ONERF_PREC_BF16 also every
+   * layer's operands (the fp32 backward re-runs the FFMA forward instead). */
   void* train_ws;
   size_t train_ws_bytes;
 } onerf_render_args;
@@ -341,15 +342,17 @@ size_t onerf_total_loss_workspace_bytes(void);
 int onerf_total_loss(onerf_ctx* ctx, const onerf_loss_args* args, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Training on the tensor cores (SURVEY.md §8 row a14: what loss.backward() does in the reference, train.py:147-180,
- * through models/rendering.py, models/nerf_model.py:97-152, models/embedding_helper.py:354-409, models/code_library.py).
- * onerf_render_rays_fwd with train_ws set runs the bf16 forward and keeps the backward operands;
+ * Training (SURVEY.md §8 row a14: what loss.backward() does in the reference, train.py:147-180, through
+ * models/rendering.py, models/nerf_model.py:97-152, models/embedding_helper.py:354-409, models/code_library.py).
+ * onerf_render_rays_fwd with train_ws set runs the forward and keeps what the backward needs;
  * onerf_render_rays_bwd turns the upstream gradients of the rendered maps into gradients of the 2 x 20 nn.Linear
  * tensors, the per-ray object codes and (voxel model) the voxel feature table, for either model (fwd->grid NULL = plain
- * PE model, whose encoding has no trainable parameters):
- *   compositing backward -> head gradients -> input-gradient chain (wgmma, transposed weight images, operand resident
- *   in registers) -> weight gradients (wgmma, sample-axis reduction) -> encoding gradient (wgmma + scatter-add) ->
- *   per-ray-constant columns (direction encoding, object code) -> reference [out,in] layout.
+ * PE model, whose encoding has no trainable parameters) and in the forward's precision:
+ *   ONERF_PREC_BF16: compositing backward -> head gradients -> input-gradient chain (wgmma, transposed weight images,
+ *   operand resident in registers) -> weight gradients (wgmma, sample-axis reduction) -> encoding gradient (wgmma +
+ *   scatter-add) -> per-ray-constant columns (direction encoding, object code) -> reference [out,in] layout.
+ *   ONERF_PREC_FP32 (verification arithmetic): compositing backward, then per chunk of rays the FFMA forward re-run with
+ *   its activation dump and the fp32 building blocks below, layer by layer.
  * No gradient flows to rays or depths (the importance samples are detached in the reference, models/rendering.py:307).
  * ------------------------------------------------------------------------------------------- */
 size_t onerf_train_workspace_bytes(int use_voxel, int n_rays, int n_samples, int n_importance);
@@ -401,7 +404,7 @@ int onerf_code_scatter_add(onerf_ctx* ctx, const float* d_codes, const int64_t* 
 
 /* ---------------------------------------------------------------------------------------------
  * fp32 backward building blocks (verification arithmetic of the training path).
- * object_nerf_b200/backward.py chains them into the gradient of render_rays for precision="fp32".
+ * onerf_render_rays_bwd chains them into the gradient of render_rays for ONERF_PREC_FP32.
  * ------------------------------------------------------------------------------------------- */
 
 /* Gradient of onerf_composite w.r.t. the per-sample fields: fwd = the forward's arguments (with noise_std > 0, NULL noise

@@ -31,6 +31,14 @@ int onerf_composite_multi_merge(onerf_ctx* ctx, const float* z_all, const float*
                                 float* weights_unsorted, float* opacity, float* rgb, float* depth, void* workspace,
                                 size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Size of the training workspace of onerf_render_rays_fwd / onerf_render_rays_bwd for either arithmetic (precision =
+ * onerf_precision); onerf_train_workspace_bytes is this with ONERF_PREC_BF16.  The fp32 workspace holds both passes'
+ * fields and one chunk (at most 65 536 samples) of the backward's activation dump and gradient buffers.  0 for an
+ * unknown precision or a bad shape.
+ * ------------------------------------------------------------------------------------------- */
+size_t onerf_train_workspace_bytes_prec(int precision, int use_voxel, int n_rays, int n_samples, int n_importance);
+
 #ifdef __cplusplus
 }
 #endif

@@ -35,7 +35,8 @@ EXPORTS = [
     "onerf_code_gather", "onerf_code_scatter_add", "onerf_render_multi_workspace_bytes", "onerf_render_multi_fwd",
 ]
 # additions to ABI version 2 declared in include/onerf_ext.h
-EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_ws", "onerf_composite_multi_merge"]
+EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_ws", "onerf_composite_multi_merge",
+               "onerf_train_workspace_bytes_prec"]
 
 _p = C.c_void_p
 
@@ -210,6 +211,8 @@ def load() -> C.CDLL:
         lib.onerf_composite_multi_workspace_bytes.restype = C.c_size_t
         for name in ("onerf_composite_multi_ws", "onerf_composite_multi_merge"):
             getattr(lib, name).argtypes = lib.onerf_composite_multi.argtypes[:-1] + [_p, C.c_size_t, _p]
+        lib.onerf_train_workspace_bytes_prec.argtypes = [C.c_int] * 5
+        lib.onerf_train_workspace_bytes_prec.restype = C.c_size_t
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

@@ -190,13 +190,13 @@ extern "C" int onerf_render_rays_fwd(onerf_ctx* ctx, const onerf_render_args* a,
   float* scene = reinterpret_cast<float*>(ws);
   ws += align256((size_t)a->n_rays * SF * 4 * sizeof(float));
   float* obj = reinterpret_cast<float*>(ws);
-  // training: both passes' fields and the backward operands are kept in the training workspace
+  // training: both passes' fields are kept in the training workspace, and with bf16 the backward operands too (the fp32
+  // backward re-runs the FFMA forward chunk by chunk instead)
   float *scene_c = scene, *obj_c = obj, *scene_f = scene, *obj_f = obj;
   void *tl_c = nullptr, *tl_f = nullptr;
   if (a->train_ws) {
-    ONERF_UNSUPPORTED(a->precision != ONERF_PREC_BF16, "training workspace: bf16 only");
     ONERF_CHECK_ARG((reinterpret_cast<uintptr_t>(a->train_ws) & 1023u) == 0, "train_ws must be 1024-byte aligned");
-    const TrainWs W = onerf_make_train_ws(onerf_train_use_voxel(a), a->n_rays, a->n_samples, a->n_importance);
+    const TrainWs W = onerf_make_train_ws(a->precision, onerf_train_use_voxel(a), a->n_rays, a->n_samples, a->n_importance);
     if (a->train_ws_bytes < (size_t)W.total) {
       onerf_set_error("onerf_render_rays_fwd: training workspace too small (%zu < %lld)", a->train_ws_bytes, (long long)W.total);
       return ONERF_ERR_WORKSPACE;
@@ -204,7 +204,7 @@ extern "C" int onerf_render_rays_fwd(onerf_ctx* ctx, const onerf_render_args* a,
     char* t = reinterpret_cast<char*>(a->train_ws);
     scene_c = reinterpret_cast<float*>(t + W.scene_c); obj_c = reinterpret_cast<float*>(t + W.obj_c);
     scene_f = reinterpret_cast<float*>(t + W.scene_f); obj_f = reinterpret_cast<float*>(t + W.obj_f);
-    tl_c = t + W.tl_coarse; tl_f = t + W.tl_fine;
+    if (a->precision == ONERF_PREC_BF16) { tl_c = t + W.tl_coarse; tl_f = t + W.tl_fine; }
   }
   // seeds: coarse depths, coarse noise, importance u, fine noise (rendering.py::_render_forward)
   int rc = onerf_sample_coarse(ctx, a->rays, a->n_rays, S, a->use_disp, a->perturb, a->jitter, a->seed, a->coarse.z_vals, stream);

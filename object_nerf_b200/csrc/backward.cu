@@ -5,7 +5,7 @@
 // samples: the FFMA field kernel re-runs the forward and dumps every layer's activations ([B x width] row-major,
 // field_fp32.cu), then per layer  dZ = dH * act'(H),  dW += dZ^T In (split over samples, atomics),  db += colsum(dZ),
 // dIn = dZ W  with the generic GEMM below; concatenations are handled with leading dimensions / column offsets.
-// Orchestration: object_nerf_b200/backward.py.
+// Orchestration: bwd_api.cu (onerf_render_rays_bwd with ONERF_PREC_FP32).
 #include "encode.cuh"
 #include "field_common.cuh"
 

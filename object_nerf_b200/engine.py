@@ -286,17 +286,10 @@ def field(rays, z, packed, grid: Optional[GridBuffers], codes=None, code_row=Non
     return (scene_out if want_scene else None), (obj_out if want_object else None)
 
 
-@_on_device
-def composite(z, scene, obj, noise_std=0.0, white_back=False, is_eval=False, zero_last_delta=False,
-              rays_in_bbox=False, frustum_bound_th=0.0, pass_through_mask=None, noise_scene=None,
-              noise_obj=None, seed=0):
-    """Returns dict(weights, opacity, rgb, depth[, rgb_instance, depth_instance, opacity_instance])."""
+def _composite_args(z, scene, obj, noise_std, white_back, is_eval, zero_last_delta, rays_in_bbox, frustum_bound_th,
+                    pass_through_mask, noise_scene, noise_obj, seed):
+    """Argument block of onerf_composite / onerf_composite_bwd (no outputs set) and the tensors it points into."""
     n, s = z.shape
-    dev = z.device
-    f = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
-    out = {"weights": f(n, s), "opacity": f(n), "rgb": f(n, 3), "depth": f(n)}
-    if obj is not None:
-        out.update(rgb_instance=f(n, 3), depth_instance=f(n), opacity_instance=f(n))
     a = _lib.CompositeArgs()
     a.z, a.scene, a.obj = z.data_ptr(), scene.data_ptr(), _lib.ptr(obj)
     a.n_rays, a.n_samples = n, s
@@ -311,6 +304,22 @@ def composite(z, scene, obj, noise_std=0.0, white_back=False, is_eval=False, zer
     if pass_through_mask is not None:
         ptm = pass_through_mask.reshape(-1).to(torch.uint8).contiguous()
     a.pass_through_mask = _lib.ptr(ptm)
+    return a, (noise_scene, noise_obj, ptm)
+
+
+@_on_device
+def composite(z, scene, obj, noise_std=0.0, white_back=False, is_eval=False, zero_last_delta=False,
+              rays_in_bbox=False, frustum_bound_th=0.0, pass_through_mask=None, noise_scene=None,
+              noise_obj=None, seed=0):
+    """Returns dict(weights, opacity, rgb, depth[, rgb_instance, depth_instance, opacity_instance])."""
+    n, s = z.shape
+    dev = z.device
+    f = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
+    out = {"weights": f(n, s), "opacity": f(n), "rgb": f(n, 3), "depth": f(n)}
+    if obj is not None:
+        out.update(rgb_instance=f(n, 3), depth_instance=f(n), opacity_instance=f(n))
+    a, _keep = _composite_args(z, scene, obj, noise_std, white_back, is_eval, zero_last_delta, rays_in_bbox,
+                               frustum_bound_th, pass_through_mask, noise_scene, noise_obj, seed)
     a.weights, a.opacity, a.rgb, a.depth = (out[k].data_ptr() for k in ("weights", "opacity", "rgb", "depth"))
     if obj is not None:
         a.rgb_instance = out["rgb_instance"].data_ptr()
@@ -318,6 +327,27 @@ def composite(z, scene, obj, noise_std=0.0, white_back=False, is_eval=False, zer
         a.opacity_instance = out["opacity_instance"].data_ptr()
     _lib.check(_lib.load().onerf_composite(_lib.ctx(dev), C.byref(a), _lib.stream()))
     return out
+
+
+@_on_device
+def composite_bwd(z, scene, obj, depth_scene, grads, noise_std=0.0, white_back=False, is_eval=False,
+                  zero_last_delta=False, frustum_bound_th=0.0, pass_through_mask=None, noise_scene=None,
+                  noise_obj=None, seed=0):
+    """Gradient of composite() w.r.t. the fields -> (dscene, dobj | None), each (N,S,4); depth_scene: the forward's scene
+    depth; grads: upstream gradients by map name (missing = 0).  Noise as the forward's (re-drawn from `seed` without
+    buffers).  No rays_in_bbox: it only selects the returned weights, which carry no gradient."""
+    n, s = z.shape
+    dev = z.device
+    dscene = torch.empty(n, s, 4, dtype=torch.float32, device=dev)
+    dobj = torch.empty(n, s, 4, dtype=torch.float32, device=dev) if obj is not None else None
+    a, _keep = _composite_args(z, scene, obj, noise_std, white_back, is_eval, zero_last_delta, False,
+                               frustum_bound_th, pass_through_mask, noise_scene, noise_obj, seed)
+    g = {k: (v.contiguous().float() if v is not None else None) for k, v in grads.items()}
+    _lib.check(_lib.load().onerf_composite_bwd(
+        _lib.ctx(dev), C.byref(a), _lib.ptr(depth_scene), _lib.ptr(g.get("rgb")), _lib.ptr(g.get("depth")),
+        _lib.ptr(g.get("opacity")), _lib.ptr(g.get("rgb_instance")), _lib.ptr(g.get("depth_instance")),
+        _lib.ptr(g.get("opacity_instance")), dscene.data_ptr(), _lib.ptr(dobj), _lib.stream()))
+    return dscene, dobj
 
 
 @_on_device
@@ -350,15 +380,17 @@ def composite_multi(z_all, field_all, white_back=False, want_ids=False, want_uns
 
 class RenderPlan:
     """Buffers + argument block of one onerf_render_rays_fwd() call (the whole forward of render_rays in ONE C call,
-    models/rendering.py:233-337 without autograd).  All outputs and the workspace are allocated once, so `run()` only
-    enqueues kernels: it can be captured in a CUDA graph and replayed."""
+    models/rendering.py:233-337).  All outputs and the workspace are allocated once, so `run()` only enqueues kernels:
+    it can be captured in a CUDA graph and replayed.  train_ws (a 1024-byte aligned uint8 tensor of
+    onerf_train_workspace_bytes_prec bytes, owned by the caller) makes it the forward of a training step, whose
+    backward (onerf_render_rays_bwd) takes `args`."""
 
     MAP_KEYS = ("weights", "opacity", "z_vals", "rgb", "depth", "rgb_instance", "depth_instance", "opacity_instance")
 
     def __init__(self, rays, packed_coarse, packed_fine, grid: Optional[GridBuffers], codes=None, n_samples=64,
                  n_importance=0, use_disp=False, perturb=0.0, noise_std=0.0, white_back=False, forward_instance=True,
                  is_eval=False, zero_last_delta=False, rays_in_bbox=False, frustum_bound_th=0.0,
-                 pass_through_mask=None, precision=None, seed=0, rand=None):
+                 pass_through_mask=None, precision=None, seed=0, rand=None, train_ws=None):
         lib = _lib.load()
         self.rays = _f32(rays)
         n, dev = self.rays.shape[0], self.rays.device
@@ -402,6 +434,8 @@ class RenderPlan:
         a.frustum_bound_th = float(frustum_bound_th)
         a.pass_through_mask = _lib.ptr(mask)
         a.workspace, a.workspace_bytes = self.workspace.data_ptr(), self.workspace.numel()
+        if train_ws is not None:
+            a.train_ws, a.train_ws_bytes = train_ws.data_ptr(), train_ws.numel()
         self.args = a
 
     def run(self):

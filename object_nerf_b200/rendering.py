@@ -112,8 +112,8 @@ def query_sigma(model, embedding_xyz, xyz: torch.Tensor, obj_code: Optional[torc
         out[i:i + n] = (scene if obj_code is None else obj)[:, 0, 3]
     return out
 
-def _render_forward(cfg, rays, codes, keep=False):
-    """The whole forward of render_rays on the CUDA kernels.  keep=True also returns what the backward needs."""
+def _render_forward(cfg, rays, codes):
+    """The whole forward of render_rays on the CUDA kernels, staged through engine (inference)."""
     rand = cfg["rand"]
     perturb, noise_std = cfg["perturb"], cfg["noise_std"]
     fi = cfg["forward_instance"]
@@ -123,22 +123,17 @@ def _render_forward(cfg, rays, codes, keep=False):
     seed = engine.new_seed() if (perturb > 0 or noise_std > 0) else 0
     z = engine.sample_coarse(rays, cfg["N_samples"], cfg["use_disp"], perturb, rand.get("jitter"), seed)
     results: Dict[str, Any] = {}
-    saved: Dict[str, Any] = {}
 
     def one_pass(typ, z_vals, seed_off):
         model = cfg["models"][typ]
-        packed = engine.packed_for(model, use_voxel, fresh=cfg.get("fresh_pack"))
+        packed = engine.packed_for(model, use_voxel)
         scene, obj = engine.field(rays, z_vals, packed, grid, codes=codes if fi else None, want_scene=True,
                                   want_object=fi, precision=cfg["precision"])
-        ns, no = rand.get(f"noise_scene_{typ}"), rand.get(f"noise_obj_{typ}")
-        if keep and noise_std > 0:      # the backward replays the noise: draw it into buffers instead of in-kernel
-            ns = ns if ns is not None else torch.randn_like(z_vals)
-            no = no if (no is not None or not fi) else torch.randn_like(z_vals)
         out = engine.composite(z_vals, scene, obj, noise_std=noise_std, white_back=cfg["white_back"],
                                is_eval=cfg["is_eval"], zero_last_delta=cfg["zero_last_delta"],
                                rays_in_bbox=cfg["rays_in_bbox"], frustum_bound_th=cfg["frustum_bound_th"],
-                               pass_through_mask=cfg["pass_through_mask"], noise_scene=ns, noise_obj=no,
-                               seed=seed + seed_off)
+                               pass_through_mask=cfg["pass_through_mask"], noise_scene=rand.get(f"noise_scene_{typ}"),
+                               noise_obj=rand.get(f"noise_obj_{typ}"), seed=seed + seed_off)
         results[f"weights_{typ}"] = out["weights"]
         results[f"opacity_{typ}"] = out["opacity"]
         results[f"z_vals_{typ}"] = z_vals
@@ -148,17 +143,13 @@ def _render_forward(cfg, rays, codes, keep=False):
             results[f"rgb_instance_{typ}"] = out["rgb_instance"]
             results[f"depth_instance_{typ}"] = out["depth_instance"]
             results[f"opacity_instance_{typ}"] = out["opacity_instance"]
-        if keep:
-            saved[typ] = dict(z=z_vals, scene=scene, obj=obj, depth=out["depth"],
-                              noise_scene=engine._f32(ns) if ns is not None else None,
-                              noise_obj=engine._f32(no) if no is not None else None)
 
     one_pass("coarse", z, 1)
     if cfg["N_importance"] > 0:
         z_fine = engine.sample_pdf_merge(z, results["weights_coarse"], cfg["N_importance"], det=(perturb == 0),
                                          u=rand.get("u"), seed=seed + 2)
         one_pass("fine", z_fine, 3)
-    return results, saved
+    return results
 
 
 def render_rays(models: Dict[str, Any], embeddings: Dict[str, Any], rays: torch.Tensor, N_samples: int = 64,
@@ -187,24 +178,18 @@ def render_rays(models: Dict[str, Any], embeddings: Dict[str, Any], rays: torch.
         any(p.requires_grad for p in trainable) or (codes is not None and codes.requires_grad)
         or (has_table and emb_xyz.embedding_space_ftr.weight.requires_grad))
     if not needs_grad:
-        return _render_forward(cfg, rays, codes)[0]
+        return _render_forward(cfg, rays, codes)
     # Training.  rays_in_bbox only swaps which weights feed the (detached) importance sampling and the returned
     # weights_* (models/rendering.py:228-229, :307): the gradients are unaffected.
     from . import backward
     cfg["has_table"], cfg["model_order"] = has_table, model_order
+    # bf16: tensor-core forward + backward; anything else selects the fp32 verification arithmetic end to end
+    cfg["precision"] = "bf16" if (cfg["precision"] or engine.default_precision()) == "bf16" else "fp32"
     params = ([emb_xyz.embedding_space_ftr.weight] if has_table else [])
     for typ in model_order:
         for w, b in engine.model_linears(models[typ]):
             params += [w, b]
-    precision = cfg["precision"] or engine.default_precision()
-    if precision == "bf16":
-        fn = backward.RenderRaysTcFn      # tensor-core forward + backward, voxel and plain-PE model alike
-    else:
-        # verification arithmetic, selected explicitly: fp32 forward AND backward, one function end to end
-        cfg["precision"] = "fp32"
-        cfg["fresh_pack"] = True          # training: never trust a cached blob (optimizers may write through .data)
-        fn = backward.RenderRaysFn
-    tensors = fn.apply(cfg, rays, codes, *params)
+    tensors = backward.RenderRaysFn.apply(cfg, rays, codes, *params)
     keys = sorted(_result_keys(model_order, forward_instance))
     return dict(zip(keys, tensors))
 

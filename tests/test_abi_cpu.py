@@ -122,3 +122,27 @@ def test_every_entry_point_rejects_a_null_context_with_a_message(lib):
     assert lib.onerf_field_train_bytes(1, 128 * 10) >= 10 * per_tile
     assert lib.onerf_train_workspace_bytes(1, 2048, 64, 64) >= (1024 + 2048) * per_tile
     assert lib.onerf_grad_buffer_floats(1) >= 891208 - 27 * 192 - 64 * 256
+
+
+def test_train_workspace_bytes_for_either_precision(lib):
+    """onerf_train_workspace_bytes_prec: 0 for an unknown precision or a bad shape; bf16 = onerf_train_workspace_bytes;
+    fp32 = both passes' fields and field gradients, the directions' PE and one backward chunk (<= 65 536 samples of whole
+    rays): 17 activation matrices, d(X), two 256-wide buffers, head gradients, fields, ray_const and per-ray sums."""
+    from object_nerf_b200 import _lib
+    f = lib.onerf_train_workspace_bytes_prec
+    for prec in (_lib.PREC_FP32, _lib.PREC_BF16):
+        assert f(prec, 1, -1, 64, 64) == 0 and f(prec, 1, 4, 0, 64) == 0 and f(prec, 0, 4, 64, -1) == 0
+    assert f(2, 1, 4, 64, 64) == 0 and f(-1, 0, 4, 64, 64) == 0
+    a1k = lambda x: (x + 1023) // 1024 * 1024
+    tail = [256] * 8 + [256, 128] + [128] * 4 + [128, 64]
+    for uv in (0, 1):
+        for n, s, si in ((1, 2, 0), (41, 64, 32), (2048, 64, 128), (4096, 64, 0), (2, 70000, 0), (0, 64, 64)):
+            assert f(_lib.PREC_BF16, uv, n, s, si) == lib.onerf_train_workspace_bytes(uv, n, s, si)
+            sf = s + si
+            rays = lambda S: min(n, max(1, 65536 // S))
+            R, B = max(rays(s), rays(sf)), max(rays(s) * s, rays(sf) * sf)
+            ko = 384 if uv else 64
+            want = (2 * a1k(n * s * 16) + 4 * a1k(n * sf * 16) + a1k(R * 128 * 4) + a1k(n * 27 * 4)
+                    + 2 * a1k(B * ko * 4) + sum(a1k(B * w * 4) for w in tail) + 2 * a1k(B * 256 * 4) + 3 * a1k(B * 16)
+                    + a1k(R * 448 * 4))
+            assert f(_lib.PREC_FP32, uv, n, s, si) == want, (uv, n, s, si)

@@ -337,7 +337,7 @@ def test_render_rays_multi_matches_reference_golden(golden, name, precision):
 
 
 def test_composite_backward_matches_oracle_autograd():
-    from object_nerf_b200 import backward as B
+    from object_nerf_b200 import engine
     rng = np.random.default_rng(41)
     n, s = 29, 96
     rays = synth.random_rays(42, n)
@@ -356,9 +356,9 @@ def test_composite_backward_matches_oracle_autograd():
     loss.backward()
     scene = torch.cat([rgb, sigma[..., None]], -1).detach().contiguous().to(DEV)
     obj = torch.cat([irgb, isigma[..., None]], -1).detach().contiguous().to(DEV)
-    dscene, dobj = B.composite_backward(z.to(DEV), scene, obj, ref["depth_x"].detach().to(DEV),
-                                        {k: v.to(DEV) for k, v in gout.items()}, 1.0, False, False, False, 0.05,
-                                        ptm.to(DEV), ns.to(DEV), no.to(DEV))
+    dscene, dobj = engine.composite_bwd(z.to(DEV), scene, obj, ref["depth_x"].detach().to(DEV),
+                                        {k: v.to(DEV) for k, v in gout.items()}, noise_std=1.0, frustum_bound_th=0.05,
+                                        pass_through_mask=ptm.to(DEV), noise_scene=ns.to(DEV), noise_obj=no.to(DEV))
     for got, want_rgb, want_sigma, nm in ((dscene, rgb.grad, sigma.grad, "scene"), (dobj, irgb.grad, isigma.grad, "obj")):
         got = got.cpu()
         scale = max(1.0, want_sigma.abs().max().item())

@@ -228,22 +228,32 @@ def _train_step(precision, inp, c, rand):
     return loss, named
 
 
-def test_plain_training_takes_the_tensor_core_path():
-    """A bf16 training call on the plain model goes to RenderRaysTcFn; fp32 keeps RenderRaysFn."""
+def test_plain_training_backward_runs_in_the_forward_precision():
+    """A bf16 training call on the plain model runs the tensor-core backward; fp32 runs the fp32 one.  Both reach
+    onerf_render_rays_bwd with the forward's precision in the argument block: the tensor-core backward is a few dozen
+    library launches, the fp32 one (FFMA forward re-run, then layer by layer) far more."""
     c = grad_plain.GRAD_CASE_PLAIN
     inp = grad_plain.build_grad_case_plain()
     rand = {k: v.to(DEV) for k, v in inp["rand"].items()}
-    from object_nerf_b200 import backward
+    L = _lib()
+    lib, dev = L.load(), torch.device(DEV)
+    orig = lib.onerf_render_rays_bwd
     seen = []
-    for fn in (backward.RenderRaysTcFn, backward.RenderRaysFn):
-        orig = fn.apply
-        fn.apply = (lambda o, name: lambda *a: (seen.append(name), o(*a))[1])(orig, fn.__name__)
+
+    def spy(ctx, fwd, bwd, stream):
+        n0 = L.launch_count(dev)
+        rc = orig(ctx, fwd, bwd, stream)
+        seen.append((fwd._obj.precision, L.launch_count(dev) - n0))
+        return rc
+
+    lib.onerf_render_rays_bwd = spy
     try:
         _train_step("bf16", inp, c, rand)
         _train_step("fp32", inp, c, rand)
     finally:
-        del backward.RenderRaysTcFn.apply, backward.RenderRaysFn.apply
-    assert seen == ["RenderRaysTcFn", "RenderRaysFn"]
+        lib.onerf_render_rays_bwd = orig
+    assert [p for p, _ in seen] == [L.PREC_BF16, L.PREC_FP32], seen
+    assert seen[0][1] < 64 < seen[1][1], seen
 
 
 def test_plain_training_step_bf16_gradients_match_reference_golden(golden):

@@ -456,7 +456,7 @@ def test_composite_bwd_matches_float64_autograd(mode, S):
     compositing forward test plus white_back / zero_last_delta with the object branch and the scene-only call, at
     sample counts around the warp width and up to the 2048 limit.  d rgb within 2e-5 and d sigma within 1e-3 of
     max(1, max |reference|) (fp32 transmittance products over S samples against float64)."""
-    from object_nerf_b200 import backward as Bk
+    from object_nerf_b200 import engine
     kw = dict(COMPOSITE_MODES[mode])
     fi = kw.pop("forward_instance", True)
     use_ptm = kw.pop("pass_through_mask", False)
@@ -474,11 +474,12 @@ def test_composite_bwd_matches_float64_autograd(mode, S):
     sum((ref[f"{k}_x"] * gout[k].double()).sum() for k in names).backward()
     scene = torch.cat([c["rgb"], c["sigma"][..., None]], -1).contiguous().to(DEV)
     obj = torch.cat([c["irgb"], c["isigma"][..., None]], -1).contiguous().to(DEV) if fi else None
-    dscene, dobj = Bk.composite_backward(
+    dscene, dobj = engine.composite_bwd(
         c["z"].to(DEV), scene, obj, ref["depth_x"].detach().float().to(DEV), {k: v.to(DEV) for k, v in gout.items()},
-        kw.get("noise_std", 0.0), kw.get("white_back", False), kw.get("is_eval", True), kw.get("zero_last_delta", False),
-        kw.get("frustum_bound_th", 0.0), c["ptm"].to(DEV) if use_ptm else None, c["ns"].to(DEV) if noise else None,
-        c["no"].to(DEV) if noise else None)
+        noise_std=kw.get("noise_std", 0.0), white_back=kw.get("white_back", False), is_eval=kw.get("is_eval", True),
+        zero_last_delta=kw.get("zero_last_delta", False), frustum_bound_th=kw.get("frustum_bound_th", 0.0),
+        pass_through_mask=c["ptm"].to(DEV) if use_ptm else None, noise_scene=c["ns"].to(DEV) if noise else None,
+        noise_obj=c["no"].to(DEV) if noise else None)
     torch.cuda.synchronize()
     pairs = [(dscene, rgb.grad, sigma.grad, "scene")] + ([(dobj, irgb.grad, isigma.grad, "obj")] if fi else [])
     for got, want_rgb, want_sigma, nm in pairs:
@@ -514,7 +515,6 @@ def test_composite_seeded_noise_forward_and_backward_match_numpy_philox():
     """noise_std = 1 with no noise buffers: the forward draws N(0, 1) from Philox stream 2 (scene) / 3 (object) at index
     ray S + i and the backward re-draws the same values.  Both must match the calls fed numpy's normals (which agree
     with the device's logf / cospif to an ulp or two), and differ from the noise-free calls."""
-    from object_nerf_b200 import backward as Bk
     from object_nerf_b200 import engine
     n, S = 29, 96
     c = _composite_inputs(n, S, seed=41)
@@ -533,10 +533,11 @@ def test_composite_seeded_noise_forward_and_backward_match_numpy_philox():
     assert (f_seed["weights"] - f_none["weights"]).abs().max().item() > 1e-2
     grads = {k: c["gout"](*f_seed[k].shape).to(DEV) for k in ("rgb", "depth", "opacity", "rgb_instance", "depth_instance",
                                                                "opacity_instance")}
-    common = (z, scene, obj, f_seed["depth"], grads, 1.0, False, False, False, 0.05, None)
-    d_seed = Bk.composite_backward(*common, None, None, seed=SEED)
-    d_buf = Bk.composite_backward(*common, ns, no)
-    d_wrong = Bk.composite_backward(*common, no, ns)        # the two streams exchanged
+    common = (z, scene, obj, f_seed["depth"], grads)
+    kw = dict(noise_std=1.0, frustum_bound_th=0.05)
+    d_seed = engine.composite_bwd(*common, seed=SEED, **kw)
+    d_buf = engine.composite_bwd(*common, noise_scene=ns, noise_obj=no, **kw)
+    d_wrong = engine.composite_bwd(*common, noise_scene=no, noise_obj=ns, **kw)        # the two streams exchanged
     torch.cuda.synchronize()
     for a, b, nm in ((d_seed[0], d_buf[0], "scene"), (d_seed[1], d_buf[1], "obj")):
         scale = max(1.0, b.abs().max().item())
@@ -580,9 +581,10 @@ def _loss(out, batch, typs, forward_instance):
     return cases.total_loss(out, batch)
 
 
-def _pool_key(c):
-    return (_lib().load().onerf_train_workspace_bytes(int(c["use_voxel"]), c["n_rays"], c["n_samples"], c["n_importance"]),
-            torch.device(DEV))
+def _pool_key(precision, c):
+    prec = _lib().PREC_BF16 if precision == "bf16" else _lib().PREC_FP32
+    return (_lib().load().onerf_train_workspace_bytes_prec(prec, int(c["use_voxel"]), c["n_rays"], c["n_samples"],
+                                                            c["n_importance"]), torch.device(DEV))
 
 
 def _step(precision, c, inp, pool_fill=None):
@@ -593,7 +595,7 @@ def _step(precision, c, inp, pool_fill=None):
     lib = helpers.CodeLib(inp["code_table"]).to(DEV)
     codes = lib.embedding_instance(inp["instance_ids"].view(-1).to(DEV))
     if pool_fill is not None:
-        assert backward._pool.free.get(_pool_key(c)), "no pooled workspace of this step's size to fill"
+        assert backward._pool.free.get(_pool_key(precision, c)), "no pooled workspace of this step's size to fill"
         for lst in backward._pool.free.values():
             for t in lst:
                 t.fill_(pool_fill)
@@ -645,19 +647,46 @@ def test_training_step_bf16_vs_fp32_untested_configurations(case):
 
 def test_pooled_training_workspace_garbage_does_not_reach_the_gradients():
     """The training workspace is pooled and not cleared between steps: a step on a pooled workspace filled with 0xFF
-    (bf16 NaN everywhere) gives finite gradients equal to a step on a zero-filled one, to run-to-run atomic noise."""
+    (bf16 and fp32 NaN everywhere) gives finite gradients equal to a step on a zero-filled one, to run-to-run atomic
+    noise, in either precision."""
     c, inp = _grad_case(dict(use_voxel=True, n_rays=41, n_importance=32))
-    _step("bf16", c, inp)                           # leaves the workspace in the pool
-    _, g0 = _step("bf16", c, inp, pool_fill=0)
-    _, gf = _step("bf16", c, inp, pool_fill=0xFF)
-    for name, a in g0.items():
-        b = gf[name]
-        if a is None:
-            assert b is None, name
-            continue
-        assert torch.isfinite(b).all(), name
-        scale = a.abs().max().item() + 1e-30
-        assert (a - b).abs().max().item() <= 1e-4 * scale, (name, (a - b).abs().max().item(), scale)
+    for precision in ("bf16", "fp32"):
+        _step(precision, c, inp)                        # leaves the workspace in the pool
+        _, g0 = _step(precision, c, inp, pool_fill=0)
+        _, gf = _step(precision, c, inp, pool_fill=0xFF)
+        for name, a in g0.items():
+            b = gf[name]
+            if a is None:
+                assert b is None, (precision, name)
+                continue
+            assert torch.isfinite(b).all(), (precision, name)
+            scale = a.abs().max().item() + 1e-30
+            assert (a - b).abs().max().item() <= 1e-4 * scale, (precision, name, (a - b).abs().max().item(), scale)
+
+
+@pytest.mark.parametrize("precision", ["bf16", "fp32"])
+def test_training_workspace_one_byte_short_is_refused(precision):
+    """onerf_render_rays_fwd and onerf_render_rays_bwd with a training workspace one byte smaller than
+    onerf_train_workspace_bytes_prec: ONERF_ERR_WORKSPACE and a message, before any kernel runs."""
+    from object_nerf_b200 import engine
+    c, inp = _grad_case(dict(use_voxel=True, n_rays=41, n_importance=32))
+    packed = {k: engine.packed_for(helpers.make_model(w, True, DEV), True, fresh=True) for k, w in inp["weights"].items()}
+    grid = engine.GridBuffers.from_module(helpers.GridModule(inp["grid"]).to(DEV))
+    codes = inp["code_table"][inp["instance_ids"].view(-1)].to(DEV)
+    ws = helpers.aligned_u8(_pool_key(precision, c)[0] - 1, DEV, fill=0)
+    L = _lib()
+    lib, ctx = L.load(), _ctx()
+    plan = engine.RenderPlan(inp["rays"].to(DEV), packed["coarse"], packed["fine"], grid, codes=codes,
+                             n_samples=c["n_samples"], n_importance=c["n_importance"], precision=precision, train_ws=ws)
+    launches = L.launch_count(torch.device(DEV))
+    assert lib.onerf_render_rays_fwd(ctx, C.byref(plan.args), L.stream()) == -4      # ONERF_ERR_WORKSPACE
+    assert b"training workspace too small" in lib.onerf_last_error()
+    b = L.RenderBwdArgs()
+    ptrs = (C.c_void_p * 20)(*([ws.data_ptr()] * 20))
+    b.W_coarse, b.dW_coarse, b.db_coarse, b.W_fine, b.dW_fine, b.db_fine = (ptrs,) * 6
+    assert lib.onerf_render_rays_bwd(ctx, C.byref(plan.args), C.byref(b), L.stream()) == -4
+    assert b"training workspace too small" in lib.onerf_last_error()
+    assert L.launch_count(torch.device(DEV)) == launches
 
 
 def _oracle_grads(c, inp, dtype):
