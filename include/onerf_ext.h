@@ -39,6 +39,24 @@ int onerf_composite_multi_merge(onerf_ctx* ctx, const float* z_all, const float*
  * ------------------------------------------------------------------------------------------- */
 size_t onerf_train_workspace_bytes_prec(int precision, int use_voxel, int n_rays, int n_samples, int n_importance);
 
+/* ---------------------------------------------------------------------------------------------
+ * One training step in one call (train.py:147-180 up to loss.backward()): onerf_render_rays_fwd, TotalLoss and
+ * onerf_render_rays_bwd with the loss and the compositing backward fused into the compositing kernels.  A batch kernel
+ * first sums what TotalLoss normalises by and skips on (it depends on the batch only); each pass's compositing kernel then
+ * composites a ray, forms its loss terms and map gradients and runs the compositing backward while the ray's alpha and
+ * transmittance are on chip; the last one writes the loss outputs and the PSNR.  The field backward follows as in
+ * onerf_render_rays_bwd.  Only enqueues work on `stream` (no host read, no allocation): CUDA-graph capturable.
+ *   fwd    onerf_render_args as for onerf_render_rays_fwd; forward_instance must be set; train_ws of
+ *          onerf_train_step_workspace_bytes(...) bytes, 1024-byte aligned.  Both passes' maps are written.
+ *   loss   batch inputs, term weights and outputs of onerf_total_loss (loss_sum_out, terms_out, present_out);
+ *          n_rays = fwd->n_rays, has_fine = (n_importance > 0); the map, grad_* and workspace fields are unused.
+ *   bwd    as for onerf_render_rays_bwd (gradients accumulated); its map gradients are unused.
+ *   psnr_out (1,) = -10 log10(mean over valid rays of (rgb - rgbs)^2) of the fine pass (coarse without one).
+ * ------------------------------------------------------------------------------------------- */
+size_t onerf_train_step_workspace_bytes(int precision, int use_voxel, int n_rays, int n_samples, int n_importance);
+int onerf_train_step(onerf_ctx* ctx, const onerf_render_args* fwd, const onerf_loss_args* loss,
+                     const onerf_render_bwd_args* bwd, float* psnr_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -36,7 +36,7 @@ EXPORTS = [
 ]
 # additions to ABI version 2 declared in include/onerf_ext.h
 EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_ws", "onerf_composite_multi_merge",
-               "onerf_train_workspace_bytes_prec"]
+               "onerf_train_workspace_bytes_prec", "onerf_train_step_workspace_bytes", "onerf_train_step"]
 
 _p = C.c_void_p
 
@@ -154,6 +154,12 @@ def load() -> C.CDLL:
                 f"{LIB_PATH} not found: run `python -c 'import __graft_entry__ as g; g.build()'` "
                 "(there is no CPU or PyTorch fallback for the render path)")
         lib = C.CDLL(LIB_PATH)
+        # ABI version 2 grows by additions only (include/onerf_ext.h): a library built before an addition has the right
+        # version but lacks the symbol
+        missing = [name for name in EXPORTS + EXPORTS_EXT if not hasattr(lib, name)]
+        if missing:
+            raise RuntimeError(f"{LIB_PATH} predates these entry points: {', '.join(missing)}; rebuild it "
+                               "(`python -c 'import __graft_entry__ as g; g.build()'`)")
         lib.onerf_abi_version.restype = C.c_int
         lib.onerf_last_error.restype = C.c_char_p
         lib.onerf_ctx_create.argtypes = [C.c_int, C.POINTER(_p)]
@@ -213,6 +219,9 @@ def load() -> C.CDLL:
             getattr(lib, name).argtypes = lib.onerf_composite_multi.argtypes[:-1] + [_p, C.c_size_t, _p]
         lib.onerf_train_workspace_bytes_prec.argtypes = [C.c_int] * 5
         lib.onerf_train_workspace_bytes_prec.restype = C.c_size_t
+        lib.onerf_train_step_workspace_bytes.argtypes = [C.c_int] * 5
+        lib.onerf_train_step_workspace_bytes.restype = C.c_size_t
+        lib.onerf_train_step.argtypes = [_p, C.POINTER(RenderArgs), C.POINTER(LossArgs), C.POINTER(RenderBwdArgs), _p, _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

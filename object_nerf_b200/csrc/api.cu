@@ -136,7 +136,8 @@ extern "C" size_t onerf_render_rays_workspace_bytes(int n_rays, int n_samples, i
 
 static int render_pass(onerf_ctx* ctx, const onerf_render_args* a, const void* packed, const float* z, int S,
                        const onerf_render_maps& m, const float* noise_scene, const float* noise_obj, uint64_t seed,
-                       float* ray_const, float* scene, float* obj, void* train_ws, void* stream) {
+                       float* ray_const, float* scene, float* obj, void* train_ws, const onerf_step_composite* step,
+                       void* stream) {
   onerf_field_args f;
   memset(&f, 0, sizeof(f));
   f.train_ws = train_ws;
@@ -160,6 +161,7 @@ static int render_pass(onerf_ctx* ctx, const onerf_render_args* a, const void* p
   c.pass_through_mask = a->pass_through_mask;
   c.weights = m.weights; c.opacity = m.opacity; c.rgb = m.rgb; c.depth = m.depth;
   c.rgb_instance = m.rgb_instance; c.depth_instance = m.depth_instance; c.opacity_instance = m.opacity_instance;
+  if (step) return onerf_launch_composite_step(ctx, &c, step, (cudaStream_t)stream);
   return onerf_composite(ctx, &c, stream);
 }
 
@@ -169,6 +171,10 @@ static bool maps_ok(const onerf_render_maps& m, int forward_instance) {
 }
 
 extern "C" int onerf_render_rays_fwd(onerf_ctx* ctx, const onerf_render_args* a, void* stream) {
+  return onerf_render_fwd_impl(ctx, a, nullptr, stream);
+}
+
+int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const onerf_step_composite* step, void* stream) {
   ONERF_CHECK_ARG(ctx && a, "null argument");
   ONERF_CHECK_ARG(a->rays && a->packed_coarse, "null rays / packed_coarse");
   ONERF_CHECK_ARG(a->n_rays >= 0 && a->n_samples >= 2 && a->n_importance >= 0, "bad shape");
@@ -206,17 +212,31 @@ extern "C" int onerf_render_rays_fwd(onerf_ctx* ctx, const onerf_render_args* a,
     scene_f = reinterpret_cast<float*>(t + W.scene_f); obj_f = reinterpret_cast<float*>(t + W.obj_f);
     if (a->precision == ONERF_PREC_BF16) { tl_c = t + W.tl_coarse; tl_f = t + W.tl_fine; }
   }
+  // training step: the coarse pass's field gradients go to the step's extension of the workspace, the fine pass's where
+  // onerf_render_rays_bwd puts them; the fine pass (or the coarse one without importance samples) finalizes the loss
+  onerf_step_composite step_c, step_f;
+  if (step) {
+    ONERF_CHECK_ARG(a->train_ws, "the training step needs a training workspace");
+    const TrainWs W = onerf_make_train_ws(a->precision, onerf_train_use_voxel(a), a->n_rays, a->n_samples, a->n_importance);
+    const TrainStepWs T = onerf_make_train_step_ws(W, a->n_rays, a->n_samples);
+    char* t = reinterpret_cast<char*>(a->train_ws);
+    step_c = step_f = *step;
+    step_c.fine = 0; step_c.finalize = a->n_importance == 0;
+    step_c.dscene = reinterpret_cast<float*>(t + T.dscene_c); step_c.dobj = reinterpret_cast<float*>(t + T.dobj_c);
+    step_f.fine = 1; step_f.finalize = 1;
+    step_f.dscene = reinterpret_cast<float*>(t + W.dscene); step_f.dobj = reinterpret_cast<float*>(t + W.dobj);
+  }
   // seeds: coarse depths, coarse noise, importance u, fine noise (rendering.py::_render_forward)
   int rc = onerf_sample_coarse(ctx, a->rays, a->n_rays, S, a->use_disp, a->perturb, a->jitter, a->seed, a->coarse.z_vals, stream);
   if (rc != ONERF_OK) return rc;
   rc = render_pass(ctx, a, a->packed_coarse, a->coarse.z_vals, S, a->coarse, a->noise_scene_coarse, a->noise_obj_coarse,
-                   a->seed + 1, ray_const, scene_c, obj_c, tl_c, stream);
+                   a->seed + 1, ray_const, scene_c, obj_c, tl_c, step ? &step_c : nullptr, stream);
   if (rc != ONERF_OK || a->n_importance == 0) return rc;
   rc = onerf_sample_pdf_merge(ctx, a->coarse.z_vals, a->coarse.weights, a->n_rays, S, a->n_importance, a->perturb == 0.0f ? 1 : 0,
                               a->u, a->seed + 2, a->fine.z_vals, stream);
   if (rc != ONERF_OK) return rc;
   return render_pass(ctx, a, a->packed_fine, a->fine.z_vals, SF, a->fine, a->noise_scene_fine, a->noise_obj_fine, a->seed + 3,
-                     ray_const, scene_f, obj_f, tl_f, stream);
+                     ray_const, scene_f, obj_f, tl_f, step ? &step_f : nullptr, stream);
 }
 
 // ------------------------------------------------------------------------------------------------

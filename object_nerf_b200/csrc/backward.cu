@@ -6,6 +6,7 @@
 // field_fp32.cu), then per layer  dZ = dH * act'(H),  dW += dZ^T In (split over samples, atomics),  db += colsum(dZ),
 // dIn = dZ W  with the generic GEMM below; concatenations are handled with leading dimensions / column offsets.
 // Orchestration: bwd_api.cu (onerf_render_rays_bwd with ONERF_PREC_FP32).
+#include "composite_bwd.cuh"
 #include "encode.cuh"
 #include "field_common.cuh"
 
@@ -22,38 +23,28 @@ __device__ __forceinline__ float warp_scan_mul(float v, int lane) {
   }
   return v;
 }
-// inclusive suffix sum: v_i <- sum_{j >= i} v_j
-__device__ __forceinline__ float warp_suffix_add(float v, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    float t = __shfl_down_sync(0xffffffffu, v, o);
-    if (lane + o < 32) v += t;
-  }
-  return v;
-}
-
 struct BranchGrad {
   const float* g_rgb;      // (N,3) or null
   const float* g_depth;    // (N,) or null
   const float* g_opacity;  // (N,) or null
 };
 
-// Recompute alpha / transmittance of one branch of one ray, then back-propagate.
-// smem (per warp): alpha[S], trans[S], gw[S]
+// Recompute alpha / transmittance of one branch of one ray, then back-propagate (composite_bwd.cuh).
+// smem (per warp): alpha[S], trans[S], sig[S], gw[S]
 __device__ __forceinline__ void composite_branch_bwd(const float* __restrict__ z, const float4* __restrict__ field, int S,
                                                      float last_delta, float noise_std, const float* __restrict__ noise,
                                                      uint64_t seed, uint32_t stream_id, int ray, bool use_mask, float z_limit, bool white, float g_r, float g_g,
                                                      float g_b, float g_d, float g_o, float4* __restrict__ dfield,
-                                                     float* s_alpha, float* s_trans, float* s_gw, int lane) {
+                                                     float* s_alpha, float* s_trans, float* s_sig, float* s_gw, int lane) {
   // forward recompute
   float carry = 1.0f;
   for (int base = 0; base < S; base += 32) {
     const int i = base + lane;
-    float alpha = 0.0f;
+    float alpha = 0.0f, s = 0.0f;
     if (i < S) {
       const float zi = __ldg(z + i);
       const float delta = (i + 1 < S) ? __fsub_rn(__ldg(z + i + 1), zi) : last_delta;
-      float s = __ldg(field + i).w;
+      s = __ldg(field + i).w;
       if (noise_std > 0.0f) {   // the forward's noise: the caller's buffer, or the same Philox draw (composite.cu)
         const float nz = noise ? __ldg(noise + i) : philox_normal(seed, stream_id, (uint64_t)ray * S + i);
         s = __fadd_rn(s, __fmul_rn(nz, noise_std));
@@ -68,48 +59,13 @@ __device__ __forceinline__ void composite_branch_bwd(const float* __restrict__ z
     if (i < S) {
       s_alpha[i] = alpha;
       s_trans[i] = carry * excl;
+      s_sig[i] = s;
     }
     carry *= __shfl_sync(0xffffffffu, incl, 31);
   }
   __syncwarp();
-  // dL/dw_i
-  const float g_o_eff = g_o - (white ? (g_r + g_g + g_b) : 0.0f);
-  for (int i = lane; i < S; i += 32) {
-    const float4 f = __ldg(field + i);
-    s_gw[i] = g_r * f.x + g_g * f.y + g_b * f.z + g_d * __ldg(z + i) + g_o_eff;
-  }
-  __syncwarp();
-  // reverse pass: suffix sums of dL/dw_k * w_k for k > i
-  float tail = 0.0f;
-  const int nchunk = (S + 31) / 32;
-  for (int c = nchunk - 1; c >= 0; --c) {
-    const int i = c * 32 + lane;
-    const bool in = i < S;
-    const float alpha = in ? s_alpha[i] : 0.0f;
-    const float T = in ? s_trans[i] : 0.0f;
-    const float w = alpha * T;
-    const float gw = in ? s_gw[i] : 0.0f;
-    const float G = gw * w;
-    const float incl = warp_suffix_add(G, lane);
-    const float after = incl - G + tail;          // sum over k > i
-    tail += __shfl_sync(0xffffffffu, incl, 0);
-    if (in) {
-      const float zi = __ldg(z + i);
-      const float delta = (i + 1 < S) ? __fsub_rn(__ldg(z + i + 1), zi) : last_delta;
-      const float4 f = __ldg(field + i);
-      float s = f.w;
-      if (noise_std > 0.0f) {
-        const float nz = noise ? __ldg(noise + i) : philox_normal(seed, stream_id, (uint64_t)ray * S + i);
-        s = __fadd_rn(s, __fmul_rn(nz, noise_std));
-      }
-      const float t = __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f);
-      const float dalpha = gw * T - after / t;
-      const bool masked = use_mask && z_limit < zi;
-      // alpha = 1 - exp(-delta relu(s)):  d alpha / d s = delta exp(-delta s) for s > 0
-      const float dsig = (masked || s <= 0.0f) ? 0.0f : dalpha * delta * expf(-delta * s);
-      dfield[i] = make_float4(g_r * w, g_g * w, g_b * w, dsig);
-    }
-  }
+  composite_branch_grad(z, field, S, last_delta, use_mask, z_limit, white, g_r, g_g, g_b, g_d, g_o, dfield, s_alpha, s_trans,
+                        s_sig, s_gw, lane);
 }
 
 struct CompositeBwdArgs {
@@ -125,9 +81,10 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(CompositeBwdArgs a) 
   const int warps_per_block = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = a.fwd.n_samples;
-  float* s_alpha = smem_c + (size_t)warp * 3 * S;
+  float* s_alpha = smem_c + (size_t)warp * 4 * S;
   float* s_trans = s_alpha + S;
-  float* s_gw = s_trans + S;
+  float* s_sig = s_trans + S;
+  float* s_gw = s_sig + S;
   for (int r = blockIdx.x * warps_per_block + warp; r < a.fwd.n_rays; r += gridDim.x * warps_per_block) {
     const float* z = a.fwd.z + (int64_t)r * S;
     auto g3 = [&](const float* p, int c) { return p ? __ldg(p + (int64_t)r * 3 + c) : 0.0f; };
@@ -136,7 +93,7 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(CompositeBwdArgs a) 
                          a.fwd.zero_last_delta ? 0.0f : 1e10f, a.fwd.noise_std,
                          a.fwd.noise_scene ? a.fwd.noise_scene + (int64_t)r * S : nullptr, a.fwd.seed, 2u, r, false, 0.0f,
                          a.fwd.white_back != 0, g3(a.gs.g_rgb, 0), g3(a.gs.g_rgb, 1), g3(a.gs.g_rgb, 2), g1(a.gs.g_depth),
-                         g1(a.gs.g_opacity), reinterpret_cast<float4*>(a.dscene) + (int64_t)r * S, s_alpha, s_trans, s_gw,
+                         g1(a.gs.g_opacity), reinterpret_cast<float4*>(a.dscene) + (int64_t)r * S, s_alpha, s_trans, s_sig, s_gw,
                          lane);
     __syncwarp();
     if (a.fwd.obj != nullptr) {
@@ -146,7 +103,7 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(CompositeBwdArgs a) 
       composite_branch_bwd(z, reinterpret_cast<const float4*>(a.fwd.obj) + (int64_t)r * S, S, 0.0f, a.fwd.noise_std,
                            a.fwd.noise_obj ? a.fwd.noise_obj + (int64_t)r * S : nullptr, a.fwd.seed, 3u, r, use_mask, z_limit, true,
                            g3(a.go.g_rgb, 0), g3(a.go.g_rgb, 1), g3(a.go.g_rgb, 2), g1(a.go.g_depth), g1(a.go.g_opacity),
-                           reinterpret_cast<float4*>(a.dobj) + (int64_t)r * S, s_alpha, s_trans, s_gw, lane);
+                           reinterpret_cast<float4*>(a.dobj) + (int64_t)r * S, s_alpha, s_trans, s_sig, s_gw, lane);
       __syncwarp();
     }
   }
@@ -350,7 +307,7 @@ extern "C" int onerf_composite_bwd(onerf_ctx* ctx, const onerf_composite_args* f
   a.dscene = dscene;
   a.dobj = dobj;
   const int warps = 4;
-  const size_t smem = (size_t)warps * 3 * fwd->n_samples * sizeof(float);
+  const size_t smem = (size_t)warps * 4 * fwd->n_samples * sizeof(float);
   ONERF_CUDA(cudaFuncSetAttribute(composite_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int blocks = (fwd->n_rays + warps - 1) / warps;
   if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;

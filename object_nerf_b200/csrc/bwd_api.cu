@@ -272,8 +272,7 @@ static int bwd_pass_fp32(onerf_ctx* ctx, const onerf_render_args* f, const onerf
 }
 #undef TRY
 
-extern "C" int onerf_render_rays_bwd(onerf_ctx* ctx, const onerf_render_args* f, const onerf_render_bwd_args* b, void* stream) {
-  ONERF_CHECK_ARG(ctx && f && b, "null argument");
+static int check_bwd_args(const onerf_render_args* f, const onerf_render_bwd_args* b) {
   ONERF_CHECK_ARG(f->train_ws, "the forward was not run with a training workspace");
   ONERF_CHECK_ARG(f->precision == ONERF_PREC_FP32 || f->precision == ONERF_PREC_BF16, "unknown precision");
   ONERF_CHECK_ARG(b->W_coarse && b->dW_coarse && b->db_coarse, "null coarse gradient arguments");
@@ -281,20 +280,78 @@ extern "C" int onerf_render_rays_bwd(onerf_ctx* ctx, const onerf_render_args* f,
   const int use_voxel = onerf_train_use_voxel(f);
   ONERF_CHECK_ARG(use_voxel || !b->table_grad, "table_grad given for the plain-PE model, which has no voxel table");
   ONERF_CHECK_ARG(!b->table_grad || onerf_aligned16(b->table_grad), "table_grad misaligned");
-  const TrainWs W = onerf_make_train_ws(f->precision, use_voxel, f->n_rays, f->n_samples, f->n_importance);
+  return ONERF_OK;
+}
+
+// The backward of both passes, fine first as autograd runs it.  step == NULL: each pass starts with the compositing
+// backward of b's map gradients; otherwise the training step's compositing kernels have already written the field
+// gradients (fine pass at W.dscene / W.dobj, coarse pass at step->dscene_c / dobj_c) and the field backward starts there.
+static int render_bwd(onerf_ctx* ctx, const onerf_render_args* f, const onerf_render_bwd_args* b, const TrainWs& W,
+                      const TrainStepWs* step, void* stream) {
+  const int use_voxel = onerf_train_use_voxel(f);
+  char* ws = reinterpret_cast<char*>(f->train_ws);
+  float* pe = reinterpret_cast<float*>(ws + W.pe);
+  int rc = onerf_dir_encode(ctx, f->rays, f->n_rays, pe, stream);
+  const auto field_bwd = f->precision == ONERF_PREC_BF16 ? bwd_pass_tc : bwd_pass_fp32;
+  for (const bool fine : {true, false}) {
+    if (rc != ONERF_OK || (fine && f->n_importance == 0)) continue;
+    TrainWs Wp = W;
+    if (!step) rc = composite_bwd_pass(ctx, f, b, W, fine, ws, stream);
+    else if (!fine) { Wp.dscene = step->dscene_c; Wp.dobj = step->dobj_c; }
+    if (rc == ONERF_OK) rc = field_bwd(ctx, f, b, Wp, use_voxel, fine, ws, pe, stream);
+  }
+  return rc;
+}
+
+extern "C" int onerf_render_rays_bwd(onerf_ctx* ctx, const onerf_render_args* f, const onerf_render_bwd_args* b, void* stream) {
+  ONERF_CHECK_ARG(ctx && f && b, "null argument");
+  int rc = check_bwd_args(f, b);
+  if (rc != ONERF_OK) return rc;
+  const TrainWs W = onerf_make_train_ws(f->precision, onerf_train_use_voxel(f), f->n_rays, f->n_samples, f->n_importance);
   if (f->train_ws_bytes < (size_t)W.total) {
     onerf_set_error("onerf_render_rays_bwd: training workspace too small (%zu < %lld)", f->train_ws_bytes, (long long)W.total);
     return ONERF_ERR_WORKSPACE;
   }
   if (f->n_rays == 0) return ONERF_OK;
-  char* ws = reinterpret_cast<char*>(f->train_ws);
-  float* pe = reinterpret_cast<float*>(ws + W.pe);
-  int rc = onerf_dir_encode(ctx, f->rays, f->n_rays, pe, stream);
-  const auto field_bwd = f->precision == ONERF_PREC_BF16 ? bwd_pass_tc : bwd_pass_fp32;
-  for (const bool fine : {true, false}) {   // fine pass first, as autograd runs it
-    if (rc != ONERF_OK || (fine && f->n_importance == 0)) continue;
-    rc = composite_bwd_pass(ctx, f, b, W, fine, ws, stream);
-    if (rc == ONERF_OK) rc = field_bwd(ctx, f, b, W, use_voxel, fine, ws, pe, stream);
+  return render_bwd(ctx, f, b, W, nullptr, stream);
+}
+
+// ---- the training step ----
+extern "C" size_t onerf_train_step_workspace_bytes(int precision, int use_voxel, int n_rays, int n_samples, int n_importance) {
+  if (precision != ONERF_PREC_FP32 && precision != ONERF_PREC_BF16) return 0;
+  if (n_rays < 0 || n_samples < 1 || n_importance < 0) return 0;
+  const TrainWs W = onerf_make_train_ws(precision, use_voxel ? 1 : 0, n_rays, n_samples, n_importance);
+  return (size_t)onerf_make_train_step_ws(W, n_rays, n_samples).total;
+}
+
+extern "C" int onerf_train_step(onerf_ctx* ctx, const onerf_render_args* f, const onerf_loss_args* l,
+                                const onerf_render_bwd_args* b, float* psnr_out, void* stream) {
+  ONERF_CHECK_ARG(ctx && f && l && b && psnr_out, "null argument");
+  int rc = check_bwd_args(f, b);
+  if (rc != ONERF_OK) return rc;
+  ONERF_CHECK_ARG(f->n_rays > 0 && l->n_rays == f->n_rays, "n_rays must be positive and equal in the render and loss arguments");
+  ONERF_CHECK_ARG(f->forward_instance, "the loss needs the object branch's maps (forward_instance)");
+  ONERF_CHECK_ARG(l->has_fine == (f->n_importance > 0 ? 1 : 0), "has_fine must say whether there is a fine pass");
+  ONERF_CHECK_ARG(l->rgbs && l->depths && l->valid_mask && l->instance_mask && l->instance_mask_weight, "null batch buffer");
+  ONERF_CHECK_ARG(l->loss_sum_out && l->terms_out && l->present_out, "null loss output");
+  ONERF_UNSUPPORTED(f->n_samples + f->n_importance > 2048, "S > 2048");
+  ONERF_CHECK_ARG((reinterpret_cast<uintptr_t>(f->train_ws) & 1023u) == 0, "train_ws must be 1024-byte aligned");
+  const TrainWs W = onerf_make_train_ws(f->precision, onerf_train_use_voxel(f), f->n_rays, f->n_samples, f->n_importance);
+  const TrainStepWs T = onerf_make_train_step_ws(W, f->n_rays, f->n_samples);
+  if (f->train_ws_bytes < (size_t)T.total) {
+    onerf_set_error("onerf_train_step: training workspace too small (%zu < %lld)", f->train_ws_bytes, (long long)T.total);
+    return ONERF_ERR_WORKSPACE;
   }
-  return rc;
+  double* acc = reinterpret_cast<double*>(reinterpret_cast<char*>(f->train_ws) + T.loss);
+  ONERF_CUDA(cudaMemsetAsync(acc, 0, ONERF_STEP_LOSS_BYTES, (cudaStream_t)stream));
+  rc = onerf_launch_batch_stats(ctx, l, acc, (cudaStream_t)stream);
+  if (rc != ONERF_OK) return rc;
+  onerf_step_composite step;
+  memset(&step, 0, sizeof(step));
+  step.loss = *l;
+  step.acc = acc;
+  step.psnr_out = psnr_out;
+  rc = onerf_render_fwd_impl(ctx, f, &step, stream);
+  if (rc != ONERF_OK) return rc;
+  return render_bwd(ctx, f, b, W, &T, stream);
 }

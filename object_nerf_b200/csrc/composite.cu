@@ -3,9 +3,14 @@
 // float4 access), multiplicative warp scan for the exclusive transmittance product.
 //
 // Reference behaviour: models/rendering.py:139-229; render_tools/multi_rendering.py:96-157.
+#include <string.h>
+
 #include <algorithm>
 
 #include "common.cuh"
+#include "composite_bwd.cuh"
+#include "loss_terms.cuh"
+#include "train_ws.h"
 #include "../../include/onerf_ext.h"
 
 namespace {
@@ -36,12 +41,14 @@ struct Acc {
 };
 
 // Composite one branch of one ray.  field = (S,4) rgb,sigma.  Returns warp-reduced sums on all lanes.
-// If w_out != nullptr the per-sample weights are stored.
+// If w_out != nullptr the per-sample weights are stored; if s_alpha != nullptr, what composite_branch_grad reads
+// (composite_bwd.cuh: alpha, transmittance, noised sigma) goes to the warp's shared memory.
 __device__ __forceinline__ Acc composite_branch(const float* __restrict__ z, const float4* __restrict__ field,
                                                 int S, float last_delta, float noise_std,
                                                 const float* __restrict__ noise, uint64_t seed,
                                                 uint32_t stream_id, int64_t ray, bool use_mask, float z_limit,
-                                                float* __restrict__ w_out, int lane) {
+                                                float* __restrict__ w_out, int lane, float* s_alpha = nullptr,
+                                                float* s_trans = nullptr, float* s_sig = nullptr) {
   Acc acc = {0.f, 0.f, 0.f, 0.f, 0.f};
   float carry = 1.0f;  // prod_{j < chunk start} (1 - alpha_j + 1e-10)
   for (int base = 0; base < S; base += 32) {
@@ -59,12 +66,17 @@ __device__ __forceinline__ Acc composite_branch(const float* __restrict__ z, con
       }
       alpha = alpha_from(s, delta);
       if (use_mask && z_limit < zi) alpha = 0.0f;  // occlusion mask, models/rendering.py:192-202
+      if (s_sig) s_sig[i] = s;
     }
     const float t = (i < S) ? __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f) : 1.0f;
     const float incl = warp_scan_mul(t, lane);
     float excl = __shfl_up_sync(0xffffffffu, incl, 1);
     if (lane == 0) excl = 1.0f;
     const float w = alpha * (carry * excl);
+    if (s_alpha && i < S) {
+      s_alpha[i] = alpha;
+      s_trans[i] = carry * excl;
+    }
     carry *= __shfl_sync(0xffffffffu, incl, 31);
     if (i < S) {
       if (w_out) w_out[i] = w;
@@ -83,43 +95,112 @@ __device__ __forceinline__ Acc composite_branch(const float* __restrict__ z, con
   return acc;
 }
 
-__global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a) {
+// kStep = false: the forward (onerf_composite).  kStep = true: the training step's compositing (onerf_train_step): the
+// same forward, then per ray the squared errors of the loss terms this pass owns and their gradients w.r.t. the ray's
+// maps (loss_terms.cuh; the normalisers depend on the batch only, so they are known before the render), then the
+// compositing backward of both branches on the alpha / transmittance the forward left in shared memory
+// (composite_bwd.cuh).  Per-block sums of the squared errors go to the fp64 accumulators; with `finalize` the last block
+// to finish turns them into the loss outputs and the PSNR.
+template <bool kStep>
+__global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, onerf_step_composite st) {
+  using namespace loss_terms;
+  extern __shared__ float smem_c[];
   const int warps_per_block = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = a.n_samples;
+  float *s_alpha = nullptr, *s_trans = nullptr, *s_sig = nullptr, *s_gw = nullptr;
+  double sq[N_TERMS] = {0.0, 0.0, 0.0, 0.0, 0.0};   // lane 0: squared-error sums of this warp's rays
+  float scale[N_TERMS];
+  if (kStep) {
+    s_alpha = smem_c + (size_t)warp * 4 * S;
+    s_trans = s_alpha + S;
+    s_sig = s_trans + S;
+    s_gw = s_sig + S;
+    grad_scales(st.loss, st.acc, scale);
+  }
   for (int r = blockIdx.x * warps_per_block + warp; r < a.n_rays; r += gridDim.x * warps_per_block) {
     const float* z = a.z + (int64_t)r * S;
     const bool obj_weights_out = (a.obj != nullptr) && a.rays_in_bbox;
-    Acc sc = composite_branch(z, reinterpret_cast<const float4*>(a.scene) + (int64_t)r * S, S,
-                              a.zero_last_delta ? 0.0f : 1e10f, a.noise_std,
+    const float scene_last_delta = a.zero_last_delta ? 0.0f : 1e10f;
+    const float4* scene = reinterpret_cast<const float4*>(a.scene) + (int64_t)r * S;
+    Acc sc = composite_branch(z, scene, S, scene_last_delta, a.noise_std,
                               a.noise_scene ? a.noise_scene + (int64_t)r * S : nullptr, a.seed, 2u, r, false,
-                              0.0f, obj_weights_out ? nullptr : a.weights + (int64_t)r * S, lane);
+                              0.0f, obj_weights_out ? nullptr : a.weights + (int64_t)r * S, lane, s_alpha, s_trans, s_sig);
+    // white background: rgb + 1 - opacity, models/rendering.py:178-179
+    const float rgb[3] = {a.white_back ? __fadd_rn(__fadd_rn(sc.r, 1.0f), -sc.opacity) : sc.r,
+                          a.white_back ? __fadd_rn(__fadd_rn(sc.g, 1.0f), -sc.opacity) : sc.g,
+                          a.white_back ? __fadd_rn(__fadd_rn(sc.b, 1.0f), -sc.opacity) : sc.b};
     if (lane == 0) {
       a.opacity[r] = sc.opacity;
       a.depth[r] = sc.depth;
-      // white background: rgb + 1 - opacity, models/rendering.py:178-179
-      a.rgb[r * 3 + 0] = a.white_back ? __fadd_rn(__fadd_rn(sc.r, 1.0f), -sc.opacity) : sc.r;
-      a.rgb[r * 3 + 1] = a.white_back ? __fadd_rn(__fadd_rn(sc.g, 1.0f), -sc.opacity) : sc.g;
-      a.rgb[r * 3 + 2] = a.white_back ? __fadd_rn(__fadd_rn(sc.b, 1.0f), -sc.opacity) : sc.b;
+      a.rgb[r * 3 + 0] = rgb[0];
+      a.rgb[r * 3 + 1] = rgb[1];
+      a.rgb[r * 3 + 2] = rgb[2];
+    }
+    Target tg;
+    if (kStep) {
+      tg = load_target(st.loss, r);
+      if (lane == 0) add_scene_sq(tg, rgb, sc.depth, sq, 1);
+      float gc[3], gd;
+      scene_grads(tg, rgb, sc.depth, scale, gc, gd);
+      __syncwarp();
+      composite_branch_grad(z, scene, S, scene_last_delta, false, 0.0f, a.white_back != 0, gc[0], gc[1], gc[2], gd, 0.0f,
+                            reinterpret_cast<float4*>(st.dscene) + (int64_t)r * S, s_alpha, s_trans, s_sig, s_gw, lane);
+      __syncwarp();
     }
     if (a.obj != nullptr) {
       bool use_mask = (!a.is_eval) && (a.frustum_bound_th > 0.0f);
       if (use_mask && a.pass_through_mask && a.pass_through_mask[r]) use_mask = false;
       const float z_limit = __fadd_rn(sc.depth, a.frustum_bound_th);
-      Acc ob = composite_branch(z, reinterpret_cast<const float4*>(a.obj) + (int64_t)r * S, S, 0.0f,
-                                a.noise_std, a.noise_obj ? a.noise_obj + (int64_t)r * S : nullptr, a.seed, 3u,
-                                r, use_mask, z_limit, obj_weights_out ? a.weights + (int64_t)r * S : nullptr,
-                                lane);
+      const float4* obj = reinterpret_cast<const float4*>(a.obj) + (int64_t)r * S;
+      Acc ob = composite_branch(z, obj, S, 0.0f, a.noise_std, a.noise_obj ? a.noise_obj + (int64_t)r * S : nullptr, a.seed,
+                                3u, r, use_mask, z_limit, obj_weights_out ? a.weights + (int64_t)r * S : nullptr, lane,
+                                s_alpha, s_trans, s_sig);
+      // always composited on white, models/rendering.py:223
+      const float irgb[3] = {__fadd_rn(__fadd_rn(ob.r, 1.0f), -ob.opacity), __fadd_rn(__fadd_rn(ob.g, 1.0f), -ob.opacity),
+                             __fadd_rn(__fadd_rn(ob.b, 1.0f), -ob.opacity)};
       if (lane == 0) {
         a.opacity_instance[r] = ob.opacity;
         a.depth_instance[r] = ob.depth;
-        // always composited on white, models/rendering.py:223
-        a.rgb_instance[r * 3 + 0] = __fadd_rn(__fadd_rn(ob.r, 1.0f), -ob.opacity);
-        a.rgb_instance[r * 3 + 1] = __fadd_rn(__fadd_rn(ob.g, 1.0f), -ob.opacity);
-        a.rgb_instance[r * 3 + 2] = __fadd_rn(__fadd_rn(ob.b, 1.0f), -ob.opacity);
+        a.rgb_instance[r * 3 + 0] = irgb[0];
+        a.rgb_instance[r * 3 + 1] = irgb[1];
+        a.rgb_instance[r * 3 + 2] = irgb[2];
+      }
+      if (kStep) {
+        if (lane == 0) add_object_sq(tg, ob.opacity, irgb, ob.depth, sq, 1);
+        float go, gi[3], gid;
+        object_grads(tg, ob.opacity, irgb, ob.depth, scale, go, gi, gid);
+        __syncwarp();
+        composite_branch_grad(z, obj, S, 0.0f, use_mask, z_limit, true, gi[0], gi[1], gi[2], gid, go,
+                              reinterpret_cast<float4*>(st.dobj) + (int64_t)r * S, s_alpha, s_trans, s_sig, s_gw, lane);
+        __syncwarp();
       }
     }
   }
+  if (!kStep) return;
+  __shared__ double red[8][N_TERMS];
+  if (lane == 0)
+    for (int t = 0; t < N_TERMS; ++t) red[warp][t] = sq[t];
+  __syncthreads();
+  if (threadIdx.x < N_TERMS) {
+    double v = 0.0;
+    for (int w = 0; w < warps_per_block; ++w) v += red[w][threadIdx.x];
+    if (v != 0.0) atomicAdd(st.acc + WS_SUM + 2 * threadIdx.x + st.fine, v);
+    __threadfence();
+  }
+  if (!st.finalize) return;
+  __shared__ bool last;
+  __syncthreads();
+  if (threadIdx.x == 0)
+    last = atomicAdd(reinterpret_cast<unsigned int*>(st.acc + WS_DOUBLES), 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!last || threadIdx.x != 0) return;
+  __threadfence();
+  double ws[WS_DOUBLES];
+  for (int i = 0; i < WS_DOUBLES; ++i) ws[i] = __ldcg(st.acc + i);
+  write_outputs(st.loss, ws);
+  // train.py:171-172: psnr of the last pass's rgb over the valid rays = -10 log10 of that pass's colour term
+  *st.psnr_out = (float)(-10.0 * log10(ws[WS_SUM + 2 * T_COLOR + st.fine] / ws[WS_COUNT + T_COLOR]));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -386,7 +467,23 @@ extern "C" int onerf_composite(onerf_ctx* ctx, const onerf_composite_args* a, vo
   int blocks = (a->n_rays + warps - 1) / warps;
   const int cap = ctx->num_sms * 8;
   if (blocks > cap) blocks = cap;
-  composite_kernel<<<blocks, warps * 32, 0, (cudaStream_t)stream>>>(*a);
+  onerf_step_composite none;
+  memset(&none, 0, sizeof(none));
+  composite_kernel<false><<<blocks, warps * 32, 0, (cudaStream_t)stream>>>(*a, none);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
+int onerf_launch_composite_step(onerf_ctx* ctx, const onerf_composite_args* a, const onerf_step_composite* t,
+                                cudaStream_t stream) {
+  ONERF_UNSUPPORTED(a->n_samples > 2048, "S > 2048");
+  if (a->n_rays == 0) return ONERF_OK;
+  const int warps = 4;
+  const size_t smem = (size_t)warps * 4 * a->n_samples * sizeof(float);
+  ONERF_CUDA(cudaFuncSetAttribute(composite_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int blocks = (a->n_rays + warps - 1) / warps;
+  if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
+  composite_kernel<true><<<blocks, warps * 32, smem, stream>>>(*a, *t);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

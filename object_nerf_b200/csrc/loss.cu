@@ -3,25 +3,39 @@
 // depth), each over the coarse and the fine maps; under autograd the reference runs ~120 elementwise / index / reduce
 // kernels and several host syncs (`mask.sum() == 0`) for 2 048 rays.  Here: one reduction pass (counts and weighted
 // squared-error sums, fp64 accumulators) and one pass that writes d(loss_sum)/d(map) for all ten maps and the loss values.
-#include "common.cuh"
+#include "loss_terms.cuh"
+#include "train_ws.h"
 
 namespace {
 
-enum { T_COLOR = 0, T_DEPTH, T_OPACITY, T_ICOLOR, T_IDEPTH, N_TERMS };
-// workspace (doubles): [0..5) mask counts per term (elements of the masked mean), [5] number of targets > 0,
-// [6..16) squared-error sums: term * 2 + (0 coarse / 1 fine)
-enum { WS_COUNT = 0, WS_TPOS = 5, WS_SUM = 6, WS_DOUBLES = 16 };
+using namespace loss_terms;
 
 struct LossParams {
   onerf_loss_args a;
 };
 
-__device__ __forceinline__ float clamp01(float x) { return fminf(fmaxf(x, 0.0f), 1.0f); }
-
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
   return v;
+}
+
+// Sums acc[0, n) over the block (256 threads) and adds the non-zero totals to ws[0, n).
+template <int n>
+__device__ __forceinline__ void block_accumulate(const double* acc, double* __restrict__ ws) {
+  __shared__ double sh[8][n];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int i = 0; i < n; ++i) {
+    const double v = warp_sum(acc[i]);
+    if (lane == 0) sh[warp][i] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < n) {
+    double v = 0.0;
+    for (int w8 = 0; w8 < 8; ++w8) v += sh[w8][threadIdx.x];
+    if (v != 0.0) atomicAdd(ws + threadIdx.x, v);
+  }
 }
 
 __global__ void __launch_bounds__(256) loss_reduce_kernel(LossParams P, double* __restrict__ ws) {
@@ -30,121 +44,59 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(LossParams P, double* 
 #pragma unroll
   for (int i = 0; i < WS_DOUBLES; ++i) acc[i] = 0.0;
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < a.n_rays; r += (int64_t)gridDim.x * blockDim.x) {
-    const bool valid = a.valid_mask[r] != 0, inst = a.instance_mask[r] != 0;
-    const float t = a.depths[r], w = a.instance_mask_weight[r];
-    const bool tpos = t > 0.0f;
-    const float tr = a.rgbs[3 * r], tg = a.rgbs[3 * r + 1], tb = a.rgbs[3 * r + 2];
-    if (tpos) acc[WS_TPOS] += 1.0;
-    if (valid) {
-      acc[WS_COUNT + T_COLOR] += 3.0;
-      acc[WS_COUNT + T_OPACITY] += 1.0;
-      if (tpos) acc[WS_COUNT + T_DEPTH] += 1.0;
-      if (inst) acc[WS_COUNT + T_ICOLOR] += 3.0;
-      if (inst && tpos) acc[WS_COUNT + T_IDEPTH] += 1.0;
-    }
+    const Target g = load_target(a, r);
+    add_counts(g, acc);
 #pragma unroll
     for (int f = 0; f < 2; ++f) {
       const onerf_loss_maps& m = f ? a.fine : a.coarse;
       if (f && !a.has_fine) break;
-      if (!valid) continue;
-      {
-        const float e0 = m.rgb[3 * r] - tr, e1 = m.rgb[3 * r + 1] - tg, e2 = m.rgb[3 * r + 2] - tb;
-        acc[WS_SUM + 2 * T_COLOR + f] += (double)(e0 * e0) + (double)(e1 * e1) + (double)(e2 * e2);
-      }
-      if (tpos) { const float e = m.depth[r] - t; acc[WS_SUM + 2 * T_DEPTH + f] += (double)(e * e); }
-      { const float e = clamp01(m.opacity_instance[r]) - (inst ? 1.0f : 0.0f); acc[WS_SUM + 2 * T_OPACITY + f] += (double)(e * e * w); }
-      if (inst) {
-        const float e0 = m.rgb_instance[3 * r] - tr, e1 = m.rgb_instance[3 * r + 1] - tg, e2 = m.rgb_instance[3 * r + 2] - tb;
-        acc[WS_SUM + 2 * T_ICOLOR + f] += (double)(e0 * e0 * w) + (double)(e1 * e1 * w) + (double)(e2 * e2 * w);
-        if (tpos) { const float e = m.depth_instance[r] - t; acc[WS_SUM + 2 * T_IDEPTH + f] += (double)(e * e * w); }
-      }
+      add_scene_sq(g, m.rgb + 3 * r, m.depth[r], acc + WS_SUM + f, 2);
+      add_object_sq(g, m.opacity_instance[r], m.rgb_instance + 3 * r, m.depth_instance[r], acc + WS_SUM + f, 2);
     }
   }
-  __shared__ double sh[8][WS_DOUBLES];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int i = 0; i < WS_DOUBLES; ++i) {
-    const double v = warp_sum(acc[i]);
-    if (lane == 0) sh[warp][i] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < WS_DOUBLES) {
-    double v = 0.0;
-    for (int w8 = 0; w8 < 8; ++w8) v += sh[w8][threadIdx.x];
-    if (v != 0.0) atomicAdd(ws + threadIdx.x, v);
-  }
+  block_accumulate<WS_DOUBLES>(acc, ws);
 }
 
-// term present (the reference returns None otherwise): models/losses.py:13-14, :46-47, :51-52, :80-81
-__device__ __forceinline__ bool term_present(const double* ws, int t) {
-  switch (t) {
-    case T_COLOR: return true;                                                   // never skipped (mean of an empty set = NaN)
-    case T_DEPTH: return ws[WS_TPOS] > 0;                                        // skipped only if no target depth at all
-    case T_OPACITY: return ws[WS_COUNT + T_OPACITY] > 0;
-    case T_ICOLOR: return ws[WS_COUNT + T_ICOLOR] > 0;
-    default: return ws[WS_TPOS] > 0 && ws[WS_COUNT + T_IDEPTH] > 0;
-  }
+// The counts half of loss_reduce_kernel: everything TotalLoss normalises by and skips on, from the batch alone.
+__global__ void __launch_bounds__(256) batch_stats_kernel(LossParams P, double* __restrict__ ws) {
+  const onerf_loss_args& a = P.a;
+  double acc[WS_SUM];
+#pragma unroll
+  for (int i = 0; i < WS_SUM; ++i) acc[i] = 0.0;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < a.n_rays; r += (int64_t)gridDim.x * blockDim.x)
+    add_counts(load_target(a, r), acc);
+  block_accumulate<WS_SUM>(acc, ws);
 }
 
 __global__ void __launch_bounds__(256) loss_grad_kernel(LossParams P, const double* __restrict__ ws) {
   const onerf_loss_args& a = P.a;
-  const float wt[N_TERMS] = {a.color_weight, a.depth_weight, a.opacity_weight, a.instance_color_weight, a.instance_depth_weight};
-  float scale[N_TERMS];   // d(weighted mean)/d(squared error) = weight / count
-  bool present[N_TERMS];
-#pragma unroll
-  for (int t = 0; t < N_TERMS; ++t) {
-    present[t] = term_present(ws, t);
-    scale[t] = present[t] ? (float)((double)wt[t] / ws[WS_COUNT + t]) : 0.0f;
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    double total = 0.0;
-    for (int t = 0; t < N_TERMS; ++t) {
-      // mean over the mask in fp32 like torch (sum / count), coarse + fine, times the weight
-      float v = 0.0f;
-      if (present[t]) {
-        v = (float)(ws[WS_SUM + 2 * t] / ws[WS_COUNT + t]);
-        if (a.has_fine) v += (float)(ws[WS_SUM + 2 * t + 1] / ws[WS_COUNT + t]);
-      }
-      a.terms_out[t] = v;                     // unweighted, as the reference's loss_dict (:129-131)
-      a.present_out[t] = present[t] ? 1 : 0;
-      if (present[t]) total += (double)(wt[t] * v);
-    }
-    *a.loss_sum_out = (float)total;
-  }
+  float scale[N_TERMS];
+  grad_scales(a, ws, scale);
+  if (blockIdx.x == 0 && threadIdx.x == 0) write_outputs(a, ws);
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < a.n_rays; r += (int64_t)gridDim.x * blockDim.x) {
-    const bool valid = a.valid_mask[r] != 0, inst = a.instance_mask[r] != 0;
-    const float t = a.depths[r], w = a.instance_mask_weight[r];
-    const bool tpos = t > 0.0f;
-    const float tr = a.rgbs[3 * r], tg = a.rgbs[3 * r + 1], tb = a.rgbs[3 * r + 2];
+    const Target g = load_target(a, r);
 #pragma unroll
     for (int f = 0; f < 2; ++f) {
       if (f && !a.has_fine) break;
       const onerf_loss_maps& m = f ? a.fine : a.coarse;
-      const onerf_loss_maps& g = f ? a.grad_fine : a.grad_coarse;
-      float gc[3] = {0.f, 0.f, 0.f}, gi[3] = {0.f, 0.f, 0.f}, gd = 0.f, go = 0.f, gid = 0.f;
-      if (valid) {
-        gc[0] = 2.0f * (m.rgb[3 * r] - tr) * scale[T_COLOR];
-        gc[1] = 2.0f * (m.rgb[3 * r + 1] - tg) * scale[T_COLOR];
-        gc[2] = 2.0f * (m.rgb[3 * r + 2] - tb) * scale[T_COLOR];
-        if (tpos) gd = 2.0f * (m.depth[r] - t) * scale[T_DEPTH];
-        const float o = m.opacity_instance[r];
-        if (o >= 0.0f && o <= 1.0f) go = 2.0f * (o - (inst ? 1.0f : 0.0f)) * w * scale[T_OPACITY];   // clamp backward
-        if (inst) {
-          gi[0] = 2.0f * (m.rgb_instance[3 * r] - tr) * w * scale[T_ICOLOR];
-          gi[1] = 2.0f * (m.rgb_instance[3 * r + 1] - tg) * w * scale[T_ICOLOR];
-          gi[2] = 2.0f * (m.rgb_instance[3 * r + 2] - tb) * w * scale[T_ICOLOR];
-          if (tpos) gid = 2.0f * (m.depth_instance[r] - t) * w * scale[T_IDEPTH];
-        }
-      }
-      float* grgb = const_cast<float*>(g.rgb);
-      float* girgb = const_cast<float*>(g.rgb_instance);
+      const onerf_loss_maps& gm = f ? a.grad_fine : a.grad_coarse;
+      float gc[3], gi[3], gd, go, gid;
+      scene_grads(g, m.rgb + 3 * r, m.depth[r], scale, gc, gd);
+      object_grads(g, m.opacity_instance[r], m.rgb_instance + 3 * r, m.depth_instance[r], scale, go, gi, gid);
+      float* grgb = const_cast<float*>(gm.rgb);
+      float* girgb = const_cast<float*>(gm.rgb_instance);
       grgb[3 * r] = gc[0]; grgb[3 * r + 1] = gc[1]; grgb[3 * r + 2] = gc[2];
       girgb[3 * r] = gi[0]; girgb[3 * r + 1] = gi[1]; girgb[3 * r + 2] = gi[2];
-      const_cast<float*>(g.depth)[r] = gd;
-      const_cast<float*>(g.opacity_instance)[r] = go;
-      const_cast<float*>(g.depth_instance)[r] = gid;
+      const_cast<float*>(gm.depth)[r] = gd;
+      const_cast<float*>(gm.opacity_instance)[r] = go;
+      const_cast<float*>(gm.depth_instance)[r] = gid;
     }
   }
+}
+
+int loss_grid(onerf_ctx* ctx, int64_t n_rays) {
+  const int64_t want = (n_rays + 255) / 256;
+  return (int)(want < (int64_t)ctx->num_sms * 4 ? want : (int64_t)ctx->num_sms * 4);
 }
 
 bool maps_ok(const onerf_loss_maps& m) { return m.rgb && m.depth && m.opacity_instance && m.rgb_instance && m.depth_instance; }
@@ -166,11 +118,18 @@ extern "C" int onerf_total_loss(onerf_ctx* ctx, const onerf_loss_args* a, void* 
   ONERF_CUDA(cudaMemsetAsync(ws, 0, WS_DOUBLES * sizeof(double), stream));
   LossParams P;
   P.a = *a;
-  const int64_t want = (a->n_rays + 255) / 256;
-  const int grid = (int)(want < (int64_t)ctx->num_sms * 4 ? want : (int64_t)ctx->num_sms * 4);
+  const int grid = loss_grid(ctx, a->n_rays);
   loss_reduce_kernel<<<grid, 256, 0, stream>>>(P, ws);
   ONERF_LAUNCH_CHECK(ctx);
   loss_grad_kernel<<<grid, 256, 0, stream>>>(P, ws);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
+int onerf_launch_batch_stats(onerf_ctx* ctx, const onerf_loss_args* a, double* ws, cudaStream_t stream) {
+  LossParams P;
+  P.a = *a;
+  batch_stats_kernel<<<loss_grid(ctx, a->n_rays), 256, 0, stream>>>(P, ws);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

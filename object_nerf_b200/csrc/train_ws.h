@@ -1,5 +1,7 @@
 // Layout of the training workspace of onerf_render_rays_fwd / onerf_render_rays_bwd (one caller-owned blob).
 #pragma once
+#include <cuda_runtime.h>
+
 #include "../../include/onerf.h"
 #include "layout.h"
 
@@ -61,3 +63,41 @@ static inline TrainWs onerf_make_train_ws(int precision, int use_voxel, int n_ra
   W.total = o;
   return W;
 }
+
+// onerf_train_step appends to the training workspace: the coarse pass's per-sample field gradients (the fine pass uses
+// TrainWs::dscene / dobj; both are written during the forward, before either field backward runs) and the loss
+// accumulators (loss_terms.cuh: WS_DOUBLES doubles, then the block counter of the last compositing kernel).
+struct TrainStepWs {
+  int64_t dscene_c, dobj_c, loss;
+  int64_t total;
+};
+#define ONERF_STEP_LOSS_BYTES 256
+
+static inline TrainStepWs onerf_make_train_step_ws(const TrainWs& W, int n_rays, int n_samples) {
+  TrainStepWs T;
+  int64_t o = W.total;
+  auto take = [&](int64_t bytes) { int64_t r = o; o += (bytes + 1023) & ~1023ll; return r; };
+  const int64_t Bc = (int64_t)n_rays * n_samples;
+  T.dscene_c = take(Bc * 16); T.dobj_c = take(Bc * 16);
+  T.loss = take(ONERF_STEP_LOSS_BYTES);
+  T.total = o;
+  return T;
+}
+
+// The training step's compositing kernel (composite.cu): forward, the loss terms this pass owns and the compositing
+// backward, per ray.
+struct onerf_step_composite {
+  onerf_loss_args loss;   // batch, term weights and (finalize) outputs; map and gradient pointers unused
+  double* acc;            // loss accumulators + block counter, counts already summed (onerf_launch_batch_stats)
+  int fine;               // 0 coarse, 1 fine: which squared-error sums this pass adds to
+  int finalize;           // last compositing kernel of the step: its last block writes the loss outputs and psnr
+  float* psnr_out;
+  float* dscene;          // (N,S,4) d(r, g, b, sigma) of the scene branch
+  float* dobj;            // (N,S,4) of the object branch
+};
+int onerf_launch_composite_step(onerf_ctx* ctx, const onerf_composite_args* c, const onerf_step_composite* t,
+                                cudaStream_t stream);
+int onerf_launch_batch_stats(onerf_ctx* ctx, const onerf_loss_args* a, double* acc, cudaStream_t stream);
+// onerf_render_rays_fwd with an optional training step: step == NULL is the plain forward; otherwise both passes'
+// compositing runs onerf_launch_composite_step with `step` (fine / finalize / dscene / dobj set per pass from ws_step).
+int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const onerf_step_composite* step, void* stream);
