@@ -57,6 +57,19 @@ size_t onerf_train_step_workspace_bytes(int precision, int use_voxel, int n_rays
 int onerf_train_step(onerf_ctx* ctx, const onerf_render_args* fwd, const onerf_loss_args* loss,
                      const onerf_render_bwd_args* bwd, float* psnr_out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Device seed.  As onerf_render_rays_fwd / onerf_train_step, with args->seed ignored: every draw the call makes without
+ * an injected buffer (jitter, u, noise_*) uses the seed *seed_dev holds when its kernel runs, exactly as the host-seed
+ * call with args->seed = *seed_dev draws, and the call's last device work adds 4 to *seed_dev (also when nothing is
+ * drawn).  seed_dev: one uint64 in device memory, 8-byte aligned.  Kernels only: CUDA-graph capturable, and each replay
+ * draws with the next seed (replay k of a graph captured with *seed_dev = s0 draws as the host-seed call with s0 + 4k).
+ * onerf_render_rays_fwd_dseed refuses train_ws != NULL (ONERF_ERR_BAD_ARG): onerf_render_rays_bwd replays the sigma noise
+ * from the host seed.
+ * ------------------------------------------------------------------------------------------- */
+int onerf_render_rays_fwd_dseed(onerf_ctx* ctx, const onerf_render_args* args, uint64_t* seed_dev, void* stream);
+int onerf_train_step_dseed(onerf_ctx* ctx, const onerf_render_args* fwd, const onerf_loss_args* loss,
+                           const onerf_render_bwd_args* bwd, float* psnr_out, uint64_t* seed_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -36,7 +36,8 @@ EXPORTS = [
 ]
 # additions to ABI version 2 declared in include/onerf_ext.h
 EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_ws", "onerf_composite_multi_merge",
-               "onerf_train_workspace_bytes_prec", "onerf_train_step_workspace_bytes", "onerf_train_step"]
+               "onerf_train_workspace_bytes_prec", "onerf_train_step_workspace_bytes", "onerf_train_step",
+               "onerf_render_rays_fwd_dseed", "onerf_train_step_dseed"]
 
 _p = C.c_void_p
 
@@ -222,6 +223,9 @@ def load() -> C.CDLL:
         lib.onerf_train_step_workspace_bytes.argtypes = [C.c_int] * 5
         lib.onerf_train_step_workspace_bytes.restype = C.c_size_t
         lib.onerf_train_step.argtypes = [_p, C.POINTER(RenderArgs), C.POINTER(LossArgs), C.POINTER(RenderBwdArgs), _p, _p]
+        lib.onerf_render_rays_fwd_dseed.argtypes = [_p, C.POINTER(RenderArgs), _p, _p]
+        lib.onerf_train_step_dseed.argtypes = [_p, C.POINTER(RenderArgs), C.POINTER(LossArgs), C.POINTER(RenderBwdArgs), _p,
+                                               _p, _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

@@ -137,7 +137,7 @@ extern "C" size_t onerf_render_rays_workspace_bytes(int n_rays, int n_samples, i
 static int render_pass(onerf_ctx* ctx, const onerf_render_args* a, const void* packed, const float* z, int S,
                        const onerf_render_maps& m, const float* noise_scene, const float* noise_obj, uint64_t seed,
                        float* ray_const, float* scene, float* obj, void* train_ws, const onerf_step_composite* step,
-                       void* stream) {
+                       uint64_t* seed_dev, void* stream) {
   onerf_field_args f;
   memset(&f, 0, sizeof(f));
   f.train_ws = train_ws;
@@ -161,8 +161,8 @@ static int render_pass(onerf_ctx* ctx, const onerf_render_args* a, const void* p
   c.pass_through_mask = a->pass_through_mask;
   c.weights = m.weights; c.opacity = m.opacity; c.rgb = m.rgb; c.depth = m.depth;
   c.rgb_instance = m.rgb_instance; c.depth_instance = m.depth_instance; c.opacity_instance = m.opacity_instance;
-  if (step) return onerf_launch_composite_step(ctx, &c, step, (cudaStream_t)stream);
-  return onerf_composite(ctx, &c, stream);
+  if (step) return onerf_launch_composite_step(ctx, &c, step, seed_dev, (cudaStream_t)stream);
+  return onerf_launch_composite(ctx, &c, seed_dev, (cudaStream_t)stream);
 }
 
 static bool maps_ok(const onerf_render_maps& m, int forward_instance) {
@@ -171,10 +171,20 @@ static bool maps_ok(const onerf_render_maps& m, int forward_instance) {
 }
 
 extern "C" int onerf_render_rays_fwd(onerf_ctx* ctx, const onerf_render_args* a, void* stream) {
-  return onerf_render_fwd_impl(ctx, a, nullptr, stream);
+  return onerf_render_fwd_impl(ctx, a, nullptr, nullptr, stream);
 }
 
-int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const onerf_step_composite* step, void* stream) {
+extern "C" int onerf_render_rays_fwd_dseed(onerf_ctx* ctx, const onerf_render_args* a, uint64_t* seed_dev, void* stream) {
+  ONERF_CHECK_ARG(ctx && a && seed_dev, "null argument");
+  ONERF_CHECK_ARG((reinterpret_cast<uintptr_t>(seed_dev) & 7u) == 0, "seed_dev must be 8-byte aligned");
+  ONERF_CHECK_ARG(!a->train_ws, "train_ws is refused: onerf_render_rays_bwd replays the noise from the host seed");
+  const int rc = onerf_render_fwd_impl(ctx, a, nullptr, seed_dev, stream);
+  if (rc != ONERF_OK) return rc;
+  return onerf_launch_seed_advance(ctx, seed_dev, (cudaStream_t)stream);
+}
+
+int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const onerf_step_composite* step, uint64_t* seed_dev,
+                          void* stream) {
   ONERF_CHECK_ARG(ctx && a, "null argument");
   ONERF_CHECK_ARG(a->rays && a->packed_coarse, "null rays / packed_coarse");
   ONERF_CHECK_ARG(a->n_rays >= 0 && a->n_samples >= 2 && a->n_importance >= 0, "bad shape");
@@ -226,17 +236,20 @@ int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const oner
     step_f.fine = 1; step_f.finalize = 1;
     step_f.dscene = reinterpret_cast<float*>(t + W.dscene); step_f.dobj = reinterpret_cast<float*>(t + W.dobj);
   }
-  // seeds: coarse depths, coarse noise, importance u, fine noise (rendering.py::_render_forward)
-  int rc = onerf_sample_coarse(ctx, a->rays, a->n_rays, S, a->use_disp, a->perturb, a->jitter, a->seed, a->coarse.z_vals, stream);
+  // seeds: coarse depths, coarse noise, importance u, fine noise (rendering.py::_render_forward); with seed_dev the kernels
+  // add *seed_dev to these offsets
+  const uint64_t seed = seed_dev ? 0 : a->seed;
+  int rc = onerf_launch_sample_coarse(ctx, a->rays, a->n_rays, S, a->use_disp, a->perturb, a->jitter, seed, seed_dev,
+                                      a->coarse.z_vals, stream);
   if (rc != ONERF_OK) return rc;
   rc = render_pass(ctx, a, a->packed_coarse, a->coarse.z_vals, S, a->coarse, a->noise_scene_coarse, a->noise_obj_coarse,
-                   a->seed + 1, ray_const, scene_c, obj_c, tl_c, step ? &step_c : nullptr, stream);
+                   seed + 1, ray_const, scene_c, obj_c, tl_c, step ? &step_c : nullptr, seed_dev, stream);
   if (rc != ONERF_OK || a->n_importance == 0) return rc;
-  rc = onerf_sample_pdf_merge(ctx, a->coarse.z_vals, a->coarse.weights, a->n_rays, S, a->n_importance, a->perturb == 0.0f ? 1 : 0,
-                              a->u, a->seed + 2, a->fine.z_vals, stream);
+  rc = onerf_launch_sample_pdf_merge(ctx, a->coarse.z_vals, a->coarse.weights, a->n_rays, S, a->n_importance,
+                                     a->perturb == 0.0f ? 1 : 0, a->u, seed + 2, seed_dev, a->fine.z_vals, stream);
   if (rc != ONERF_OK) return rc;
-  return render_pass(ctx, a, a->packed_fine, a->fine.z_vals, SF, a->fine, a->noise_scene_fine, a->noise_obj_fine, a->seed + 3,
-                     ray_const, scene_f, obj_f, tl_f, step ? &step_f : nullptr, stream);
+  return render_pass(ctx, a, a->packed_fine, a->fine.z_vals, SF, a->fine, a->noise_scene_fine, a->noise_obj_fine, seed + 3,
+                     ray_const, scene_f, obj_f, tl_f, step ? &step_f : nullptr, seed_dev, stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -324,8 +324,8 @@ extern "C" size_t onerf_train_step_workspace_bytes(int precision, int use_voxel,
   return (size_t)onerf_make_train_step_ws(W, n_rays, n_samples).total;
 }
 
-extern "C" int onerf_train_step(onerf_ctx* ctx, const onerf_render_args* f, const onerf_loss_args* l,
-                                const onerf_render_bwd_args* b, float* psnr_out, void* stream) {
+static int train_step(onerf_ctx* ctx, const onerf_render_args* f, const onerf_loss_args* l, const onerf_render_bwd_args* b,
+                      float* psnr_out, uint64_t* seed_dev, void* stream) {
   ONERF_CHECK_ARG(ctx && f && l && b && psnr_out, "null argument");
   int rc = check_bwd_args(f, b);
   if (rc != ONERF_OK) return rc;
@@ -351,7 +351,20 @@ extern "C" int onerf_train_step(onerf_ctx* ctx, const onerf_render_args* f, cons
   step.loss = *l;
   step.acc = acc;
   step.psnr_out = psnr_out;
-  rc = onerf_render_fwd_impl(ctx, f, &step, stream);
+  // the finalizing compositing kernel advances *seed_dev: the field backward draws nothing
+  rc = onerf_render_fwd_impl(ctx, f, &step, seed_dev, stream);
   if (rc != ONERF_OK) return rc;
   return render_bwd(ctx, f, b, W, &T, stream);
+}
+
+extern "C" int onerf_train_step(onerf_ctx* ctx, const onerf_render_args* f, const onerf_loss_args* l,
+                                const onerf_render_bwd_args* b, float* psnr_out, void* stream) {
+  return train_step(ctx, f, l, b, psnr_out, nullptr, stream);
+}
+
+extern "C" int onerf_train_step_dseed(onerf_ctx* ctx, const onerf_render_args* f, const onerf_loss_args* l,
+                                      const onerf_render_bwd_args* b, float* psnr_out, uint64_t* seed_dev, void* stream) {
+  ONERF_CHECK_ARG(seed_dev, "null seed_dev");
+  ONERF_CHECK_ARG((reinterpret_cast<uintptr_t>(seed_dev) & 7u) == 0, "seed_dev must be 8-byte aligned");
+  return train_step(ctx, f, l, b, psnr_out, seed_dev, stream);
 }

@@ -100,14 +100,17 @@ __device__ __forceinline__ Acc composite_branch(const float* __restrict__ z, con
 // maps (loss_terms.cuh; the normalisers depend on the batch only, so they are known before the render), then the
 // compositing backward of both branches on the alpha / transmittance the forward left in shared memory
 // (composite_bwd.cuh).  Per-block sums of the squared errors go to the fp64 accumulators; with `finalize` the last block
-// to finish turns them into the loss outputs and the PSNR.
+// to finish turns them into the loss outputs and the PSNR, and advances *seed_dev (train_ws.h: device seed), which every
+// block has read by then.
 template <bool kStep>
-__global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, onerf_step_composite st) {
+__global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, onerf_step_composite st, uint64_t* seed_dev) {
   using namespace loss_terms;
   extern __shared__ float smem_c[];
   const int warps_per_block = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = a.n_samples;
+  uint64_t seed = a.seed;
+  if (seed_dev && a.noise_std > 0.0f) seed += *seed_dev;
   float *s_alpha = nullptr, *s_trans = nullptr, *s_sig = nullptr, *s_gw = nullptr;
   double sq[N_TERMS] = {0.0, 0.0, 0.0, 0.0, 0.0};   // lane 0: squared-error sums of this warp's rays
   float scale[N_TERMS];
@@ -124,7 +127,7 @@ __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, 
     const float scene_last_delta = a.zero_last_delta ? 0.0f : 1e10f;
     const float4* scene = reinterpret_cast<const float4*>(a.scene) + (int64_t)r * S;
     Acc sc = composite_branch(z, scene, S, scene_last_delta, a.noise_std,
-                              a.noise_scene ? a.noise_scene + (int64_t)r * S : nullptr, a.seed, 2u, r, false,
+                              a.noise_scene ? a.noise_scene + (int64_t)r * S : nullptr, seed, 2u, r, false,
                               0.0f, obj_weights_out ? nullptr : a.weights + (int64_t)r * S, lane, s_alpha, s_trans, s_sig);
     // white background: rgb + 1 - opacity, models/rendering.py:178-179
     const float rgb[3] = {a.white_back ? __fadd_rn(__fadd_rn(sc.r, 1.0f), -sc.opacity) : sc.r,
@@ -153,7 +156,7 @@ __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, 
       if (use_mask && a.pass_through_mask && a.pass_through_mask[r]) use_mask = false;
       const float z_limit = __fadd_rn(sc.depth, a.frustum_bound_th);
       const float4* obj = reinterpret_cast<const float4*>(a.obj) + (int64_t)r * S;
-      Acc ob = composite_branch(z, obj, S, 0.0f, a.noise_std, a.noise_obj ? a.noise_obj + (int64_t)r * S : nullptr, a.seed,
+      Acc ob = composite_branch(z, obj, S, 0.0f, a.noise_std, a.noise_obj ? a.noise_obj + (int64_t)r * S : nullptr, seed,
                                 3u, r, use_mask, z_limit, obj_weights_out ? a.weights + (int64_t)r * S : nullptr, lane,
                                 s_alpha, s_trans, s_sig);
       // always composited on white, models/rendering.py:223
@@ -201,7 +204,11 @@ __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, 
   write_outputs(st.loss, ws);
   // train.py:171-172: psnr of the last pass's rgb over the valid rays = -10 log10 of that pass's colour term
   *st.psnr_out = (float)(-10.0 * log10(ws[WS_SUM + 2 * T_COLOR + st.fine] / ws[WS_COUNT + T_COLOR]));
+  if (seed_dev) *seed_dev += ONERF_SEED_ADVANCE;
 }
+
+// The forward-only call's last device work (onerf_render_rays_fwd_dseed).
+__global__ void seed_advance_kernel(uint64_t* seed_dev) { *seed_dev += ONERF_SEED_ADVANCE; }
 
 // ---------------------------------------------------------------------------------------------
 // multi-object: joint stable sort by depth, then composite (last delta = 0)
@@ -457,6 +464,16 @@ merge_composite_kernel(const float4* __restrict__ field_all, int n_rays, int n_o
 }  // namespace
 
 extern "C" int onerf_composite(onerf_ctx* ctx, const onerf_composite_args* a, void* stream) {
+  return onerf_launch_composite(ctx, a, nullptr, (cudaStream_t)stream);
+}
+
+int onerf_launch_seed_advance(onerf_ctx* ctx, uint64_t* seed_dev, cudaStream_t stream) {
+  seed_advance_kernel<<<1, 1, 0, stream>>>(seed_dev);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
+int onerf_launch_composite(onerf_ctx* ctx, const onerf_composite_args* a, uint64_t* seed_dev, cudaStream_t stream) {
   ONERF_CHECK_ARG(ctx && a, "null argument");
   ONERF_CHECK_ARG(a->z && a->scene && a->weights && a->opacity && a->rgb && a->depth, "null buffer");
   ONERF_CHECK_ARG(a->n_rays >= 0 && a->n_samples >= 1, "bad shape");
@@ -469,13 +486,13 @@ extern "C" int onerf_composite(onerf_ctx* ctx, const onerf_composite_args* a, vo
   if (blocks > cap) blocks = cap;
   onerf_step_composite none;
   memset(&none, 0, sizeof(none));
-  composite_kernel<false><<<blocks, warps * 32, 0, (cudaStream_t)stream>>>(*a, none);
+  composite_kernel<false><<<blocks, warps * 32, 0, stream>>>(*a, none, seed_dev);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }
 
 int onerf_launch_composite_step(onerf_ctx* ctx, const onerf_composite_args* a, const onerf_step_composite* t,
-                                cudaStream_t stream) {
+                                uint64_t* seed_dev, cudaStream_t stream) {
   ONERF_UNSUPPORTED(a->n_samples > 2048, "S > 2048");
   if (a->n_rays == 0) return ONERF_OK;
   const int warps = 4;
@@ -483,7 +500,7 @@ int onerf_launch_composite_step(onerf_ctx* ctx, const onerf_composite_args* a, c
   ONERF_CUDA(cudaFuncSetAttribute(composite_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int blocks = (a->n_rays + warps - 1) / warps;
   if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
-  composite_kernel<true><<<blocks, warps * 32, smem, stream>>>(*a, *t);
+  composite_kernel<true><<<blocks, warps * 32, smem, stream>>>(*a, *t, seed_dev);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

@@ -3,6 +3,7 @@
 //
 // Reference behaviour: models/rendering.py:259-277 (stratified), :11-61 (sample_pdf), :301-313 (merge).
 #include "common.cuh"
+#include "train_ws.h"
 
 namespace {
 
@@ -23,9 +24,11 @@ __device__ __forceinline__ float coarse_depth(float near, float far, int i, int 
   return __fdiv_rn(1.0f, __fadd_rn(a, b));
 }
 
+// seed_dev != null: the draws use seed + *seed_dev (the caller passes only the offset in `seed`); see onerf_ext.h
 __global__ void __launch_bounds__(256)
 sample_coarse_kernel(const float* __restrict__ rays, int n_rays, int S, int use_disp, float perturb,
-                     const float* __restrict__ jitter, uint64_t seed, float* __restrict__ z_out) {
+                     const float* __restrict__ jitter, uint64_t seed, const uint64_t* seed_dev, float* __restrict__ z_out) {
+  if (seed_dev && perturb > 0.0f && !jitter) seed += *seed_dev;
   const int64_t total = (int64_t)n_rays * S;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total;
        e += (int64_t)gridDim.x * blockDim.x) {
@@ -67,10 +70,12 @@ __device__ __forceinline__ double warp_scan_add(double v, int lane) {
 __global__ void __launch_bounds__(256)
 sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restrict__ weights, int n_rays,
                         int S, int K, int P, int det, const float* __restrict__ u_in, uint64_t seed,
-                        float* __restrict__ z_out, const float* __restrict__ bins_in) {
+                        const uint64_t* seed_dev, float* __restrict__ z_out, const float* __restrict__ bins_in) {
   // bins_in != null: stand-alone sample_pdf on explicit bins (N, S-1) and weights (N, S-2): no merge,
   // z_out (N, K) in draw order.  Otherwise the fused form on coarse depths / full coarse weights.
+  // seed_dev != null: as in sample_coarse_kernel.
   extern __shared__ float smem[];
+  if (seed_dev && !det && !u_in) seed += *seed_dev;
   const int warps_per_block = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int per_warp = 2 * S + P;
@@ -155,9 +160,8 @@ sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restr
 
 }  // namespace
 
-extern "C" int onerf_sample_coarse(onerf_ctx* ctx, const float* rays, int n_rays, int n_samples,
-                                   int use_disp, float perturb, const float* jitter, uint64_t seed,
-                                   float* z_out, void* stream) {
+int onerf_launch_sample_coarse(onerf_ctx* ctx, const float* rays, int n_rays, int n_samples, int use_disp, float perturb,
+                               const float* jitter, uint64_t seed, const uint64_t* seed_dev, float* z_out, void* stream) {
   ONERF_CHECK_ARG(ctx && rays && z_out, "null argument");
   ONERF_CHECK_ARG(n_rays >= 0 && n_samples >= 1, "bad shape");
   if (n_rays == 0) return ONERF_OK;
@@ -166,14 +170,27 @@ extern "C" int onerf_sample_coarse(onerf_ctx* ctx, const float* rays, int n_rays
   const int cap = ctx->num_sms * 16;
   if (blocks > cap) blocks = cap;
   sample_coarse_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(rays, n_rays, n_samples, use_disp, perturb,
-                                                                 jitter, seed, z_out);
+                                                                 jitter, seed, seed_dev, z_out);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
+}
+
+extern "C" int onerf_sample_coarse(onerf_ctx* ctx, const float* rays, int n_rays, int n_samples,
+                                   int use_disp, float perturb, const float* jitter, uint64_t seed,
+                                   float* z_out, void* stream) {
+  return onerf_launch_sample_coarse(ctx, rays, n_rays, n_samples, use_disp, perturb, jitter, seed, nullptr, z_out, stream);
 }
 
 extern "C" int onerf_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, const float* weights,
                                       int n_rays, int n_samples, int n_importance, int det, const float* u,
                                       uint64_t seed, float* z_out, void* stream) {
+  return onerf_launch_sample_pdf_merge(ctx, z_coarse, weights, n_rays, n_samples, n_importance, det, u, seed, nullptr, z_out,
+                                       stream);
+}
+
+int onerf_launch_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, const float* weights, int n_rays, int n_samples,
+                                  int n_importance, int det, const float* u, uint64_t seed, const uint64_t* seed_dev,
+                                  float* z_out, void* stream) {
   ONERF_CHECK_ARG(ctx && z_coarse && weights && z_out, "null argument");
   ONERF_CHECK_ARG(n_rays >= 0 && n_samples >= 3 && n_importance >= 1, "bad shape (need S >= 3, K >= 1)");
   ONERF_UNSUPPORTED(n_samples + n_importance > 2048, "S + K > 2048");
@@ -187,7 +204,7 @@ extern "C" int onerf_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, con
   const int cap = ctx->num_sms * 8;
   if (blocks > cap) blocks = cap;
   sample_pdf_merge_kernel<<<blocks, warps * 32, smem, (cudaStream_t)stream>>>(
-      z_coarse, weights, n_rays, n_samples, n_importance, P, det, u, seed, z_out, nullptr);
+      z_coarse, weights, n_rays, n_samples, n_importance, P, det, u, seed, seed_dev, z_out, nullptr);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }
@@ -209,7 +226,7 @@ extern "C" int onerf_sample_pdf(onerf_ctx* ctx, const float* bins, const float* 
   const int cap = ctx->num_sms * 8;
   if (blocks > cap) blocks = cap;
   sample_pdf_merge_kernel<<<blocks, warps * 32, smem, (cudaStream_t)stream>>>(
-      nullptr, weights, n_rays, S, n_importance, P, det, u, seed, out, bins);
+      nullptr, weights, n_rays, S, n_importance, P, det, u, seed, nullptr, out, bins);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

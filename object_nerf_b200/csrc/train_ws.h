@@ -95,9 +95,23 @@ struct onerf_step_composite {
   float* dscene;          // (N,S,4) d(r, g, b, sigma) of the scene branch
   float* dobj;            // (N,S,4) of the object branch
 };
+// Device seed (onerf_ext.h: onerf_render_rays_fwd_dseed, onerf_train_step_dseed): every launcher below that takes
+// `seed_dev` draws with seed + *seed_dev read when its kernel runs if seed_dev != NULL (the caller then passes only the
+// per-draw offset in `seed`), and with `seed` alone otherwise.  With finalize set, the step's compositing kernel adds
+// ONERF_SEED_ADVANCE to *seed_dev once every block has read it.
+#define ONERF_SEED_ADVANCE 4
 int onerf_launch_composite_step(onerf_ctx* ctx, const onerf_composite_args* c, const onerf_step_composite* t,
-                                cudaStream_t stream);
+                                uint64_t* seed_dev, cudaStream_t stream);
+int onerf_launch_composite(onerf_ctx* ctx, const onerf_composite_args* c, uint64_t* seed_dev, cudaStream_t stream);
+int onerf_launch_seed_advance(onerf_ctx* ctx, uint64_t* seed_dev, cudaStream_t stream);   // one thread: *seed_dev += 4
+int onerf_launch_sample_coarse(onerf_ctx* ctx, const float* rays, int n_rays, int n_samples, int use_disp, float perturb,
+                               const float* jitter, uint64_t seed, const uint64_t* seed_dev, float* z_out, void* stream);
+int onerf_launch_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, const float* weights, int n_rays, int n_samples,
+                                  int n_importance, int det, const float* u, uint64_t seed, const uint64_t* seed_dev,
+                                  float* z_out, void* stream);
 int onerf_launch_batch_stats(onerf_ctx* ctx, const onerf_loss_args* a, double* acc, cudaStream_t stream);
 // onerf_render_rays_fwd with an optional training step: step == NULL is the plain forward; otherwise both passes'
-// compositing runs onerf_launch_composite_step with `step` (fine / finalize / dscene / dobj set per pass from ws_step).
-int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const onerf_step_composite* step, void* stream);
+// compositing runs onerf_launch_composite_step with `step` (fine / finalize / dscene / dobj set per pass from ws_step),
+// and the finalizing one advances *seed_dev.  seed_dev as above; a->seed is ignored when it is set.
+int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const onerf_step_composite* step, uint64_t* seed_dev,
+                          void* stream);

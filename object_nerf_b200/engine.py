@@ -438,8 +438,17 @@ class RenderPlan:
             a.train_ws, a.train_ws_bytes = train_ws.data_ptr(), train_ws.numel()
         self.args = a
 
-    def run(self):
-        """Enqueue the forward on the current stream; returns the reference's result dict (views of the plan's buffers)."""
+    def run(self, seed_dev: Optional[torch.Tensor] = None):
+        """Enqueue the forward on the current stream; returns the reference's result dict (views of the plan's buffers).
+        seed_dev: a one-element int64 tensor on the plan's device holding the Philox seed; the draws then use the value it
+        holds when the kernels run instead of args.seed, and the call adds 4 to it (onerf_render_rays_fwd_dseed), so
+        every replay of a captured run draws fresh numbers."""
         with torch.cuda.device(self.rays.device):
-            _lib.check(_lib.load().onerf_render_rays_fwd(_lib.ctx(self.rays.device), C.byref(self.args), _lib.stream()))
+            ctx, lib = _lib.ctx(self.rays.device), _lib.load()
+            if seed_dev is None:
+                _lib.check(lib.onerf_render_rays_fwd(ctx, C.byref(self.args), _lib.stream()))
+            else:
+                if seed_dev.dtype != torch.int64 or seed_dev.numel() != 1 or seed_dev.device != self.rays.device:
+                    raise ValueError("seed_dev must be a one-element int64 tensor on the plan's device")
+                _lib.check(lib.onerf_render_rays_fwd_dseed(ctx, C.byref(self.args), seed_dev.data_ptr(), _lib.stream()))
         return {f"{k}_{typ}": v for typ, m in self.maps.items() for k, v in m.items()}

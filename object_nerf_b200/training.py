@@ -10,12 +10,18 @@ CUDA graph together with `torch.optim.Adam(..., capturable=True)` and replayed. 
 steps (`optimizer.zero_grad(set_to_none=False)`): a missing `.grad` is created (zero-filled) on the call that finds it
 missing.
 
-A replay repeats what the capture saw on the host, in particular:
-  - the voxel grid's buffers.  Grid maintenance (EmbeddingVoxel.voxel_subdivision, .self_pruning_empty_voxels) replaces
-    or reshapes them, so recapture the graph after it; eager calls pick the current grid up on every call;
-  - the Philox seed of the random draws (stratified jitter, importance u, sigma noise), so every replay draws the same
-    numbers.  For fresh draws per replay pass `_rand` buffers and refill them inside the captured region with torch's
-    generator (`torch.rand(..., out=...)`, `torch.randn(..., out=...)`), which advances on every replay.
+A replay repeats what the capture saw on the host, in particular the voxel grid's buffers.  Grid maintenance
+(EmbeddingVoxel.voxel_subdivision, .self_pruning_empty_voxels) replaces or reshapes them, so recapture the graph after
+it; eager calls pick the current grid up on every call.
+
+The random draws (stratified jitter, importance u, sigma noise) are fresh on every replay.  An eager call draws a new
+Philox seed from torch's generator (`engine.new_seed`) and passes it by value (onerf_train_step).  A call made while
+the current stream is capturing runs onerf_train_step_dseed instead: its kernels read the seed from the plan's device
+counter `seed_dev` when they run, and the step's last compositing kernel adds 4 to it.  Replay k of a graph captured
+with the counter at s0 therefore draws exactly what an eager step with seed s0 + 4k draws.  The counter is written once,
+when the plan is made, with the seed of that (eager) first call plus 4; `step_seed` reads it.  The first call for a
+configuration must therefore run eagerly (the usual warm-up before a capture): a plan made inside a capture would have
+its counter reset on every replay, so that is refused.  Injected `_rand` buffers take precedence over either seed.
 
 The returned tensors are the plan's output buffers and are overwritten by the next step of the same plan.
 """
@@ -30,7 +36,7 @@ import torch
 from . import _lib, backward, engine
 from .losses import TERMS
 
-__all__ = ["train_step"]
+__all__ = ["train_step", "step_seed"]
 
 _RAND_KEYS = ("jitter", "u", "noise_scene_coarse", "noise_obj_coarse", "noise_scene_fine", "noise_obj_fine")
 # coarse model -> {configuration: plan}; a plan references no module, so it lives exactly as long as the model
@@ -44,9 +50,11 @@ def _is_voxel(emb) -> bool:
 class _StepPlan:
     """Every buffer one configuration of the step needs, allocated once."""
 
-    def __init__(self, models, emb_xyz, n, cfg, rand, dev):
+    def __init__(self, models, emb_xyz, n, cfg, rand, dev, seed):
         lib = _lib.load()
         self.n, self.dev, self.cfg = n, dev, cfg
+        # the device seed of captured steps (onerf_train_step_dseed), continuing from the creating call's host seed
+        self.seed_dev = torch.full((1,), seed + 4, dtype=torch.int64, device=dev)
         self.model_order = ["coarse"] + (["fine"] if cfg["N_importance"] > 0 else [])
         self.use_voxel = _is_voxel(emb_xyz)
         f = lambda *shape, dtype=torch.float32: torch.empty(*shape, dtype=dtype, device=dev)
@@ -80,6 +88,20 @@ class _StepPlan:
          la.instance_depth_weight) = cfg["loss_weights"]
         la.loss_sum_out, la.terms_out, la.present_out = self.out.data_ptr(), self.out[1:].data_ptr(), self.present.data_ptr()
         self.loss_args = la
+
+
+def _capturing(dev) -> bool:
+    return dev.type == "cuda" and torch.cuda.is_current_stream_capturing()
+
+
+def step_seed(models: Dict[str, Any]) -> torch.Tensor:
+    """A copy of the device seed counter of the model's train_step plan (one int64 on the device): the Philox seed the
+    next captured step's replay draws with.  Taken inside a captured region, the copy is made on every replay.  The
+    model must have exactly one plan (one train_step configuration)."""
+    plans = list(_plans.get(models["coarse"], {}).values())
+    if len(plans) != 1:
+        raise ValueError(f"step_seed needs exactly one train_step plan for this model, found {len(plans)}")
+    return plans[0].seed_dev.clone()
 
 
 def _grad_of(p: torch.Tensor) -> torch.Tensor:
@@ -127,10 +149,15 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
     table = emb_xyz.embedding_space_ftr.weight if use_voxel else None
     key = (dev, n, use_voxel, tuple(sorted(cfg.items())),
            tuple(rand[k].data_ptr() if rand.get(k) is not None else 0 for k in _RAND_KEYS))
+    capturing = _capturing(dev)
+    seed = engine.new_seed() if not capturing and (cfg["perturb"] > 0 or cfg["noise_std"] > 0) else 0
     plans = _plans.setdefault(models["coarse"], {})
     plan = plans.get(key)
     if plan is None:
-        plan = plans[key] = _StepPlan(models, emb_xyz, n, cfg, rand, dev)
+        if capturing:
+            raise RuntimeError("train_step: the first call for a configuration must run before the CUDA-graph capture "
+                               "(warm up eagerly): its plan's device seed counter would be reset on every replay")
+        plan = plans[key] = _StepPlan(models, emb_xyz, n, cfg, rand, dev, seed)
     # the grid as it is now (host-side argument block only)
     plan.grid = engine.GridBuffers.from_module(emb_xyz) if use_voxel else None
     plan.render.args.grid = C.pointer(plan.grid.c) if use_voxel else None
@@ -167,8 +194,13 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
         b.d_codes = plan.d_codes.data_ptr()
         b.table_grad = _grad_of(table).data_ptr() if table is not None else None
         a = plan.render.args
-        a.seed = engine.new_seed() if (cfg["perturb"] > 0 or cfg["noise_std"] > 0) else 0
-        _lib.check(lib.onerf_train_step(ctx, C.byref(a), C.byref(plan.loss_args), C.byref(b), plan.psnr.data_ptr(), stream))
+        if capturing:
+            _lib.check(lib.onerf_train_step_dseed(ctx, C.byref(a), C.byref(plan.loss_args), C.byref(b),
+                                                  plan.psnr.data_ptr(), plan.seed_dev.data_ptr(), stream))
+        else:
+            a.seed = seed
+            _lib.check(lib.onerf_train_step(ctx, C.byref(a), C.byref(plan.loss_args), C.byref(b), plan.psnr.data_ptr(),
+                                            stream))
         _lib.check(lib.onerf_code_scatter_add(ctx, plan.d_codes.data_ptr(), plan.ids.data_ptr(), n, code_table.shape[0],
                                               _grad_of(code_table).data_ptr(), stream))
     return plan.out[0], plan.out[1:], plan.present, plan.psnr[0]

@@ -1,9 +1,12 @@
 """One training step of 2048 rays (configs[2]: 64 + 64 samples, jitter, sigma noise, occlusion mask, pass-through rays)
-by three routes, alternated step by step in one process, for the voxel model and the plain positional-encoding model,
-both on the tensor cores (bf16):
-  existing   render_rays -> TotalLoss -> loss.backward() -> Adam(fused=True)
-  fused      training.train_step (onerf_train_step) -> Adam(fused=True, capturable=True)
-  graph      the fused step and its Adam step captured once in a CUDA graph, then replayed
+by four routes, alternated step by step in one process, for the voxel model and the plain positional-encoding model,
+all on the tensor cores (bf16):
+  existing     render_rays -> TotalLoss -> loss.backward() -> Adam(fused=True)
+  fused        training.train_step (onerf_train_step) -> Adam(fused=True, capturable=True)
+  graph        the fused step and its Adam step captured once in a CUDA graph through the host-seed entry
+               (onerf_train_step), then replayed: every replay draws with the seed the capture froze
+  graph-dseed  the same, captured as train_step captures by default (onerf_train_step_dseed, no `_rand` buffers):
+               every replay reads and advances the plan's device seed, so it draws fresh numbers
 Reports per route the device time per step (CUDA events around the step), the wall time per step (host clock around the
 step and a synchronize) and the library kernel launches per step (the graph replays the fused route's launches).
 The card's name and power limit are printed with the numbers."""
@@ -76,10 +79,16 @@ class Arm:
             for _ in range(3):
                 self._eager()
         torch.cuda.current_stream().wait_stream(s)
-        if self.route == "graph":
+        if self.route.startswith("graph"):
             self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
-                self._eager()
+            capturing = training._capturing
+            if self.route == "graph":       # the host-seed entry: the capture freezes the seed
+                training._capturing = lambda dev: False
+            try:
+                with torch.cuda.graph(self.graph):
+                    self._eager()
+            finally:
+                training._capturing = capturing
         torch.cuda.synchronize()
 
     def step(self):
@@ -99,19 +108,19 @@ def main():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True).stdout.strip()
     print("device:", torch.cuda.get_device_name(dev), "|", q)
-    arms = [Arm(v, r) for v in (True, False) for r in ("existing", "fused", "graph")]
+    arms = [Arm(v, r) for v in (True, False) for r in ("existing", "fused", "graph", "graph-dseed")]
     lib, ctx = _lib.load(), _lib.ctx(dev)
     launches = {}
     for arm in arms:
         arm.prepare()
-        if arm.route != "graph":
+        if not arm.route.startswith("graph"):
             c0 = lib.onerf_ctx_launch_count(ctx)
             arm._eager()
             torch.cuda.synchronize()
             launches[arm.name] = lib.onerf_ctx_launch_count(ctx) - c0
     for arm in arms:
-        if arm.route == "graph":
-            launches[arm.name] = launches[arm.name.replace("graph", "fused")]
+        if arm.route.startswith("graph"):
+            launches[arm.name] = launches[arm.name.split()[0] + " fused"]
     ts = {arm.name: [] for arm in arms}
     for _ in range(STEPS):
         for arm in arms:
@@ -120,7 +129,7 @@ def main():
     for arm in arms:
         dt = np.array([t[0] for t in ts[arm.name]])
         wt = np.array([t[1] for t in ts[arm.name]])
-        print(f"  {arm.name:16s} device {np.median(dt):7.2f} ms (min {dt.min():6.2f})  wall {np.median(wt):7.2f} ms "
+        print(f"  {arm.name:18s} device {np.median(dt):7.2f} ms (min {dt.min():6.2f})  wall {np.median(wt):7.2f} ms "
               f"(min {wt.min():6.2f})  library launches {launches[arm.name]}")
 
 
