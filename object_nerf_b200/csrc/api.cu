@@ -188,6 +188,8 @@ int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const oner
   ONERF_CHECK_ARG(ctx && a, "null argument");
   ONERF_CHECK_ARG(a->rays && a->packed_coarse, "null rays / packed_coarse");
   ONERF_CHECK_ARG(a->n_rays >= 0 && a->n_samples >= 2 && a->n_importance >= 0, "bad shape");
+  // the importance sampler sorts S + K depths per ray in shared memory; refused here, before the coarse pass runs
+  ONERF_UNSUPPORTED(a->n_importance > 0 && (int64_t)a->n_samples + a->n_importance > 2048, "S + K > 2048");
   ONERF_CHECK_ARG(!a->forward_instance || a->codes, "forward_instance needs codes");
   ONERF_CHECK_ARG(a->n_importance == 0 || a->packed_fine, "n_importance > 0 needs packed_fine");
   ONERF_CHECK_ARG(maps_ok(a->coarse, a->forward_instance), "null coarse output map");

@@ -7,8 +7,9 @@
 
 namespace {
 
-// torch.linspace(0, 1, S)[i] in fp32: symmetric two-sided formula (ATen RangeFactories), every
-// operation individually rounded (no FMA contraction) so the CPU oracle and the GPU agree.
+// torch.linspace(0, 1, S)[i] in fp32: symmetric two-sided formula (ATen RangeFactories), every operation individually
+// rounded (no FMA contraction).  torch's vectorised CPU kernel fuses the upper half's 1 - step * (n - 1 - i) into one
+// multiply-add, so there it can differ by one ulp of t (5 of 64 points at S = 64; tests/test_sampling_stages_cpu.py).
 __device__ __forceinline__ float linspace01(int i, int n) {
   if (n <= 1) return 0.0f;
   const float step = __fdiv_rn(1.0f, (float)(n - 1));
@@ -192,7 +193,8 @@ int onerf_launch_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, const f
                                   int n_importance, int det, const float* u, uint64_t seed, const uint64_t* seed_dev,
                                   float* z_out, void* stream) {
   ONERF_CHECK_ARG(ctx && z_coarse && weights && z_out, "null argument");
-  ONERF_CHECK_ARG(n_rays >= 0 && n_samples >= 3 && n_importance >= 1, "bad shape (need S >= 3, K >= 1)");
+  // S = 2 leaves no pdf weight (weights[:, 1:-1] is empty): every sample is the one mid-point bin, as in the reference
+  ONERF_CHECK_ARG(n_rays >= 0 && n_samples >= 2 && n_importance >= 1, "bad shape (need S >= 2, K >= 1)");
   ONERF_UNSUPPORTED(n_samples + n_importance > 2048, "S + K > 2048");
   if (n_rays == 0) return ONERF_OK;
   int P = 1;
@@ -212,8 +214,9 @@ int onerf_launch_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, const f
 extern "C" int onerf_sample_pdf(onerf_ctx* ctx, const float* bins, const float* weights, int n_rays, int n_bins,
                                 int n_importance, int det, const float* u, uint64_t seed, float* out,
                                 void* stream) {
-  ONERF_CHECK_ARG(ctx && bins && weights && out, "null argument");
-  ONERF_CHECK_ARG(n_rays >= 0 && n_bins >= 2 && n_importance >= 1, "bad shape (need >= 2 bins, K >= 1)");
+  // one bin has no weights: the (N, 0) weight tensor may have a null data pointer
+  ONERF_CHECK_ARG(ctx && bins && (weights || n_bins == 1) && out, "null argument");
+  ONERF_CHECK_ARG(n_rays >= 0 && n_bins >= 1 && n_importance >= 1, "bad shape (need >= 1 bin, K >= 1)");
   ONERF_UNSUPPORTED(n_bins + 1 + n_importance > 2048, "bins + K > 2047");
   if (n_rays == 0) return ONERF_OK;
   const int S = n_bins + 1;  // the kernel's "S": S-1 bins, S-2 weights

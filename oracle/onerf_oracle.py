@@ -207,7 +207,10 @@ def sample_pdf(bins, weights, n_importance, det=False, u=None, eps=1e-5):
     wts = weights + eps
     pdf = wts / wts.sum(-1, keepdim=True)
     cdf = torch.cumsum(pdf, -1)
-    cdf = torch.cat([torch.zeros_like(cdf[:, :1]), cdf], -1)
+    # An extension of the reference, not a port: models/rendering.py prepends zeros_like(cdf[:, :1]), which is empty when
+    # there are no weights (two coarse samples), and then gathers from an empty cdf.  A zero column of its own is the same
+    # for m >= 1 and gives m = 0 the cdf [0]: every sample is the one bin, as the library's kernel gives it.
+    cdf = torch.cat([torch.zeros(n, 1, dtype=cdf.dtype, device=cdf.device), cdf], -1)
     if det:
         u = torch.linspace(0, 1, n_importance, dtype=bins.dtype).expand(n, n_importance)
     u = u.contiguous()

@@ -45,23 +45,6 @@ def close_but(a, b, tol, name, max_outlier_frac, outlier_tol):
     assert err.max().item() <= outlier_tol, f"{name}: max abs err {err.max().item():.3e} > {outlier_tol:.1e}"
 
 
-def test_sample_coarse_matches_oracle():
-    from object_nerf_b200 import engine
-    rays = synth.random_rays(3, 77)
-    jit = synth.random_buffers(4, 77, 64, 64)["jitter"]
-    for use_disp in (False, True):
-        for perturb in (0.0, 1.0):
-            ref = O.stratified_z(rays, 64, use_disp, perturb, jit)
-            got = engine.sample_coarse(rays.to(DEV), 64, use_disp, perturb, jit.to(DEV))
-            close(got, ref, 1e-6, f"z disp={use_disp} perturb={perturb}")
-    # device RNG path: stratified property only
-    z = engine.sample_coarse(rays.to(DEV), 64, False, 1.0, None, seed=123).cpu()
-    base = O.stratified_z(rays, 64, False, 0.0)
-    mid = 0.5 * (base[:, 1:] + base[:, :-1])
-    assert (z[:, 1:-1] >= mid[:, :-1] - 1e-6).all() and (z[:, 1:-1] <= mid[:, 1:] + 1e-6).all()
-    assert (z[:, 1:] >= z[:, :-1]).all()
-
-
 def test_sample_pdf_matches_golden(golden):
     from object_nerf_b200 import rendering
     g = golden("stage_sample_pdf")
@@ -71,23 +54,6 @@ def test_sample_pdf_matches_golden(golden):
                                _u=si["pdf_u"].to(DEV))
     close_but(det, g["det"], 2e-5, "sample_pdf det", 0.01, 0.1)
     close_but(rnd, g["rnd"], 2e-5, "sample_pdf rnd", 0.01, 0.1)
-
-
-def test_sample_pdf_merge_matches_oracle():
-    from object_nerf_b200 import engine
-    rng = np.random.default_rng(9)
-    n = 50
-    rays = synth.random_rays(5, n)
-    z = O.stratified_z(rays, 64)
-    w = torch.from_numpy((rng.random((n, 64)) ** 6).astype(np.float32))
-    w[:3] = 0
-    u = torch.from_numpy(rng.random((n, 64)).astype(np.float32))
-    mid = 0.5 * (z[:, :-1] + z[:, 1:])
-    for det in (True, False):
-        ref = O.merge_sorted(z, O.sample_pdf(mid, w[:, 1:-1], 64, det=det, u=u))
-        got = engine.sample_pdf_merge(z.to(DEV), w.to(DEV), 64, det, u=None if det else u.to(DEV))
-        close_but(got, ref, 2e-5, f"pdf_merge det={det}", 0.01, 0.1)
-        assert (got[:, 1:] >= got[:, :-1]).all()
 
 
 def test_encode_matches_golden(golden):
@@ -129,35 +95,6 @@ def test_field_matches_oracle(precision, use_voxel):
     close(oo[:, :3], ref["inst_rgb"], rgb_tol, "obj rgb")
     close(so[:, 3], ref["sigma"], sig_tol, "scene sigma")
     close(oo[:, 3], ref["inst_sigma"], sig_tol, "obj sigma")
-
-
-def test_composite_matches_oracle():
-    from object_nerf_b200 import engine
-    rng = np.random.default_rng(31)
-    n, s = 37, 128
-    rays = synth.random_rays(32, n)
-    z = O.merge_sorted(O.stratified_z(rays, 64), O.stratified_z(rays, 64) + 0.01)
-    f = lambda *sh: torch.from_numpy(rng.standard_normal(sh).astype(np.float32))
-    sigma, isigma = f(n, s) * 6, f(n, s) * 6
-    rgb, irgb = torch.sigmoid(f(n, s, 3)), torch.sigmoid(f(n, s, 3))
-    ns, no = f(n, s), f(n, s)
-    ptm = torch.from_numpy(rng.random((n, 1)) < 0.5)
-    scene = torch.cat([rgb, sigma[..., None]], -1).contiguous()
-    obj = torch.cat([irgb, isigma[..., None]], -1).contiguous()
-    for kw in (dict(), dict(white_back=True, rays_in_bbox=True), dict(zero_last_delta=True),
-               dict(noise_std=1.0, is_eval=False, frustum_bound_th=0.05, pass_through_mask=ptm)):
-        ref = {}
-        O.composite_pass(ref, "x", sigma, rgb, isigma, irgb, z, noise_scene=ns, noise_obj=no,
-                         **{"is_eval": True, **kw})
-        kk = dict(kw)
-        if "pass_through_mask" in kk:
-            kk["pass_through_mask"] = ptm.to(DEV)
-        got = engine.composite(z.to(DEV), scene.to(DEV), obj.to(DEV), noise_scene=ns.to(DEV),
-                               noise_obj=no.to(DEV), **{"is_eval": True, **kk})
-        for k_ref, k_got in (("weights_x", "weights"), ("opacity_x", "opacity"), ("rgb_x", "rgb"),
-                             ("depth_x", "depth"), ("rgb_instance_x", "rgb_instance"),
-                             ("depth_instance_x", "depth_instance"), ("opacity_instance_x", "opacity_instance")):
-            close(got[k_got], ref[k_ref], 2e-5, f"{k_ref} {kw.keys()}")
 
 
 def _run_render_case(c, precision):

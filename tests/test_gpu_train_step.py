@@ -4,7 +4,7 @@ seeded batch, and against the reference's own backward (fixtures)."""
 import pytest
 import torch
 
-from tests import cases, grad_plain, helpers
+from tests import cases, grad_plain, helpers, synth
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -143,11 +143,24 @@ def test_skipped_terms_match_total_loss(empty):
     _compare(inp, True, "fp32", rand, batch=batch)
 
 
-@pytest.mark.parametrize("mode", ["rays_in_bbox", "no_pass_through", "is_eval", "coarse_only"])
+SHAPE_MODES = {"shape_33_30": (33, 30), "shape_3_1": (3, 1), "shape_2_1": (2, 1), "shape_1024_1024": (1024, 1024)}
+
+
+@pytest.mark.parametrize("mode", ["rays_in_bbox", "no_pass_through", "is_eval", "coarse_only"] + list(SHAPE_MODES))
 def test_modes_match_existing_route(mode):
     """rays_in_bbox, the occlusion mask without pass-through rays, is_eval and N_importance = 0 (the coarse pass writes
-    the loss outputs and the PSNR)."""
+    the loss outputs and the PSNR); and (S, K) shapes off the 64 + 64 default on a few rays: a partial last warp chunk,
+    the smallest sort buffers (S = 2: no pdf weight at all) and S + K = 2048, the shared-memory limit of the step's
+    compositing kernel (4 warps x 4 S floats)."""
     inp, rand = _voxel_case()
+    if mode in SHAPE_MODES:
+        S, K = SHAPE_MODES[mode]
+        n = 4 if S + K > 256 else 9
+        inp = cases.build_grad_case(n_rays=n)
+        inp["rand"] = synth.random_buffers(cases.GRAD_CASE["seed"] + 4, n, S, K)
+        rand = {k: v.to(DEV) for k, v in inp["rand"].items()}
+        _compare(inp, True, "fp32", rand, N_samples=S, N_importance=K)
+        return
     over = {"rays_in_bbox": dict(rays_in_bbox=True),
             "no_pass_through": dict(pass_through_mask=None),
             "is_eval": dict(is_eval=True),
