@@ -70,6 +70,56 @@ int onerf_render_rays_fwd_dseed(onerf_ctx* ctx, const onerf_render_args* args, u
 int onerf_train_step_dseed(onerf_ctx* ctx, const onerf_render_args* fwd, const onerf_loss_args* loss,
                            const onerf_render_bwd_args* bwd, float* psnr_out, uint64_t* seed_dev, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * An edited frame from a camera (EditableRenderer.render_edit, editable_renderer.py:203-294), or a contiguous tile of it.
+ * Pixels [pixel_begin, pixel_end) (row-major) of the H x W frame are rendered in chunks of chunk_rays pixels; for each
+ * chunk every set's rays are generated on the device exactly as onerf_camera_rays generates them for those pixels, the
+ * chunk runs through onerf_render_multi_fwd's path (perturb = 0, so nothing is random) and its maps are written to rows
+ * [chunk - pixel_begin, ...) of the tile-sized outputs.  Every result row depends on its pixel only, never on chunk_rays
+ * or the tile bounds.
+ *   sets_host  n_obj ray sets (host array).  obj_id 0 = scene branch (box NULL: near / far = near, far / scale_factor),
+ *              otherwise the object branch with code_table[obj_id] (box required, bbox_enlarge applied: near / far from
+ *              the slab test, 0 / 0 for a miss).  Toc: row-major (3,4) camera-to-set pose, translation at NeRF scale.
+ *   maps       tile-sized (N = pixel_end - pixel_begin rows), shapes of onerf_render_multi_maps.  Any array may be NULL:
+ *              it is not written (its values go to chunk scratch in the workspace).
+ *   workspace  >= onerf_render_edit_workspace_bytes(chunk_rays, n_obj, n_samples, n_importance) bytes, 256-byte aligned
+ *              (0 for a bad shape).
+ * Limits and refusals of onerf_render_multi_fwd, plus: a tile outside [0, H*W], chunk_rays < 1, an object set without a
+ * box or the scene set with one, a bad camera (H, W or focal not positive).  Kernels only, no host read.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct onerf_edit_set {
+  int obj_id;
+  float Toc[12];
+  const onerf_box_host* box;
+} onerf_edit_set;
+
+typedef struct onerf_render_edit_args {
+  const onerf_edit_set* sets_host;
+  int n_obj;
+  int H, W;
+  float focal;
+  int64_t pixel_begin, pixel_end;
+  double near, far, scale_factor;
+  int n_samples, n_importance;
+  const onerf_grid* grid;
+  const void* packed_coarse;
+  const void* packed_fine;            /* required iff n_importance > 0 */
+  const float* code_table;            /* (n_codes,64) */
+  int n_codes;
+  int precision;                      /* onerf_precision */
+  int use_disp, white_back;
+  const float* boxes;                 /* (n_boxes,18) removed-object boxes of the scene set, or NULL */
+  int n_boxes;
+  int chunk_rays;
+  onerf_render_multi_maps coarse;
+  onerf_render_multi_maps fine;       /* written iff n_importance > 0 */
+  void* workspace;
+  size_t workspace_bytes;
+} onerf_render_edit_args;
+
+size_t onerf_render_edit_workspace_bytes(int chunk_rays, int n_obj, int n_samples, int n_importance);
+int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -37,7 +37,8 @@ EXPORTS = [
 # additions to ABI version 2 declared in include/onerf_ext.h
 EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_ws", "onerf_composite_multi_merge",
                "onerf_train_workspace_bytes_prec", "onerf_train_step_workspace_bytes", "onerf_train_step",
-               "onerf_render_rays_fwd_dseed", "onerf_train_step_dseed"]
+               "onerf_render_rays_fwd_dseed", "onerf_train_step_dseed", "onerf_render_edit_workspace_bytes",
+               "onerf_render_edit_frame"]
 
 _p = C.c_void_p
 
@@ -114,6 +115,21 @@ class RenderMultiArgs(C.Structure):
         ("n_samples", C.c_int), ("n_importance", C.c_int), ("grid", C.POINTER(Grid)), ("packed_coarse", _p),
         ("packed_fine", _p), ("code_table", _p), ("n_codes", C.c_int), ("precision", C.c_int), ("use_disp", C.c_int),
         ("perturb", C.c_float), ("seed", C.c_uint64), ("white_back", C.c_int), ("boxes", _p), ("n_boxes", C.c_int),
+        ("coarse", RenderMultiMaps), ("fine", RenderMultiMaps), ("workspace", _p), ("workspace_bytes", C.c_size_t),
+    ]
+
+
+class EditSet(C.Structure):
+    _fields_ = [("obj_id", C.c_int), ("Toc", C.c_float * 12), ("box", C.POINTER(BoxHost))]
+
+
+class RenderEditArgs(C.Structure):
+    _fields_ = [
+        ("sets_host", C.POINTER(EditSet)), ("n_obj", C.c_int), ("H", C.c_int), ("W", C.c_int), ("focal", C.c_float),
+        ("pixel_begin", C.c_int64), ("pixel_end", C.c_int64), ("near", C.c_double), ("far", C.c_double),
+        ("scale_factor", C.c_double), ("n_samples", C.c_int), ("n_importance", C.c_int), ("grid", C.POINTER(Grid)),
+        ("packed_coarse", _p), ("packed_fine", _p), ("code_table", _p), ("n_codes", C.c_int), ("precision", C.c_int),
+        ("use_disp", C.c_int), ("white_back", C.c_int), ("boxes", _p), ("n_boxes", C.c_int), ("chunk_rays", C.c_int),
         ("coarse", RenderMultiMaps), ("fine", RenderMultiMaps), ("workspace", _p), ("workspace_bytes", C.c_size_t),
     ]
 
@@ -226,6 +242,9 @@ def load() -> C.CDLL:
         lib.onerf_render_rays_fwd_dseed.argtypes = [_p, C.POINTER(RenderArgs), _p, _p]
         lib.onerf_train_step_dseed.argtypes = [_p, C.POINTER(RenderArgs), C.POINTER(LossArgs), C.POINTER(RenderBwdArgs), _p,
                                                _p, _p]
+        lib.onerf_render_edit_workspace_bytes.argtypes = [C.c_int] * 4
+        lib.onerf_render_edit_workspace_bytes.restype = C.c_size_t
+        lib.onerf_render_edit_frame.argtypes = [_p, C.POINTER(RenderEditArgs), _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

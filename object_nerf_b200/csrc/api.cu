@@ -2,6 +2,8 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <vector>
+
 #include "field_common.cuh"
 #include "train_ws.h"
 #include "../../include/onerf_ext.h"
@@ -340,28 +342,58 @@ static int multi_fields(onerf_ctx* ctx, const onerf_render_multi_args* a, const 
   return ONERF_OK;
 }
 
+// The argument checks of onerf_render_multi_fwd, reported under the entry `fn`.  with_rays_and_maps = 0 leaves out the ray
+// sets and the outputs (onerf_render_edit_frame makes both itself).
+#define FN_CHECK_ARG(cond, msg)                                                      \
+  do {                                                                               \
+    if (!(cond)) { onerf_set_error("%s: %s", fn, msg); return ONERF_ERR_BAD_ARG; }   \
+  } while (0)
+#define FN_UNSUPPORTED(cond, msg)                                                                 \
+  do {                                                                                            \
+    if (cond) { onerf_set_error("%s: unsupported: %s", fn, msg); return ONERF_ERR_UNSUPPORTED; }  \
+  } while (0)
+
+static int check_multi_args(const char* fn, const onerf_render_multi_args* a, bool with_rays_and_maps) {
+  FN_CHECK_ARG((a->rays_list_host || !with_rays_and_maps) && a->obj_ids_host && a->packed_coarse && a->grid && a->code_table,
+               "null input");
+  FN_CHECK_ARG(a->n_rays >= 0 && a->n_obj >= 1 && a->n_samples >= 2 && a->n_importance >= 0, "bad shape");
+  FN_UNSUPPORTED((int64_t)a->n_obj * (a->n_samples + a->n_importance) > INT32_MAX, "n_obj * samples >= 2^31");
+  FN_UNSUPPORTED(a->n_samples + a->n_importance > 2048, "more than 2048 samples per ray set");
+  FN_CHECK_ARG(a->n_importance == 0 || a->packed_fine, "n_importance > 0 needs packed_fine");
+  FN_CHECK_ARG(a->n_boxes == 0 || a->boxes, "n_boxes > 0 with null boxes");
+  for (int i = 0; i < a->n_obj; ++i) {
+    if (with_rays_and_maps) FN_CHECK_ARG(a->rays_list_host[i], "null ray set");
+    FN_CHECK_ARG(a->obj_ids_host[i] >= 0 && a->obj_ids_host[i] < a->n_codes, "object id outside the code table");
+  }
+  if (!with_rays_and_maps) return ONERF_OK;
+  const onerf_render_multi_maps& c = a->coarse;
+  FN_CHECK_ARG(c.weights && c.opacity && c.z_vals && c.rgb && c.depth && c.obj_ids, "null coarse output");
+  if (a->n_importance > 0)
+    FN_CHECK_ARG(a->fine.weights && a->fine.opacity && a->fine.z_vals && a->fine.rgb && a->fine.depth, "null fine output");
+  return ONERF_OK;
+}
+#undef FN_CHECK_ARG
+#undef FN_UNSUPPORTED
+
+static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, void* stream);
+
 extern "C" int onerf_render_multi_fwd(onerf_ctx* ctx, const onerf_render_multi_args* a, void* stream) {
   ONERF_CHECK_ARG(ctx && a, "null argument");
-  ONERF_CHECK_ARG(a->rays_list_host && a->obj_ids_host && a->packed_coarse && a->grid && a->code_table, "null input");
-  ONERF_CHECK_ARG(a->n_rays >= 0 && a->n_obj >= 1 && a->n_samples >= 2 && a->n_importance >= 0, "bad shape");
-  ONERF_UNSUPPORTED((int64_t)a->n_obj * (a->n_samples + a->n_importance) > INT32_MAX, "n_obj * samples >= 2^31");
-  ONERF_UNSUPPORTED(a->n_samples + a->n_importance > 2048, "more than 2048 samples per ray set");
-  ONERF_CHECK_ARG(a->n_importance == 0 || a->packed_fine, "n_importance > 0 needs packed_fine");
-  ONERF_CHECK_ARG(a->n_boxes == 0 || a->boxes, "n_boxes > 0 with null boxes");
-  for (int i = 0; i < a->n_obj; ++i) {
-    ONERF_CHECK_ARG(a->rays_list_host[i], "null ray set");
-    ONERF_CHECK_ARG(a->obj_ids_host[i] >= 0 && a->obj_ids_host[i] < a->n_codes, "object id outside the code table");
-  }
-  const onerf_render_multi_maps& c = a->coarse;
-  ONERF_CHECK_ARG(c.weights && c.opacity && c.z_vals && c.rgb && c.depth && c.obj_ids, "null coarse output");
-  if (a->n_importance > 0)
-    ONERF_CHECK_ARG(a->fine.weights && a->fine.opacity && a->fine.z_vals && a->fine.rgb && a->fine.depth, "null fine output");
+  const int rc = check_multi_args(__func__, a, true);
+  if (rc != ONERF_OK) return rc;
   const size_t need = onerf_render_multi_workspace_bytes(a->n_rays, a->n_obj, a->n_samples, a->n_importance);
   ONERF_CHECK_ARG(a->workspace && (reinterpret_cast<uintptr_t>(a->workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
   if (a->workspace_bytes < need) {
     onerf_set_error("onerf_render_multi_fwd: workspace too small (%zu < %zu)", a->workspace_bytes, need);
     return ONERF_ERR_WORKSPACE;
   }
+  return multi_forward(ctx, a, stream);
+}
+
+// The forward of onerf_render_multi_fwd on checked arguments: n_rays rays of every set in a->rays_list_host, maps written
+// to a->coarse / a->fine, scratch in a->workspace.
+static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, void* stream) {
+  const onerf_render_multi_maps& c = a->coarse;
   if (a->n_rays == 0) return ONERF_OK;
   const int S = a->n_samples, SF = a->n_samples + a->n_importance, N = a->n_rays, NO = a->n_obj;
   const MultiWs w = multi_ws_layout(reinterpret_cast<char*>(a->workspace), N, NO, S, a->n_importance);
@@ -386,4 +418,112 @@ extern "C" int onerf_render_multi_fwd(onerf_ctx* ctx, const onerf_render_multi_a
   if (rc != ONERF_OK) return rc;
   return onerf_composite_multi_ws(ctx, w.z_fine, w.field_all, N, NO, SF, a->white_back, a->fine.z_vals, a->fine.weights, nullptr,
                                   nullptr, a->fine.opacity, a->fine.rgb, a->fine.depth, w.sort, w.sort_bytes, stream);
+}
+
+// ------------------------------------------------------------------------------------------------
+// An edited frame from a camera (EditableRenderer.render_edit, editable_renderer.py:203-294): per chunk of pixels, every
+// set's camera rays (onerf_camera_rays' kernel on the chunk's pixels), then multi_forward with the chunk's rows of the
+// caller's maps.  Chunks are independent: every stage works per ray.
+// ------------------------------------------------------------------------------------------------
+struct EditWs {
+  float* rays;                            // (n_obj, chunk, 8): every set's rays of the current chunk
+  onerf_render_multi_maps coarse, fine;   // one chunk of each map, for the maps the caller leaves NULL
+  void* multi;                            // workspace of multi_forward for one chunk
+  size_t multi_bytes;
+  size_t total;
+};
+
+static EditWs edit_ws_layout(char* base, int chunk, int n_obj, int n_samples, int n_importance) {
+  const size_t n = chunk, nf = n_importance > 0 ? n : 0, no = n_obj;
+  const size_t tc = no * n_samples, tf = no * (n_samples + n_importance);
+  EditWs w;
+  size_t off = 0;
+  auto take = [&](size_t floats) { float* p = reinterpret_cast<float*>(base + off); off += align256(floats * sizeof(float)); return p; };
+  w.rays = take(no * n * 8);
+  w.coarse.weights = take(n * tc); w.coarse.opacity = take(n); w.coarse.z_vals = take(n * tc);
+  w.coarse.rgb = take(n * 3); w.coarse.depth = take(n); w.coarse.obj_ids = take(n * tc);
+  w.fine.weights = take(nf * tf); w.fine.opacity = take(nf); w.fine.z_vals = take(nf * tf);
+  w.fine.rgb = take(nf * 3); w.fine.depth = take(nf); w.fine.obj_ids = nullptr;
+  w.multi_bytes = onerf_render_multi_workspace_bytes(chunk, n_obj, n_samples, n_importance);
+  w.multi = base + off;
+  off += align256(w.multi_bytes);
+  w.total = off;
+  return w;
+}
+
+// rows [r0, r0 + chunk) of the tile's maps (T samples per row), or the chunk scratch where a map is NULL
+static onerf_render_multi_maps chunk_maps(const onerf_render_multi_maps& out, const onerf_render_multi_maps& scratch,
+                                          int64_t r0, int64_t T) {
+  auto at = [&](float* o, float* s, int64_t width) { return o ? o + r0 * width : s; };
+  onerf_render_multi_maps m;
+  m.weights = at(out.weights, scratch.weights, T);
+  m.opacity = at(out.opacity, scratch.opacity, 1);
+  m.z_vals = at(out.z_vals, scratch.z_vals, T);
+  m.rgb = at(out.rgb, scratch.rgb, 3);
+  m.depth = at(out.depth, scratch.depth, 1);
+  m.obj_ids = at(out.obj_ids, scratch.obj_ids, T);
+  return m;
+}
+
+extern "C" size_t onerf_render_edit_workspace_bytes(int chunk_rays, int n_obj, int n_samples, int n_importance) {
+  if (chunk_rays < 1 || onerf_render_multi_workspace_bytes(chunk_rays, n_obj, n_samples, n_importance) == 0) return 0;
+  return edit_ws_layout(nullptr, chunk_rays, n_obj, n_samples, n_importance).total;
+}
+
+extern "C" int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_args* a, void* stream) {
+  ONERF_CHECK_ARG(ctx && a && a->sets_host, "null argument");
+  ONERF_CHECK_ARG(a->n_obj >= 1, "bad shape");
+  ONERF_CHECK_ARG(a->H > 0 && a->W > 0 && a->focal > 0, "bad camera");
+  const int64_t n_tile = a->pixel_end - a->pixel_begin;
+  ONERF_CHECK_ARG(a->pixel_begin >= 0 && n_tile >= 0 && a->pixel_end <= (int64_t)a->H * a->W, "tile outside the frame");
+  ONERF_CHECK_ARG(a->chunk_rays >= 1, "chunk_rays < 1");
+  ONERF_CHECK_ARG(a->scale_factor > 0, "scale_factor must be positive");
+  const int NO = a->n_obj;
+  std::vector<int> ids(NO);
+  for (int i = 0; i < NO; ++i) {
+    const onerf_edit_set& s = a->sets_host[i];
+    ONERF_CHECK_ARG(s.obj_id == 0 || s.box, "an object set needs its box");
+    ONERF_CHECK_ARG(s.obj_id != 0 || !s.box, "the scene set takes no box");
+    ids[i] = s.obj_id;
+  }
+  const int chunk = a->chunk_rays;
+  onerf_render_multi_args m;
+  memset(&m, 0, sizeof(m));
+  m.obj_ids_host = ids.data();
+  m.n_obj = NO; m.n_rays = (int)(n_tile < chunk ? n_tile : chunk);
+  m.n_samples = a->n_samples; m.n_importance = a->n_importance;
+  m.grid = a->grid; m.packed_coarse = a->packed_coarse; m.packed_fine = a->packed_fine;
+  m.code_table = a->code_table; m.n_codes = a->n_codes;
+  m.precision = a->precision; m.use_disp = a->use_disp; m.perturb = 0.0f; m.seed = 0; m.white_back = a->white_back;
+  m.boxes = a->boxes; m.n_boxes = a->n_boxes;
+  int rc = check_multi_args(__func__, &m, false);
+  if (rc != ONERF_OK) return rc;
+  const size_t need = onerf_render_edit_workspace_bytes(chunk, NO, a->n_samples, a->n_importance);
+  ONERF_CHECK_ARG(a->workspace && (reinterpret_cast<uintptr_t>(a->workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
+  if (a->workspace_bytes < need) {
+    onerf_set_error("onerf_render_edit_frame: workspace too small (%zu < %zu)", a->workspace_bytes, need);
+    return ONERF_ERR_WORKSPACE;
+  }
+  const EditWs w = edit_ws_layout(reinterpret_cast<char*>(a->workspace), chunk, NO, a->n_samples, a->n_importance);
+  std::vector<const float*> rays(NO);
+  for (int i = 0; i < NO; ++i) rays[i] = w.rays + (size_t)i * chunk * 8;
+  m.rays_list_host = rays.data();
+  m.workspace = w.multi;
+  m.workspace_bytes = w.multi_bytes;
+  const int64_t TC = (int64_t)NO * a->n_samples, TF = (int64_t)NO * (a->n_samples + a->n_importance);
+  for (int64_t r0 = 0; r0 < n_tile; r0 += chunk) {
+    const int n = (int)(n_tile - r0 < chunk ? n_tile - r0 : chunk);
+    for (int i = 0; i < NO; ++i) {
+      const onerf_edit_set& s = a->sets_host[i];
+      rc = onerf_launch_camera_rays(ctx, a->H, a->W, a->focal, s.Toc, s.box, a->scale_factor, a->near, a->far,
+                                    a->pixel_begin + r0, n, const_cast<float*>(rays[i]), nullptr, (cudaStream_t)stream);
+      if (rc != ONERF_OK) return rc;
+    }
+    m.n_rays = n;
+    m.coarse = chunk_maps(a->coarse, w.coarse, r0, TC);
+    if (a->n_importance > 0) m.fine = chunk_maps(a->fine, w.fine, r0, TF);
+    rc = multi_forward(ctx, &m, stream);
+    if (rc != ONERF_OK) return rc;
+  }
+  return ONERF_OK;
 }

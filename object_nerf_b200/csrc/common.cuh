@@ -20,6 +20,12 @@ void onerf_free_pack_tables(onerf_ctx* ctx);
 
 void onerf_set_error(const char* fmt, ...);
 
+// rays.cu: pixels [p0, p0 + n) of onerf_camera_rays' H x W frame, written as rows 0 .. n-1 of rays_out (and hit_out).
+// The camera and rays_out are the caller's to check.
+int onerf_launch_camera_rays(onerf_ctx* ctx, int H, int W, float focal, const float* c2w_host, const onerf_box_host* box,
+                             double scale_factor, double near, double far, int64_t p0, int64_t n, float* rays_out,
+                             uint8_t* hit_out, cudaStream_t stream);
+
 #define ONERF_CHECK_ARG(cond, msg)                       \
   do {                                                   \
     if (!(cond)) {                                       \

@@ -119,12 +119,13 @@ __global__ void __launch_bounds__(256) generate_rays_kernel(BoxParams b, const f
               rays_d[3 * i + 2]);
 }
 
-// pixel -> (N,8) ray in one pass: get_ray_directions + get_rays + generate_rays
-__global__ void __launch_bounds__(256) camera_rays_kernel(Cam c, BoxParams b, float* __restrict__ out,
+// pixel -> (N,8) ray in one pass: get_ray_directions + get_rays + generate_rays.  Row i of out is pixel p0 + i (row-major),
+// i < n: a tile of the frame gets the rays the whole frame has at those pixels.
+__global__ void __launch_bounds__(256) camera_rays_kernel(Cam c, BoxParams b, int64_t p0, int64_t n, float* __restrict__ out,
                                                           uint8_t* __restrict__ hit_out) {
-  const int64_t n = (int64_t)c.H * c.W;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const int y = (int)(i / c.W), x = (int)(i - (int64_t)y * c.W);
+    const int64_t p = p0 + i;
+    const int y = (int)(p / c.W), x = (int)(p - (int64_t)y * c.W);
     float dx, dy, dz, wx, wy, wz;
     pixel_direction(c, x, y, dx, dy, dz);
     rotate_normalise(c, dx, dy, dz, wx, wy, wz);
@@ -210,16 +211,24 @@ extern "C" int onerf_generate_rays(onerf_ctx* ctx, const float* rays_o, const fl
   return ONERF_OK;
 }
 
+int onerf_launch_camera_rays(onerf_ctx* ctx, int H, int W, float focal, const float* c2w_host, const onerf_box_host* box,
+                             double scale_factor, double near, double far, int64_t p0, int64_t n, float* rays_out,
+                             uint8_t* hit_out, cudaStream_t stream) {
+  BoxParams b;
+  const int rc = make_box(box, scale_factor, near, far, b);
+  if (rc != ONERF_OK) return rc;
+  if (n == 0) return ONERF_OK;
+  const Cam c = make_cam(H, W, focal, c2w_host);
+  camera_rays_kernel<<<grid_for(ctx, n), 256, 0, stream>>>(c, b, p0, n, rays_out, hit_out);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
 extern "C" int onerf_camera_rays(onerf_ctx* ctx, int H, int W, float focal, const float* c2w_host, const onerf_box_host* box,
                                  double scale_factor, double near, double far, float* rays_out, uint8_t* hit_out,
                                  void* stream) {
   ONERF_CHECK_ARG(ctx && c2w_host && rays_out, "null argument");
   ONERF_CHECK_ARG(H > 0 && W > 0 && focal > 0 && onerf_aligned16(rays_out), "bad camera or misaligned output");
-  BoxParams b;
-  const int rc = make_box(box, scale_factor, near, far, b);
-  if (rc != ONERF_OK) return rc;
-  const Cam c = make_cam(H, W, focal, c2w_host);
-  camera_rays_kernel<<<grid_for(ctx, (int64_t)H * W), 256, 0, (cudaStream_t)stream>>>(c, b, rays_out, hit_out);
-  ONERF_LAUNCH_CHECK(ctx);
-  return ONERF_OK;
+  return onerf_launch_camera_rays(ctx, H, W, focal, c2w_host, box, scale_factor, near, far, 0, (int64_t)H * W, rays_out,
+                                  hit_out, (cudaStream_t)stream);
 }
