@@ -120,6 +120,62 @@ typedef struct onerf_render_edit_args {
 size_t onerf_render_edit_workspace_bytes(int chunk_rays, int n_obj, int n_samples, int n_importance);
 int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_args* args, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Training batches drawn on the device (GenericDataset.__getitem__ through DataLoader(shuffle=True), and under DDP
+ * DistributedSampler; datasets/generic_dataset.py:475-490, train.py:121-129).  The dataset's R rays stay in device
+ * memory; one launch draws batch `step` of rank `rank` into B-row outputs:
+ *   P = floor(R / (B * W)) full batches per epoch (the last R - P*B*W positions of each epoch's order are not drawn);
+ *   epoch e = step / P, j = step mod P; element b takes position p = (j*B + b)*W + rank of epoch e's permutation
+ *   pi_{seed,e} of [0, R) (a 6-round Feistel network on [0, 2^m), m the smallest even m >= 2 with 2^m >= R, round
+ *   function philox4x32 keyed by seed with counter (right half, (uint32)e, 5, round), cycle-walked into [0, R));
+ *   ray i = pi(p) gives rays, rgbs, depths, valid_mask and frame_idx; instance column c = (w * I) >> 32, with w word
+ *   (n & 3) of philox4x32((n >> 2, n >> 34, 4, 0), seed) at n = (step*B + b)*W + rank, gives instance_mask,
+ *   instance_mask_weight, instance_ids and pass_through_mask (row i, column c).
+ * Every rank with the same seed shares the permutation and draws a disjoint stride of it.
+ *   data       device buffers of the dataset.  frame_idx may be NULL (frame_idx_out is then filled with -1).
+ *   outputs    B rows: rays (B,8), rgbs (B,3), depths, valid_mask, frame_idx (B,); instance_mask, instance_mask_weight,
+ *              instance_ids, pass_through_mask (B,) (the layout of onerf_loss_args and onerf_train_step's batch).
+ *              frame_idx and index_out may be NULL; index_out (B,2) = (ray i, column c) per row.
+ * Refusals (ONERF_ERR_BAD_ARG): a null ctx, argument block or required buffer, B < 1, W < 1, rank outside [0, W),
+ * I < 1, R < B*W (P = 0), R >= 2^40.  Kernels only, no host read: CUDA-graph capturable.
+ * onerf_draw_batch_dstep ignores args->step: its kernel reads the step from *step_dev (one uint64, 8-byte aligned) and a
+ * one-thread follow-up launch adds 1 to it, so each replay of a captured call draws the next batch.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct onerf_ray_dataset {
+  int64_t n_rays;                       /* R */
+  int n_instances;                      /* I: instance columns per ray */
+  const float* rays;                    /* (R,8) */
+  const float* rgbs;                    /* (R,3) */
+  const float* depths;                  /* (R,) */
+  const uint8_t* valid_mask;            /* (R,) 0 / 1 */
+  const int64_t* frame_idx;             /* (R,) or NULL */
+  const uint8_t* instance_mask;         /* (R,I) 0 / 1 */
+  const float* instance_mask_weight;    /* (R,I) */
+  const int64_t* instance_ids;          /* (R,I) */
+  const uint8_t* pass_through_mask;     /* (R,I) 0 / 1 */
+} onerf_ray_dataset;
+
+typedef struct onerf_batch_args {
+  onerf_ray_dataset data;
+  int batch;                            /* B */
+  int rank, world;                      /* W = world */
+  uint64_t seed;
+  uint64_t step;                        /* onerf_draw_batch only */
+  float* rays;
+  float* rgbs;
+  float* depths;
+  uint8_t* valid_mask;
+  int64_t* frame_idx;                   /* or NULL */
+  uint8_t* instance_mask;
+  float* instance_mask_weight;
+  int64_t* instance_ids;
+  uint8_t* pass_through_mask;
+  int64_t* index_out;                   /* (B,2) or NULL */
+} onerf_batch_args;
+
+int onerf_draw_batch(onerf_ctx* ctx, const onerf_batch_args* args, void* stream);
+int onerf_draw_batch_dstep(onerf_ctx* ctx, const onerf_batch_args* args, uint64_t* step_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -4,3 +4,4 @@ from .rendering import render_rays, inference_model, query_sigma  # noqa: F401
 from .nerf_model import ObjectNeRF  # noqa: F401
 from .embedding_helper import Embedding, EmbeddingVoxel  # noqa: F401
 from .code_library import CodeLibrary  # noqa: F401
+from .batches import RaySampler  # noqa: F401

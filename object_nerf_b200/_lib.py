@@ -38,7 +38,7 @@ EXPORTS = [
 EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_ws", "onerf_composite_multi_merge",
                "onerf_train_workspace_bytes_prec", "onerf_train_step_workspace_bytes", "onerf_train_step",
                "onerf_render_rays_fwd_dseed", "onerf_train_step_dseed", "onerf_render_edit_workspace_bytes",
-               "onerf_render_edit_frame"]
+               "onerf_render_edit_frame", "onerf_draw_batch", "onerf_draw_batch_dstep"]
 
 _p = C.c_void_p
 
@@ -131,6 +131,21 @@ class RenderEditArgs(C.Structure):
         ("packed_coarse", _p), ("packed_fine", _p), ("code_table", _p), ("n_codes", C.c_int), ("precision", C.c_int),
         ("use_disp", C.c_int), ("white_back", C.c_int), ("boxes", _p), ("n_boxes", C.c_int), ("chunk_rays", C.c_int),
         ("coarse", RenderMultiMaps), ("fine", RenderMultiMaps), ("workspace", _p), ("workspace_bytes", C.c_size_t),
+    ]
+
+
+class RayDataset(C.Structure):
+    _fields_ = [("n_rays", C.c_int64), ("n_instances", C.c_int), ("rays", _p), ("rgbs", _p), ("depths", _p),
+                ("valid_mask", _p), ("frame_idx", _p), ("instance_mask", _p), ("instance_mask_weight", _p),
+                ("instance_ids", _p), ("pass_through_mask", _p)]
+
+
+class BatchArgs(C.Structure):
+    _fields_ = [
+        ("data", RayDataset), ("batch", C.c_int), ("rank", C.c_int), ("world", C.c_int), ("seed", C.c_uint64),
+        ("step", C.c_uint64), ("rays", _p), ("rgbs", _p), ("depths", _p), ("valid_mask", _p), ("frame_idx", _p),
+        ("instance_mask", _p), ("instance_mask_weight", _p), ("instance_ids", _p), ("pass_through_mask", _p),
+        ("index_out", _p),
     ]
 
 
@@ -245,6 +260,8 @@ def load() -> C.CDLL:
         lib.onerf_render_edit_workspace_bytes.argtypes = [C.c_int] * 4
         lib.onerf_render_edit_workspace_bytes.restype = C.c_size_t
         lib.onerf_render_edit_frame.argtypes = [_p, C.POINTER(RenderEditArgs), _p]
+        lib.onerf_draw_batch.argtypes = [_p, C.POINTER(BatchArgs), _p]
+        lib.onerf_draw_batch_dstep.argtypes = [_p, C.POINTER(BatchArgs), _p, _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib
