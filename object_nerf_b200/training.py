@@ -24,6 +24,26 @@ configuration must therefore run eagerly (the usual warm-up before a capture): a
 its counter reset on every replay, so that is refused.  Injected `_rand` buffers take precedence over either seed.
 
 The returned tensors are the plan's output buffers and are overwritten by the next step of the same plan.
+
+Data-parallel training (`group=`, a torch.distributed process group; DDP's semantics without DDP's hooks, which never
+fire because the step writes `.grad` without autograd):
+  - the plan made by the first call with a group allocates one fp32 gradient bucket and points the `.grad` of every
+    trained tensor at a view of it: the 40 tensors of each model in engine.model_linears order (fine model first), the
+    code table, the voxel table last, every offset 16-byte aligned.  Values already in `.grad` are copied in.  Keep
+    them there: a later call whose `.grad` no longer aliases the bucket (`zero_grad(set_to_none=True)`, a replaced
+    parameter) is refused;
+  - after the step, one all-reduce (SUM, then a scale by 1/W: the mean over ranks, as DDP) of the bucket's prefix runs
+    on the current stream.  The prefix ends after voxel-table row n_used: only rows the index map references,
+    [0, n_used), can receive gradient, so the rows above are zero on every rank.  The whole prefix is reduced, including
+    what `.grad` held before the step (as DDP without no_sync): zero the gradients before each step.  With NCCL the
+    reduction captures in the step's CUDA graph;
+  - `sync_replicas` must have run since the last change to the grid: it broadcasts rank 0's parameters and grid (DDP's
+    construction-time broadcast and broadcast_buffers) and counts n_used.  Call it before training and after every
+    grid maintenance (pruning draws its jitter per rank, so the ranks' grids differ after it);
+  - rank r draws with the seed a group-less call would use plus r * 2^52 (mod 2^62), both the host seed and the start of
+    the device counter.  A deliberate difference from the reference: its ranks start from identical torch generators
+    and would draw the same jitter and noise at the same batch positions.  Injected `_rand` buffers still win;
+  - the returned loss, terms, flags and PSNR are this rank's (train.py logs them per rank).
 """
 from __future__ import annotations
 
@@ -36,15 +56,67 @@ import torch
 from . import _lib, backward, engine
 from .losses import TERMS
 
-__all__ = ["train_step", "step_seed"]
+__all__ = ["train_step", "step_seed", "sync_replicas"]
 
 _RAND_KEYS = ("jitter", "u", "noise_scene_coarse", "noise_obj_coarse", "noise_scene_fine", "noise_obj_fine")
 # coarse model -> {configuration: plan}; a plan references no module, so it lives exactly as long as the model
 _plans: "weakref.WeakKeyDictionary[Any, Dict[tuple, _StepPlan]]" = weakref.WeakKeyDictionary()
+# coarse model -> (grid stamp or None, n_used) of its last sync_replicas
+_synced: "weakref.WeakKeyDictionary[Any, tuple]" = weakref.WeakKeyDictionary()
+RANK_SEED_STRIDE = 1 << 52
+# EmbeddingVoxel's grid state besides the table (voxel_occupancy and voxel_count are absent from bare grid modules)
+GRID_BUFFERS = ("voxel_shape", "voxel_size", "voxel_offset", "voxel_count", "voxel_idx_map", "voxel_occupancy")
 
 
 def _is_voxel(emb) -> bool:
     return hasattr(emb, "voxel_idx_map")
+
+
+def _grid_stamp(emb) -> tuple:
+    """What grid maintenance changes, readable without the device: the index map's address, shape and in-place
+    version (pruning writes it in place, subdivision replaces it)."""
+    m = emb.voxel_idx_map
+    return m.data_ptr(), tuple(m.shape), m._version
+
+
+def _trained_tensors(models, model_order, code_table, table) -> list:
+    """The tensors a step writes gradients for, in bucket order."""
+    out = []
+    for typ in reversed(model_order):            # fine first
+        for w, b in engine.model_linears(models[typ]):
+            out += [w, b]
+    out.append(code_table)
+    if table is not None:
+        out.append(table)
+    return out
+
+
+def _grad_ptrs(tensors) -> list:
+    return [t.grad.data_ptr() if t.grad is not None else 0 for t in tensors]
+
+
+class _GradBucket:
+    """One fp32 buffer that the `.grad` of every trained tensor views (layout: _trained_tensors, each offset rounded up
+    to 4 floats), so that a step's gradients are reduced by one all-reduce."""
+
+    def __init__(self, tensors, has_table, dev):
+        self.offsets, off = [], 0
+        for t in tensors:
+            self.offsets.append(off)
+            off += -(-t.numel() // 4) * 4
+        self.flat = torch.zeros(off, dtype=torch.float32, device=dev)
+        self.table_offset = self.offsets[-1] if has_table else None
+        self.table_row = tensors[-1].shape[1] if has_table else 0
+        for t, o in zip(tensors, self.offsets):
+            view = self.flat[o:o + t.numel()].view(t.shape)
+            if t.grad is not None:
+                view.copy_(t.grad)
+            t.grad = view
+        self.ptrs = _grad_ptrs(tensors)
+
+    def prefix(self, n_used: int) -> int:
+        """Floats the all-reduce covers: all of it, or up to the end of voxel-table row n_used."""
+        return self.flat.numel() if self.table_offset is None else self.table_offset + self.table_row * n_used
 
 
 class _StepPlan:
@@ -53,6 +125,7 @@ class _StepPlan:
     def __init__(self, models, emb_xyz, n, cfg, rand, dev, seed):
         lib = _lib.load()
         self.n, self.dev, self.cfg = n, dev, cfg
+        self.bucket = None              # _GradBucket of a plan made with a process group
         # the device seed of captured steps (onerf_train_step_dseed), continuing from the creating call's host seed
         self.seed_dev = torch.full((1,), seed + 4, dtype=torch.int64, device=dev)
         self.model_order = ["coarse"] + (["fine"] if cfg["N_importance"] > 0 else [])
@@ -104,6 +177,44 @@ def step_seed(models: Dict[str, Any]) -> torch.Tensor:
     return plans[0].seed_dev.clone()
 
 
+def sync_replicas(models: Dict[str, Any], embeddings: Dict[str, Any], code_library, group) -> None:
+    """Make every rank's replica rank 0's: broadcast the parameters of `models`, `embeddings` and `code_library` and the
+    voxel grid's buffers (GRID_BUFFERS; a rank whose index map has another shape gets new buffers of rank 0's shape), then
+    count the table rows the index map references (one host read).  The eager counterpart of DDP's construction-time
+    broadcast and broadcast_buffers: call it before the first train_step(group=...) and after every grid maintenance,
+    before recapturing."""
+    import torch.distributed as dist
+
+    def bcast(t):
+        dist.broadcast(t.view(torch.uint8) if t.dtype == torch.bool else t, group_src=0, group=group)
+
+    emb = embeddings["xyz"]
+    use_voxel = _is_voxel(emb)
+    n_used = 0
+    with torch.no_grad():
+        if use_voxel:
+            bcast(emb.voxel_shape)
+            shape = tuple(int(v) for v in emb.voxel_shape.tolist())
+            for name in ("voxel_idx_map", "voxel_occupancy"):
+                t = getattr(emb, name, None)
+                if t is not None and tuple(t.shape) != shape:
+                    setattr(emb, name, torch.empty(shape, dtype=t.dtype, device=t.device))
+            for name in GRID_BUFFERS[1:]:
+                if getattr(emb, name, None) is not None:
+                    bcast(getattr(emb, name))
+        seen = set()
+        for m in list(models.values()) + list(embeddings.values()) + [code_library]:
+            for p in m.parameters() if m is not None else ():
+                if id(p) not in seen:
+                    seen.add(id(p))
+                    bcast(p.detach())
+        if use_voxel:
+            m = emb.voxel_idx_map
+            rows = emb.embedding_space_ftr.weight.shape[0]
+            n_used = min(int(m.max().item()) + 1, rows) if m.numel() else 0
+    _synced[models["coarse"]] = (_grid_stamp(emb) if use_voxel else None, n_used)
+
+
 def _grad_of(p: torch.Tensor) -> torch.Tensor:
     if p.grad is None:
         p.grad = torch.zeros_like(p, memory_format=torch.contiguous_format)
@@ -122,10 +233,12 @@ def _f32_param(p: torch.Tensor) -> torch.Tensor:
 def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library, batch: Dict[str, torch.Tensor],
                loss_conf, N_samples: int = 64, use_disp: bool = False, perturb: float = 0, noise_std: float = 1,
                N_importance: int = 0, white_back: bool = False, forward_instance: bool = True,
-               frustum_bound_th: float = 0, pass_through_mask=None, rays_in_bbox: bool = False, **render_kwargs):
+               frustum_bound_th: float = 0, pass_through_mask=None, rays_in_bbox: bool = False, group=None,
+               **render_kwargs):
     """render_rays(models, embeddings, batch["rays"], ...) with the codes code_library(batch) looks up, then
     TotalLoss(loss_conf) and its backward, as one call.  Takes render_rays' keyword arguments (train.py:84-98, 155-165;
     is_eval, use_zero_as_last_delta, precision and _rand included, the rest ignored as render_rays ignores them).
+    group: a torch.distributed process group; the gradients are then averaged over its ranks (module docstring).
 
     Returns (loss_sum, terms, present, psnr) as device tensors: loss_sum (), the five unweighted terms (5,) in
     losses.TERMS order (0 where skipped), present (5,) int32 flags (TotalLoss's loss_dict holds term i iff present[i]),
@@ -148,16 +261,39 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
     use_voxel = _is_voxel(emb_xyz)
     table = emb_xyz.embedding_space_ftr.weight if use_voxel else None
     key = (dev, n, use_voxel, tuple(sorted(cfg.items())),
-           tuple(rand[k].data_ptr() if rand.get(k) is not None else 0 for k in _RAND_KEYS))
+           tuple(rand[k].data_ptr() if rand.get(k) is not None else 0 for k in _RAND_KEYS), group)
     capturing = _capturing(dev)
     seed = engine.new_seed() if not capturing and (cfg["perturb"] > 0 or cfg["noise_std"] > 0) else 0
+    code_table = code_library.embedding_instance.weight
+    if group is not None:
+        import torch.distributed as dist
+        synced = _synced.get(models["coarse"])
+        if synced is None:
+            raise RuntimeError("train_step(group=...): call training.sync_replicas(models, embeddings, code_library, "
+                               "group) before the first step, so that every rank starts from rank 0's replica")
+        if use_voxel and synced[0] != _grid_stamp(emb_xyz):
+            raise RuntimeError("train_step(group=...): the voxel grid changed since the last sync_replicas (grid "
+                               "maintenance); call training.sync_replicas again, then recapture")
+        world = dist.get_world_size(group)
+        seed = (seed + dist.get_rank(group) * RANK_SEED_STRIDE) % (1 << 62)
     plans = _plans.setdefault(models["coarse"], {})
     plan = plans.get(key)
     if plan is None:
         if capturing:
             raise RuntimeError("train_step: the first call for a configuration must run before the CUDA-graph capture "
                                "(warm up eagerly): its plan's device seed counter would be reset on every replay")
-        plan = plans[key] = _StepPlan(models, emb_xyz, n, cfg, rand, dev, seed)
+        plan = _StepPlan(models, emb_xyz, n, cfg, rand, dev, seed)
+        if group is not None:
+            trained = _trained_tensors(models, plan.model_order, code_table, table)
+            ptrs = _grad_ptrs(trained)
+            # another configuration's bucket, if the gradients still view it
+            plan.bucket = next((p.bucket for p in plans.values() if p.bucket is not None and p.bucket.ptrs == ptrs),
+                               None) or _GradBucket(trained, table is not None, dev)
+        plans[key] = plan
+    if group is not None and _grad_ptrs(_trained_tensors(models, plan.model_order, code_table, table)) != plan.bucket.ptrs:
+        raise RuntimeError("train_step(group=...): a .grad no longer views the gradient bucket this step all-reduces "
+                           "(zero_grad(set_to_none=True) or a replaced parameter?); zero the gradients with "
+                           "set_to_none=False")
     # the grid as it is now (host-side argument block only)
     plan.grid = engine.GridBuffers.from_module(emb_xyz) if use_voxel else None
     plan.render.args.grid = C.pointer(plan.grid.c) if use_voxel else None
@@ -172,7 +308,6 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
     if pass_through_mask is not None:
         plan.ptm.copy_(pass_through_mask.reshape(n))
     plan.d_codes.zero_()
-    code_table = code_library.embedding_instance.weight
     ctx, stream = _lib.ctx(dev), _lib.stream()
     keep = []
     with torch.cuda.device(dev):
@@ -203,4 +338,8 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
                                             stream))
         _lib.check(lib.onerf_code_scatter_add(ctx, plan.d_codes.data_ptr(), plan.ids.data_ptr(), n, code_table.shape[0],
                                               _grad_of(code_table).data_ptr(), stream))
+        if group is not None:
+            reduced = plan.bucket.flat[:plan.bucket.prefix(synced[1])]
+            dist.all_reduce(reduced, op=dist.ReduceOp.SUM, group=group)     # gloo has no AVG
+            reduced.mul_(1.0 / world)
     return plan.out[0], plan.out[1:], plan.present, plan.psnr[0]
