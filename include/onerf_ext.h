@@ -176,6 +176,63 @@ typedef struct onerf_batch_args {
 int onerf_draw_batch(onerf_ctx* ctx, const onerf_batch_args* args, void* stream);
 int onerf_draw_batch_dstep(onerf_ctx* ctx, const onerf_batch_args* args, uint64_t* step_dev, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * One validation image, or a contiguous tile of it, in one call (train.py:73-105, 182-223: ObjectNeRFSystem.forward over
+ * the image, TotalLoss, psnr).  Rays [ray_begin, ray_end) of the image's batch are rendered in chunks of chunk_rays rays
+ * through onerf_render_rays_fwd's passes (is_eval, nothing random); the compositing kernel of each pass also adds the
+ * ray's squared errors of the five TotalLoss terms and of the validation PSNR to `record`.  Per-sample arrays (weights,
+ * z_vals) exist only for one chunk, in the workspace.
+ *   record   ONERF_VALIDATE_RECORD_DOUBLES doubles, 8-byte aligned, zeroed by the call before it adds to it:
+ *            [0..5) element counts of the five masked means, [5] number of depths > 0 (both from the tile's batch rows),
+ *            [6..16) squared-error sums, term * 2 + (0 coarse / 1 fine), [16] PSNR squared-error sum, [17] PSNR element
+ *            count.  All sums over rays: the record of a frame is the sum of the records of its tiles, which is what a
+ *            process group all-reduces before onerf_validate_finalize.
+ *   render   as for onerf_render_rays_fwd, for the whole image: rays (n_rays,8), n_rays, models, grid, precision, sample
+ *            counts, use_disp, white_back, rays_in_bbox.  forward_instance and is_eval must be set, perturb and noise_std 0,
+ *            train_ws NULL.  codes is ignored: each chunk's codes are gathered from code_table by instance_ids.
+ *            coarse / fine: tile-sized maps (ray_end - ray_begin rows); any may be NULL: it is not written (its values
+ *            go to chunk scratch).  weights and z_vals are ignored (never tile-sized).  workspace: >=
+ *            onerf_validate_workspace_bytes(chunk_rays, n_samples, n_importance) bytes (0 for a bad shape), 256-byte
+ *            aligned; its size does not depend on the image.
+ *   loss     the image's batch rows (n_rays = render.n_rays), the term weights and, with `finalize`, the outputs
+ *            loss_sum_out, terms_out, present_out as for onerf_total_loss; maps, grad_* and workspace are unused.
+ *   psnr_mask  which rays the PSNR of the last pass's rgb averages over (train.py:185-190): ONERF_PSNR_VALID_INSTANCE =
+ *            valid_mask * instance_mask, ONERF_PSNR_ALL_RAYS = every ray, valid or not (a batch without instance_mask).
+ *   finalize 1: onerf_validate_finalize runs on the record as the call's last launch (the single-process frame);
+ *            psnr_out (1,) is then required.
+ * Every map row depends on its ray only, never on chunk_rays or the tile bounds, and is bit-identical to
+ * onerf_render_rays_fwd (is_eval = 1) over the same rays.  Refusals (ONERF_ERR_BAD_ARG): a tile outside [0, n_rays],
+ * chunk_rays < 1, forward_instance or is_eval off, a training workspace, perturb or noise_std non-zero, a NULL or
+ * misaligned record, a NULL batch buffer, a misaligned or undersized workspace.  Kernels and one memset only, no host
+ * read, no allocation: CUDA-graph capturable.
+ *
+ * onerf_validate_finalize: one single-block launch that turns a record into loss_sum (1,), the five unweighted terms
+ * (5,), the present flags (5,) (skip rules of onerf_total_loss; an empty color mask gives NaN as the reference's mean of
+ * an empty set does) and psnr (1,) = -10 log10(record[16] / record[17]) (NaN for an empty mask).  weights: host array of
+ * the five loss.*_weight.  A launch of its own, so that the record can be reduced across ranks in between.
+ * ------------------------------------------------------------------------------------------- */
+#define ONERF_VALIDATE_RECORD_DOUBLES 18
+typedef enum onerf_psnr_mask { ONERF_PSNR_VALID_INSTANCE = 0, ONERF_PSNR_ALL_RAYS = 1 } onerf_psnr_mask;
+
+typedef struct onerf_validate_args {
+  onerf_render_args render;
+  onerf_loss_args loss;
+  const int64_t* instance_ids;          /* (n_rays,) */
+  const float* code_table;              /* (n_codes,64) */
+  int n_codes;
+  int64_t ray_begin, ray_end;
+  int chunk_rays;
+  int psnr_mask;                        /* onerf_psnr_mask */
+  double* record;
+  int finalize;
+  float* psnr_out;                      /* (1,), with finalize */
+} onerf_validate_args;
+
+size_t onerf_validate_workspace_bytes(int chunk_rays, int n_samples, int n_importance);
+int onerf_validate_frame(onerf_ctx* ctx, const onerf_validate_args* args, void* stream);
+int onerf_validate_finalize(onerf_ctx* ctx, const double* record, const float weights[5], int has_fine,
+                            float* loss_sum_out, float* terms_out, int* present_out, float* psnr_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

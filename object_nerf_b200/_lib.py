@@ -38,7 +38,10 @@ EXPORTS = [
 EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_ws", "onerf_composite_multi_merge",
                "onerf_train_workspace_bytes_prec", "onerf_train_step_workspace_bytes", "onerf_train_step",
                "onerf_render_rays_fwd_dseed", "onerf_train_step_dseed", "onerf_render_edit_workspace_bytes",
-               "onerf_render_edit_frame", "onerf_draw_batch", "onerf_draw_batch_dstep"]
+               "onerf_render_edit_frame", "onerf_draw_batch", "onerf_draw_batch_dstep",
+               "onerf_validate_workspace_bytes", "onerf_validate_frame", "onerf_validate_finalize"]
+VALIDATE_RECORD_DOUBLES = 18
+PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
 
 _p = C.c_void_p
 
@@ -146,6 +149,14 @@ class BatchArgs(C.Structure):
         ("step", C.c_uint64), ("rays", _p), ("rgbs", _p), ("depths", _p), ("valid_mask", _p), ("frame_idx", _p),
         ("instance_mask", _p), ("instance_mask_weight", _p), ("instance_ids", _p), ("pass_through_mask", _p),
         ("index_out", _p),
+    ]
+
+
+class ValidateArgs(C.Structure):
+    _fields_ = [
+        ("render", RenderArgs), ("loss", LossArgs), ("instance_ids", _p), ("code_table", _p), ("n_codes", C.c_int),
+        ("ray_begin", C.c_int64), ("ray_end", C.c_int64), ("chunk_rays", C.c_int), ("psnr_mask", C.c_int),
+        ("record", _p), ("finalize", C.c_int), ("psnr_out", _p),
     ]
 
 
@@ -262,6 +273,10 @@ def load() -> C.CDLL:
         lib.onerf_render_edit_frame.argtypes = [_p, C.POINTER(RenderEditArgs), _p]
         lib.onerf_draw_batch.argtypes = [_p, C.POINTER(BatchArgs), _p]
         lib.onerf_draw_batch_dstep.argtypes = [_p, C.POINTER(BatchArgs), _p, _p]
+        lib.onerf_validate_workspace_bytes.argtypes = [C.c_int] * 3
+        lib.onerf_validate_workspace_bytes.restype = C.c_size_t
+        lib.onerf_validate_frame.argtypes = [_p, C.POINTER(ValidateArgs), _p]
+        lib.onerf_validate_finalize.argtypes = [_p, _p, C.POINTER(C.c_float), C.c_int, _p, _p, _p, _p, _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

@@ -163,6 +163,7 @@ static int render_pass(onerf_ctx* ctx, const onerf_render_args* a, const void* p
   c.pass_through_mask = a->pass_through_mask;
   c.weights = m.weights; c.opacity = m.opacity; c.rgb = m.rgb; c.depth = m.depth;
   c.rgb_instance = m.rgb_instance; c.depth_instance = m.depth_instance; c.opacity_instance = m.opacity_instance;
+  if (step && step->eval) return onerf_launch_composite_eval(ctx, &c, step, (cudaStream_t)stream);
   if (step) return onerf_launch_composite_step(ctx, &c, step, seed_dev, (cudaStream_t)stream);
   return onerf_launch_composite(ctx, &c, seed_dev, (cudaStream_t)stream);
 }
@@ -229,7 +230,12 @@ int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const oner
   // training step: the coarse pass's field gradients go to the step's extension of the workspace, the fine pass's where
   // onerf_render_rays_bwd puts them; the fine pass (or the coarse one without importance samples) finalizes the loss
   onerf_step_composite step_c, step_f;
-  if (step) {
+  if (step && step->eval) {
+    // validation: both passes add their squared errors to the record; the last pass carries the PSNR
+    step_c = step_f = *step;
+    step_c.fine = 0; step_f.fine = 1;
+    if (a->n_importance > 0) step_c.psnr = 0;
+  } else if (step) {
     ONERF_CHECK_ARG(a->train_ws, "the training step needs a training workspace");
     const TrainWs W = onerf_make_train_ws(a->precision, onerf_train_use_voxel(a), a->n_rays, a->n_samples, a->n_importance);
     const TrainStepWs T = onerf_make_train_step_ws(W, a->n_rays, a->n_samples);
@@ -526,4 +532,123 @@ extern "C" int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_a
     if (rc != ONERF_OK) return rc;
   }
   return ONERF_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// A validation image (or a tile of it) in one call: the batch counts of the tile once, then per chunk a code gather and
+// onerf_render_fwd_impl with the evaluation compositing, on the chunk's rows of the caller's maps.  Chunks are
+// independent (every stage works per ray) and only add to the record.
+// ------------------------------------------------------------------------------------------------
+struct ValidateWs {
+  float* codes;                     // (chunk,64)
+  onerf_render_maps coarse, fine;   // one chunk of each map: the per-sample arrays, and the maps the caller leaves NULL
+  void* render;                     // workspace of onerf_render_rays_fwd for one chunk
+  size_t render_bytes;
+  size_t total;
+};
+
+static ValidateWs validate_ws_layout(char* base, int chunk, int n_samples, int n_importance) {
+  const size_t n = chunk, nf = n_importance > 0 ? n : 0;
+  ValidateWs w;
+  size_t off = 0;
+  auto take = [&](size_t floats) { float* p = reinterpret_cast<float*>(base + off); off += align256(floats * sizeof(float)); return p; };
+  auto maps = [&](size_t rows, size_t S) {
+    onerf_render_maps m;
+    m.weights = take(rows * S); m.opacity = take(rows); m.z_vals = take(rows * S); m.rgb = take(rows * 3);
+    m.depth = take(rows); m.rgb_instance = take(rows * 3); m.depth_instance = take(rows); m.opacity_instance = take(rows);
+    return m;
+  };
+  w.codes = take(n * 64);
+  w.coarse = maps(n, n_samples);
+  w.fine = maps(nf, (size_t)n_samples + n_importance);
+  w.render_bytes = onerf_render_rays_workspace_bytes(chunk, n_samples, n_importance);
+  w.render = base + off;
+  off += align256(w.render_bytes);
+  w.total = off;
+  return w;
+}
+
+// rows [r0, ...) of the tile's maps, or the chunk scratch where a map is NULL; per-sample arrays always scratch
+static onerf_render_maps validate_chunk_maps(const onerf_render_maps& out, const onerf_render_maps& scratch, int64_t r0) {
+  auto at = [&](float* o, float* s, int64_t width) { return o ? o + r0 * width : s; };
+  onerf_render_maps m = scratch;
+  m.opacity = at(out.opacity, scratch.opacity, 1);
+  m.rgb = at(out.rgb, scratch.rgb, 3);
+  m.depth = at(out.depth, scratch.depth, 1);
+  m.rgb_instance = at(out.rgb_instance, scratch.rgb_instance, 3);
+  m.depth_instance = at(out.depth_instance, scratch.depth_instance, 1);
+  m.opacity_instance = at(out.opacity_instance, scratch.opacity_instance, 1);
+  return m;
+}
+
+extern "C" size_t onerf_validate_workspace_bytes(int chunk_rays, int n_samples, int n_importance) {
+  if (chunk_rays < 1 || n_samples < 2 || n_importance < 0) return 0;
+  return validate_ws_layout(nullptr, chunk_rays, n_samples, n_importance).total;
+}
+
+extern "C" int onerf_validate_frame(onerf_ctx* ctx, const onerf_validate_args* v, void* stream) {
+  ONERF_CHECK_ARG(ctx && v, "null argument");
+  const onerf_render_args& ra = v->render;
+  const onerf_loss_args& la = v->loss;
+  const int64_t n_tile = v->ray_end - v->ray_begin;
+  ONERF_CHECK_ARG(ra.n_rays >= 0 && ra.n_samples >= 2 && ra.n_importance >= 0, "bad shape");
+  ONERF_CHECK_ARG(v->ray_begin >= 0 && n_tile >= 0 && v->ray_end <= ra.n_rays, "tile outside the image");
+  ONERF_CHECK_ARG(v->chunk_rays >= 1, "chunk_rays < 1");
+  ONERF_CHECK_ARG(ra.forward_instance, "TotalLoss needs the object branch's maps: forward_instance must be set");
+  ONERF_CHECK_ARG(ra.is_eval, "validation renders with is_eval set");
+  ONERF_CHECK_ARG(!ra.train_ws, "a training workspace is refused: validation keeps nothing for a backward");
+  ONERF_CHECK_ARG(ra.perturb == 0.0f && ra.noise_std == 0.0f, "perturb and noise_std must be 0");
+  ONERF_CHECK_ARG(v->record && (reinterpret_cast<uintptr_t>(v->record) & 7u) == 0, "record null or not 8-byte aligned");
+  ONERF_CHECK_ARG(ra.rays && v->instance_ids && v->code_table, "null rays / instance_ids / code_table");
+  ONERF_CHECK_ARG(la.rgbs && la.depths && la.valid_mask && la.instance_mask && la.instance_mask_weight, "null batch buffer");
+  ONERF_CHECK_ARG(la.n_rays == ra.n_rays, "loss.n_rays differs from render.n_rays");
+  ONERF_CHECK_ARG(v->psnr_mask == ONERF_PSNR_VALID_INSTANCE || v->psnr_mask == ONERF_PSNR_ALL_RAYS, "unknown psnr_mask");
+  ONERF_CHECK_ARG(!v->finalize || (la.loss_sum_out && la.terms_out && la.present_out && v->psnr_out), "finalize with a null output");
+  const int chunk = v->chunk_rays;
+  const size_t need = onerf_validate_workspace_bytes(chunk, ra.n_samples, ra.n_importance);
+  ONERF_CHECK_ARG(ra.workspace && (reinterpret_cast<uintptr_t>(ra.workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
+  if (ra.workspace_bytes < need) {
+    onerf_set_error("onerf_validate_frame: workspace too small (%zu < %zu)", ra.workspace_bytes, need);
+    return ONERF_ERR_BAD_ARG;
+  }
+  const ValidateWs w = validate_ws_layout(reinterpret_cast<char*>(ra.workspace), chunk, ra.n_samples, ra.n_importance);
+  ONERF_CUDA(cudaMemsetAsync(v->record, 0, ONERF_VALIDATE_RECORD_DOUBLES * sizeof(double), (cudaStream_t)stream));
+  // rows [first, first + n) of the image's batch
+  auto batch_rows = [&](int64_t first, int64_t n) {
+    onerf_loss_args l = la;
+    l.n_rays = n;
+    l.rgbs += first * 3; l.depths += first; l.valid_mask += first; l.instance_mask += first; l.instance_mask_weight += first;
+    return l;
+  };
+  int rc = ONERF_OK;
+  if (n_tile > 0) {
+    const onerf_loss_args tile = batch_rows(v->ray_begin, n_tile);
+    rc = onerf_launch_batch_stats(ctx, &tile, v->record, (cudaStream_t)stream);
+    if (rc != ONERF_OK) return rc;
+  }
+  onerf_step_composite step;
+  memset(&step, 0, sizeof(step));
+  step.eval = 1;
+  step.psnr = 1 + v->psnr_mask;
+  step.acc = v->record;
+  onerf_render_args c = ra;
+  c.codes = w.codes;
+  c.workspace = w.render; c.workspace_bytes = w.render_bytes;
+  for (int64_t r0 = 0; r0 < n_tile; r0 += chunk) {
+    const int n = (int)(n_tile - r0 < chunk ? n_tile - r0 : chunk);
+    const int64_t first = v->ray_begin + r0;
+    rc = onerf_code_gather(ctx, v->code_table, v->instance_ids + first, n, v->n_codes, w.codes, stream);
+    if (rc != ONERF_OK) return rc;
+    c.rays = ra.rays + first * 8;
+    c.n_rays = n;
+    c.coarse = validate_chunk_maps(ra.coarse, w.coarse, r0);
+    if (ra.n_importance > 0) c.fine = validate_chunk_maps(ra.fine, w.fine, r0);
+    step.loss = batch_rows(first, n);
+    rc = onerf_render_fwd_impl(ctx, &c, &step, nullptr, stream);
+    if (rc != ONERF_OK) return rc;
+  }
+  if (!v->finalize) return ONERF_OK;
+  const float wt[5] = {la.color_weight, la.depth_weight, la.opacity_weight, la.instance_color_weight, la.instance_depth_weight};
+  return onerf_validate_finalize(ctx, v->record, wt, ra.n_importance > 0, la.loss_sum_out, la.terms_out, la.present_out,
+                                 v->psnr_out, stream);
 }

@@ -102,7 +102,11 @@ __device__ __forceinline__ Acc composite_branch(const float* __restrict__ z, con
 // (composite_bwd.cuh).  Per-block sums of the squared errors go to the fp64 accumulators; with `finalize` the last block
 // to finish turns them into the loss outputs and the PSNR, and advances *seed_dev (train_ws.h: device seed), which every
 // block has read by then.
-template <bool kStep>
+// kEval (with kStep = false): the validation frame's compositing (onerf_validate_frame): the forward, then the ray's
+// squared errors added to the same accumulators and, on the pass `st.psnr` selects, to the validation PSNR pair
+// (loss_terms.cuh: VR_PSNR_*).  No gradients, no backward, no finalisation: the record is summed over chunks, tiles and
+// ranks before validate_finalize_kernel (loss.cu) reads it.
+template <bool kStep, bool kEval = false>
 __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, onerf_step_composite st, uint64_t* seed_dev) {
   using namespace loss_terms;
   extern __shared__ float smem_c[];
@@ -113,6 +117,7 @@ __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, 
   if (seed_dev && a.noise_std > 0.0f) seed += *seed_dev;
   float *s_alpha = nullptr, *s_trans = nullptr, *s_sig = nullptr, *s_gw = nullptr;
   double sq[N_TERMS] = {0.0, 0.0, 0.0, 0.0, 0.0};   // lane 0: squared-error sums of this warp's rays
+  double psnr[2] = {0.0, 0.0};                       // lane 0, kEval: masked squared-error sum and element count
   float scale[N_TERMS];
   if (kStep) {
     s_alpha = smem_c + (size_t)warp * 4 * S;
@@ -141,6 +146,13 @@ __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, 
       a.rgb[r * 3 + 2] = rgb[2];
     }
     Target tg;
+    if (kEval) {
+      tg = load_target(st.loss, r);
+      if (lane == 0) {
+        add_scene_sq(tg, rgb, sc.depth, sq, 1);
+        add_psnr_sq(tg, st.psnr, rgb, psnr);
+      }
+    }
     if (kStep) {
       tg = load_target(st.loss, r);
       if (lane == 0) add_scene_sq(tg, rgb, sc.depth, sq, 1);
@@ -169,6 +181,7 @@ __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, 
         a.rgb_instance[r * 3 + 1] = irgb[1];
         a.rgb_instance[r * 3 + 2] = irgb[2];
       }
+      if (kEval && lane == 0) add_object_sq(tg, ob.opacity, irgb, ob.depth, sq, 1);
       if (kStep) {
         if (lane == 0) add_object_sq(tg, ob.opacity, irgb, ob.depth, sq, 1);
         float go, gi[3], gid;
@@ -179,6 +192,23 @@ __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, 
         __syncwarp();
       }
     }
+  }
+  if (kEval) {
+    __shared__ double red_e[8][N_TERMS + 2];
+    if (lane == 0) {
+      for (int t = 0; t < N_TERMS; ++t) red_e[warp][t] = sq[t];
+      red_e[warp][N_TERMS] = psnr[0];
+      red_e[warp][N_TERMS + 1] = psnr[1];
+    }
+    __syncthreads();
+    if (threadIdx.x < N_TERMS + 2) {
+      double v = 0.0;
+      for (int w = 0; w < warps_per_block; ++w) v += red_e[w][threadIdx.x];
+      double* dst = threadIdx.x < N_TERMS ? st.acc + WS_SUM + 2 * threadIdx.x + st.fine
+                                          : st.acc + VR_PSNR_SUM + (threadIdx.x - N_TERMS);
+      if (v != 0.0) atomicAdd(dst, v);
+    }
+    return;
   }
   if (!kStep) return;
   __shared__ double red[8][N_TERMS];
@@ -487,6 +517,17 @@ int onerf_launch_composite(onerf_ctx* ctx, const onerf_composite_args* a, uint64
   onerf_step_composite none;
   memset(&none, 0, sizeof(none));
   composite_kernel<false><<<blocks, warps * 32, 0, stream>>>(*a, none, seed_dev);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
+int onerf_launch_composite_eval(onerf_ctx* ctx, const onerf_composite_args* a, const onerf_step_composite* t,
+                                cudaStream_t stream) {
+  if (a->n_rays == 0) return ONERF_OK;
+  const int warps = 8;
+  int blocks = (a->n_rays + warps - 1) / warps;
+  if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
+  composite_kernel<false, true><<<blocks, warps * 32, 0, stream>>>(*a, *t, nullptr);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

@@ -3,6 +3,8 @@
 // depth), each over the coarse and the fine maps; under autograd the reference runs ~120 elementwise / index / reduce
 // kernels and several host syncs (`mask.sum() == 0`) for 2 048 rays.  Here: one reduction pass (counts and weighted
 // squared-error sums, fp64 accumulators) and one pass that writes d(loss_sum)/d(map) for all ten maps and the loss values.
+#include <string.h>
+
 #include "loss_terms.cuh"
 #include "train_ws.h"
 
@@ -94,6 +96,14 @@ __global__ void __launch_bounds__(256) loss_grad_kernel(LossParams P, const doub
   }
 }
 
+// A validation record (onerf_validate_frame) to the loss outputs, with loss_grad_kernel's arithmetic (write_outputs), and
+// the validation PSNR.  One thread: 18 doubles in, 12 values out.
+__global__ void validate_finalize_kernel(LossParams P, const double* __restrict__ record, float* __restrict__ psnr_out) {
+  if (threadIdx.x != 0) return;
+  write_outputs(P.a, record);
+  *psnr_out = (float)(-10.0 * log10(record[VR_PSNR_SUM] / record[VR_PSNR_COUNT]));   // 0 / 0: NaN, as mean([])
+}
+
 int loss_grid(onerf_ctx* ctx, int64_t n_rays) {
   const int64_t want = (n_rays + 255) / 256;
   return (int)(want < (int64_t)ctx->num_sms * 4 ? want : (int64_t)ctx->num_sms * 4);
@@ -130,6 +140,23 @@ int onerf_launch_batch_stats(onerf_ctx* ctx, const onerf_loss_args* a, double* w
   LossParams P;
   P.a = *a;
   batch_stats_kernel<<<loss_grid(ctx, a->n_rays), 256, 0, stream>>>(P, ws);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
+extern "C" int onerf_validate_finalize(onerf_ctx* ctx, const double* record, const float weights[5], int has_fine,
+                                       float* loss_sum_out, float* terms_out, int* present_out, float* psnr_out,
+                                       void* stream) {
+  ONERF_CHECK_ARG(ctx && record && weights, "null argument");
+  ONERF_CHECK_ARG(loss_sum_out && terms_out && present_out && psnr_out, "null output");
+  ONERF_CHECK_ARG((reinterpret_cast<uintptr_t>(record) & 7u) == 0, "record must be 8-byte aligned");
+  LossParams P;
+  memset(&P, 0, sizeof(P));
+  P.a.has_fine = has_fine;
+  P.a.color_weight = weights[0]; P.a.depth_weight = weights[1]; P.a.opacity_weight = weights[2];
+  P.a.instance_color_weight = weights[3]; P.a.instance_depth_weight = weights[4];
+  P.a.loss_sum_out = loss_sum_out; P.a.terms_out = terms_out; P.a.present_out = present_out;
+  validate_finalize_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(P, record, psnr_out);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

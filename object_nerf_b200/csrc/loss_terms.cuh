@@ -3,6 +3,7 @@
 // one ray.  The scene maps (rgb, depth) carry the color and depth terms, the object maps the other three.
 #pragma once
 #include "common.cuh"
+#include "../../include/onerf_ext.h"
 
 namespace loss_terms {
 
@@ -10,6 +11,10 @@ enum { T_COLOR = 0, T_DEPTH, T_OPACITY, T_ICOLOR, T_IDEPTH, N_TERMS };
 // accumulators (doubles): [0..5) mask counts per term (elements of the masked mean), [5] number of targets > 0,
 // [6..16) squared-error sums: term * 2 + (0 coarse / 1 fine)
 enum { WS_COUNT = 0, WS_TPOS = 5, WS_SUM = 6, WS_DOUBLES = 16 };
+// the validation record (onerf_validate_frame) is the accumulators followed by the validation PSNR's masked
+// squared-error sum and element count (train.py:185-190, :220)
+enum { VR_PSNR_SUM = WS_DOUBLES, VR_PSNR_COUNT, VR_DOUBLES };
+static_assert(VR_DOUBLES == ONERF_VALIDATE_RECORD_DOUBLES, "record size declared in onerf_ext.h");
 
 __device__ __forceinline__ float clamp01(float x) { return fminf(fmaxf(x, 0.0f), 1.0f); }
 
@@ -59,6 +64,15 @@ __device__ __forceinline__ void add_object_sq(const Target& g, float opacity, co
     sum[stride * T_ICOLOR] += (double)(e0 * e0 * g.w) + (double)(e1 * e1 * g.w) + (double)(e2 * e2 * g.w);
     if (g.tpos) { const float e = depth - g.t; sum[stride * T_IDEPTH] += (double)(e * e * g.w); }
   }
+}
+
+// the validation PSNR's share of one ray: psnr = 0 (this pass is not the one measured), 1 + ONERF_PSNR_VALID_INSTANCE
+// (mask = valid_mask * instance_mask) or 1 + ONERF_PSNR_ALL_RAYS (mask = None: every ray, valid or not)
+__device__ __forceinline__ void add_psnr_sq(const Target& g, int psnr, const float* rgb, double* acc) {
+  if (psnr == 0 || (psnr == 1 + ONERF_PSNR_VALID_INSTANCE && !(g.valid && g.inst))) return;
+  const float e0 = rgb[0] - g.rgb[0], e1 = rgb[1] - g.rgb[1], e2 = rgb[2] - g.rgb[2];
+  acc[0] += (double)(e0 * e0) + (double)(e1 * e1) + (double)(e2 * e2);
+  acc[1] += 3.0;
 }
 
 // term present (the reference returns None otherwise): models/losses.py:13-14, :46-47, :51-52, :80-81

@@ -94,6 +94,10 @@ struct onerf_step_composite {
   float* psnr_out;
   float* dscene;          // (N,S,4) d(r, g, b, sigma) of the scene branch
   float* dobj;            // (N,S,4) of the object branch
+  // validation (onerf_validate_frame, onerf_launch_composite_eval): `loss` holds the chunk's batch rows, `acc` is the
+  // frame's record; the kernel only adds the pass's squared errors - finalize, psnr_out, dscene and dobj are unused
+  int eval;
+  int psnr;               // eval: 0 = this pass adds nothing to the PSNR pair, else 1 + onerf_psnr_mask
 };
 // Device seed (onerf_ext.h: onerf_render_rays_fwd_dseed, onerf_train_step_dseed): every launcher below that takes
 // `seed_dev` draws with seed + *seed_dev read when its kernel runs if seed_dev != NULL (the caller then passes only the
@@ -102,6 +106,8 @@ struct onerf_step_composite {
 #define ONERF_SEED_ADVANCE 4
 int onerf_launch_composite_step(onerf_ctx* ctx, const onerf_composite_args* c, const onerf_step_composite* t,
                                 uint64_t* seed_dev, cudaStream_t stream);
+int onerf_launch_composite_eval(onerf_ctx* ctx, const onerf_composite_args* c, const onerf_step_composite* t,
+                                cudaStream_t stream);
 int onerf_launch_composite(onerf_ctx* ctx, const onerf_composite_args* c, uint64_t* seed_dev, cudaStream_t stream);
 int onerf_launch_seed_advance(onerf_ctx* ctx, uint64_t* seed_dev, cudaStream_t stream);   // one thread: *seed_dev += 4
 int onerf_launch_sample_coarse(onerf_ctx* ctx, const float* rays, int n_rays, int n_samples, int use_disp, float perturb,
@@ -112,6 +118,8 @@ int onerf_launch_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, const f
 int onerf_launch_batch_stats(onerf_ctx* ctx, const onerf_loss_args* a, double* acc, cudaStream_t stream);
 // onerf_render_rays_fwd with an optional training step: step == NULL is the plain forward; otherwise both passes'
 // compositing runs onerf_launch_composite_step with `step` (fine / finalize / dscene / dobj set per pass from ws_step),
-// and the finalizing one advances *seed_dev.  seed_dev as above; a->seed is ignored when it is set.
+// and the finalizing one advances *seed_dev.  seed_dev as above; a->seed is ignored when it is set.  With step->eval
+// the passes composite with onerf_launch_composite_eval instead (fine set per pass, psnr kept on the last pass only)
+// and no training workspace is involved.
 int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const onerf_step_composite* step, uint64_t* seed_dev,
                           void* stream);

@@ -44,6 +44,19 @@ fire because the step writes `.grad` without autograd):
     the device counter.  A deliberate difference from the reference: its ranks start from identical torch generators
     and would draw the same jitter and noise at the same batch positions.  Injected `_rand` buffers still win;
   - the returned loss, terms, flags and PSNR are this rank's (train.py logs them per rank).
+
+Validation (`validate_frame`, `install_validation`): the other half of train.py's loop, one validation image per call
+(onerf_validate_frame, include/onerf_ext.h).  The image runs through render_rays' passes (is_eval, perturb = 0,
+noise_std = 0: nothing is random) in chunks of `chunk` rays; each pass's compositing kernel also adds the ray's squared
+errors of the five TotalLoss terms and of the validation PSNR to an 18-double record, and one more launch turns the
+record into the loss outputs.  Only the requested maps of the last pass are image-sized; weights and z_vals exist for
+one chunk at a time.  Like the step it reads nothing back, allocates nothing after the first call for a shape (a plan
+per coarse model and configuration owns the buffers; the returned tensors are overwritten by the next call of the same
+plan) and can be captured: the batch tensors are read in place when they already have the kernels' types (float32,
+int64 ids, bool or uint8 masks, 8 ray columns), so a replay validates whatever they hold by then, with the weights
+re-packed from the parameters as they are by then.  With `group=` rank r renders parallel.shard_bounds(n_rays, W, r),
+the records are all-reduced (SUM, float64) before the finalising launch, so every rank returns the loss and PSNR of the
+whole image, and the maps are all-gathered (parallel.gather_tiles, which allocates the gathered tensors).
 """
 from __future__ import annotations
 
@@ -53,10 +66,10 @@ from typing import Any, Dict
 
 import torch
 
-from . import _lib, backward, engine
+from . import _lib, backward, editing, engine, parallel
 from .losses import TERMS
 
-__all__ = ["train_step", "step_seed", "sync_replicas"]
+__all__ = ["train_step", "step_seed", "sync_replicas", "validate_frame", "install_validation"]
 
 _RAND_KEYS = ("jitter", "u", "noise_scene_coarse", "noise_obj_coarse", "noise_scene_fine", "noise_obj_fine")
 # coarse model -> {configuration: plan}; a plan references no module, so it lives exactly as long as the model
@@ -343,3 +356,177 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
             dist.all_reduce(reduced, op=dist.ReduceOp.SUM, group=group)     # gloo has no AVG
             reduced.mul_(1.0 / world)
     return plan.out[0], plan.out[1:], plan.present, plan.psnr[0]
+
+
+# ------------------------------------------------------------------------------------------------
+# validation
+# ------------------------------------------------------------------------------------------------
+# what utils/train_helper.visualize_val_image reads of the last pass
+VAL_KEYS = ("rgb", "depth", "rgb_instance", "depth_instance", "opacity_instance")
+_VAL_WIDTHS = {"opacity": 1, "rgb": 3, "depth": 1, "rgb_instance": 3, "depth_instance": 1, "opacity_instance": 1}
+_val_plans: "weakref.WeakKeyDictionary[Any, Dict[tuple, _ValPlan]]" = weakref.WeakKeyDictionary()
+
+
+class _ValPlan:
+    """Every buffer one configuration of validate_frame owns: the record, the outputs, the packed weights, the tile's
+    maps and, for a batch without instance_mask, the all-zero mask and weight."""
+
+    def __init__(self, models, n, tile, cfg, keys, dev, use_voxel):
+        lib = _lib.load()
+        self.model_order = ["coarse"] + (["fine"] if cfg["N_importance"] > 0 else [])
+        self.typ = self.model_order[-1]
+        f = lambda *shape, dtype=torch.float32: torch.empty(*shape, dtype=dtype, device=dev)
+        self.record = torch.zeros(_lib.VALIDATE_RECORD_DOUBLES, dtype=torch.float64, device=dev)
+        self.out, self.present, self.psnr = f(1 + len(TERMS)), f(len(TERMS), dtype=torch.int32), f(1)
+        self.no_inst = self.no_weight = None
+        if not cfg["has_instance_mask"]:
+            self.no_inst = torch.zeros(n, dtype=torch.uint8, device=dev)
+            self.no_weight = torch.zeros(n, dtype=torch.float32, device=dev)
+        nbytes = lib.onerf_packed_weights_bytes(int(use_voxel))
+        self.packed = {}
+        for typ in self.model_order:
+            engine.check_architecture(models[typ], use_voxel)
+            blob = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
+            off = (-blob.data_ptr()) % 1024
+            self.packed[typ] = blob[off:off + nbytes]
+        self.maps = {f"{k}_{self.typ}": f(tile, 3) if _VAL_WIDTHS[k] == 3 else f(tile) for k in keys}
+        self.weights = (C.c_float * len(TERMS))(*cfg["loss_weights"])
+        a = self.args = _lib.ValidateArgs()
+        r, la = a.render, a.loss
+        r.n_rays, r.n_samples, r.n_importance = n, cfg["N_samples"], cfg["N_importance"]
+        r.precision = engine.PRECISIONS[cfg["precision"]]
+        r.use_disp, r.white_back, r.rays_in_bbox = int(cfg["use_disp"]), int(cfg["white_back"]), int(cfg["rays_in_bbox"])
+        r.forward_instance, r.is_eval = 1, 1
+        r.packed_coarse = self.packed["coarse"].data_ptr()
+        r.packed_fine = self.packed["fine"].data_ptr() if "fine" in self.packed else None
+        for k in keys:
+            setattr(getattr(r, self.typ), k, self.maps[f"{k}_{self.typ}"].data_ptr())
+        la.n_rays, la.has_fine = n, int(self.typ == "fine")
+        (la.color_weight, la.depth_weight, la.opacity_weight, la.instance_color_weight,
+         la.instance_depth_weight) = cfg["loss_weights"]
+        la.loss_sum_out, la.terms_out, la.present_out = self.out.data_ptr(), self.out[1:].data_ptr(), self.present.data_ptr()
+        a.chunk_rays = cfg["chunk"]
+        a.psnr_mask = _lib.PSNR_VALID_INSTANCE if cfg["has_instance_mask"] else _lib.PSNR_ALL_RAYS
+        a.record, a.psnr_out = self.record.data_ptr(), self.psnr.data_ptr()
+
+
+def _batch_rows(t: torch.Tensor, n: int, width: int, dtype) -> torch.Tensor:
+    """batch[key] with the loader's leading dimension of 1 dropped, in the kernels' type; the tensor itself when it has
+    that type already."""
+    t = t.reshape((n, width) if width > 1 else (n,))
+    if t.dtype == torch.bool and dtype == torch.uint8:
+        t = t.view(torch.uint8)
+    return t.to(dtype).contiguous()
+
+
+def validate_frame(models: Dict[str, Any], embeddings: Dict[str, Any], code_library, batch: Dict[str, torch.Tensor],
+                   loss_conf, *, N_samples: int, N_importance: int, use_disp: bool, white_back: bool,
+                   rays_in_bbox: bool = False, chunk: int = 65536, keys=VAL_KEYS, precision: str = "bf16", group=None):
+    """One validation image as train.py's validation_step computes it (train.py:182-223): render_rays over batch["rays"]
+    with is_eval=True and the codes of batch["instance_ids"], TotalLoss(loss_conf) on the maps and the PSNR of the last
+    pass's rgb, as one library call.  `batch` is what val_dataloader yields (leading dimension 1; the first 8 ray columns
+    are used).  The PSNR averages over valid_mask * instance_mask, or over every ray when the batch has no
+    instance_mask; such a batch is taken as one without instance pixels (mask and weight 0).
+
+    Returns {"loss_sum": (), "terms": (5,) unweighted in losses.TERMS order (0 where skipped), "present": (5,) int32,
+    "psnr": ()} plus, for every k in `keys` (of opacity, rgb, depth, rgb_instance, depth_instance, opacity_instance),
+    the image-sized map f"{k}_fine" (f"{k}_coarse" without a fine pass), all on the device.  The default keys are what
+    utils/train_helper.visualize_val_image reads.  group: see the module docstring."""
+    keys = tuple(keys)
+    unknown = [k for k in keys if k not in _VAL_WIDTHS]
+    if unknown:
+        raise KeyError(f"validate_frame: no such map {unknown} (choose from {sorted(_VAL_WIDTHS)})")
+    if int(chunk) < 1:
+        raise ValueError("validate_frame: chunk must be at least 1 ray")
+    rays = batch["rays"]
+    if rays.shape[-1] < 8:
+        raise ValueError(f"validate_frame: rays need 8 columns (o, d, near, far), got {rays.shape[-1]}")
+    rays = rays.reshape(-1, rays.shape[-1])[:, :8]
+    n, dev = rays.shape[0], rays.device
+    lib = _lib.load()
+    ctx = _lib.ctx(dev)
+    emb_xyz = embeddings["xyz"]
+    use_voxel = _is_voxel(emb_xyz)
+    has_mask = "instance_mask" in batch
+    cfg = dict(N_samples=int(N_samples), N_importance=int(N_importance), use_disp=bool(use_disp),
+               white_back=bool(white_back), rays_in_bbox=bool(rays_in_bbox), chunk=int(chunk),
+               precision="bf16" if precision == "bf16" else "fp32", has_instance_mask=has_mask,
+               loss_weights=tuple(float(loss_conf[f"{t}_weight"]) for t in TERMS))
+    begin, end = 0, n
+    if group is not None:
+        import torch.distributed as dist
+        begin, end = parallel.shard_bounds(n, dist.get_world_size(group), dist.get_rank(group))
+    plans = _val_plans.setdefault(models["coarse"], {})
+    key = (dev, n, begin, end, use_voxel, tuple(sorted(cfg.items())), keys)
+    plan = plans.get(key)
+    if plan is None:
+        plan = plans[key] = _ValPlan(models, n, end - begin, cfg, keys, dev, use_voxel)
+    a = plan.args
+    code_table = _f32_param(code_library.embedding_instance.weight)
+    # what the call reads, alive until it has been enqueued (a captured call reads the same tensors on every replay)
+    held = [_batch_rows(rays, n, 8, torch.float32), _batch_rows(batch["rgbs"], n, 3, torch.float32),
+            _batch_rows(batch["depths"], n, 1, torch.float32), _batch_rows(batch["valid_mask"], n, 1, torch.uint8),
+            _batch_rows(batch["instance_mask"], n, 1, torch.uint8) if has_mask else plan.no_inst,
+            _batch_rows(batch["instance_mask_weight"], n, 1, torch.float32) if has_mask else plan.no_weight,
+            _batch_rows(batch["instance_ids"], n, 1, torch.int64)]
+    (a.render.rays, a.loss.rgbs, a.loss.depths, a.loss.valid_mask, a.loss.instance_mask, a.loss.instance_mask_weight,
+     a.instance_ids) = (t.data_ptr() for t in held)
+    a.code_table, a.n_codes = code_table.data_ptr(), code_table.shape[0]
+    grid = engine.GridBuffers.from_module(emb_xyz) if use_voxel else None
+    a.render.grid = C.pointer(grid.c) if use_voxel else None
+    a.ray_begin, a.ray_end, a.finalize = begin, end, int(group is None)
+    ws = editing._workspace(lib.onerf_validate_workspace_bytes(cfg["chunk"], cfg["N_samples"], cfg["N_importance"]), dev)
+    a.render.workspace, a.render.workspace_bytes = ws.data_ptr(), ws.numel()
+    stream = _lib.stream()
+    with torch.cuda.device(dev):
+        for typ in plan.model_order:
+            lin = engine.model_linears(models[typ])
+            Wp = (C.c_void_p * 20)(*[_f32_param(w).data_ptr() for w, _ in lin])
+            Bp = (C.c_void_p * 20)(*[_f32_param(b).data_ptr() for _, b in lin])
+            _lib.check(lib.onerf_pack_weights(ctx, int(use_voxel), Wp, Bp, plan.packed[typ].data_ptr(),
+                                              plan.packed[typ].numel(), stream))
+        _lib.check(lib.onerf_validate_frame(ctx, C.byref(a), stream))
+        maps = dict(plan.maps)
+        if group is not None:
+            dist.all_reduce(plan.record, op=dist.ReduceOp.SUM, group=group)
+            _lib.check(lib.onerf_validate_finalize(ctx, plan.record.data_ptr(), plan.weights, a.loss.has_fine,
+                                                   plan.out.data_ptr(), plan.out[1:].data_ptr(), plan.present.data_ptr(),
+                                                   plan.psnr.data_ptr(), stream))
+            maps = {k: parallel.gather_tiles(v, n, group) for k, v in maps.items()}
+    return {"loss_sum": plan.out[0], "terms": plan.out[1:], "present": plan.present, "psnr": plan.psnr[0], **maps}
+
+
+def install_validation(system_cls, *, chunk: int = 65536, group=None):
+    """Replace `validation_step` of `system_cls` (the reference's ObjectNeRFSystem, train.py:182-223) by one that runs
+    validate_frame: the same `log` dict (val_loss, the present terms under the reference's names, val_psnr), the same
+    `self.log("val/...")` calls, and visualize_val_image for the first image.  The image renders without jitter and
+    sigma noise whatever config.model.perturb / noise_std say.  Leaving absent terms out of the dict needs the five
+    flags on the host: one 20-byte read per image, the only one.  The logged values are copies (validation_epoch_end
+    stacks them over the images; validate_frame's own outputs are overwritten by the next image).
+    chunk, group: as validate_frame."""
+    import sys
+
+    def validation_step(self, batch, batch_nb):
+        conf = self.config
+        res = validate_frame(self.models, self.embeddings, self.code_library, batch, conf.loss,
+                             N_samples=conf.model.N_samples, N_importance=conf.model.N_importance,
+                             use_disp=conf.model.use_disp, white_back=self.val_dataset.white_back,
+                             rays_in_bbox=getattr(self.val_dataset, "is_rays_in_bbox", lambda: False)(),
+                             chunk=chunk, group=group)
+        flags = res["present"].tolist()
+        terms = res["terms"].clone()
+        loss_dict = {t: terms[i] for i, t in enumerate(TERMS) if flags[i]}
+        for k, v in loss_dict.items():
+            self.log(f"val/{k}", v)
+        log = {"val_loss": res["loss_sum"].clone()}
+        log.update(loss_dict)
+        typ = "fine" if conf.model.N_importance > 0 else "coarse"
+        if batch_nb == 0:
+            visualize = sys.modules[system_cls.__module__].visualize_val_image
+            stack_image = visualize(conf.img_wh, batch, res, typ=typ)
+            self.logger.experiment.add_images("val/GT_pred_depth", stack_image, self.global_step)
+        log["val_psnr"] = res["psnr"].clone()
+        return log
+
+    system_cls.validation_step = validation_step
+    return system_cls
