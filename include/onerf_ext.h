@@ -233,6 +233,55 @@ int onerf_validate_frame(onerf_ctx* ctx, const onerf_validate_args* args, void* 
 int onerf_validate_finalize(onerf_ctx* ctx, const double* record, const float weights[5], int has_fine,
                             float* loss_sum_out, float* terms_out, int* present_out, float* psnr_out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Voxel pruning (EmbeddingVoxel.self_pruning_empty_voxels, models/embedding_helper.py:202-245), in two launches so that a
+ * process group can all-gather the per-voxel maxima in between.
+ *
+ * onerf_prune_measure: for every voxel k of the shard [cell_begin, cell_end) of cells (K = n_cells rows (i, j, l), the
+ * order of torch.nonzero(voxel_occupancy)), max_alpha_out[k - cell_begin] = the largest alpha = 1 - exp(-relu(sigma))
+ * of the scene branch's density over the voxel's 4096 samples.  Sample s of voxel k sits at
+ *   centre + (r * voxel_size - voxel_size / 2),   centre = float(cell) * voxel_size - voxel_offset
+ * (fp32, each operation rounded on its own, the reference's order), r = jitter row k * 4096 + s, or without jitter
+ * component c of r = philox4x32 uniform of stream 6 at element (k * 4096 + s) * 3 + c, keyed by seed (the draw of
+ * onerf_sample_coarse's stream 0 with another stream id).  Rows of a voxel depend on k, never on the shard.
+ *   grid       required: the voxel model only.  packed: its onerf_pack_weights blob.
+ *   precision  ONERF_PREC_BF16: one fused tensor-core pass (sigma bit-identical to onerf_field_fwd's scene branch on the
+ *              same points); ONERF_PREC_FP32: per chunk of 32 voxels, the points, onerf_field_fwd's FFMA field (scene
+ *              only) and a per-voxel maximum.
+ *   jitter     (n_cells * 4096, 3) U[0,1), indexed by the global k, or NULL.
+ *   max_alpha_out  (cell_end - cell_begin,) floats, 4-byte aligned; zeroed by the call first.
+ *   workspace  >= onerf_prune_workspace_bytes(precision) bytes, 256-byte aligned (0 bytes for bf16: may be NULL).
+ * Refusals (ONERF_ERR_BAD_ARG): null ctx / args / grid / packed, null cells with K > 0, null max_alpha_out with a
+ * non-empty shard, a shard outside [0, K], misaligned cells / jitter / max_alpha_out / workspace, an unknown precision;
+ * ONERF_ERR_WORKSPACE: a workspace that is too small.
+ *
+ * onerf_prune_apply: every voxel k in [0, n_cells) with max_alpha[k] < max_alpha_th gets occupancy[cell] = 0 and
+ * idx_map[cell] = -1 (dense (X, dim_y, dim_z) arrays, uint8 and int64); *n_pruned (int64, device) = their count.
+ * Table rows are not renumbered.  Refusals (ONERF_ERR_BAD_ARG): null pointers, K < 0, dim_y or dim_z < 1, misaligned
+ * buffers.
+ * Both calls enqueue kernels and memsets only, with no host read.
+ * ------------------------------------------------------------------------------------------- */
+#define ONERF_PRUNE_SAMPLES 4096
+
+typedef struct onerf_prune_args {
+  const onerf_grid* grid;
+  const void* packed;
+  int precision;                        /* onerf_precision */
+  const int64_t* cells;                 /* (n_cells,3) */
+  int64_t n_cells;
+  int64_t cell_begin, cell_end;
+  const float* jitter;                  /* (n_cells * 4096,3) or NULL */
+  uint64_t seed;
+  float* max_alpha_out;                 /* (cell_end - cell_begin,) */
+  void* workspace;
+  size_t workspace_bytes;
+} onerf_prune_args;
+
+size_t onerf_prune_workspace_bytes(int precision);
+int onerf_prune_measure(onerf_ctx* ctx, const onerf_prune_args* args, void* stream);
+int onerf_prune_apply(onerf_ctx* ctx, const int64_t* cells, int64_t n_cells, const float* max_alpha, float max_alpha_th,
+                      int64_t dim_y, int64_t dim_z, uint8_t* occupancy, int64_t* idx_map, int64_t* n_pruned, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

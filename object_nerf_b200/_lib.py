@@ -39,8 +39,10 @@ EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_w
                "onerf_train_workspace_bytes_prec", "onerf_train_step_workspace_bytes", "onerf_train_step",
                "onerf_render_rays_fwd_dseed", "onerf_train_step_dseed", "onerf_render_edit_workspace_bytes",
                "onerf_render_edit_frame", "onerf_draw_batch", "onerf_draw_batch_dstep",
-               "onerf_validate_workspace_bytes", "onerf_validate_frame", "onerf_validate_finalize"]
+               "onerf_validate_workspace_bytes", "onerf_validate_frame", "onerf_validate_finalize",
+               "onerf_prune_workspace_bytes", "onerf_prune_measure", "onerf_prune_apply"]
 VALIDATE_RECORD_DOUBLES = 18
+PRUNE_SAMPLES = 4096
 PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
 
 _p = C.c_void_p
@@ -157,6 +159,14 @@ class ValidateArgs(C.Structure):
         ("render", RenderArgs), ("loss", LossArgs), ("instance_ids", _p), ("code_table", _p), ("n_codes", C.c_int),
         ("ray_begin", C.c_int64), ("ray_end", C.c_int64), ("chunk_rays", C.c_int), ("psnr_mask", C.c_int),
         ("record", _p), ("finalize", C.c_int), ("psnr_out", _p),
+    ]
+
+
+class PruneArgs(C.Structure):
+    _fields_ = [
+        ("grid", C.POINTER(Grid)), ("packed", _p), ("precision", C.c_int), ("cells", _p), ("n_cells", C.c_int64),
+        ("cell_begin", C.c_int64), ("cell_end", C.c_int64), ("jitter", _p), ("seed", C.c_uint64), ("max_alpha_out", _p),
+        ("workspace", _p), ("workspace_bytes", C.c_size_t),
     ]
 
 
@@ -277,6 +287,10 @@ def load() -> C.CDLL:
         lib.onerf_validate_workspace_bytes.restype = C.c_size_t
         lib.onerf_validate_frame.argtypes = [_p, C.POINTER(ValidateArgs), _p]
         lib.onerf_validate_finalize.argtypes = [_p, _p, C.POINTER(C.c_float), C.c_int, _p, _p, _p, _p, _p]
+        lib.onerf_prune_workspace_bytes.argtypes = [C.c_int]
+        lib.onerf_prune_workspace_bytes.restype = C.c_size_t
+        lib.onerf_prune_measure.argtypes = [_p, C.POINTER(PruneArgs), _p]
+        lib.onerf_prune_apply.argtypes = [_p, _p, C.c_int64, _p, C.c_float, C.c_int64, C.c_int64, _p, _p, _p, _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

@@ -22,6 +22,7 @@
 #include "field_common.cuh"
 #include "tc_chain.cuh"
 #include "field_pe.cuh"
+#include "prune.cuh"
 
 namespace {
 
@@ -451,6 +452,144 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
   }
 }
 
+// =============================== pruning pass (sigma only, voxel model) ===============================
+// EmbeddingVoxel.self_pruning_empty_voxels (reference models/embedding_helper.py:202-245) on the tensor cores: the
+// samples are generated in the encoder warps (prune.cuh), only the scene branch's layers S0..S7 and the sigma head run,
+// and each warp folds the alpha of its 16 rows into the voxel's maximum with one atomicMax.  A 128-row tile lies inside
+// one voxel (4096 % 128 == 0): tile t of the launch is tiles [32 k, 32 k + 32) of voxel k = cell_begin + t / 32.
+struct PruneTcParams {
+  TcParams t;              // t.f: grid, packed, L; t.layers: G_S0..G_S7
+  PruneSource src;
+  int64_t cell_begin, n_cells;   // the shard [cell_begin, cell_begin + n_cells) of src.cells
+  uint32_t* max_alpha;     // (n_cells,) float bits, zeroed by the caller
+};
+constexpr int kPruneTilesPerVoxel = kPruneSamples / TM;
+static_assert(kPruneSamples % TM == 0, "a tile must lie inside one voxel");
+
+// encoder_loop<true> with the sample positions of prune_point instead of rays and depths: the same jobs and helpers,
+// so a point's X is bit for bit what field_tc_kernel builds for the same xyz.  No row metadata: every row is live.
+__device__ __forceinline__ void prune_encoder_loop(const PruneTcParams& Q, uint32_t sX, uint32_t x_full, uint32_t x_free,
+                                                   int64_t n_tiles) {
+  const int et = threadIdx.x - NUM_CONSUMER - 32;
+  const GridView g = load_grid_view(Q.t.f.grid);
+  uint32_t it = 0;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+    const int64_t k = Q.cell_begin + tile / kPruneTilesPerVoxel;
+    const int s0 = (int)(tile % kPruneTilesPerVoxel) * TM;
+#pragma unroll 1
+    for (int job = et; job < 4 * TM; job += NUM_ENCODER) {
+      const int row = job & (TM - 1), cq = job / TM;
+      float p[3];
+      prune_point(Q.src, g, k, s0 + row, p);
+      if (cq < 3) {
+        float f[8];
+        if (cq == 0) voxel_trilinear<0, 8, false>(g, p[0], p[1], p[2], f);
+        else if (cq == 1) voxel_trilinear<8, 8, false>(g, p[0], p[1], p[2], f);
+        else voxel_trilinear<16, 8, false>(g, p[0], p[1], p[2], f);
+        mbar_wait(x_free, (it & 1) ^ 1, Q.t.diag);
+        pe8_to_chunks(sX, row, cq < 2 ? cq : 34, cq < 2 ? 2 : 1, f);
+      } else {
+        mbar_wait(x_free, (it & 1) ^ 1, Q.t.diag);
+        pe_xyz_to_chunks(sX, row, 26, p[0], p[1], p[2]);
+        st_chunk(a_chunk_addr(sX, row, 47), 0u, 0u, 0u, 0u);
+      }
+    }
+    mbar_wait(x_free, (it & 1) ^ 1, Q.t.diag);
+    fence_async_smem();
+    mbar_arrive(x_full);
+  }
+}
+
+__global__ void __launch_bounds__(NUM_THREADS, 1) prune_tc_kernel(const __grid_constant__ PruneTcParams Q) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const TcParams& P = Q.t;
+  const FieldParams& p = P.f;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  constexpr int X_ATOMS = 6, XS = 9;
+
+  // shared memory: field_tc_kernel's carve-up without the row metadata
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t sX = sbase;
+  const uint32_t sB = sX + X_ATOMS * ATOM_BYTES;
+  const uint32_t sBias = sB + NSTAGE * STAGE_BYTES;
+  const uint32_t sBar = sBias + G_COUNT * 256 * 4;
+  const uint32_t x_full = sBar + 16 * NSTAGE, x_free = x_full + 8;
+  float* bias_tab = reinterpret_cast<float*>(smem_raw + (sBias - smem_u32(smem_raw)));
+  const float* Pf = reinterpret_cast<const float*>(p.packed);
+  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u, P.diag};
+
+  if (threadIdx.x == 0) {
+    mbar_init(x_full, NUM_ENCODER);
+    mbar_init(x_free, NUM_CONSUMER / 32);
+    ring_init_bars(ring.full, ring.empty);
+  }
+  for (int i = threadIdx.x; i < G_COUNT * 256; i += NUM_THREADS) {
+    const int g = i >> 8, c = i & 255;
+    bias_tab[i] = (c < p.L.g[g].N) ? __ldg(Pf + p.L.g[g].bias_off + c) : 0.0f;
+  }
+  __syncthreads();
+
+  const int64_t n_tiles = Q.n_cells * kPruneTilesPerVoxel;
+  if (warp >= PRODUCER_WARP) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == PRODUCER_WARP)
+      tc_producer_loop(P.layers, P.n_layers, reinterpret_cast<const uint8_t*>(p.packed), ring, n_tiles);
+    else
+      prune_encoder_loop(Q, sX, x_full, x_free, n_tiles);
+    return;
+  }
+  setmaxnreg_inc<CONSUMER_REGS>();
+
+  const int wg = warp >> 2;
+  const uint32_t sXw = sX + (uint32_t)wg * 64u * 128u;
+  const float* sw = Pf + p.L.sigma_w;
+  const float sb = __ldg(Pf + p.L.sigma_b);
+  Rows R;
+  R.row[0] = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  R.row[1] = R.row[0] + 8;
+  R.live[0] = R.live[1] = 1;
+#ifdef ONERF_FIELD_TIMELINE
+  R.tl = nullptr;
+#endif
+  uint32_t it = 0;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+    R.tile = tile;
+    mbar_wait(x_full, it & 1, P.diag);
+    // the scene branch of field_tc_kernel up to its sigma head (models/nerf_model.py:97-112)
+    float acc[128];
+    uint32_t h[64];
+    float part[2][4] = {};
+    run_layer<256, XS, 0, EPI_HIDDEN, false>(P, R, ring, sXw, acc, h, h, bias_tab + G_S0 * 256, 0, nullptr, part, 1, -1,
+                                             x_free, false);
+#pragma unroll 1
+    for (int l = 1; l < 4; ++l)
+      run_layer<256, 0, 8, EPI_HIDDEN, false>(P, R, ring, sXw, acc, h, h, bias_tab + (G_S0 + l) * 256, 0, nullptr, part,
+                                              1 + l, -1);
+    run_layer<256, XS, 8, EPI_HIDDEN, false>(P, R, ring, sXw, acc, h, h, bias_tab + G_S4 * 256, 0, nullptr, part, 5, -1,
+                                             x_free, true);
+#pragma unroll 1
+    for (int l = 5; l < 7; ++l)
+      run_layer<256, 0, 8, EPI_HIDDEN, false>(P, R, ring, sXw, acc, h, h, bias_tab + (G_S0 + l) * 256, 0, nullptr, part,
+                                              1 + l, -1);
+    run_layer<256, 0, 8, EPI_HIDDEN_SIGMA, false>(P, R, ring, sXw, acc, h, h, bias_tab + G_S7 * 256, 0, sw, part, 8, -1);
+    // sigma as write_heads forms it (same lane sums, same bias add), then the warp's largest alpha
+    float m = 0.0f;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      part[r][0] += __shfl_xor_sync(0xffffffffu, part[r][0], 1);
+      part[r][0] += __shfl_xor_sync(0xffffffffu, part[r][0], 2);
+      m = fmaxf(m, prune_alpha(part[r][0] + sb));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    // lane 0 folds it into the voxel's slot; the lane test is a predicate inside the asm statement (see ring_release)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, %2, 0;\n\t@p red.global.max.u32 [%0], %1;\n\t}" ::"l"(
+                     Q.max_alpha + tile / kPruneTilesPerVoxel),
+                 "r"(__float_as_uint(m)), "r"(lane)
+                 : "memory");
+  }
+}
+
 }  // namespace
 
 int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t stream) {
@@ -487,6 +626,27 @@ int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t 
   };
   if (L.use_voxel) return fp.train_ws ? launch(field_tc_kernel<true, true>) : launch(field_tc_kernel<true, false>);
   return fp.train_ws ? launch(field_tc_kernel<false, true>) : launch(field_tc_kernel<false, false>);
+}
+
+int onerf_launch_prune_bf16(onerf_ctx* ctx, const FieldParams& fp, const PruneSource& src, int64_t cell_begin,
+                            int64_t n_cells, float* max_alpha, cudaStream_t stream) {
+  const PackLayout& L = fp.L;
+  PruneTcParams Q;
+  memset(&Q, 0, sizeof(Q));
+  Q.t.f = fp;
+  for (int g = G_S0; g <= G_S7; ++g) Q.t.layers[Q.t.n_layers++] = WLayer{L.g[g].img_off, L.g[g].N, L.g[g].K / 32};
+  Q.t.diag = ctx->tc_diag;
+  Q.src = src;
+  Q.cell_begin = cell_begin;
+  Q.n_cells = n_cells;
+  Q.max_alpha = reinterpret_cast<uint32_t*>(max_alpha);
+  const int64_t tiles = n_cells * kPruneTilesPerVoxel;
+  const int blocks = (int)(tiles < ctx->num_sms ? tiles : ctx->num_sms);
+  const size_t smem = 1024 + (size_t)6 * ATOM_BYTES + NSTAGE * STAGE_BYTES + G_COUNT * 256 * 4 + 16 * NSTAGE + 16;
+  ONERF_CUDA(cudaFuncSetAttribute(prune_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  prune_tc_kernel<<<blocks, NUM_THREADS, smem, stream>>>(Q);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
 }
 
 #ifdef ONERF_FIELD_TIMELINE

@@ -7,6 +7,8 @@ fused CUDA kernels; calling these modules directly uses the stand-alone encode k
 """
 from __future__ import annotations
 
+import ctypes as C
+
 import numpy as np
 import torch
 import torch.nn.functional as F
@@ -96,25 +98,42 @@ class EmbeddingVoxel(nn.Module):
         voxel_xyz = idx_occu.float() * self.voxel_size - self.voxel_offset
         return idx_occu, voxel_xyz
 
-    def self_pruning_empty_voxels(self, model, max_alpha_th=0.5, precision=None, _rand=None, _sigma_fn=None):
+    def self_pruning_empty_voxels(self, model, max_alpha_th=0.5, precision=None, _rand=None, _sigma_fn=None, *,
+                                  seed=None, group=None):
         """Reference :202-245: drop every occupied voxel whose largest alpha over 16^3 jittered samples
         (`1 - exp(-relu(sigma))`, scene branch of `model`) stays below max_alpha_th: occupancy -> False, index map -> -1.
-        The density comes from the fused kernel (`rendering.query_sigma`) instead of `self.forward` + `model(...,
-        sigma_only=True)` (upstream's call at :223 passes a tensor to `forward(inputs: dict)`; the intended semantics
-        are kept).  precision: arithmetic of the density query (None = the library default).  _rand: optional list of U[0,1) tensors, one (32 * 4096, 3) block per 32-voxel chunk (tests);
-        _sigma_fn(xyz) -> sigma overrides the density query (CPU tests of the grid logic)."""
-        from . import rendering
+        Returns the number of voxels dropped (one host read).  Table rows are not renumbered.
+
+        The pass runs on the device in two library calls (include/onerf_ext.h): onerf_prune_measure generates every
+        voxel's samples and reduces them to the voxel's largest alpha (bf16: one fused tensor-core launch that evaluates
+        only the layers sigma needs; fp32: the FFMA field chunk by chunk), onerf_prune_apply clears the cells below the
+        threshold.  The density is the scene branch's, as `self.forward` + `model(..., sigma_only=True)` intend
+        (upstream's call at :223 passes a tensor to `forward(inputs: dict)`).
+          precision  arithmetic of the density (None = the library default).
+          seed       Philox seed of the jitter (None: engine.new_seed(), so torch.manual_seed makes a run reproducible).
+                     The jitter has torch.rand_like's distribution, not its bits.
+          group      torch.distributed process group: rank 0's seed is broadcast, rank r measures the voxels
+                     parallel.shard_bounds(K, W, r), the maxima are all-gathered and every rank applies the same mask,
+                     so the grids stay identical across ranks.  A grouped train_step still wants sync_replicas after it
+                     (training.py: any grid change).
+          _rand      list of U[0,1) tensors, one (32 * 4096, 3) block per 32-voxel chunk: the jitter instead of Philox
+                     (tests).
+          _sigma_fn  xyz -> sigma: the reference's host loop over 32-voxel chunks with this density (CPU tests of the
+                     grid logic)."""
+        if _sigma_fn is None:
+            return self._prune_on_device(model, max_alpha_th, precision, _rand, seed, group)
+        if group is not None:
+            raise ValueError("group= needs the device pass: _sigma_fn runs the host loop on one process")
         idx_occu, voxel_xyz = self._occupied()
         n_occu = voxel_xyz.shape[0]
         n_per_voxel, per_batch = 16 ** 3, 32
-        sigma_fn = _sigma_fn or (lambda pts: rendering.query_sigma(model, self, pts, precision=precision))
         empty = []
         for k, i in enumerate(range(0, n_occu, per_batch)):
             centres = voxel_xyz[i:i + per_batch]
             samples = centres[:, None, :].expand(-1, n_per_voxel, -1).reshape(-1, 3).clone()
             r = _rand[k][:samples.shape[0]].to(samples) if _rand is not None else torch.rand_like(samples)
             samples += r * self.voxel_size - self.voxel_size / 2
-            sigmas = sigma_fn(samples).reshape(-1)
+            sigmas = _sigma_fn(samples).reshape(-1)
             alphas = 1 - torch.exp(-torch.relu(sigmas))
             empty.append(alphas.view(-1, n_per_voxel).max(-1)[0] < max_alpha_th)
         empty_mask = torch.cat(empty, 0) if empty else torch.zeros(0, dtype=torch.bool, device=voxel_xyz.device)
@@ -122,6 +141,60 @@ class EmbeddingVoxel(nn.Module):
         self.voxel_occupancy[idx_empty[:, 0], idx_empty[:, 1], idx_empty[:, 2]] = False
         self.voxel_idx_map[idx_empty[:, 0], idx_empty[:, 1], idx_empty[:, 2]] = -1
         return int(idx_empty.shape[0])
+
+    def _prune_on_device(self, model, max_alpha_th, precision, _rand, seed, group):
+        from . import _lib, parallel
+        occ = self.voxel_occupancy
+        cells = torch.nonzero(occ).contiguous()        # (CPU nonzero returns a column-major result)
+        n_cells = cells.shape[0]
+        if n_cells == 0:
+            return 0
+        dev = occ.device
+        world, rank = 1, 0
+        if group is not None:
+            import torch.distributed as dist
+            world, rank = dist.get_world_size(group), dist.get_rank(group)
+        jitter = None
+        if _rand is not None:
+            # block i holds chunk i's rows: concatenated, row k * 4096 + s is sample s of voxel k
+            per = 32 * _lib.PRUNE_SAMPLES
+            blocks = [r[:min(per, (n_cells - i * 32) * _lib.PRUNE_SAMPLES)] for i, r in enumerate(_rand[:(n_cells + 31) // 32])]
+            jitter = torch.cat(blocks).to(device=dev, dtype=torch.float32).contiguous()
+            if jitter.shape != (n_cells * _lib.PRUNE_SAMPLES, 3):
+                raise ValueError(f"_rand holds {jitter.shape[0]} jitter rows for {n_cells} voxels x 4096 samples")
+            seed = 0
+        elif seed is None:
+            seed = engine.new_seed()
+        if group is not None and jitter is None:
+            t = torch.tensor([seed], dtype=torch.int64, device=dev)
+            dist.broadcast(t, group_src=0, group=group)
+            seed = int(t.item())
+        begin, end = parallel.shard_bounds(n_cells, world, rank)
+        max_alpha = torch.zeros(end - begin, dtype=torch.float32, device=dev)
+        grid = self.grid_buffers()
+        packed = engine.packed_for(model, True)
+        prec = engine.PRECISIONS[precision or engine.default_precision()]
+        lib = _lib.load()
+        with torch.cuda.device(dev):
+            ctx = _lib.ctx(dev)
+            ws = torch.empty(lib.onerf_prune_workspace_bytes(prec), dtype=torch.uint8, device=dev)
+            a = _lib.PruneArgs()
+            a.grid, a.packed, a.precision = C.pointer(grid.c), packed.data_ptr(), prec
+            a.cells, a.n_cells, a.cell_begin, a.cell_end = _lib.ptr(cells), n_cells, begin, end
+            a.jitter, a.seed = _lib.ptr(jitter), seed
+            a.max_alpha_out = _lib.ptr(max_alpha)
+            a.workspace, a.workspace_bytes = (ws.data_ptr() if ws.numel() else None), ws.numel()
+            _lib.check(lib.onerf_prune_measure(ctx, C.byref(a), _lib.stream()))
+            if group is not None:
+                max_alpha = parallel.gather_tiles(max_alpha, n_cells, group)
+            n_pruned = torch.zeros(1, dtype=torch.int64, device=dev)
+            _lib.check(lib.onerf_prune_apply(ctx, _lib.ptr(cells), n_cells, _lib.ptr(max_alpha), float(max_alpha_th),
+                                             occ.shape[1], occ.shape[2], _lib.ptr(occ), _lib.ptr(self.voxel_idx_map),
+                                             n_pruned.data_ptr(), _lib.stream()))
+        # the library wrote the buffers in place: count it as an in-place change (training._grid_stamp)
+        torch.autograd.graph.increment_version(occ)
+        torch.autograd.graph.increment_version(self.voxel_idx_map)
+        return int(n_pruned.item())
 
     def voxel_subdivision(self, _features_fn=None):
         """Reference :247-302: halve the voxel size.  Every occupied voxel spawns its 8 children

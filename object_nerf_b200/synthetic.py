@@ -181,6 +181,23 @@ class GridModule(torch.nn.Module):
         self.register_buffer("voxel_shape", g["shape"].clone())
 
 
+def make_embedding(g):
+    """An EmbeddingVoxel holding grid `g` (make_grid) with occupancy = idx_map >= 0 (the state the reference's grid has
+    after construction, here without a point cloud), so that grid maintenance can run on it."""
+    from .embedding_helper import EmbeddingVoxel
+    emb = EmbeddingVoxel.__new__(EmbeddingVoxel)
+    torch.nn.Module.__init__(emb)
+    emb.channels, emb.instance_ftr_C = N_VOX_CH, 8
+    emb.embedding_space_ftr = torch.nn.Embedding.from_pretrained(g["table"].clone(), freeze=False)
+    emb.register_buffer("voxel_size", g["voxel_size"].clone())
+    emb.register_buffer("voxel_offset", g["offset"].clone())
+    emb.register_buffer("voxel_shape", g["shape"].clone())
+    emb.register_buffer("voxel_count", torch.scalar_tensor(int(g["idx_map"].numel())))
+    emb.register_buffer("voxel_occupancy", g["idx_map"] >= 0)
+    emb.register_buffer("voxel_idx_map", g["idx_map"].clone())
+    return emb
+
+
 def make_code_library(table):
     from .code_library import CodeLibrary
     lib = CodeLibrary(model_config())

@@ -39,7 +39,8 @@ fire because the step writes `.grad` without autograd):
     reduction captures in the step's CUDA graph;
   - `sync_replicas` must have run since the last change to the grid: it broadcasts rank 0's parameters and grid (DDP's
     construction-time broadcast and broadcast_buffers) and counts n_used.  Call it before training and after every
-    grid maintenance (pruning draws its jitter per rank, so the ranks' grids differ after it);
+    grid maintenance (pruning without `group=` draws its jitter per rank, so the ranks' grids differ after it; with
+    `group=` they stay identical, and the rule still holds);
   - rank r draws with the seed a group-less call would use plus r * 2^52 (mod 2^62), both the host seed and the start of
     the device counter.  A deliberate difference from the reference: its ranks start from identical torch generators
     and would draw the same jitter and noise at the same batch positions.  Injected `_rand` buffers still win;
