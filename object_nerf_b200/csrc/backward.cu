@@ -6,7 +6,7 @@
 // field_fp32.cu), then per layer  dZ = dH * act'(H),  dW += dZ^T In (split over samples, atomics),  db += colsum(dZ),
 // dIn = dZ W  with the generic GEMM below; concatenations are handled with leading dimensions / column offsets.
 // Orchestration: bwd_api.cu (onerf_render_rays_bwd with ONERF_PREC_FP32).
-#include "composite_bwd.cuh"
+#include "composite_core.cuh"
 #include "encode.cuh"
 #include "field_common.cuh"
 
@@ -15,58 +15,11 @@ namespace {
 // ------------------------------------------------------------------------------------------------
 // compositing backward: one warp per ray
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float warp_scan_mul(float v, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    float t = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v *= t;
-  }
-  return v;
-}
 struct BranchGrad {
   const float* g_rgb;      // (N,3) or null
   const float* g_depth;    // (N,) or null
   const float* g_opacity;  // (N,) or null
 };
-
-// Recompute alpha / transmittance of one branch of one ray, then back-propagate (composite_bwd.cuh).
-// smem (per warp): alpha[S], trans[S], sig[S], gw[S]
-__device__ __forceinline__ void composite_branch_bwd(const float* __restrict__ z, const float4* __restrict__ field, int S,
-                                                     float last_delta, float noise_std, const float* __restrict__ noise,
-                                                     uint64_t seed, uint32_t stream_id, int ray, bool use_mask, float z_limit, bool white, float g_r, float g_g,
-                                                     float g_b, float g_d, float g_o, float4* __restrict__ dfield,
-                                                     float* s_alpha, float* s_trans, float* s_sig, float* s_gw, int lane) {
-  // forward recompute
-  float carry = 1.0f;
-  for (int base = 0; base < S; base += 32) {
-    const int i = base + lane;
-    float alpha = 0.0f, s = 0.0f;
-    if (i < S) {
-      const float zi = __ldg(z + i);
-      const float delta = (i + 1 < S) ? __fsub_rn(__ldg(z + i + 1), zi) : last_delta;
-      s = __ldg(field + i).w;
-      if (noise_std > 0.0f) {   // the forward's noise: the caller's buffer, or the same Philox draw (composite.cu)
-        const float nz = noise ? __ldg(noise + i) : philox_normal(seed, stream_id, (uint64_t)ray * S + i);
-        s = __fadd_rn(s, __fmul_rn(nz, noise_std));
-      }
-      alpha = __fsub_rn(1.0f, expf(__fmul_rn(-delta, fmaxf(s, 0.0f))));
-      if (use_mask && z_limit < zi) alpha = 0.0f;
-    }
-    const float t = (i < S) ? __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f) : 1.0f;
-    const float incl = warp_scan_mul(t, lane);
-    float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-    if (lane == 0) excl = 1.0f;
-    if (i < S) {
-      s_alpha[i] = alpha;
-      s_trans[i] = carry * excl;
-      s_sig[i] = s;
-    }
-    carry *= __shfl_sync(0xffffffffu, incl, 31);
-  }
-  __syncwarp();
-  composite_branch_grad(z, field, S, last_delta, use_mask, z_limit, white, g_r, g_g, g_b, g_d, g_o, dfield, s_alpha, s_trans,
-                        s_sig, s_gw, lane);
-}
 
 struct CompositeBwdArgs {
   onerf_composite_args fwd;   // same inputs as the forward (outputs unused)
@@ -76,6 +29,9 @@ struct CompositeBwdArgs {
   float* dobj;                // (N,S,4) or null
 };
 
+// Per branch: composite_branch recomputes the forward's alpha / transmittance / noised sigma (the caller's noise buffer
+// or the same Philox draw) into the warp's shared memory, then composite_branch_grad back-propagates, the sequence
+// composite_kernel<true> (composite.cu) runs.  smem (per warp): alpha[S], trans[S], sig[S], gw[S]
 __global__ void __launch_bounds__(128) composite_bwd_kernel(CompositeBwdArgs a) {
   extern __shared__ float smem_c[];
   const int warps_per_block = blockDim.x >> 5;
@@ -89,21 +45,27 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(CompositeBwdArgs a) 
     const float* z = a.fwd.z + (int64_t)r * S;
     auto g3 = [&](const float* p, int c) { return p ? __ldg(p + (int64_t)r * 3 + c) : 0.0f; };
     auto g1 = [&](const float* p) { return p ? __ldg(p + r) : 0.0f; };
-    composite_branch_bwd(z, reinterpret_cast<const float4*>(a.fwd.scene) + (int64_t)r * S, S,
-                         a.fwd.zero_last_delta ? 0.0f : 1e10f, a.fwd.noise_std,
-                         a.fwd.noise_scene ? a.fwd.noise_scene + (int64_t)r * S : nullptr, a.fwd.seed, 2u, r, false, 0.0f,
-                         a.fwd.white_back != 0, g3(a.gs.g_rgb, 0), g3(a.gs.g_rgb, 1), g3(a.gs.g_rgb, 2), g1(a.gs.g_depth),
-                         g1(a.gs.g_opacity), reinterpret_cast<float4*>(a.dscene) + (int64_t)r * S, s_alpha, s_trans, s_sig, s_gw,
-                         lane);
+    const float4* scene = reinterpret_cast<const float4*>(a.fwd.scene) + (int64_t)r * S;
+    const float scene_last_delta = a.fwd.zero_last_delta ? 0.0f : 1e10f;
+    composite_branch(z, scene, S, scene_last_delta, a.fwd.noise_std,
+                     a.fwd.noise_scene ? a.fwd.noise_scene + (int64_t)r * S : nullptr, a.fwd.seed, 2u, r, false, 0.0f,
+                     nullptr, lane, s_alpha, s_trans, s_sig);
+    __syncwarp();
+    composite_branch_grad(z, scene, S, scene_last_delta, false, 0.0f, a.fwd.white_back != 0, g3(a.gs.g_rgb, 0),
+                          g3(a.gs.g_rgb, 1), g3(a.gs.g_rgb, 2), g1(a.gs.g_depth), g1(a.gs.g_opacity),
+                          reinterpret_cast<float4*>(a.dscene) + (int64_t)r * S, s_alpha, s_trans, s_sig, s_gw, lane);
     __syncwarp();
     if (a.fwd.obj != nullptr) {
       bool use_mask = (!a.fwd.is_eval) && (a.fwd.frustum_bound_th > 0.0f);
       if (use_mask && a.fwd.pass_through_mask && a.fwd.pass_through_mask[r]) use_mask = false;
       const float z_limit = __fadd_rn(__ldg(a.depth_scene + r), a.fwd.frustum_bound_th);
-      composite_branch_bwd(z, reinterpret_cast<const float4*>(a.fwd.obj) + (int64_t)r * S, S, 0.0f, a.fwd.noise_std,
-                           a.fwd.noise_obj ? a.fwd.noise_obj + (int64_t)r * S : nullptr, a.fwd.seed, 3u, r, use_mask, z_limit, true,
-                           g3(a.go.g_rgb, 0), g3(a.go.g_rgb, 1), g3(a.go.g_rgb, 2), g1(a.go.g_depth), g1(a.go.g_opacity),
-                           reinterpret_cast<float4*>(a.dobj) + (int64_t)r * S, s_alpha, s_trans, s_sig, s_gw, lane);
+      const float4* obj = reinterpret_cast<const float4*>(a.fwd.obj) + (int64_t)r * S;
+      composite_branch(z, obj, S, 0.0f, a.fwd.noise_std, a.fwd.noise_obj ? a.fwd.noise_obj + (int64_t)r * S : nullptr,
+                       a.fwd.seed, 3u, r, use_mask, z_limit, nullptr, lane, s_alpha, s_trans, s_sig);
+      __syncwarp();
+      composite_branch_grad(z, obj, S, 0.0f, use_mask, z_limit, true, g3(a.go.g_rgb, 0), g3(a.go.g_rgb, 1),
+                            g3(a.go.g_rgb, 2), g1(a.go.g_depth), g1(a.go.g_opacity),
+                            reinterpret_cast<float4*>(a.dobj) + (int64_t)r * S, s_alpha, s_trans, s_sig, s_gw, lane);
       __syncwarp();
     }
   }
@@ -309,9 +271,7 @@ extern "C" int onerf_composite_bwd(onerf_ctx* ctx, const onerf_composite_args* f
   const int warps = 4;
   const size_t smem = (size_t)warps * 4 * fwd->n_samples * sizeof(float);
   ONERF_CUDA(cudaFuncSetAttribute(composite_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int blocks = (fwd->n_rays + warps - 1) / warps;
-  if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
-  composite_bwd_kernel<<<blocks, warps * 32, smem, (cudaStream_t)stream>>>(a);
+  composite_bwd_kernel<<<composite_blocks(ctx, fwd->n_rays, warps), warps * 32, smem, (cudaStream_t)stream>>>(a);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

@@ -69,6 +69,35 @@ int onerf_launch_camera_rays(onerf_ctx* ctx, int H, int W, float focal, const fl
 static inline bool onerf_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // ---------------------------------------------------------------------------------------------
+// warp helpers
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// Ascending bitonic sort of keys[0, P) (P a power of two, shared memory) by the whole warp, after the warp's writes to
+// keys.  Pad with keys that sort last.  The compare-exchange is (a > b) == up: float keys holding NaN end where that
+// rule puts them.
+template <typename T>
+__device__ __forceinline__ void warp_bitonic_sort(T* keys, int P, int lane) {
+  __syncwarp();
+  for (int k2 = 2; k2 <= P; k2 <<= 1) {
+    for (int j = k2 >> 1; j > 0; j >>= 1) {
+      for (int t = lane; t < (P >> 1); t += 32) {
+        const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));  // index with bit j cleared
+        const int l = i | j;
+        const bool up = ((i & k2) == 0);
+        const T a = keys[i], b = keys[l];
+        if ((a > b) == up) { keys[i] = b; keys[l] = a; }
+      }
+      __syncwarp();
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Philox4x32-10 counter RNG (used only when the caller does not inject its own random buffers)
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint4 philox4x32(uint4 ctr, uint2 key) {

@@ -1,6 +1,6 @@
 // sigma -> alpha -> transmittance-weighted compositing, single-scene (scene + object branch) and the
 // multi-object joint-sort variant.  One warp per ray, samples strided over lanes (coalesced float /
-// float4 access), multiplicative warp scan for the exclusive transmittance product.
+// float4 access); the scan itself is composite_core.cuh's composite_scan.
 //
 // Reference behaviour: models/rendering.py:139-229; render_tools/multi_rendering.py:96-157.
 #include <string.h>
@@ -8,98 +8,18 @@
 #include <algorithm>
 
 #include "common.cuh"
-#include "composite_bwd.cuh"
+#include "composite_core.cuh"
 #include "loss_terms.cuh"
 #include "train_ws.h"
 #include "../../include/onerf_ext.h"
 
 namespace {
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// inclusive multiplicative warp scan
-__device__ __forceinline__ float warp_scan_mul(float v, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    float t = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v *= t;
-  }
-  return v;
-}
-
-__device__ __forceinline__ float alpha_from(float sigma, float delta) {
-  // 1 - exp(-delta * relu(sigma))   (models/rendering.py:157)
-  return __fsub_rn(1.0f, expf(__fmul_rn(-delta, fmaxf(sigma, 0.0f))));
-}
-
-struct Acc {
-  float opacity, r, g, b, depth;
-};
-
-// Composite one branch of one ray.  field = (S,4) rgb,sigma.  Returns warp-reduced sums on all lanes.
-// If w_out != nullptr the per-sample weights are stored; if s_alpha != nullptr, what composite_branch_grad reads
-// (composite_bwd.cuh: alpha, transmittance, noised sigma) goes to the warp's shared memory.
-__device__ __forceinline__ Acc composite_branch(const float* __restrict__ z, const float4* __restrict__ field,
-                                                int S, float last_delta, float noise_std,
-                                                const float* __restrict__ noise, uint64_t seed,
-                                                uint32_t stream_id, int64_t ray, bool use_mask, float z_limit,
-                                                float* __restrict__ w_out, int lane, float* s_alpha = nullptr,
-                                                float* s_trans = nullptr, float* s_sig = nullptr) {
-  Acc acc = {0.f, 0.f, 0.f, 0.f, 0.f};
-  float carry = 1.0f;  // prod_{j < chunk start} (1 - alpha_j + 1e-10)
-  for (int base = 0; base < S; base += 32) {
-    const int i = base + lane;
-    float alpha = 0.0f, zi = 0.0f;
-    float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (i < S) {
-      zi = __ldg(z + i);
-      const float delta = (i + 1 < S) ? __fsub_rn(__ldg(z + i + 1), zi) : last_delta;
-      f = __ldg(field + i);
-      float s = f.w;
-      if (noise_std > 0.0f) {
-        const float nz = noise ? __ldg(noise + i) : philox_normal(seed, stream_id, (uint64_t)ray * S + i);
-        s = __fadd_rn(s, __fmul_rn(nz, noise_std));
-      }
-      alpha = alpha_from(s, delta);
-      if (use_mask && z_limit < zi) alpha = 0.0f;  // occlusion mask, models/rendering.py:192-202
-      if (s_sig) s_sig[i] = s;
-    }
-    const float t = (i < S) ? __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f) : 1.0f;
-    const float incl = warp_scan_mul(t, lane);
-    float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-    if (lane == 0) excl = 1.0f;
-    const float w = alpha * (carry * excl);
-    if (s_alpha && i < S) {
-      s_alpha[i] = alpha;
-      s_trans[i] = carry * excl;
-    }
-    carry *= __shfl_sync(0xffffffffu, incl, 31);
-    if (i < S) {
-      if (w_out) w_out[i] = w;
-      acc.opacity += w;
-      acc.r += w * f.x;
-      acc.g += w * f.y;
-      acc.b += w * f.z;
-      acc.depth += w * zi;
-    }
-  }
-  acc.opacity = warp_sum(acc.opacity);
-  acc.r = warp_sum(acc.r);
-  acc.g = warp_sum(acc.g);
-  acc.b = warp_sum(acc.b);
-  acc.depth = warp_sum(acc.depth);
-  return acc;
-}
-
 // kStep = false: the forward (onerf_composite).  kStep = true: the training step's compositing (onerf_train_step): the
 // same forward, then per ray the squared errors of the loss terms this pass owns and their gradients w.r.t. the ray's
 // maps (loss_terms.cuh; the normalisers depend on the batch only, so they are known before the render), then the
 // compositing backward of both branches on the alpha / transmittance the forward left in shared memory
-// (composite_bwd.cuh).  Per-block sums of the squared errors go to the fp64 accumulators; with `finalize` the last block
+// (composite_core.cuh).  Per-block sums of the squared errors go to the fp64 accumulators; with `finalize` the last block
 // to finish turns them into the loss outputs and the PSNR, and advances *seed_dev (train_ws.h: device seed), which every
 // block has read by then.
 // kEval (with kStep = false): the validation frame's compositing (onerf_validate_frame): the forward, then the ray's
@@ -131,9 +51,10 @@ __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, 
     const bool obj_weights_out = (a.obj != nullptr) && a.rays_in_bbox;
     const float scene_last_delta = a.zero_last_delta ? 0.0f : 1e10f;
     const float4* scene = reinterpret_cast<const float4*>(a.scene) + (int64_t)r * S;
-    Acc sc = composite_branch(z, scene, S, scene_last_delta, a.noise_std,
-                              a.noise_scene ? a.noise_scene + (int64_t)r * S : nullptr, seed, 2u, r, false,
-                              0.0f, obj_weights_out ? nullptr : a.weights + (int64_t)r * S, lane, s_alpha, s_trans, s_sig);
+    const Acc sc = warp_sum(composite_branch(z, scene, S, scene_last_delta, a.noise_std,
+                                             a.noise_scene ? a.noise_scene + (int64_t)r * S : nullptr, seed, 2u, r, false,
+                                             0.0f, obj_weights_out ? nullptr : a.weights + (int64_t)r * S, lane, s_alpha,
+                                             s_trans, s_sig));
     // white background: rgb + 1 - opacity, models/rendering.py:178-179
     const float rgb[3] = {a.white_back ? __fadd_rn(__fadd_rn(sc.r, 1.0f), -sc.opacity) : sc.r,
                           a.white_back ? __fadd_rn(__fadd_rn(sc.g, 1.0f), -sc.opacity) : sc.g,
@@ -168,9 +89,10 @@ __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, 
       if (use_mask && a.pass_through_mask && a.pass_through_mask[r]) use_mask = false;
       const float z_limit = __fadd_rn(sc.depth, a.frustum_bound_th);
       const float4* obj = reinterpret_cast<const float4*>(a.obj) + (int64_t)r * S;
-      Acc ob = composite_branch(z, obj, S, 0.0f, a.noise_std, a.noise_obj ? a.noise_obj + (int64_t)r * S : nullptr, seed,
-                                3u, r, use_mask, z_limit, obj_weights_out ? a.weights + (int64_t)r * S : nullptr, lane,
-                                s_alpha, s_trans, s_sig);
+      const Acc ob = warp_sum(composite_branch(z, obj, S, 0.0f, a.noise_std,
+                                               a.noise_obj ? a.noise_obj + (int64_t)r * S : nullptr, seed, 3u, r, use_mask,
+                                               z_limit, obj_weights_out ? a.weights + (int64_t)r * S : nullptr, lane,
+                                               s_alpha, s_trans, s_sig));
       // always composited on white, models/rendering.py:223
       const float irgb[3] = {__fadd_rn(__fadd_rn(ob.r, 1.0f), -ob.opacity), __fadd_rn(__fadd_rn(ob.g, 1.0f), -ob.opacity),
                              __fadd_rn(__fadd_rn(ob.b, 1.0f), -ob.opacity)};
@@ -248,6 +170,24 @@ __device__ __forceinline__ uint32_t float_order_key(float f) {
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
+// Offset of concatenated index c = obj * S + s of a ray in object-major storage [obj][ray][s] (obj_stride = n_rays * S),
+// relative to sample 0 of the ray's first set.
+__device__ __forceinline__ int64_t src_off(int c, int S, int64_t obj_stride) {
+  return (int64_t)(c / S) * obj_stride + (c % S);
+}
+
+// lane 0 writes a multi-object ray's maps from the warp's sums
+__device__ __forceinline__ void store_multi_maps(const Acc& acc, int white_back, int r, int lane, float* __restrict__ opacity,
+                                                 float* __restrict__ rgb, float* __restrict__ depth) {
+  if (lane == 0) {
+    opacity[r] = acc.opacity;
+    depth[r] = acc.depth;
+    rgb[r * 3 + 0] = white_back ? __fadd_rn(__fadd_rn(acc.r, 1.0f), -acc.opacity) : acc.r;
+    rgb[r * 3 + 1] = white_back ? __fadd_rn(__fadd_rn(acc.g, 1.0f), -acc.opacity) : acc.g;
+    rgb[r * 3 + 2] = white_back ? __fadd_rn(__fadd_rn(acc.b, 1.0f), -acc.opacity) : acc.b;
+  }
+}
+
 // One warp per ray.  Shared memory per warp: keys[P] (uint64: orderable z << 32 | concat index).
 __global__ void __launch_bounds__(128)
 composite_multi_kernel(const float* __restrict__ z_all, const float4* __restrict__ field_all, int n_rays,
@@ -261,77 +201,32 @@ composite_multi_kernel(const float* __restrict__ z_all, const float4* __restrict
   unsigned long long* keys = keys_all + (size_t)warp * P;
   const int T = n_obj * S;
   for (int r = blockIdx.x * warps_per_block + warp; r < n_rays; r += gridDim.x * warps_per_block) {
-    // concatenated index c = obj * S + s  <->  object-major storage [obj][ray][s]
     const int64_t obj_stride = (int64_t)n_rays * S;
     const float* z = z_all + (int64_t)r * S;
     const float4* fld = field_all + (int64_t)r * S;
-#define SRC_OFF(c) ((int64_t)((c) / S) * obj_stride + ((c) % S))
     for (int i = lane; i < P; i += 32)
-      keys[i] = (i < T) ? (((unsigned long long)float_order_key(__ldg(z + SRC_OFF(i))) << 32) | (unsigned)i)
+      keys[i] = (i < T) ? (((unsigned long long)float_order_key(__ldg(z + src_off(i, S, obj_stride))) << 32) | (unsigned)i)
                         : 0xffffffffffffffffull;
-    __syncwarp();
-    for (int k2 = 2; k2 <= P; k2 <<= 1) {
-      for (int j = k2 >> 1; j > 0; j >>= 1) {
-        for (int t = lane; t < (P >> 1); t += 32) {
-          const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-          const int l = i | j;
-          const bool up = ((i & k2) == 0);
-          const unsigned long long a = keys[i], b = keys[l];
-          if ((a > b) == up) { keys[i] = b; keys[l] = a; }
-        }
-        __syncwarp();
-      }
-    }
+    warp_bitonic_sort(keys, P, lane);
     // composite in sorted order
-    Acc acc = {0.f, 0.f, 0.f, 0.f, 0.f};
-    float carry = 1.0f;
-    for (int base = 0; base < T; base += 32) {
-      const int i = base + lane;
-      float alpha = 0.0f, zi = 0.0f;
-      float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
-      int src = 0;
-      if (i < T) {
-        src = (int)(keys[i] & 0xffffffffu);
-        zi = __ldg(z + SRC_OFF(src));
-        const float zn = (i + 1 < T) ? __ldg(z + SRC_OFF((int)(keys[i + 1] & 0xffffffffu))) : zi;
-        const float delta = (i + 1 < T) ? __fsub_rn(zn, zi) : 0.0f;  // multi_rendering.py:125-128
-        f = __ldg(fld + SRC_OFF(src));
-        alpha = alpha_from(f.w, delta);
-      }
-      const float t = (i < T) ? __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f) : 1.0f;
-      const float incl = warp_scan_mul(t, lane);
-      float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-      if (lane == 0) excl = 1.0f;
-      const float w = alpha * (carry * excl);
-      carry *= __shfl_sync(0xffffffffu, incl, 31);
-      if (i < T) {
-        const int64_t o = (int64_t)r * T + i;
-        z_sorted[o] = zi;
-        weights[o] = w;
-        if (obj_ids) obj_ids[o] = (float)(src / S);
-        if (weights_unsorted) weights_unsorted[(int64_t)r * S + SRC_OFF(src)] = w;
-        acc.opacity += w;
-        acc.r += w * f.x;
-        acc.g += w * f.y;
-        acc.b += w * f.z;
-        acc.depth += w * zi;
-      }
-    }
-    acc.opacity = warp_sum(acc.opacity);
-    acc.r = warp_sum(acc.r);
-    acc.g = warp_sum(acc.g);
-    acc.b = warp_sum(acc.b);
-    acc.depth = warp_sum(acc.depth);
-    if (lane == 0) {
-      opacity[r] = acc.opacity;
-      depth[r] = acc.depth;
-      rgb[r * 3 + 0] = white_back ? __fadd_rn(__fadd_rn(acc.r, 1.0f), -acc.opacity) : acc.r;
-      rgb[r * 3 + 1] = white_back ? __fadd_rn(__fadd_rn(acc.g, 1.0f), -acc.opacity) : acc.g;
-      rgb[r * 3 + 2] = white_back ? __fadd_rn(__fadd_rn(acc.b, 1.0f), -acc.opacity) : acc.b;
-    }
+    auto load = [&](int i) {
+      const int src = (int)(keys[i] & 0xffffffffu);
+      const float zi = __ldg(z + src_off(src, S, obj_stride));
+      const float zn = (i + 1 < T) ? __ldg(z + src_off((int)(keys[i + 1] & 0xffffffffu), S, obj_stride)) : zi;
+      const float delta = (i + 1 < T) ? __fsub_rn(zn, zi) : 0.0f;  // multi_rendering.py:125-128
+      const float4 f = __ldg(fld + src_off(src, S, obj_stride));
+      return Sample{zi, delta, f.w, f, false, src};
+    };
+    auto sink = [&](int i, const Sample& s, float, float, float w) {
+      const int64_t o = (int64_t)r * T + i;
+      z_sorted[o] = s.z;
+      weights[o] = w;
+      if (obj_ids) obj_ids[o] = (float)(s.src / S);
+      if (weights_unsorted) weights_unsorted[(int64_t)r * S + src_off(s.src, S, obj_stride)] = w;
+    };
+    store_multi_maps(warp_sum(composite_scan(T, lane, load, sink)), white_back, r, lane, opacity, rgb, depth);
     __syncwarp();
   }
-#undef SRC_OFF
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -370,19 +265,7 @@ merge_sort_sets_kernel(const float* __restrict__ z_all, int n_rays, int n_obj, i
     }
     for (int i = lane; i < P; i += 32)
       keys[i] = (i < S) ? (((unsigned long long)float_order_key(__ldg(z + i)) << 32) | (unsigned)i) : 0xffffffffffffffffull;
-    __syncwarp();
-    for (int k2 = 2; k2 <= P; k2 <<= 1) {
-      for (int j = k2 >> 1; j > 0; j >>= 1) {
-        for (int t = lane; t < (P >> 1); t += 32) {
-          const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-          const int m = i | j;
-          const bool up = ((i & k2) == 0);
-          const unsigned long long a = keys[i], b = keys[m];
-          if ((a > b) == up) { keys[i] = b; keys[m] = a; }
-        }
-        __syncwarp();
-      }
-    }
+    warp_bitonic_sort(keys, P, lane);
     for (int s = lane; s < S; s += 32) {
       ko[s] = (uint32_t)(keys[s] >> 32);
       io[s] = (uint16_t)(keys[s] & 0xffffu);
@@ -427,8 +310,8 @@ merge_rank_kernel(const float* __restrict__ z_all, int n_rays, int n_obj, int S,
   }
 }
 
-// One warp per ray: composite_multi_kernel's compositing loop (same arithmetic, same 32-wide scan blocks) over the
-// order the rank kernel left in weights[] / z_sorted[].
+// One warp per ray: composite_scan, as in composite_multi_kernel, over the order the rank kernel left in weights[] /
+// z_sorted[].
 __global__ void __launch_bounds__(128)
 merge_composite_kernel(const float4* __restrict__ field_all, int n_rays, int n_obj, int S,
                        int white_back, const float* __restrict__ z_sorted, float* __restrict__ weights,
@@ -442,52 +325,21 @@ merge_composite_kernel(const float4* __restrict__ field_all, int n_rays, int n_o
     const float4* fld = field_all + (int64_t)r * S;
     const float* zs = z_sorted + (int64_t)r * T;
     float* wr = weights + (int64_t)r * T;
-#define SRC_OFF(c) ((int64_t)((c) / S) * obj_stride + ((c) % S))
-    Acc acc = {0.f, 0.f, 0.f, 0.f, 0.f};
-    float carry = 1.0f;
-    for (int base = 0; base < T; base += 32) {
-      const int i = base + lane;
-      float alpha = 0.0f, zi = 0.0f;
-      float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
-      int src = 0;
-      if (i < T) {
-        src = (int)__float_as_uint(wr[i]);
-        zi = zs[i];
-        const float zn = (i + 1 < T) ? zs[i + 1] : zi;
-        const float delta = (i + 1 < T) ? __fsub_rn(zn, zi) : 0.0f;  // multi_rendering.py:125-128
-        f = __ldg(fld + SRC_OFF(src));
-        alpha = alpha_from(f.w, delta);
-      }
-      const float t = (i < T) ? __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f) : 1.0f;
-      const float incl = warp_scan_mul(t, lane);
-      float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-      if (lane == 0) excl = 1.0f;
-      const float w = alpha * (carry * excl);
-      carry *= __shfl_sync(0xffffffffu, incl, 31);
-      if (i < T) {
-        wr[i] = w;
-        if (obj_ids) obj_ids[(int64_t)r * T + i] = (float)(src / S);
-        if (weights_unsorted) weights_unsorted[(int64_t)r * S + SRC_OFF(src)] = w;
-        acc.opacity += w;
-        acc.r += w * f.x;
-        acc.g += w * f.y;
-        acc.b += w * f.z;
-        acc.depth += w * zi;
-      }
-    }
-    acc.opacity = warp_sum(acc.opacity);
-    acc.r = warp_sum(acc.r);
-    acc.g = warp_sum(acc.g);
-    acc.b = warp_sum(acc.b);
-    acc.depth = warp_sum(acc.depth);
-    if (lane == 0) {
-      opacity[r] = acc.opacity;
-      depth[r] = acc.depth;
-      rgb[r * 3 + 0] = white_back ? __fadd_rn(__fadd_rn(acc.r, 1.0f), -acc.opacity) : acc.r;
-      rgb[r * 3 + 1] = white_back ? __fadd_rn(__fadd_rn(acc.g, 1.0f), -acc.opacity) : acc.g;
-      rgb[r * 3 + 2] = white_back ? __fadd_rn(__fadd_rn(acc.b, 1.0f), -acc.opacity) : acc.b;
-    }
-#undef SRC_OFF
+    // each lane reads its order word wr[i] before its sink overwrites it with the weight
+    auto load = [&](int i) {
+      const int src = (int)__float_as_uint(wr[i]);
+      const float zi = zs[i];
+      const float zn = (i + 1 < T) ? zs[i + 1] : zi;
+      const float delta = (i + 1 < T) ? __fsub_rn(zn, zi) : 0.0f;  // multi_rendering.py:125-128
+      const float4 f = __ldg(fld + src_off(src, S, obj_stride));
+      return Sample{zi, delta, f.w, f, false, src};
+    };
+    auto sink = [&](int i, const Sample& s, float, float, float w) {
+      wr[i] = w;
+      if (obj_ids) obj_ids[(int64_t)r * T + i] = (float)(s.src / S);
+      if (weights_unsorted) weights_unsorted[(int64_t)r * S + src_off(s.src, S, obj_stride)] = w;
+    };
+    store_multi_maps(warp_sum(composite_scan(T, lane, load, sink)), white_back, r, lane, opacity, rgb, depth);
   }
 }
 
@@ -511,12 +363,9 @@ int onerf_launch_composite(onerf_ctx* ctx, const onerf_composite_args* a, uint64
   if (a->obj) ONERF_CHECK_ARG(a->rgb_instance && a->depth_instance && a->opacity_instance, "null instance output");
   if (a->n_rays == 0) return ONERF_OK;
   const int warps = 8;
-  int blocks = (a->n_rays + warps - 1) / warps;
-  const int cap = ctx->num_sms * 8;
-  if (blocks > cap) blocks = cap;
   onerf_step_composite none;
   memset(&none, 0, sizeof(none));
-  composite_kernel<false><<<blocks, warps * 32, 0, stream>>>(*a, none, seed_dev);
+  composite_kernel<false><<<composite_blocks(ctx, a->n_rays, warps), warps * 32, 0, stream>>>(*a, none, seed_dev);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }
@@ -525,9 +374,7 @@ int onerf_launch_composite_eval(onerf_ctx* ctx, const onerf_composite_args* a, c
                                 cudaStream_t stream) {
   if (a->n_rays == 0) return ONERF_OK;
   const int warps = 8;
-  int blocks = (a->n_rays + warps - 1) / warps;
-  if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
-  composite_kernel<false, true><<<blocks, warps * 32, 0, stream>>>(*a, *t, nullptr);
+  composite_kernel<false, true><<<composite_blocks(ctx, a->n_rays, warps), warps * 32, 0, stream>>>(*a, *t, nullptr);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }
@@ -539,9 +386,7 @@ int onerf_launch_composite_step(onerf_ctx* ctx, const onerf_composite_args* a, c
   const int warps = 4;
   const size_t smem = (size_t)warps * 4 * a->n_samples * sizeof(float);
   ONERF_CUDA(cudaFuncSetAttribute(composite_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int blocks = (a->n_rays + warps - 1) / warps;
-  if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
-  composite_kernel<true><<<blocks, warps * 32, smem, stream>>>(*a, *t, seed_dev);
+  composite_kernel<true><<<composite_blocks(ctx, a->n_rays, warps), warps * 32, smem, stream>>>(*a, *t, seed_dev);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }
@@ -567,10 +412,7 @@ static int composite_multi_run(onerf_ctx* ctx, int path, const float* z_all, con
     while (P < T) P <<= 1;
     const size_t smem = (size_t)warps * P * sizeof(unsigned long long);
     ONERF_CUDA(cudaFuncSetAttribute(composite_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int blocks = (n_rays + warps - 1) / warps;
-    const int cap = ctx->num_sms * 8;
-    if (blocks > cap) blocks = cap;
-    composite_multi_kernel<<<blocks, warps * 32, smem, stream>>>(
+    composite_multi_kernel<<<composite_blocks(ctx, n_rays, warps), warps * 32, smem, stream>>>(
         z_all, reinterpret_cast<const float4*>(field_all), n_rays, n_obj, n_samples, P, white_back, z_sorted,
         weights, obj_ids, weights_unsorted, opacity, rgb, depth);
     ONERF_LAUNCH_CHECK(ctx);
@@ -589,8 +431,7 @@ static int composite_multi_run(onerf_ctx* ctx, int path, const float* z_all, con
   ONERF_LAUNCH_CHECK(ctx);
   merge_rank_kernel<<<list_blocks, warps * 32, 0, stream>>>(z_all, n_rays, n_obj, n_samples, skey, sidx, z_sorted, weights);
   ONERF_LAUNCH_CHECK(ctx);
-  const int ray_blocks = (int)std::min<int64_t>((n_rays + warps - 1) / warps, (int64_t)ctx->num_sms * 8);
-  merge_composite_kernel<<<ray_blocks, warps * 32, 0, stream>>>(
+  merge_composite_kernel<<<composite_blocks(ctx, n_rays, warps), warps * 32, 0, stream>>>(
       reinterpret_cast<const float4*>(field_all), n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
       weights_unsorted, opacity, rgb, depth);
   ONERF_LAUNCH_CHECK(ctx);

@@ -48,12 +48,6 @@ sample_coarse_kernel(const float* __restrict__ rays, int n_rays, int S, int use_
   }
 }
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // inclusive additive warp scan in double: torch's CPU cumsum accumulates fp32 rows in double and rounds
 // each prefix to fp32 (ATen cumsum_cpu_kernel, acc_type<float> = double); doing the same keeps cdf[M]
 // on the same side of 1.0 as the reference, which decides where the u = 1 sample lands when the tail
@@ -139,20 +133,7 @@ sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restr
       continue;
     }
     for (int i = S + K + lane; i < P; i += 32) merged[i] = __int_as_float(0x7f800000);
-    __syncwarp();
-    // bitonic sort (ascending) of P values by one warp
-    for (int k2 = 2; k2 <= P; k2 <<= 1) {
-      for (int j = k2 >> 1; j > 0; j >>= 1) {
-        for (int t = lane; t < (P >> 1); t += 32) {
-          const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));  // index with bit j cleared
-          const int l = i | j;
-          const bool up = ((i & k2) == 0);
-          const float a = merged[i], b = merged[l];
-          if ((a > b) == up) { merged[i] = b; merged[l] = a; }
-        }
-        __syncwarp();
-      }
-    }
+    warp_bitonic_sort(merged, P, lane);
     float* out = z_out + (int64_t)r * (S + K);
     for (int i = lane; i < S + K; i += 32) out[i] = merged[i];
     __syncwarp();
