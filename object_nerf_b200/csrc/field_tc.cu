@@ -62,6 +62,11 @@ struct Rows {
 #endif
 };
 
+__device__ __forceinline__ void fragment_rows(int (&row)[2], int warp, int lane) {
+  row[0] = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
+  row[1] = row[0] + 8;
+}
+
 #ifdef ONERF_FIELD_TIMELINE
 // Phase timeline, built only by tools/field_timeline.py: lane 0 of each warpgroup stores clock64 stamps of the first
 // TL_TILES tiles of CTAs [0, TL_CTAS) at tl[((cta * 3 + warpgroup) * TL_TILES + k) * TL_SLOTS + slot] (slot meanings in
@@ -173,6 +178,13 @@ __device__ __forceinline__ void epilogue(const float (&acc)[N / 2], uint32_t* pk
   }
 }
 
+// sum of the partial sums that the four lanes of a row hold (every lane gets it)
+__device__ __forceinline__ float row_sum(float part) {
+  part += __shfl_xor_sync(0xffffffffu, part, 1);
+  part += __shfl_xor_sync(0xffffffffu, part, 2);
+  return part;
+}
+
 // finish the heads of one branch: sum the four lanes of each row, add the head biases, write (rgb, sigma)
 __device__ __forceinline__ void write_heads(const FieldParams& p, const Rows& R, int branch, float (&part)[2][4]) {
   const float* Pf = reinterpret_cast<const float*>(p.packed);
@@ -181,10 +193,7 @@ __device__ __forceinline__ void write_heads(const FieldParams& p, const Rows& R,
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      part[r][k] += __shfl_xor_sync(0xffffffffu, part[r][k], 1);
-      part[r][k] += __shfl_xor_sync(0xffffffffu, part[r][k], 2);
-    }
+    for (int k = 0; k < 4; ++k) part[r][k] = row_sum(part[r][k]);
     if ((threadIdx.x & 3) == 0 && R.live[r]) {
       float sg = part[r][0] + sb;
       const float cr = 1.0f / (1.0f + __expf(-(part[r][1] + __ldg(hb + 0))));
@@ -226,6 +235,30 @@ __device__ __forceinline__ void run_layer(const TcParams& P, const Rows& R, Ring
   TL_AT(R.tl, 3 * slot + 2);
 }
 
+// The scene branch up to its sigma head (models/nerf_model.py:97-112): layers S0..S7, XS K slabs of X into S0 and the
+// skip layer.  Leaves S7's output in h and the sigma partial sums in part[r][0].
+template <int XS, bool DUMP>
+__device__ __forceinline__ void scene_trunk(const TcParams& P, const Rows& R, Ring& ring, uint32_t sXw, float (&acc)[128],
+                                            uint32_t (&h)[64], const float* bias_tab, float (&part)[2][4],
+                                            uint32_t x_free) {
+  const float* sw = reinterpret_cast<const float*>(P.f.packed) + P.f.L.sigma_w;
+  run_layer<256, XS, 0, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_S0 * 256, 0, nullptr, part, 1,
+                                          onerf_mask_word0(1), x_free, false);
+#pragma unroll 1
+  for (int l = 1; l < 4; ++l)
+    run_layer<256, 0, 8, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + (G_S0 + l) * 256, 0, nullptr, part,
+                                           1 + l, onerf_mask_word0(1 + l));
+  // skip layer [X | h3]: the last reader of X
+  run_layer<256, XS, 8, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_S4 * 256, 0, nullptr, part, 5,
+                                          onerf_mask_word0(5), x_free, true);
+#pragma unroll 1
+  for (int l = 5; l < 7; ++l)
+    run_layer<256, 0, 8, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + (G_S0 + l) * 256, 0, nullptr, part,
+                                           1 + l, onerf_mask_word0(1 + l));
+  run_layer<256, 0, 8, EPI_HIDDEN_SIGMA, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_S7 * 256, 0, sw, part, 8,
+                                               onerf_mask_word0(8));
+}
+
 // =============================== encoder warps (warps 1-3 of the producer warpgroup) ===============================
 // They write X (bf16, K-major SWIZZLE_128B atoms) and the row metadata of tile t + gridDim.x while the consumers still
 // run tile t: (row, column quarter) jobs, each gathering before it waits for X to be free, so the first job's loads
@@ -247,6 +280,25 @@ __device__ __forceinline__ void prefetch_rows(const void* base, int64_t pitch, i
   const int lines = (nbytes + 127) >> 7;
   for (int i = et; i < (r1 - r0 + 1) * lines; i += NUM_ENCODER)
     prefetch_l2(reinterpret_cast<const char*>(base) + (r0 + i / lines) * pitch + bytes0 + (int64_t)(i % lines) * 128);
+}
+
+// Column quarter cq (0..3) of row `row` of a voxel-model tile, for the point (x, y, z).  Each quarter gathers before it
+// waits for X to be free (`parity` of x_free), so the first job's loads overlap the consumers' last X-fed layer.
+__device__ __forceinline__ void voxel_encode_job(const GridView& g, uint32_t sX, int row, int cq, float x, float y,
+                                                 float z, uint32_t x_free, uint32_t parity, uint32_t* diag) {
+  if (cq < 3) {
+    float f[8];
+    // scene channels 0-7: chunks 0, 2, 4, ...; 8-15: chunks 1, 3, 5, ...; object channels: chunk 34 (column 272) on
+    if (cq == 0) voxel_trilinear<0, 8, false>(g, x, y, z, f);
+    else if (cq == 1) voxel_trilinear<8, 8, false>(g, x, y, z, f);
+    else voxel_trilinear<16, 8, false>(g, x, y, z, f);
+    mbar_wait(x_free, parity, diag);
+    pe8_to_chunks(sX, row, cq < 2 ? cq : 34, cq < 2 ? 2 : 1, f);
+  } else if (cq == 3) {
+    mbar_wait(x_free, parity, diag);
+    pe_xyz_to_chunks(sX, row, 26, x, y, z);                     // columns 208..271
+    st_chunk(a_chunk_addr(sX, row, 47), 0u, 0u, 0u, 0u);        // columns 376..383
+  }
 }
 
 template <bool VOXEL>
@@ -295,19 +347,11 @@ __device__ __forceinline__ void encoder_loop(const TcParams& P, uint32_t sX, Row
         mbar_wait(x_free, (it & 1) ^ 1, P.diag);
         meta[row] = RowMeta{ray, si, mute, live ? 1 : 0};
       }
-      if (VOXEL && cq < 3) {
-        const GridView g = load_grid_view(p.grid);
-        float f[8];
-        // scene channels 0-7: chunks 0, 2, 4, ...; 8-15: chunks 1, 3, 5, ...; object channels: chunk 34 (column 272) on
-        if (cq == 0) voxel_trilinear<0, 8, false>(g, x, y, z, f);
-        else if (cq == 1) voxel_trilinear<8, 8, false>(g, x, y, z, f);
-        else voxel_trilinear<16, 8, false>(g, x, y, z, f);
+      if (VOXEL) {
+        voxel_encode_job(load_grid_view(p.grid), sX, row, cq, x, y, z, x_free, (it & 1) ^ 1, P.diag);
+      } else if (cq == 0) {
         mbar_wait(x_free, (it & 1) ^ 1, P.diag);
-        pe8_to_chunks(sX, row, cq < 2 ? cq : 34, cq < 2 ? 2 : 1, f);
-      } else if (cq == (VOXEL ? 3 : 0)) {
-        mbar_wait(x_free, (it & 1) ^ 1, P.diag);
-        pe_xyz_to_chunks(sX, row, VOXEL ? 26 : 0, x, y, z);                   // columns 208..271 (voxel model)
-        if (VOXEL) st_chunk(a_chunk_addr(sX, row, 47), 0u, 0u, 0u, 0u);       // columns 376..383
+        pe_xyz_to_chunks(sX, row, 0, x, y, z);
       }
     }
     mbar_wait(x_free, (it & 1) ^ 1, P.diag);   // (a no-op after the first job: keeps one arrival per phase)
@@ -318,31 +362,32 @@ __device__ __forceinline__ void encoder_loop(const TcParams& P, uint32_t sX, Row
   }
 }
 
-template <bool VOXEL, bool DUMP>
-__global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_constant__ TcParams P) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
+// Dynamic shared memory of a CTA as offsets from its 1024-byte aligned base (the 128B swizzle of X needs the
+// alignment): the X atoms at 0, the weight ring, [G_COUNT][256] bias floats, [TM] RowMeta where the kernel keeps row
+// metadata, then the barriers (ring full[], empty[], x_full, x_free).  `bytes` is what a launch asks for.
+struct FieldSmem {
+  uint32_t sB, sBias, sMeta, sBar, x_full, x_free, bytes;
+};
+__host__ __device__ constexpr FieldSmem field_smem(int x_atoms, bool has_meta) {
+  FieldSmem s{};
+  s.sB = x_atoms * ATOM_BYTES;
+  s.sBias = s.sB + NSTAGE * STAGE_BYTES;
+  s.sMeta = s.sBias + G_COUNT * 256 * 4;
+  s.sBar = s.sMeta + (has_meta ? TM * (uint32_t)sizeof(RowMeta) : 0u);
+  s.x_full = s.sBar + 16 * NSTAGE;
+  s.x_free = s.x_full + 8;
+  s.bytes = 1024 + s.x_free + 8;
+  return s;
+}
+
+// Every thread of the CTA, once: the barriers of plan S at base sX, the bias table, __syncthreads().  Returns the ring.
+__device__ __forceinline__ Ring cta_prologue(const FieldSmem& S, const TcParams& P, uint32_t sX, float* bias_tab) {
   const FieldParams& p = P.f;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int X_ATOMS = VOXEL ? 6 : 1;
-  constexpr int XS = VOXEL ? 9 : 2, XO = VOXEL ? 12 : 2;   // K slabs of X read by the scene / object branch (KX, KO)
-
-  // ---- shared memory carve-up (base is 1024-byte aligned: required by the 128B swizzle) ----
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sX = sbase;
-  const uint32_t sB = sX + X_ATOMS * ATOM_BYTES;
-  const uint32_t sBias = sB + NSTAGE * STAGE_BYTES;                 // [G_COUNT][256] floats
-  const uint32_t sMeta = sBias + G_COUNT * 256 * 4;                 // [128] RowMeta
-  const uint32_t sBar = sMeta + TM * sizeof(RowMeta);               // ring full[], empty[], then x_full, x_free
-  const uint32_t x_full = sBar + 16 * NSTAGE, x_free = x_full + 8;
-  uint8_t* gen_base = smem_raw + (sbase - smem_u32(smem_raw));
-  float* bias_tab = reinterpret_cast<float*>(gen_base + (sBias - sbase));
-  RowMeta* meta = reinterpret_cast<RowMeta*>(gen_base + (sMeta - sbase));
   const float* Pf = reinterpret_cast<const float*>(p.packed);
-  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u, P.diag};
-
+  Ring ring{sX + S.sB, sX + S.sBar, sX + S.sBar + 8 * NSTAGE, 0u, 0u, P.diag};
   if (threadIdx.x == 0) {
-    mbar_init(x_full, NUM_ENCODER);
-    mbar_init(x_free, NUM_CONSUMER / 32);
+    mbar_init(sX + S.x_full, NUM_ENCODER);
+    mbar_init(sX + S.x_free, NUM_CONSUMER / 32);
     ring_init_bars(ring.full, ring.empty);   // (its fence covers the two above)
   }
   // per-column biases of every GEMM -> shared memory (layers with a per-ray constant read ray_const instead)
@@ -351,6 +396,24 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
     bias_tab[i] = (c < p.L.g[g].N) ? __ldg(Pf + p.L.g[g].bias_off + c) : 0.0f;
   }
   __syncthreads();
+  return ring;
+}
+
+template <bool VOXEL, bool DUMP>
+__global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_constant__ TcParams P) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const FieldParams& p = P.f;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  constexpr int X_ATOMS = VOXEL ? 6 : 1;
+  constexpr int XS = VOXEL ? 9 : 2, XO = VOXEL ? 12 : 2;   // K slabs of X read by the scene / object branch (KX, KO)
+  constexpr FieldSmem S = field_smem(X_ATOMS, true);
+  const uint32_t sX = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* gen_base = smem_raw + (sX - smem_u32(smem_raw));
+  float* bias_tab = reinterpret_cast<float*>(gen_base + S.sBias);
+  RowMeta* meta = reinterpret_cast<RowMeta*>(gen_base + S.sMeta);
+  const uint32_t x_full = sX + S.x_full, x_free = sX + S.x_free;
+  const float* Pf = reinterpret_cast<const float*>(p.packed);
+  Ring ring = cta_prologue(S, P, sX, bias_tab);
 
   const int64_t total = (int64_t)field_rays(p) * p.S;
   const int64_t n_tiles = (total + TM - 1) / TM;
@@ -372,8 +435,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
   const uint32_t sXw = sX + (uint32_t)wg * 64u * 128u;
   const bool free_after_o2 = !p.want_scene;
   Rows R;
-  R.row[0] = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  R.row[1] = R.row[0] + 8;
+  fragment_rows(R.row, warp, lane);
   uint32_t it = 0;
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
     R.tile = tile;
@@ -424,22 +486,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
       float acc[128];
       uint32_t h[64];
       float part[2][4] = {};
-      const float* sw = Pf + p.L.sigma_w;
-      run_layer<256, XS, 0, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_S0 * 256, 0, nullptr, part, 1,
-                                              onerf_mask_word0(1), x_free, false);
-#pragma unroll 1
-      for (int l = 1; l < 4; ++l)
-        run_layer<256, 0, 8, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + (G_S0 + l) * 256, 0, nullptr, part,
-                                               1 + l, onerf_mask_word0(1 + l));
-      // skip layer [X | h3]: the last reader of X
-      run_layer<256, XS, 8, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_S4 * 256, 0, nullptr, part, 5,
-                                              onerf_mask_word0(5), x_free, true);
-#pragma unroll 1
-      for (int l = 5; l < 7; ++l)
-        run_layer<256, 0, 8, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + (G_S0 + l) * 256, 0, nullptr, part,
-                                               1 + l, onerf_mask_word0(1 + l));
-      run_layer<256, 0, 8, EPI_HIDDEN_SIGMA, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_S7 * 256, 0, sw, part, 8,
-                                                   onerf_mask_word0(8));
+      scene_trunk<XS, DUMP>(P, R, ring, sXw, acc, h, bias_tab, part, x_free);
       run_layer<256, 0, 8, EPI_FINAL, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_SFIN * 256, 0, nullptr, part, 9, -1);
       float accd[64];
       uint32_t hd[32];
@@ -466,8 +513,8 @@ struct PruneTcParams {
 constexpr int kPruneTilesPerVoxel = kPruneSamples / TM;
 static_assert(kPruneSamples % TM == 0, "a tile must lie inside one voxel");
 
-// encoder_loop<true> with the sample positions of prune_point instead of rays and depths: the same jobs and helpers,
-// so a point's X is bit for bit what field_tc_kernel builds for the same xyz.  No row metadata: every row is live.
+// The encoder warps of the pruning pass: the points come from prune_point instead of rays and depths.  No row
+// metadata: every row is live.
 __device__ __forceinline__ void prune_encoder_loop(const PruneTcParams& Q, uint32_t sX, uint32_t x_full, uint32_t x_free,
                                                    int64_t n_tiles) {
   const int et = threadIdx.x - NUM_CONSUMER - 32;
@@ -478,21 +525,10 @@ __device__ __forceinline__ void prune_encoder_loop(const PruneTcParams& Q, uint3
     const int s0 = (int)(tile % kPruneTilesPerVoxel) * TM;
 #pragma unroll 1
     for (int job = et; job < 4 * TM; job += NUM_ENCODER) {
-      const int row = job & (TM - 1), cq = job / TM;
+      const int row = job & (TM - 1);
       float p[3];
       prune_point(Q.src, g, k, s0 + row, p);
-      if (cq < 3) {
-        float f[8];
-        if (cq == 0) voxel_trilinear<0, 8, false>(g, p[0], p[1], p[2], f);
-        else if (cq == 1) voxel_trilinear<8, 8, false>(g, p[0], p[1], p[2], f);
-        else voxel_trilinear<16, 8, false>(g, p[0], p[1], p[2], f);
-        mbar_wait(x_free, (it & 1) ^ 1, Q.t.diag);
-        pe8_to_chunks(sX, row, cq < 2 ? cq : 34, cq < 2 ? 2 : 1, f);
-      } else {
-        mbar_wait(x_free, (it & 1) ^ 1, Q.t.diag);
-        pe_xyz_to_chunks(sX, row, 26, p[0], p[1], p[2]);
-        st_chunk(a_chunk_addr(sX, row, 47), 0u, 0u, 0u, 0u);
-      }
+      voxel_encode_job(g, sX, row, job / TM, p[0], p[1], p[2], x_free, (it & 1) ^ 1, Q.t.diag);
     }
     mbar_wait(x_free, (it & 1) ^ 1, Q.t.diag);
     fence_async_smem();
@@ -505,29 +541,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) prune_tc_kernel(const __grid_c
   const TcParams& P = Q.t;
   const FieldParams& p = P.f;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int X_ATOMS = 6, XS = 9;
-
-  // shared memory: field_tc_kernel's carve-up without the row metadata
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sX = sbase;
-  const uint32_t sB = sX + X_ATOMS * ATOM_BYTES;
-  const uint32_t sBias = sB + NSTAGE * STAGE_BYTES;
-  const uint32_t sBar = sBias + G_COUNT * 256 * 4;
-  const uint32_t x_full = sBar + 16 * NSTAGE, x_free = x_full + 8;
-  float* bias_tab = reinterpret_cast<float*>(smem_raw + (sBias - smem_u32(smem_raw)));
-  const float* Pf = reinterpret_cast<const float*>(p.packed);
-  Ring ring{sB, sBar, sBar + 8 * NSTAGE, 0u, 0u, P.diag};
-
-  if (threadIdx.x == 0) {
-    mbar_init(x_full, NUM_ENCODER);
-    mbar_init(x_free, NUM_CONSUMER / 32);
-    ring_init_bars(ring.full, ring.empty);
-  }
-  for (int i = threadIdx.x; i < G_COUNT * 256; i += NUM_THREADS) {
-    const int g = i >> 8, c = i & 255;
-    bias_tab[i] = (c < p.L.g[g].N) ? __ldg(Pf + p.L.g[g].bias_off + c) : 0.0f;
-  }
-  __syncthreads();
+  constexpr FieldSmem S = field_smem(6, false);
+  const uint32_t sX = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  float* bias_tab = reinterpret_cast<float*>(smem_raw + (sX - smem_u32(smem_raw)) + S.sBias);
+  const uint32_t x_full = sX + S.x_full, x_free = sX + S.x_free;
+  Ring ring = cta_prologue(S, P, sX, bias_tab);
 
   const int64_t n_tiles = Q.n_cells * kPruneTilesPerVoxel;
   if (warp >= PRODUCER_WARP) {
@@ -540,14 +558,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) prune_tc_kernel(const __grid_c
   }
   setmaxnreg_inc<CONSUMER_REGS>();
 
-  const int wg = warp >> 2;
-  const uint32_t sXw = sX + (uint32_t)wg * 64u * 128u;
-  const float* sw = Pf + p.L.sigma_w;
-  const float sb = __ldg(Pf + p.L.sigma_b);
-  Rows R;
-  R.row[0] = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  R.row[1] = R.row[0] + 8;
-  R.live[0] = R.live[1] = 1;
+  const uint32_t sXw = sX + (uint32_t)(warp >> 2) * 64u * 128u;
+  const float sb = __ldg(reinterpret_cast<const float*>(p.packed) + p.L.sigma_b);
+  Rows R;   // scene_trunk without DUMP reads row and tile only (and tl): the per-ray fields stay unset
+  fragment_rows(R.row, warp, lane);
 #ifdef ONERF_FIELD_TIMELINE
   R.tl = nullptr;
 #endif
@@ -555,31 +569,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) prune_tc_kernel(const __grid_c
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
     R.tile = tile;
     mbar_wait(x_full, it & 1, P.diag);
-    // the scene branch of field_tc_kernel up to its sigma head (models/nerf_model.py:97-112)
     float acc[128];
     uint32_t h[64];
     float part[2][4] = {};
-    run_layer<256, XS, 0, EPI_HIDDEN, false>(P, R, ring, sXw, acc, h, h, bias_tab + G_S0 * 256, 0, nullptr, part, 1, -1,
-                                             x_free, false);
-#pragma unroll 1
-    for (int l = 1; l < 4; ++l)
-      run_layer<256, 0, 8, EPI_HIDDEN, false>(P, R, ring, sXw, acc, h, h, bias_tab + (G_S0 + l) * 256, 0, nullptr, part,
-                                              1 + l, -1);
-    run_layer<256, XS, 8, EPI_HIDDEN, false>(P, R, ring, sXw, acc, h, h, bias_tab + G_S4 * 256, 0, nullptr, part, 5, -1,
-                                             x_free, true);
-#pragma unroll 1
-    for (int l = 5; l < 7; ++l)
-      run_layer<256, 0, 8, EPI_HIDDEN, false>(P, R, ring, sXw, acc, h, h, bias_tab + (G_S0 + l) * 256, 0, nullptr, part,
-                                              1 + l, -1);
-    run_layer<256, 0, 8, EPI_HIDDEN_SIGMA, false>(P, R, ring, sXw, acc, h, h, bias_tab + G_S7 * 256, 0, sw, part, 8, -1);
-    // sigma as write_heads forms it (same lane sums, same bias add), then the warp's largest alpha
+    scene_trunk<9, false>(P, R, ring, sXw, acc, h, bias_tab, part, x_free);
+    // the warp's largest alpha
     float m = 0.0f;
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      part[r][0] += __shfl_xor_sync(0xffffffffu, part[r][0], 1);
-      part[r][0] += __shfl_xor_sync(0xffffffffu, part[r][0], 2);
-      m = fmaxf(m, prune_alpha(part[r][0] + sb));
-    }
+    for (int r = 0; r < 2; ++r) m = fmaxf(m, prune_alpha(row_sum(part[r][0]) + sb));
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     // lane 0 folds it into the voxel's slot; the lane test is a predicate inside the asm statement (see ring_release)
@@ -590,63 +587,58 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) prune_tc_kernel(const __grid_c
   }
 }
 
+// appends GEMMs [g0, g1] of the packed layout to the producer program
+void add_layers(TcParams& P, int g0, int g1) {
+  for (int g = g0; g <= g1; ++g) P.layers[P.n_layers++] = WLayer{P.f.L.g[g].img_off, P.f.L.g[g].N, P.f.L.g[g].K / 32};
+}
+
+// persistent grid: one CTA per SM, or per tile where there are fewer
+template <class Params>
+int launch_persistent(onerf_ctx* ctx, void (*kernel)(Params), const Params& P, int64_t tiles, size_t smem,
+                      cudaStream_t stream) {
+  const int blocks = (int)(tiles < ctx->num_sms ? tiles : ctx->num_sms);
+  ONERF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<blocks, NUM_THREADS, smem, stream>>>(P);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
 }  // namespace
 
 int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t stream) {
-  const PackLayout& L = fp.L;
   TcParams P;
   memset(&P, 0, sizeof(P));
   P.f = fp;
-  int n = 0;
-  auto add = [&](int g) { P.layers[n++] = WLayer{L.g[g].img_off, L.g[g].N, L.g[g].K / 32}; };
-  if (fp.want_object)
-    for (int g = G_O0; g <= G_ODIR; ++g) add(g);
-  if (fp.want_scene)
-    for (int g = G_S0; g <= G_SDIR; ++g) add(g);
-  P.n_layers = n;
+  if (fp.want_object) add_layers(P, G_O0, G_ODIR);
+  if (fp.want_scene) add_layers(P, G_S0, G_SDIR);
   P.diag = ctx->tc_diag;
 #ifdef ONERF_FIELD_TIMELINE
   P.tl = g_timeline;
 #endif
+  const bool voxel = fp.L.use_voxel, train = fp.train_ws != nullptr;
   const int64_t total = (int64_t)fp.n_rays * fp.S;
-  const int64_t tiles = (total + TM - 1) / TM;
-  if (fp.train_ws) {
+  if (train) {
     P.dump = reinterpret_cast<uint8_t*>(fp.train_ws);
-    P.TL = onerf_make_train_layout(L.use_voxel, total);
+    P.TL = onerf_make_train_layout(voxel, total);
   }
-  const int blocks = (int)(tiles < ctx->num_sms ? tiles : ctx->num_sms);
-  const int x_atoms = L.use_voxel ? 6 : 1;
-  const size_t smem = 1024 + (size_t)x_atoms * ATOM_BYTES + NSTAGE * STAGE_BYTES + G_COUNT * 256 * 4 + TM * sizeof(RowMeta) +
-                      16 * NSTAGE + 16;
-  auto launch = [&](auto kernel) -> int {
-    ONERF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel<<<blocks, NUM_THREADS, smem, stream>>>(P);
-    ONERF_LAUNCH_CHECK(ctx);
-    return ONERF_OK;
-  };
-  if (L.use_voxel) return fp.train_ws ? launch(field_tc_kernel<true, true>) : launch(field_tc_kernel<true, false>);
-  return fp.train_ws ? launch(field_tc_kernel<false, true>) : launch(field_tc_kernel<false, false>);
+  auto* kernel = voxel ? (train ? field_tc_kernel<true, true> : field_tc_kernel<true, false>)
+                       : (train ? field_tc_kernel<false, true> : field_tc_kernel<false, false>);
+  return launch_persistent(ctx, kernel, P, (total + TM - 1) / TM, field_smem(voxel ? 6 : 1, true).bytes, stream);
 }
 
 int onerf_launch_prune_bf16(onerf_ctx* ctx, const FieldParams& fp, const PruneSource& src, int64_t cell_begin,
                             int64_t n_cells, float* max_alpha, cudaStream_t stream) {
-  const PackLayout& L = fp.L;
   PruneTcParams Q;
   memset(&Q, 0, sizeof(Q));
   Q.t.f = fp;
-  for (int g = G_S0; g <= G_S7; ++g) Q.t.layers[Q.t.n_layers++] = WLayer{L.g[g].img_off, L.g[g].N, L.g[g].K / 32};
+  add_layers(Q.t, G_S0, G_S7);
   Q.t.diag = ctx->tc_diag;
   Q.src = src;
   Q.cell_begin = cell_begin;
   Q.n_cells = n_cells;
   Q.max_alpha = reinterpret_cast<uint32_t*>(max_alpha);
-  const int64_t tiles = n_cells * kPruneTilesPerVoxel;
-  const int blocks = (int)(tiles < ctx->num_sms ? tiles : ctx->num_sms);
-  const size_t smem = 1024 + (size_t)6 * ATOM_BYTES + NSTAGE * STAGE_BYTES + G_COUNT * 256 * 4 + 16 * NSTAGE + 16;
-  ONERF_CUDA(cudaFuncSetAttribute(prune_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  prune_tc_kernel<<<blocks, NUM_THREADS, smem, stream>>>(Q);
-  ONERF_LAUNCH_CHECK(ctx);
-  return ONERF_OK;
+  return launch_persistent(ctx, prune_tc_kernel, Q, n_cells * kPruneTilesPerVoxel,
+                           field_smem(6, false).bytes, stream);
 }
 
 #ifdef ONERF_FIELD_TIMELINE

@@ -13,7 +13,7 @@ import torch
 
 from tests import cases
 from tests.test_graph_rng_cpu import _ext_declarations
-from tests.test_sass_pipeline_cpu import LIB, _cuobjdump
+from tests.test_sass_pipeline_cpu import LIB
 from tests.test_train_step_cpu import _FakeLib
 
 S = 4096
@@ -308,34 +308,3 @@ def test_two_gloo_ranks_apply_the_same_gathered_mask():
         n, shard, seed, occ, idx = ret[rank]
         assert n == n_want and shard == parallel.shard_bounds(K, 2, rank) and seed == 100
         assert torch.equal(occ, occ_want) and torch.equal(idx, idx_want)
-
-
-# ------------------------------------------------------------------------------------------------
-# the fused kernel's wgmma stream
-# ------------------------------------------------------------------------------------------------
-def test_prune_tc_kernel_wgmma_is_pipelined():
-    import re
-    import subprocess
-    exe = _cuobjdump()
-    if exe is None:
-        pytest.skip("cuobjdump not found (CUDA toolkit bin/ not on PATH): cannot disassemble the library")
-    assert os.path.exists(LIB), f"{LIB} is missing: build the library first (__graft_entry__.build())"
-    sass = subprocess.run([exe, "-sass", LIB], check=True, capture_output=True, text=True).stdout
-    counts, fn = {}, None
-    for line in sass.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            fn = m.group(1) if "prune_tc_kernel" in m.group(1) else None
-            if fn:
-                counts[fn] = {"hgmma": 0, "wait_all": 0, "wait_one": 0}
-            continue
-        if fn is None:
-            continue
-        c = counts[fn]
-        c["hgmma"] += bool(re.search(r"\bHGMMA\.", line))
-        c["wait_all"] += "WARPGROUP.DEPBAR.LE gsb0, 0x0" in line
-        c["wait_one"] += "WARPGROUP.DEPBAR.LE gsb0, 0x1" in line
-    assert len(counts) == 1, sorted(counts)
-    (c,) = counts.values()
-    assert c["hgmma"] > 0 and c["wait_one"] > 0, c
-    assert 4 * c["wait_all"] <= c["hgmma"], c

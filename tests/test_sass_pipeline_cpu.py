@@ -2,8 +2,8 @@
 
 ptxas serialises every wgmma of a kernel (a full WARPGROUP.DEPBAR after each HGMMA) when the code between two of them
 calls a function, branches divergently or lacks registers.  This disassembles the built library and checks that each
-field_tc_kernel instance waits with one group still in flight (gsb0, 0x1) and waits for all groups only rarely
-(about once per layer), not after every HGMMA.
+field_tc_kernel instance and prune_tc_kernel, which runs the same scene trunk, wait with one group still in flight
+(gsb0, 0x1) and wait for all groups only rarely (about once per layer), not after every HGMMA.
 """
 import os
 import re
@@ -36,7 +36,7 @@ def _wait_counts():
     for line in sass.splitlines():
         m = re.search(r"Function : (\S+)", line)
         if m:
-            fn = m.group(1) if "field_tc_kernel" in m.group(1) else None
+            fn = m.group(1) if re.search("field_tc_kernel|prune_tc_kernel", m.group(1)) else None
             if fn:
                 counts[fn] = {"hgmma": 0, "wait_all": 0, "wait_one": 0}
             continue
@@ -54,8 +54,8 @@ def _wait_counts():
 
 def test_field_tc_kernel_wgmma_is_pipelined():
     counts = _wait_counts()
-    # <VOXEL, DUMP> in {false, true}^2
-    assert len(counts) == 4, sorted(counts)
+    # field_tc_kernel<VOXEL, DUMP> in {false, true}^2, and prune_tc_kernel
+    assert len(counts) == 5, sorted(counts)
     for fn, c in counts.items():
         assert c["hgmma"] > 0, (fn, c)
         assert c["wait_one"] > 0, (fn, c)                  # per-stage waits leave a group in flight
