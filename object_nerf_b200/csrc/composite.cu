@@ -165,8 +165,13 @@ __global__ void seed_advance_kernel(uint64_t* seed_dev) { *seed_dev += ONERF_SEE
 // ---------------------------------------------------------------------------------------------
 // multi-object: joint stable sort by depth, then composite (last delta = 0)
 // ---------------------------------------------------------------------------------------------
+// Unsigned key ordered as the float's value.  -0.0 gets +0.0's key and every NaN, whatever its sign, the largest key, so
+// with the concatenated index as the tie-break both paths give torch.sort(stable=True)'s order: zeros of either sign in
+// index order, NaN last.
 __device__ __forceinline__ uint32_t float_order_key(float f) {
+  if (f != f) return 0xffffffffu;
   uint32_t u = __float_as_uint(f);
+  if (u == 0x80000000u) u = 0u;
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
