@@ -5,6 +5,7 @@ gradients of onerf_bwd_wgrad), per-ray sums (onerf_bwd_raysums), the chain and w
 batches, the compositing backward in every mode, the seeded (Philox) noise path, and whole training steps the other
 files do not run.  The references themselves are checked in tests/test_train_stages_cpu.py."""
 import ctypes as C
+import time
 
 import numpy as np
 import pytest
@@ -13,6 +14,7 @@ import torch
 from tests import cases, helpers, synth
 from tests.test_gpu_train_plain import _torch_chain as _chain_plain
 from tests.test_gpu_train_tc import GEMM_K, GEMM_N, GEMM_OF_DZ, _torch_chain as _chain_voxel, grad_layout
+from tests.test_fp32_backward_cpu import ORACLE_TWO_CHUNKS
 from tests.test_train_stages_cpu import (DX_LAYERS, dx_from_dz, edge_points, grid_coords, philox_normal, philox_uniform,
                                          table_grad_autograd, table_grad_matched)
 from oracle import onerf_oracle as O
@@ -718,17 +720,25 @@ def _oracle_grads(c, inp, dtype):
     return loss.item(), {k: (t.grad.reshape(-1) if t.grad is not None else None) for k, t in leaves.items()}
 
 
-@pytest.mark.parametrize("case", ["scene_only_voxel", "scene_only_plain", "coarse_only"])
+# coarse_only_two_chunks: 1 030 rays x 64 samples, the smallest coarse-only batch the fp32 backward runs in two chunks
+# (1 024 + 6 rays)
+ORACLE_CASES = dict(STEP_CASES, coarse_only_two_chunks=ORACLE_TWO_CHUNKS)
+
+
+@pytest.mark.parametrize("case", ["scene_only_voxel", "scene_only_plain", "coarse_only", "coarse_only_two_chunks"])
 def test_training_step_fp32_matches_float64_oracle(case):
-    """The fp32 path of the scene-only and coarse-only steps against float64 autograd of the oracle (leaf table for the
-    voxel grid), with the gates of the plain fixture's fp32 test: loss 2e-4, per-tensor norm 2e-3, sampled entries within
-    1 % of the tensor's RMS entry.  An entry that the oracle's own float32 restatement already moves by more than that
-    cannot decide the gate: it is reported, not asserted, and at least 95 % of the entries must be decidable.  Without
-    the object branch the object layers and codes get no gradient."""
-    c, inp = _grad_case(STEP_CASES[case])
+    """The fp32 path of the scene-only and coarse-only steps, and of a coarse-only step across a chunk boundary of the
+    fp32 backward, against float64 autograd of the oracle (leaf table for the voxel grid), with the gates of the plain
+    fixture's fp32 test: loss 2e-4, per-tensor norm 2e-3, sampled entries within 1 % of the tensor's RMS entry.  An
+    entry that the oracle's own float32 restatement already moves by more than that cannot decide the gate: it is
+    reported, not asserted, and at least 95 % of the entries must be decidable.  Without the object branch the object
+    layers and codes get no gradient."""
+    c, inp = _grad_case(ORACLE_CASES[case])
     loss, ours = _step("fp32", c, inp)
+    t0 = time.perf_counter()
     loss64, exact = _oracle_grads(c, inp, torch.float64)
     _, rounded = _oracle_grads(c, inp, torch.float32)
+    print(f"{case}: {c['n_rays']} rays, the float64 and float32 oracle steps took {time.perf_counter() - t0:.1f} s")
     assert abs(loss - loss64) <= 2e-4 * abs(loss64), (loss, loss64)
     checked, total, undecidable = 0, 0, []
     for name, ref in exact.items():

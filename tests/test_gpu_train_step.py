@@ -5,6 +5,7 @@ import pytest
 import torch
 
 from tests import cases, grad_plain, helpers, synth
+from tests.test_fp32_backward_cpu import FUSED_STEP_SHAPES
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -181,6 +182,22 @@ def test_psnr_is_the_reference_formula_on_the_returned_rgb(n_importance):
     mask = batch["valid_mask"].view(-1, 1).repeat(1, 3)
     mse = torch.mean((maps[f"rgb_{typ}"] - batch["rgbs"])[mask] ** 2)
     want = (-10 * torch.log10(mse)).item()
+    assert abs(psnr.item() - want) <= 1e-4 * abs(want), (psnr.item(), want)
+
+
+@pytest.mark.parametrize("shape", list(FUSED_STEP_SHAPES))
+def test_fp32_step_at_batch_size_matches_existing_route(shape):
+    """The fp32 comparison of test_fp32_step_matches_existing_route at batch size: 2 048 rays x 64 + 64 samples (512
+    compositing blocks, more than the SMs, so the last block that finalises the loss runs in a later wave than the
+    first; two fp32 chunks per pass) and 1 100 rays x 64 + 63 (ragged last chunks in both passes: 1 024 + 76 and
+    516 + 516 + 68).  The PSNR output is the reference formula on the returned rgb."""
+    n, S, K = FUSED_STEP_SHAPES[shape]
+    inp = cases.build_grad_case(n_rays=n)
+    inp["rand"] = synth.random_buffers(cases.GRAD_CASE["seed"] + 4, n, S, K)
+    rand = {k: v.to(DEV) for k, v in inp["rand"].items()}
+    _, psnr, maps, batch, _ = _compare(inp, True, "fp32", rand, N_samples=S, N_importance=K)
+    mask = batch["valid_mask"].view(-1, 1).repeat(1, 3)
+    want = (-10 * torch.log10(torch.mean((maps["rgb_fine"] - batch["rgbs"])[mask] ** 2))).item()
     assert abs(psnr.item() - want) <= 1e-4 * abs(want), (psnr.item(), want)
 
 
