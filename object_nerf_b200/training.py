@@ -46,6 +46,11 @@ fire because the step writes `.grad` without autograd):
     and would draw the same jitter and noise at the same batch positions.  Injected `_rand` buffers still win;
   - the returned loss, terms, flags and PSNR are this rank's (train.py logs them per rank).
 
+Through autograd (`TrainStepFn`, `install_training`): for host loops that call loss.backward() themselves (Lightning,
+DDP, GradScaler).  The step writes its gradients into a bucket its plan owns (`grad_sink=True`, the `group=` bucket's
+layout) and leaves `.grad` alone; the backward hands copies of them, times the incoming gradient, to autograd.
+`install_training(ObjectNeRFSystem)` binds this as the reference's `training_step`.
+
 Validation (`validate_frame`, `install_validation`): the other half of train.py's loop, one validation image per call
 (onerf_validate_frame, include/onerf_ext.h).  The image runs through render_rays' passes (is_eval, perturb = 0,
 noise_std = 0: nothing is random) in chunks of `chunk` rays; each pass's compositing kernel also adds the ray's squared
@@ -70,7 +75,8 @@ import torch
 from . import _lib, backward, editing, engine, parallel
 from .losses import TERMS
 
-__all__ = ["train_step", "step_seed", "sync_replicas", "validate_frame", "install_validation"]
+__all__ = ["train_step", "step_seed", "sync_replicas", "TrainStepFn", "install_training", "validate_frame",
+           "install_validation"]
 
 _RAND_KEYS = ("jitter", "u", "noise_scene_coarse", "noise_obj_coarse", "noise_scene_fine", "noise_obj_fine")
 # coarse model -> {configuration: plan}; a plan references no module, so it lives exactly as long as the model
@@ -110,8 +116,9 @@ def _grad_ptrs(tensors) -> list:
 
 
 class _GradBucket:
-    """One fp32 buffer that the `.grad` of every trained tensor views (layout: _trained_tensors, each offset rounded up
-    to 4 floats), so that a step's gradients are reduced by one all-reduce."""
+    """One fp32 buffer with a gradient view per trained tensor (layout: _trained_tensors, each offset rounded up to 4
+    floats): either the `.grad` of every trained tensor views it (`adopt`), so that a step's gradients are reduced by one
+    all-reduce, or it is the step's own gradient sink (train_step(grad_sink=True))."""
 
     def __init__(self, tensors, has_table, dev):
         self.offsets, off = [], 0
@@ -121,15 +128,22 @@ class _GradBucket:
         self.flat = torch.zeros(off, dtype=torch.float32, device=dev)
         self.table_offset = self.offsets[-1] if has_table else None
         self.table_row = tensors[-1].shape[1] if has_table else 0
-        for t, o in zip(tensors, self.offsets):
-            view = self.flat[o:o + t.numel()].view(t.shape)
+        self.shapes = [tuple(t.shape) for t in tensors]
+        self.views = [self.flat[o:o + t.numel()].view(t.shape) for t, o in zip(tensors, self.offsets)]
+        self.ptrs = None
+
+    def adopt(self, tensors) -> "_GradBucket":
+        """Point the `.grad` of `tensors` at the views, keeping the values they held."""
+        for t, view in zip(tensors, self.views):
             if t.grad is not None:
                 view.copy_(t.grad)
             t.grad = view
         self.ptrs = _grad_ptrs(tensors)
+        return self
 
     def prefix(self, n_used: int) -> int:
-        """Floats the all-reduce covers: all of it, or up to the end of voxel-table row n_used."""
+        """Floats up to the end of voxel-table row n_used (all of them without a table): the only ones a step can write
+        when the index map references rows [0, n_used)."""
         return self.flat.numel() if self.table_offset is None else self.table_offset + self.table_row * n_used
 
 
@@ -140,6 +154,9 @@ class _StepPlan:
         lib = _lib.load()
         self.n, self.dev, self.cfg = n, dev, cfg
         self.bucket = None              # _GradBucket of a plan made with a process group
+        self.sink = None                # _GradBucket of a plan made with grad_sink=True
+        # table rows the sink may hold gradient in (the most the grid has referenced) and the grid they were counted on
+        self.sink_rows, self.sink_grid = 0, None
         # the device seed of captured steps (onerf_train_step_dseed), continuing from the creating call's host seed
         self.seed_dev = torch.full((1,), seed + 4, dtype=torch.int64, device=dev)
         self.model_order = ["coarse"] + (["fine"] if cfg["N_importance"] > 0 else [])
@@ -223,10 +240,15 @@ def sync_replicas(models: Dict[str, Any], embeddings: Dict[str, Any], code_libra
                     seen.add(id(p))
                     bcast(p.detach())
         if use_voxel:
-            m = emb.voxel_idx_map
-            rows = emb.embedding_space_ftr.weight.shape[0]
-            n_used = min(int(m.max().item()) + 1, rows) if m.numel() else 0
+            n_used = _rows_used(emb)
     _synced[models["coarse"]] = (_grid_stamp(emb) if use_voxel else None, n_used)
+
+
+def _rows_used(emb) -> int:
+    """Voxel-table rows the index map references, [0, n_used): the only rows a step can write gradient to (one host
+    read)."""
+    m = emb.voxel_idx_map
+    return min(int(m.max().item()) + 1, emb.embedding_space_ftr.weight.shape[0]) if m.numel() else 0
 
 
 def _grad_of(p: torch.Tensor) -> torch.Tensor:
@@ -248,17 +270,26 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
                loss_conf, N_samples: int = 64, use_disp: bool = False, perturb: float = 0, noise_std: float = 1,
                N_importance: int = 0, white_back: bool = False, forward_instance: bool = True,
                frustum_bound_th: float = 0, pass_through_mask=None, rays_in_bbox: bool = False, group=None,
-               **render_kwargs):
+               grad_sink: bool = False, **render_kwargs):
     """render_rays(models, embeddings, batch["rays"], ...) with the codes code_library(batch) looks up, then
     TotalLoss(loss_conf) and its backward, as one call.  Takes render_rays' keyword arguments (train.py:84-98, 155-165;
     is_eval, use_zero_as_last_delta, precision and _rand included, the rest ignored as render_rays ignores them).
     group: a torch.distributed process group; the gradients are then averaged over its ranks (module docstring).
+    grad_sink: write the gradients into an fp32 bucket the plan owns instead of `.grad` (which stays untouched), and
+    return them (TrainStepFn hands them to autograd).  The call zeroes the bucket first (with the voxel model only up
+    to the last table row the grid has referenced; the rows above were never written).
 
     Returns (loss_sum, terms, present, psnr) as device tensors: loss_sum (), the five unweighted terms (5,) in
     losses.TERMS order (0 where skipped), present (5,) int32 flags (TotalLoss's loss_dict holds term i iff present[i]),
-    and the PSNR of the fine pass's rgb (coarse without a fine pass) over the valid rays (train.py:171-172)."""
+    and the PSNR of the fine pass's rgb (coarse without a fine pass) over the valid rays (train.py:171-172).  With
+    grad_sink a fifth element follows: the gradients as views of the bucket, one per tensor of _trained_tensors (fine
+    model first, then coarse, each in engine.model_linears order with weight before bias; the code table; the voxel
+    table), overwritten by the next call of the same plan."""
     if not forward_instance:
         raise NotImplementedError("TotalLoss needs the object branch's maps: train_step runs with forward_instance=True")
+    if grad_sink and group is not None:
+        raise ValueError("train_step: grad_sink returns the gradients for the caller to reduce (DDP does it through "
+                         "autograd); group= reduces .grad itself: choose one")
     lib = _lib.load()
     rays = batch["rays"].reshape(-1, 8)
     dev = rays.device
@@ -275,7 +306,7 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
     use_voxel = _is_voxel(emb_xyz)
     table = emb_xyz.embedding_space_ftr.weight if use_voxel else None
     key = (dev, n, use_voxel, tuple(sorted(cfg.items())),
-           tuple(rand[k].data_ptr() if rand.get(k) is not None else 0 for k in _RAND_KEYS), group)
+           tuple(rand[k].data_ptr() if rand.get(k) is not None else 0 for k in _RAND_KEYS), group, bool(grad_sink))
     capturing = _capturing(dev)
     seed = engine.new_seed() if not capturing and (cfg["perturb"] > 0 or cfg["noise_std"] > 0) else 0
     code_table = code_library.embedding_instance.weight
@@ -292,22 +323,38 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
         seed = (seed + dist.get_rank(group) * RANK_SEED_STRIDE) % (1 << 62)
     plans = _plans.setdefault(models["coarse"], {})
     plan = plans.get(key)
-    if plan is None:
+    made = plan is None
+    if made:
         if capturing:
             raise RuntimeError("train_step: the first call for a configuration must run before the CUDA-graph capture "
                                "(warm up eagerly): its plan's device seed counter would be reset on every replay")
         plan = _StepPlan(models, emb_xyz, n, cfg, rand, dev, seed)
+    trained = _trained_tensors(models, plan.model_order, code_table, table)
+    if made:
         if group is not None:
-            trained = _trained_tensors(models, plan.model_order, code_table, table)
             ptrs = _grad_ptrs(trained)
             # another configuration's bucket, if the gradients still view it
             plan.bucket = next((p.bucket for p in plans.values() if p.bucket is not None and p.bucket.ptrs == ptrs),
-                               None) or _GradBucket(trained, table is not None, dev)
+                               None) or _GradBucket(trained, table is not None, dev).adopt(trained)
+        if grad_sink:
+            plan.sink = _GradBucket(trained, table is not None, dev)
         plans[key] = plan
-    if group is not None and _grad_ptrs(_trained_tensors(models, plan.model_order, code_table, table)) != plan.bucket.ptrs:
+    if group is not None and _grad_ptrs(trained) != plan.bucket.ptrs:
         raise RuntimeError("train_step(group=...): a .grad no longer views the gradient bucket this step all-reduces "
                            "(zero_grad(set_to_none=True) or a replaced parameter?); zero the gradients with "
                            "set_to_none=False")
+    if grad_sink:
+        if [tuple(t.shape) for t in trained] != plan.sink.shapes:
+            raise RuntimeError("train_step(grad_sink=True): a trained tensor changed shape since this configuration's "
+                               "first call")
+        if use_voxel and plan.sink_grid != _grid_stamp(emb_xyz):
+            # one host read after each grid change; pruning can lower n_used, so keep the most rows ever referenced
+            plan.sink_rows, plan.sink_grid = max(plan.sink_rows, _rows_used(emb_xyz)), _grid_stamp(emb_xyz)
+        plan.sink.flat[:plan.sink.prefix(plan.sink_rows)].zero_()
+        grads = plan.sink.views
+    else:
+        grads = [_grad_of(t) for t in trained]
+    first = {typ: 40 * k for k, typ in enumerate(reversed(plan.model_order))}     # grads: fine model first
     # the grid as it is now (host-side argument block only)
     plan.grid = engine.GridBuffers.from_module(emb_xyz) if use_voxel else None
     plan.render.args.grid = C.pointer(plan.grid.c) if use_voxel else None
@@ -332,8 +379,9 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
             lin = engine.model_linears(models[typ])
             Wp = (C.c_void_p * 20)(*[_f32_param(w).data_ptr() for w, _ in lin])
             Bp = (C.c_void_p * 20)(*[_f32_param(bb).data_ptr() for _, bb in lin])
-            dWp = (C.c_void_p * 20)(*[_grad_of(w).data_ptr() for w, _ in lin])
-            dbp = (C.c_void_p * 20)(*[_grad_of(bb).data_ptr() for _, bb in lin])
+            g = grads[first[typ]:first[typ] + 40]
+            dWp = (C.c_void_p * 20)(*[d.data_ptr() for d in g[0::2]])
+            dbp = (C.c_void_p * 20)(*[d.data_ptr() for d in g[1::2]])
             keep += [Wp, Bp, dWp, dbp]
             _lib.check(lib.onerf_pack_weights(ctx, int(plan.use_voxel), Wp, Bp, plan.packed[typ].data_ptr(),
                                               plan.packed[typ].numel(), stream))
@@ -341,7 +389,7 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
             setattr(b, "dW_" + typ, dWp)
             setattr(b, "db_" + typ, dbp)
         b.d_codes = plan.d_codes.data_ptr()
-        b.table_grad = _grad_of(table).data_ptr() if table is not None else None
+        b.table_grad = grads[-1].data_ptr() if table is not None else None
         a = plan.render.args
         if capturing:
             _lib.check(lib.onerf_train_step_dseed(ctx, C.byref(a), C.byref(plan.loss_args), C.byref(b),
@@ -351,12 +399,95 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
             _lib.check(lib.onerf_train_step(ctx, C.byref(a), C.byref(plan.loss_args), C.byref(b), plan.psnr.data_ptr(),
                                             stream))
         _lib.check(lib.onerf_code_scatter_add(ctx, plan.d_codes.data_ptr(), plan.ids.data_ptr(), n, code_table.shape[0],
-                                              _grad_of(code_table).data_ptr(), stream))
+                                              grads[40 * len(plan.model_order)].data_ptr(), stream))
         if group is not None:
             reduced = plan.bucket.flat[:plan.bucket.prefix(synced[1])]
             dist.all_reduce(reduced, op=dist.ReduceOp.SUM, group=group)     # gloo has no AVG
             reduced.mul_(1.0 / world)
+    if grad_sink:
+        return plan.out[0], plan.out[1:], plan.present, plan.psnr[0], grads
     return plan.out[0], plan.out[1:], plan.present, plan.psnr[0]
+
+
+class TrainStepFn(torch.autograd.Function):
+    """train_step as an autograd node, for host loops that own the backward (Lightning, DDP, GradScaler, gradient
+    accumulation).  The inputs are the trained tensors in _trained_tensors order; forward runs the whole step into the
+    plan's gradient sink (train_step(grad_sink=True)), so `.grad` is only written by autograd, through AccumulateGrad,
+    where DDP's reducer hooks fire.  Returns (loss_sum, terms, present, psnr) as fresh tensors; only loss_sum is
+    differentiable.  backward returns each sink gradient times grad_output as a new tensor (never a view of the sink:
+    autograd may adopt a returned gradient as `.grad`, and the next step would overwrite it), so `(loss / N).backward()`
+    and a GradScaler's scaled loss come out right.  Run backward before the next step of the same configuration: that
+    step zeroes the sink, and a backward after it is refused.  Call through `run`."""
+
+    @staticmethod
+    def forward(ctx, step, *trained):
+        models, embeddings, code_library, batch, loss_conf, kwargs = step
+        loss_sum, terms, present, psnr, grads = train_step(models, embeddings, code_library, batch, loss_conf,
+                                                           grad_sink=True, **kwargs)
+        ctx.grads = grads
+        ctx.sink_version = grads[0]._version if grads else None      # the views share the sink's version counter
+        out = loss_sum.clone(), terms.clone(), present.clone(), psnr.clone()
+        ctx.mark_non_differentiable(*out[1:])
+        return out
+
+    @staticmethod
+    def backward(ctx, g_loss, *_):
+        if ctx.grads and ctx.grads[0]._version != ctx.sink_version:
+            raise RuntimeError("TrainStepFn: a later step of the same configuration has overwritten this step's "
+                               "gradients; run backward before the next step")
+        return (None,) + tuple(g * g_loss for g in ctx.grads)
+
+    @classmethod
+    def run(cls, models: Dict[str, Any], embeddings: Dict[str, Any], code_library, batch: Dict[str, torch.Tensor],
+            loss_conf, **kwargs):
+        """train_step(models, embeddings, code_library, batch, loss_conf, **kwargs) through autograd (group= is not
+        taken: DDP reduces the gradients).  Refused when grad mode is off or no trained tensor requires grad: the
+        step's backward would have nowhere to go."""
+        emb_xyz = embeddings["xyz"]
+        model_order = ["coarse"] + (["fine"] if int(kwargs.get("N_importance", 0)) > 0 else [])
+        trained = _trained_tensors(models, model_order, code_library.embedding_instance.weight,
+                                   emb_xyz.embedding_space_ftr.weight if _is_voxel(emb_xyz) else None)
+        if not torch.is_grad_enabled():
+            raise RuntimeError("TrainStepFn: grad mode is off (torch.no_grad() / inference_mode); the step exists for "
+                               "its gradients: call training.train_step for a step that writes .grad directly")
+        if not any(t.requires_grad for t in trained):
+            raise RuntimeError("TrainStepFn: no trained tensor (model linears, code table, voxel table) requires grad")
+        return cls.apply((models, embeddings, code_library, batch, loss_conf, kwargs), *trained)
+
+
+def install_training(system_cls, *, precision=None):
+    """Replace `training_step` of `system_cls` (the reference's ObjectNeRFSystem, train.py:147-180) by one that runs the
+    step through TrainStepFn with the arguments the reference passes to render_rays: is_eval=False, the batch's
+    pass_through_mask, rays_in_bbox from train_dataset.is_rays_in_bbox(), frustum_bound_th = config.model.frustum_bound
+    / config.dataset_extra.scale_factor, N_samples, N_importance, use_disp, perturb and noise_std from config.model,
+    white_back from train_dataset, and the codes of the batch's instance ids.  It makes the same `self.log` calls (lr,
+    train/loss, train/<term> for each present term, train/psnr) and returns loss_sum, whose backward hands the step's
+    gradients to autograd (and so to Lightning's gradient accumulation, AMP scaling and DDP).  Leaving absent terms out
+    of the log needs the five flags on the host: one 20-byte read per step, the only one.  Grid maintenance in
+    on_epoch_start needs nothing: each step reads the current grid.
+    precision: the step's arithmetic (None = the library default)."""
+    import sys
+    get_learning_rate = sys.modules[system_cls.__module__].get_learning_rate      # train.py's own import
+
+    def training_step(self, batch, batch_nb):
+        conf, m = self.config, self.config.model
+        loss_sum, terms, present, psnr = TrainStepFn.run(
+            self.models, self.embeddings, self.code_library, batch, conf.loss, N_samples=m.N_samples,
+            use_disp=m.use_disp, perturb=m.perturb, noise_std=m.noise_std, N_importance=m.N_importance,
+            white_back=self.train_dataset.white_back, is_eval=False, pass_through_mask=batch["pass_through_mask"],
+            rays_in_bbox=getattr(self.train_dataset, "is_rays_in_bbox", lambda: False)(),
+            frustum_bound_th=m.frustum_bound / conf["dataset_extra"]["scale_factor"], precision=precision)
+        flags = present.tolist()
+        self.log("lr", get_learning_rate(self.optimizer))
+        self.log("train/loss", loss_sum)
+        for i, t in enumerate(TERMS):
+            if flags[i]:
+                self.log(f"train/{t}", terms[i])
+        self.log("train/psnr", psnr, prog_bar=True)
+        return loss_sum
+
+    system_cls.training_step = training_step
+    return system_cls
 
 
 # ------------------------------------------------------------------------------------------------
