@@ -1,7 +1,8 @@
 """Per-object latent codes (reference models/code_library.py:5-28): an embedding table looked up by instance id.
 On a CUDA device the lookup and its gradient (scatter-add of the per-ray code gradients into the table) are kernels of
-libonerf_sm100.so (`onerf_code_gather` / `onerf_code_scatter_add`); the parameter keeps the reference's name
-(`embedding_instance.weight`), so checkpoints and optimizers are interchangeable."""
+libonerf_sm90.so (`onerf_code_gather` / `onerf_code_scatter_add`); the parameter keeps the reference's name
+(`embedding_instance.weight`), so checkpoints and optimizers are interchangeable.  An id outside [0, n_codes) reads the
+nearest row (0 or n_codes - 1), and its gradient goes to that same row."""
 import torch
 from torch import nn
 

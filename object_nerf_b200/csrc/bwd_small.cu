@@ -153,12 +153,17 @@ __global__ void __launch_bounds__(256) vec4_sum_kernel(const float4* __restrict_
   }
 }
 
+// The table row of an instance id: ids outside [0, n_codes) are clamped to the nearest row (the ids are device data, so
+// checking them on the host would cost a sync).  Gather and scatter share the rule, so a ray's code gradient goes to
+// the row its code was read from.
+__device__ __forceinline__ int64_t code_row(int64_t id, int n_codes) {
+  return id < 0 ? 0 : (id >= n_codes ? n_codes - 1 : id);
+}
 __global__ void code_gather_kernel(const float* __restrict__ table, const int64_t* __restrict__ ids, int n, int n_codes,
                                    float* __restrict__ out) {
   for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n * 16; e += gridDim.x * blockDim.x) {
     const int r = e >> 4, c4 = e & 15;
-    int64_t id = ids[r];
-    id = id < 0 ? 0 : (id >= n_codes ? n_codes - 1 : id);
+    const int64_t id = code_row(ids[r], n_codes);
     reinterpret_cast<float4*>(out)[e] = __ldg(reinterpret_cast<const float4*>(table) + id * 16 + c4);
   }
 }
@@ -166,8 +171,7 @@ __global__ void code_scatter_kernel(const float* __restrict__ d_codes, const int
                                     float* __restrict__ table_grad) {
   for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n * 64; e += gridDim.x * blockDim.x) {
     const int r = e >> 6, c = e & 63;
-    const int64_t id = ids[r];
-    if (id >= 0 && id < n_codes) atomicAdd(table_grad + id * 64 + c, d_codes[e]);
+    atomicAdd(table_grad + code_row(ids[r], n_codes) * 64 + c, d_codes[e]);
   }
 }
 
@@ -243,6 +247,7 @@ extern "C" int onerf_code_gather(onerf_ctx* ctx, const float* table, const int64
                                  void* stream) {
   ONERF_CHECK_ARG(ctx && table && ids && out, "null argument");
   ONERF_CHECK_ARG(onerf_aligned16(table) && onerf_aligned16(out), "misaligned buffer");
+  ONERF_CHECK_ARG(n >= 0 && (n == 0 || n_codes >= 1), "an empty code table has no row to read");
   if (n == 0) return ONERF_OK;
   code_gather_kernel<<<(n * 16 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(table, ids, n, n_codes, out);
   ONERF_LAUNCH_CHECK(ctx);
@@ -252,6 +257,7 @@ extern "C" int onerf_code_gather(onerf_ctx* ctx, const float* table, const int64
 extern "C" int onerf_code_scatter_add(onerf_ctx* ctx, const float* d_codes, const int64_t* ids, int n, int n_codes,
                                       float* table_grad, void* stream) {
   ONERF_CHECK_ARG(ctx && d_codes && ids && table_grad, "null argument");
+  ONERF_CHECK_ARG(n >= 0 && (n == 0 || n_codes >= 1), "an empty code table has no row to add to");
   if (n == 0) return ONERF_OK;
   code_scatter_kernel<<<(n * 64 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(d_codes, ids, n, n_codes, table_grad);
   ONERF_LAUNCH_CHECK(ctx);
