@@ -32,6 +32,62 @@ int onerf_composite_multi_merge(onerf_ctx* ctx, const float* z_all, const float*
                                 size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Sigma noise and box-clipped ray sets on the editing path (render_tools/multi_rendering.py:131-132, 278-287).
+ *
+ * onerf_composite_multi_noise_ws / _merge: onerf_composite_multi_ws / _merge with alpha taken from
+ * relu(sigma + noise * noise_std) (the multiply rounded first).  The noise is indexed by SORTED position: sample p of ray r
+ * takes noise[r * T + p] ((N, T) row-major, T = n_obj * n_samples) if `noise` is given, else the Philox normal of stream
+ * ONERF_STREAM_MULTI_NOISE_COARSE (pass 0) or ONERF_STREAM_MULTI_NOISE_FINE (pass 1) at element r * T + p keyed by
+ * `seed` (the draw of onerf_composite's streams 2 / 3 with another stream id).  Both paths give the same bits for the same
+ * order.  noise_std = 0 draws nothing and gives the bits of the entries without noise.  Refusals (ONERF_ERR_BAD_ARG):
+ * noise_std negative or not finite, a noise buffer with noise_std = 0, a noise buffer not 4-byte aligned, pass not 0 / 1.
+ *
+ * onerf_sample_pdf_merge_clip: onerf_sample_pdf_merge whose merged row is stored through the box clip of a 10-column ray
+ * set: with (near_box, far_box) = clip[r] ((N,2) row-major), every z with near_box < z < far_box (both strict) becomes
+ * far_box.  Comparisons only: bit-exact, and the row stays ascending.  clip NULL is onerf_sample_pdf_merge.  Refusals: a
+ * clip not 8-byte aligned or a u not 4-byte aligned, and those of onerf_sample_pdf_merge.
+ * ------------------------------------------------------------------------------------------- */
+#define ONERF_STREAM_MULTI_NOISE_COARSE 7
+#define ONERF_STREAM_MULTI_NOISE_FINE 8
+int onerf_composite_multi_noise_ws(onerf_ctx* ctx, const float* z_all, const float* field_all, int n_rays, int n_obj,
+                                   int n_samples, int white_back, float noise_std, const float* noise, uint64_t seed,
+                                   int pass, float* z_sorted, float* weights, float* obj_ids, float* weights_unsorted,
+                                   float* opacity, float* rgb, float* depth, void* workspace, size_t workspace_bytes,
+                                   void* stream);
+int onerf_composite_multi_noise_merge(onerf_ctx* ctx, const float* z_all, const float* field_all, int n_rays, int n_obj,
+                                      int n_samples, int white_back, float noise_std, const float* noise, uint64_t seed,
+                                      int pass, float* z_sorted, float* weights, float* obj_ids, float* weights_unsorted,
+                                      float* opacity, float* rgb, float* depth, void* workspace, size_t workspace_bytes,
+                                      void* stream);
+int onerf_sample_pdf_merge_clip(onerf_ctx* ctx, const float* z_coarse, const float* weights, int n_rays, int n_samples,
+                                int n_importance, int det, const float* u, uint64_t seed, const float* clip, float* z_out,
+                                void* stream);
+
+/* onerf_render_multi_fwd with what render_rays_multi takes beyond it.  onerf_render_multi_fwd is this call with a zeroed
+ * onerf_render_multi_ext (ext == NULL is the same).  The coarse pass composites with noise_coarse (or stream 7), the
+ * fine pass with noise_fine (or stream 8), both keyed by args->seed; the coarse weights that feed each set's importance
+ * sampling are the noised ones.  Set i draws its importance u from u_list_host[i] when given, else as
+ * onerf_render_multi_fwd does (Philox stream 1 keyed by args->seed + i; linspace when perturb = 0).  A set with
+ * clip_list_host[i] != NULL is a 10-column set: its fine depths go through onerf_sample_pdf_merge_clip's clip, which the
+ * muting test (z[:, -1] == 0) and the box culling see; its coarse depths are not clipped, and without a fine pass the
+ * clip is unused.  Sets with and without a clip may be mixed.
+ * Refusals (ONERF_ERR_BAD_ARG), besides those of onerf_render_multi_fwd: noise_std negative or not finite; a noise buffer
+ * with noise_std = 0, or noise_fine without a fine pass; a u with perturb = 0 or without a fine pass; a noise or u buffer
+ * not 4-byte aligned, a clip not 8-byte aligned. */
+typedef struct onerf_render_multi_ext {
+  float noise_std;                    /* 0: no noise, nothing drawn */
+  const float* noise_coarse;          /* (N, n_obj * n_samples) N(0,1) in sorted order, or NULL */
+  const float* noise_fine;            /* (N, n_obj * (n_samples + n_importance)), or NULL */
+  const float* const* clip_list_host; /* NULL, or n_obj DEVICE pointers (host array) to (N,2) (near_box, far_box), NULL
+                                         for a set without a clip */
+  const float* const* u_list_host;    /* NULL, or n_obj DEVICE pointers (host array) to (N, n_importance) U[0,1), NULL
+                                         entries drawn */
+} onerf_render_multi_ext;
+
+int onerf_render_multi_fwd_ext(onerf_ctx* ctx, const onerf_render_multi_args* args, const onerf_render_multi_ext* ext,
+                               void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Size of the training workspace of onerf_render_rays_fwd / onerf_render_rays_bwd for either arithmetic (precision =
  * onerf_precision); onerf_train_workspace_bytes is this with ONERF_PREC_BF16.  The fp32 workspace holds both passes'
  * fields and one chunk (at most 65 536 samples) of the backward's activation dump and gradient buffers.  0 for an
@@ -74,7 +130,8 @@ int onerf_train_step_dseed(onerf_ctx* ctx, const onerf_render_args* fwd, const o
  * An edited frame from a camera (EditableRenderer.render_edit, editable_renderer.py:203-294), or a contiguous tile of it.
  * Pixels [pixel_begin, pixel_end) (row-major) of the H x W frame are rendered in chunks of chunk_rays pixels; for each
  * chunk every set's rays are generated on the device exactly as onerf_camera_rays generates them for those pixels, the
- * chunk runs through onerf_render_multi_fwd's path (perturb = 0, so nothing is random) and its maps are written to rows
+ * chunk runs through onerf_render_multi_fwd's path (perturb = 0 and no noise, so nothing is random; 8-column sets) and
+ * its maps are written to rows
  * [chunk - pixel_begin, ...) of the tile-sized outputs.  Every result row depends on its pixel only, never on chunk_rays
  * or the tile bounds.
  *   sets_host  n_obj ray sets (host array).  obj_id 0 = scene branch (box NULL: near / far = near, far / scale_factor),

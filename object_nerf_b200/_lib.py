@@ -40,10 +40,13 @@ EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_w
                "onerf_render_rays_fwd_dseed", "onerf_train_step_dseed", "onerf_render_edit_workspace_bytes",
                "onerf_render_edit_frame", "onerf_draw_batch", "onerf_draw_batch_dstep",
                "onerf_validate_workspace_bytes", "onerf_validate_frame", "onerf_validate_finalize",
-               "onerf_prune_workspace_bytes", "onerf_prune_measure", "onerf_prune_apply"]
+               "onerf_prune_workspace_bytes", "onerf_prune_measure", "onerf_prune_apply",
+               "onerf_composite_multi_noise_ws", "onerf_composite_multi_noise_merge", "onerf_sample_pdf_merge_clip",
+               "onerf_render_multi_fwd_ext"]
 VALIDATE_RECORD_DOUBLES = 18
 PRUNE_SAMPLES = 4096
 PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
+STREAM_MULTI_NOISE_COARSE, STREAM_MULTI_NOISE_FINE = 7, 8   # Philox streams of the joint compositing's sigma noise
 
 _p = C.c_void_p
 
@@ -122,6 +125,11 @@ class RenderMultiArgs(C.Structure):
         ("perturb", C.c_float), ("seed", C.c_uint64), ("white_back", C.c_int), ("boxes", _p), ("n_boxes", C.c_int),
         ("coarse", RenderMultiMaps), ("fine", RenderMultiMaps), ("workspace", _p), ("workspace_bytes", C.c_size_t),
     ]
+
+
+class RenderMultiExt(C.Structure):
+    _fields_ = [("noise_std", C.c_float), ("noise_coarse", _p), ("noise_fine", _p), ("clip_list_host", C.POINTER(_p)),
+                ("u_list_host", C.POINTER(_p))]
 
 
 class EditSet(C.Structure):
@@ -270,6 +278,11 @@ def load() -> C.CDLL:
         lib.onerf_composite_multi_workspace_bytes.restype = C.c_size_t
         for name in ("onerf_composite_multi_ws", "onerf_composite_multi_merge"):
             getattr(lib, name).argtypes = lib.onerf_composite_multi.argtypes[:-1] + [_p, C.c_size_t, _p]
+        for name in ("onerf_composite_multi_noise_ws", "onerf_composite_multi_noise_merge"):
+            getattr(lib, name).argtypes = ([_p, _p, _p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _p, C.c_uint64, C.c_int]
+                                           + [_p] * 7 + [_p, C.c_size_t, _p])
+        lib.onerf_sample_pdf_merge_clip.argtypes = [_p, _p, _p, C.c_int, C.c_int, C.c_int, C.c_int, _p, C.c_uint64, _p, _p, _p]
+        lib.onerf_render_multi_fwd_ext.argtypes = [_p, C.POINTER(RenderMultiArgs), C.POINTER(RenderMultiExt), _p]
         lib.onerf_train_workspace_bytes_prec.argtypes = [C.c_int] * 5
         lib.onerf_train_workspace_bytes_prec.restype = C.c_size_t
         lib.onerf_train_step_workspace_bytes.argtypes = [C.c_int] * 5

@@ -1,4 +1,5 @@
 // C-ABI plumbing: context, errors, and the field entry point's argument validation / dispatch.
+#include <float.h>
 #include <stdarg.h>
 #include <string.h>
 
@@ -378,27 +379,62 @@ static int check_multi_args(const char* fn, const onerf_render_multi_args* a, bo
     FN_CHECK_ARG(a->fine.weights && a->fine.opacity && a->fine.z_vals && a->fine.rgb && a->fine.depth, "null fine output");
   return ONERF_OK;
 }
+
+// The checks of onerf_render_multi_fwd_ext's extension block against the call's arguments.
+static int check_multi_ext(const char* fn, const onerf_render_multi_args* a, const onerf_render_multi_ext* x) {
+  FN_CHECK_ARG(x->noise_std >= 0.0f && x->noise_std <= FLT_MAX, "noise_std must be finite and >= 0");
+  FN_CHECK_ARG(!(x->noise_coarse || x->noise_fine) || x->noise_std != 0.0f, "a noise buffer with noise_std = 0");
+  FN_CHECK_ARG(!x->noise_fine || a->n_importance > 0, "noise_fine without a fine pass");
+  FN_CHECK_ARG(onerf_aligned4(x->noise_coarse) && onerf_aligned4(x->noise_fine), "noise buffers must be 4-byte aligned");
+  for (int i = 0; i < a->n_obj; ++i) {
+    const float* u = x->u_list_host ? x->u_list_host[i] : nullptr;
+    const float* clip = x->clip_list_host ? x->clip_list_host[i] : nullptr;
+    FN_CHECK_ARG(!u || (a->n_importance > 0 && a->perturb != 0.0f), "a u buffer with perturb = 0 or without a fine pass");
+    FN_CHECK_ARG(onerf_aligned4(u), "u buffers must be 4-byte aligned");
+    FN_CHECK_ARG(onerf_aligned8(clip), "clip buffers must be 8-byte aligned");
+  }
+  return ONERF_OK;
+}
 #undef FN_CHECK_ARG
 #undef FN_UNSUPPORTED
 
-static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, void* stream);
+static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const onerf_render_multi_ext& x, void* stream);
+
+static int render_multi_fwd(const char* fn, onerf_ctx* ctx, const onerf_render_multi_args* a,
+                            const onerf_render_multi_ext* ext, void* stream) {
+  int rc = check_multi_args(fn, a, true);
+  if (rc != ONERF_OK) return rc;
+  onerf_render_multi_ext none;
+  memset(&none, 0, sizeof(none));
+  const onerf_render_multi_ext& x = ext ? *ext : none;
+  rc = check_multi_ext(fn, a, &x);
+  if (rc != ONERF_OK) return rc;
+  const size_t need = onerf_render_multi_workspace_bytes(a->n_rays, a->n_obj, a->n_samples, a->n_importance);
+  if (!a->workspace || (reinterpret_cast<uintptr_t>(a->workspace) & 255u) != 0) {
+    onerf_set_error("%s: workspace null or not 256-byte aligned", fn);
+    return ONERF_ERR_BAD_ARG;
+  }
+  if (a->workspace_bytes < need) {
+    onerf_set_error("%s: workspace too small (%zu < %zu)", fn, a->workspace_bytes, need);
+    return ONERF_ERR_WORKSPACE;
+  }
+  return multi_forward(ctx, a, x, stream);
+}
 
 extern "C" int onerf_render_multi_fwd(onerf_ctx* ctx, const onerf_render_multi_args* a, void* stream) {
   ONERF_CHECK_ARG(ctx && a, "null argument");
-  const int rc = check_multi_args(__func__, a, true);
-  if (rc != ONERF_OK) return rc;
-  const size_t need = onerf_render_multi_workspace_bytes(a->n_rays, a->n_obj, a->n_samples, a->n_importance);
-  ONERF_CHECK_ARG(a->workspace && (reinterpret_cast<uintptr_t>(a->workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
-  if (a->workspace_bytes < need) {
-    onerf_set_error("onerf_render_multi_fwd: workspace too small (%zu < %zu)", a->workspace_bytes, need);
-    return ONERF_ERR_WORKSPACE;
-  }
-  return multi_forward(ctx, a, stream);
+  return render_multi_fwd(__func__, ctx, a, nullptr, stream);
 }
 
-// The forward of onerf_render_multi_fwd on checked arguments: n_rays rays of every set in a->rays_list_host, maps written
-// to a->coarse / a->fine, scratch in a->workspace.
-static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, void* stream) {
+extern "C" int onerf_render_multi_fwd_ext(onerf_ctx* ctx, const onerf_render_multi_args* a, const onerf_render_multi_ext* ext,
+                                          void* stream) {
+  ONERF_CHECK_ARG(ctx && a, "null argument");
+  return render_multi_fwd(__func__, ctx, a, ext, stream);
+}
+
+// The forward of onerf_render_multi_fwd_ext on checked arguments: n_rays rays of every set in a->rays_list_host, maps
+// written to a->coarse / a->fine, scratch in a->workspace.
+static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const onerf_render_multi_ext& x, void* stream) {
   const onerf_render_multi_maps& c = a->coarse;
   if (a->n_rays == 0) return ONERF_OK;
   const int S = a->n_samples, SF = a->n_samples + a->n_importance, N = a->n_rays, NO = a->n_obj;
@@ -410,20 +446,24 @@ static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, void*
   }
   rc = multi_fields(ctx, a, a->packed_coarse, w.z_all, S, w, stream);
   if (rc != ONERF_OK) return rc;
-  rc = onerf_composite_multi_ws(ctx, w.z_all, w.field_all, N, NO, S, a->white_back, c.z_vals, c.weights, c.obj_ids,
-                                a->n_importance > 0 ? w.w_unsorted : nullptr, c.opacity, c.rgb, c.depth, w.sort, w.sort_bytes,
-                                stream);
+  rc = onerf_composite_multi_noise_ws(ctx, w.z_all, w.field_all, N, NO, S, a->white_back, x.noise_std, x.noise_coarse, a->seed,
+                                      0, c.z_vals, c.weights, c.obj_ids, a->n_importance > 0 ? w.w_unsorted : nullptr,
+                                      c.opacity, c.rgb, c.depth, w.sort, w.sort_bytes, stream);
   if (rc != ONERF_OK || a->n_importance == 0) return rc;
   const int det = a->perturb == 0.0f ? 1 : 0;
   for (int i = 0; i < NO; ++i) {
-    rc = onerf_sample_pdf_merge(ctx, w.z_all + (size_t)i * N * S, w.w_unsorted + (size_t)i * N * S, N, S, a->n_importance, det,
-                                nullptr, det ? 0 : a->seed + (uint64_t)i, w.z_fine + (size_t)i * N * SF, stream);
+    const float* u = x.u_list_host ? x.u_list_host[i] : nullptr;
+    const float* clip = x.clip_list_host ? x.clip_list_host[i] : nullptr;
+    rc = onerf_launch_sample_pdf_merge(ctx, w.z_all + (size_t)i * N * S, w.w_unsorted + (size_t)i * N * S, N, S,
+                                       a->n_importance, det, u, det ? 0 : a->seed + (uint64_t)i, nullptr,
+                                       w.z_fine + (size_t)i * N * SF, stream, clip);
     if (rc != ONERF_OK) return rc;
   }
   rc = multi_fields(ctx, a, a->packed_fine, w.z_fine, SF, w, stream);
   if (rc != ONERF_OK) return rc;
-  return onerf_composite_multi_ws(ctx, w.z_fine, w.field_all, N, NO, SF, a->white_back, a->fine.z_vals, a->fine.weights, nullptr,
-                                  nullptr, a->fine.opacity, a->fine.rgb, a->fine.depth, w.sort, w.sort_bytes, stream);
+  return onerf_composite_multi_noise_ws(ctx, w.z_fine, w.field_all, N, NO, SF, a->white_back, x.noise_std, x.noise_fine,
+                                        a->seed, 1, a->fine.z_vals, a->fine.weights, nullptr, nullptr, a->fine.opacity,
+                                        a->fine.rgb, a->fine.depth, w.sort, w.sort_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -495,6 +535,8 @@ extern "C" int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_a
   const int chunk = a->chunk_rays;
   onerf_render_multi_args m;
   memset(&m, 0, sizeof(m));
+  onerf_render_multi_ext no_ext;
+  memset(&no_ext, 0, sizeof(no_ext));
   m.obj_ids_host = ids.data();
   m.n_obj = NO; m.n_rays = (int)(n_tile < chunk ? n_tile : chunk);
   m.n_samples = a->n_samples; m.n_importance = a->n_importance;
@@ -528,7 +570,7 @@ extern "C" int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_a
     m.n_rays = n;
     m.coarse = chunk_maps(a->coarse, w.coarse, r0, TC);
     if (a->n_importance > 0) m.fine = chunk_maps(a->fine, w.fine, r0, TF);
-    rc = multi_forward(ctx, &m, stream);
+    rc = multi_forward(ctx, &m, no_ext, stream);
     if (rc != ONERF_OK) return rc;
   }
   return ONERF_OK;

@@ -67,6 +67,8 @@ int onerf_launch_camera_rays(onerf_ctx* ctx, int H, int W, float focal, const fl
   } while (0)
 
 static inline bool onerf_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+static inline bool onerf_aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
+static inline bool onerf_aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 
 // ---------------------------------------------------------------------------------------------
 // warp helpers

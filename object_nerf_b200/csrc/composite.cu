@@ -3,6 +3,7 @@
 // float4 access); the scan itself is composite_core.cuh's composite_scan.
 //
 // Reference behaviour: models/rendering.py:139-229; render_tools/multi_rendering.py:96-157.
+#include <float.h>
 #include <string.h>
 
 #include <algorithm>
@@ -193,10 +194,30 @@ __device__ __forceinline__ void store_multi_maps(const Acc& acc, int white_back,
   }
 }
 
+// Sigma noise of the joint compositing (render_tools/multi_rendering.py:131-132: one randn_like over the sorted sigmas):
+// sorted sample p of ray r takes buf[r * T + p] if the caller gives a buffer, else Philox stream `stream_id`
+// (ONERF_STREAM_MULTI_NOISE_COARSE / _FINE) at element r * T + p, keyed by `seed`.  Only read by the kNoise instances of
+// the two compositing kernels; std == 0 launches the noise-free ones.
+struct MultiNoise {
+  float std;
+  const float* buf;
+  uint64_t seed;
+  uint32_t stream_id;
+};
+
+// relu's argument sigma + noise * std, the multiply rounded first as the reference's (randn * std) + sigma
+template <bool kNoise>
+__device__ __forceinline__ float multi_sigma(float sigma, const MultiNoise& nz, int64_t e) {
+  if (!kNoise) return sigma;
+  const float v = nz.buf ? __ldg(nz.buf + e) : philox_normal(nz.seed, nz.stream_id, (uint64_t)e);
+  return __fadd_rn(sigma, __fmul_rn(v, nz.std));
+}
+
 // One warp per ray.  Shared memory per warp: keys[P] (uint64: orderable z << 32 | concat index).
+template <bool kNoise>
 __global__ void __launch_bounds__(128)
 composite_multi_kernel(const float* __restrict__ z_all, const float4* __restrict__ field_all, int n_rays,
-                       int n_obj, int S, int P, int white_back, float* __restrict__ z_sorted,
+                       int n_obj, int S, int P, int white_back, MultiNoise nz, float* __restrict__ z_sorted,
                        float* __restrict__ weights, float* __restrict__ obj_ids,
                        float* __restrict__ weights_unsorted, float* __restrict__ opacity,
                        float* __restrict__ rgb, float* __restrict__ depth) {
@@ -220,7 +241,7 @@ composite_multi_kernel(const float* __restrict__ z_all, const float4* __restrict
       const float zn = (i + 1 < T) ? __ldg(z + src_off((int)(keys[i + 1] & 0xffffffffu), S, obj_stride)) : zi;
       const float delta = (i + 1 < T) ? __fsub_rn(zn, zi) : 0.0f;  // multi_rendering.py:125-128
       const float4 f = __ldg(fld + src_off(src, S, obj_stride));
-      return Sample{zi, delta, f.w, f, false, src};
+      return Sample{zi, delta, multi_sigma<kNoise>(f.w, nz, (int64_t)r * T + i), f, false, src};
     };
     auto sink = [&](int i, const Sample& s, float, float, float w) {
       const int64_t o = (int64_t)r * T + i;
@@ -317,9 +338,10 @@ merge_rank_kernel(const float* __restrict__ z_all, int n_rays, int n_obj, int S,
 
 // One warp per ray: composite_scan, as in composite_multi_kernel, over the order the rank kernel left in weights[] /
 // z_sorted[].
+template <bool kNoise>
 __global__ void __launch_bounds__(128)
 merge_composite_kernel(const float4* __restrict__ field_all, int n_rays, int n_obj, int S,
-                       int white_back, const float* __restrict__ z_sorted, float* __restrict__ weights,
+                       int white_back, MultiNoise nz, const float* __restrict__ z_sorted, float* __restrict__ weights,
                        float* __restrict__ obj_ids, float* __restrict__ weights_unsorted, float* __restrict__ opacity,
                        float* __restrict__ rgb, float* __restrict__ depth) {
   const int warps_per_block = blockDim.x >> 5;
@@ -337,7 +359,7 @@ merge_composite_kernel(const float4* __restrict__ field_all, int n_rays, int n_o
       const float zn = (i + 1 < T) ? zs[i + 1] : zi;
       const float delta = (i + 1 < T) ? __fsub_rn(zn, zi) : 0.0f;  // multi_rendering.py:125-128
       const float4 f = __ldg(fld + src_off(src, S, obj_stride));
-      return Sample{zi, delta, f.w, f, false, src};
+      return Sample{zi, delta, multi_sigma<kNoise>(f.w, nz, (int64_t)r * T + i), f, false, src};
     };
     auto sink = [&](int i, const Sample& s, float, float, float w) {
       wr[i] = w;
@@ -404,21 +426,24 @@ extern "C" size_t onerf_composite_multi_workspace_bytes(int n_rays, int n_obj, i
   return merge_ws_bytes(n_rays, (int64_t)n_obj * n_samples);
 }
 
-// path: 0 = bitonic kernel (T <= 4096, no workspace), 1 = rank merge (any T up to the int32 / per-set bounds)
+// path: 0 = bitonic kernel (T <= 4096, no workspace), 1 = rank merge (any T up to the int32 / per-set bounds).
+// nz.std == 0 runs the noise-free kernels.
 static int composite_multi_run(onerf_ctx* ctx, int path, const float* z_all, const float* field_all, int n_rays, int n_obj,
-                               int n_samples, int white_back, float* z_sorted, float* weights, float* obj_ids,
-                               float* weights_unsorted, float* opacity, float* rgb, float* depth, void* workspace,
-                               size_t workspace_bytes, cudaStream_t stream) {
+                               int n_samples, int white_back, const MultiNoise& nz, float* z_sorted, float* weights,
+                               float* obj_ids, float* weights_unsorted, float* opacity, float* rgb, float* depth,
+                               void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   const int T = n_obj * n_samples;
   if (n_rays == 0) return ONERF_OK;
   const int warps = 4;
+  const bool noise = nz.std != 0.0f;
   if (path == 0) {
     int P = 2;
     while (P < T) P <<= 1;
     const size_t smem = (size_t)warps * P * sizeof(unsigned long long);
-    ONERF_CUDA(cudaFuncSetAttribute(composite_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    composite_multi_kernel<<<composite_blocks(ctx, n_rays, warps), warps * 32, smem, stream>>>(
-        z_all, reinterpret_cast<const float4*>(field_all), n_rays, n_obj, n_samples, P, white_back, z_sorted,
+    auto kernel = noise ? composite_multi_kernel<true> : composite_multi_kernel<false>;
+    ONERF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<composite_blocks(ctx, n_rays, warps), warps * 32, smem, stream>>>(
+        z_all, reinterpret_cast<const float4*>(field_all), n_rays, n_obj, n_samples, P, white_back, nz, z_sorted,
         weights, obj_ids, weights_unsorted, opacity, rgb, depth);
     ONERF_LAUNCH_CHECK(ctx);
     return ONERF_OK;
@@ -436,12 +461,15 @@ static int composite_multi_run(onerf_ctx* ctx, int path, const float* z_all, con
   ONERF_LAUNCH_CHECK(ctx);
   merge_rank_kernel<<<list_blocks, warps * 32, 0, stream>>>(z_all, n_rays, n_obj, n_samples, skey, sidx, z_sorted, weights);
   ONERF_LAUNCH_CHECK(ctx);
-  merge_composite_kernel<<<composite_blocks(ctx, n_rays, warps), warps * 32, 0, stream>>>(
-      reinterpret_cast<const float4*>(field_all), n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
+  auto kernel = noise ? merge_composite_kernel<true> : merge_composite_kernel<false>;
+  kernel<<<composite_blocks(ctx, n_rays, warps), warps * 32, 0, stream>>>(
+      reinterpret_cast<const float4*>(field_all), n_rays, n_obj, n_samples, white_back, nz, z_sorted, weights, obj_ids,
       weights_unsorted, opacity, rgb, depth);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }
+
+static const MultiNoise kNoNoise = {0.0f, nullptr, 0, 0};
 
 #define MULTI_ARGS_OK()                                                                                                 \
   ONERF_CHECK_ARG(ctx && z_all && field_all && z_sorted && weights && opacity && rgb && depth, "null argument");        \
@@ -454,14 +482,14 @@ extern "C" int onerf_composite_multi(onerf_ctx* ctx, const float* z_all, const f
                                      float* rgb, float* depth, void* stream) {
   MULTI_ARGS_OK();
   ONERF_UNSUPPORTED((int64_t)n_obj * n_samples > 4096, "n_obj * n_samples > 4096 (onerf_composite_multi_ws has no such limit)");
-  return composite_multi_run(ctx, 0, z_all, field_all, n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
-                             weights_unsorted, opacity, rgb, depth, nullptr, 0, (cudaStream_t)stream);
+  return composite_multi_run(ctx, 0, z_all, field_all, n_rays, n_obj, n_samples, white_back, kNoNoise, z_sorted, weights,
+                             obj_ids, weights_unsorted, opacity, rgb, depth, nullptr, 0, (cudaStream_t)stream);
 }
 
 static int composite_multi_ws(onerf_ctx* ctx, int force_merge, const float* z_all, const float* field_all, int n_rays,
-                              int n_obj, int n_samples, int white_back, float* z_sorted, float* weights, float* obj_ids,
-                              float* weights_unsorted, float* opacity, float* rgb, float* depth, void* workspace,
-                              size_t workspace_bytes, void* stream) {
+                              int n_obj, int n_samples, int white_back, const MultiNoise& nz, float* z_sorted,
+                              float* weights, float* obj_ids, float* weights_unsorted, float* opacity, float* rgb,
+                              float* depth, void* workspace, size_t workspace_bytes, void* stream) {
   MULTI_ARGS_OK();
   const int64_t T = (int64_t)n_obj * n_samples;
   const int path = (force_merge || T > 4096) ? 1 : 0;
@@ -475,22 +503,57 @@ static int composite_multi_ws(onerf_ctx* ctx, int force_merge, const float* z_al
       return ONERF_ERR_WORKSPACE;
     }
   }
-  return composite_multi_run(ctx, path, z_all, field_all, n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
-                             weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, (cudaStream_t)stream);
+  return composite_multi_run(ctx, path, z_all, field_all, n_rays, n_obj, n_samples, white_back, nz, z_sorted, weights,
+                             obj_ids, weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int onerf_composite_multi_ws(onerf_ctx* ctx, const float* z_all, const float* field_all, int n_rays, int n_obj,
                                         int n_samples, int white_back, float* z_sorted, float* weights, float* obj_ids,
                                         float* weights_unsorted, float* opacity, float* rgb, float* depth, void* workspace,
                                         size_t workspace_bytes, void* stream) {
-  return composite_multi_ws(ctx, 0, z_all, field_all, n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
-                            weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, stream);
+  return composite_multi_ws(ctx, 0, z_all, field_all, n_rays, n_obj, n_samples, white_back, kNoNoise, z_sorted, weights,
+                            obj_ids, weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, stream);
 }
 
 extern "C" int onerf_composite_multi_merge(onerf_ctx* ctx, const float* z_all, const float* field_all, int n_rays, int n_obj,
                                            int n_samples, int white_back, float* z_sorted, float* weights, float* obj_ids,
                                            float* weights_unsorted, float* opacity, float* rgb, float* depth, void* workspace,
                                            size_t workspace_bytes, void* stream) {
-  return composite_multi_ws(ctx, 1, z_all, field_all, n_rays, n_obj, n_samples, white_back, z_sorted, weights, obj_ids,
-                            weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, stream);
+  return composite_multi_ws(ctx, 1, z_all, field_all, n_rays, n_obj, n_samples, white_back, kNoNoise, z_sorted, weights,
+                            obj_ids, weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, stream);
+}
+
+// onerf_composite_multi_ws / _merge with sigma noise (include/onerf_ext.h)
+static int composite_multi_noise(onerf_ctx* ctx, int force_merge, const float* z_all, const float* field_all, int n_rays,
+                                 int n_obj, int n_samples, int white_back, float noise_std, const float* noise,
+                                 uint64_t seed, int pass, float* z_sorted, float* weights, float* obj_ids,
+                                 float* weights_unsorted, float* opacity, float* rgb, float* depth, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+  ONERF_CHECK_ARG(noise_std >= 0.0f && noise_std <= FLT_MAX, "noise_std must be finite and >= 0");
+  ONERF_CHECK_ARG(!noise || noise_std != 0.0f, "a noise buffer with noise_std = 0");
+  ONERF_CHECK_ARG(onerf_aligned4(noise), "noise buffer must be 4-byte aligned");
+  ONERF_CHECK_ARG(pass == 0 || pass == 1, "pass must be 0 (coarse) or 1 (fine)");
+  const MultiNoise nz = {noise_std, noise, seed, pass ? ONERF_STREAM_MULTI_NOISE_FINE : ONERF_STREAM_MULTI_NOISE_COARSE};
+  return composite_multi_ws(ctx, force_merge, z_all, field_all, n_rays, n_obj, n_samples, white_back, nz, z_sorted, weights,
+                            obj_ids, weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, stream);
+}
+
+extern "C" int onerf_composite_multi_noise_ws(onerf_ctx* ctx, const float* z_all, const float* field_all, int n_rays,
+                                              int n_obj, int n_samples, int white_back, float noise_std, const float* noise,
+                                              uint64_t seed, int pass, float* z_sorted, float* weights, float* obj_ids,
+                                              float* weights_unsorted, float* opacity, float* rgb, float* depth,
+                                              void* workspace, size_t workspace_bytes, void* stream) {
+  return composite_multi_noise(ctx, 0, z_all, field_all, n_rays, n_obj, n_samples, white_back, noise_std, noise, seed, pass,
+                               z_sorted, weights, obj_ids, weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes,
+                               stream);
+}
+
+extern "C" int onerf_composite_multi_noise_merge(onerf_ctx* ctx, const float* z_all, const float* field_all, int n_rays,
+                                                 int n_obj, int n_samples, int white_back, float noise_std,
+                                                 const float* noise, uint64_t seed, int pass, float* z_sorted, float* weights,
+                                                 float* obj_ids, float* weights_unsorted, float* opacity, float* rgb,
+                                                 float* depth, void* workspace, size_t workspace_bytes, void* stream) {
+  return composite_multi_noise(ctx, 1, z_all, field_all, n_rays, n_obj, n_samples, white_back, noise_std, noise, seed, pass,
+                               z_sorted, weights, obj_ids, weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes,
+                               stream);
 }

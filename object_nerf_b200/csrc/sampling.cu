@@ -4,6 +4,7 @@
 // Reference behaviour: models/rendering.py:259-277 (stratified), :11-61 (sample_pdf), :301-313 (merge).
 #include "common.cuh"
 #include "train_ws.h"
+#include "../../include/onerf_ext.h"
 
 namespace {
 
@@ -62,10 +63,15 @@ __device__ __forceinline__ double warp_scan_add(double v, int lane) {
 }
 
 // One warp per ray.  Shared memory per warp: bins[S-1] | cdf[S-1] | merged[P], P = pow2 >= S+K.
+// kClip (fused form only): the merged depths are stored through the box clip of a 10-column ray set
+// (render_tools/multi_rendering.py:278-287): z with clip[r][0] < z < clip[r][1] (both strict) becomes clip[r][1].
+// The map is monotone, so the stored row stays sorted.
+template <bool kClip>
 __global__ void __launch_bounds__(256)
 sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restrict__ weights, int n_rays,
                         int S, int K, int P, int det, const float* __restrict__ u_in, uint64_t seed,
-                        const uint64_t* seed_dev, float* __restrict__ z_out, const float* __restrict__ bins_in) {
+                        const uint64_t* seed_dev, float* __restrict__ z_out, const float* __restrict__ bins_in,
+                        const float* __restrict__ clip) {
   // bins_in != null: stand-alone sample_pdf on explicit bins (N, S-1) and weights (N, S-2): no merge,
   // z_out (N, K) in draw order.  Otherwise the fused form on coarse depths / full coarse weights.
   // seed_dev != null: as in sample_coarse_kernel.
@@ -135,7 +141,15 @@ sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restr
     for (int i = S + K + lane; i < P; i += 32) merged[i] = __int_as_float(0x7f800000);
     warp_bitonic_sort(merged, P, lane);
     float* out = z_out + (int64_t)r * (S + K);
-    for (int i = lane; i < S + K; i += 32) out[i] = merged[i];
+    if (kClip) {
+      const float near_box = __ldg(clip + 2 * (int64_t)r), far_box = __ldg(clip + 2 * (int64_t)r + 1);
+      for (int i = lane; i < S + K; i += 32) {
+        const float z = merged[i];
+        out[i] = (near_box < z && z < far_box) ? far_box : z;
+      }
+    } else {
+      for (int i = lane; i < S + K; i += 32) out[i] = merged[i];
+    }
     __syncwarp();
   }
 }
@@ -170,9 +184,17 @@ extern "C" int onerf_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, con
                                        stream);
 }
 
+extern "C" int onerf_sample_pdf_merge_clip(onerf_ctx* ctx, const float* z_coarse, const float* weights, int n_rays,
+                                           int n_samples, int n_importance, int det, const float* u, uint64_t seed,
+                                           const float* clip, float* z_out, void* stream) {
+  ONERF_CHECK_ARG(onerf_aligned8(clip) && onerf_aligned4(u), "clip must be 8-byte and u 4-byte aligned");
+  return onerf_launch_sample_pdf_merge(ctx, z_coarse, weights, n_rays, n_samples, n_importance, det, u, seed, nullptr, z_out,
+                                       stream, clip);
+}
+
 int onerf_launch_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, const float* weights, int n_rays, int n_samples,
                                   int n_importance, int det, const float* u, uint64_t seed, const uint64_t* seed_dev,
-                                  float* z_out, void* stream) {
+                                  float* z_out, void* stream, const float* clip) {
   ONERF_CHECK_ARG(ctx && z_coarse && weights && z_out, "null argument");
   // S = 2 leaves no pdf weight (weights[:, 1:-1] is empty): every sample is the one mid-point bin, as in the reference
   ONERF_CHECK_ARG(n_rays >= 0 && n_samples >= 2 && n_importance >= 1, "bad shape (need S >= 2, K >= 1)");
@@ -182,12 +204,13 @@ int onerf_launch_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, const f
   while (P < n_samples + n_importance) P <<= 1;
   const int warps = 8;
   const size_t smem = (size_t)warps * (2 * n_samples + P) * sizeof(float);
-  ONERF_CUDA(cudaFuncSetAttribute(sample_pdf_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  auto kernel = clip ? sample_pdf_merge_kernel<true> : sample_pdf_merge_kernel<false>;
+  ONERF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int blocks = (n_rays + warps - 1) / warps;
   const int cap = ctx->num_sms * 8;
   if (blocks > cap) blocks = cap;
-  sample_pdf_merge_kernel<<<blocks, warps * 32, smem, (cudaStream_t)stream>>>(
-      z_coarse, weights, n_rays, n_samples, n_importance, P, det, u, seed, seed_dev, z_out, nullptr);
+  kernel<<<blocks, warps * 32, smem, (cudaStream_t)stream>>>(
+      z_coarse, weights, n_rays, n_samples, n_importance, P, det, u, seed, seed_dev, z_out, nullptr, clip);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }
@@ -205,12 +228,12 @@ extern "C" int onerf_sample_pdf(onerf_ctx* ctx, const float* bins, const float* 
   while (P < S + n_importance) P <<= 1;
   const int warps = 8;
   const size_t smem = (size_t)warps * (2 * S + P) * sizeof(float);
-  ONERF_CUDA(cudaFuncSetAttribute(sample_pdf_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  ONERF_CUDA(cudaFuncSetAttribute(sample_pdf_merge_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int blocks = (n_rays + warps - 1) / warps;
   const int cap = ctx->num_sms * 8;
   if (blocks > cap) blocks = cap;
-  sample_pdf_merge_kernel<<<blocks, warps * 32, smem, (cudaStream_t)stream>>>(
-      nullptr, weights, n_rays, S, n_importance, P, det, u, seed, nullptr, out, bins);
+  sample_pdf_merge_kernel<false><<<blocks, warps * 32, smem, (cudaStream_t)stream>>>(
+      nullptr, weights, n_rays, S, n_importance, P, det, u, seed, nullptr, out, bins, nullptr);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

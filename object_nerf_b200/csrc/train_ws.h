@@ -114,7 +114,7 @@ int onerf_launch_sample_coarse(onerf_ctx* ctx, const float* rays, int n_rays, in
                                const float* jitter, uint64_t seed, const uint64_t* seed_dev, float* z_out, void* stream);
 int onerf_launch_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, const float* weights, int n_rays, int n_samples,
                                   int n_importance, int det, const float* u, uint64_t seed, const uint64_t* seed_dev,
-                                  float* z_out, void* stream);
+                                  float* z_out, void* stream, const float* clip = nullptr);   // clip: onerf_sample_pdf_merge_clip
 int onerf_launch_batch_stats(onerf_ctx* ctx, const onerf_loss_args* a, double* acc, cudaStream_t stream);
 // onerf_render_rays_fwd with an optional training step: step == NULL is the plain forward; otherwise both passes'
 // compositing runs onerf_launch_composite_step with `step` (fine / finalize / dscene / dobj set per pass from ws_step),

@@ -191,16 +191,24 @@ def sample_coarse(rays, n_samples, use_disp=False, perturb=0.0, jitter=None, see
 
 
 @_on_device
-def sample_pdf_merge(z_coarse, weights, n_importance, det, u=None, seed=0, out=None):
+def sample_pdf_merge(z_coarse, weights, n_importance, det, u=None, seed=0, out=None, clip=None):
+    """clip (N,2) = (near_box, far_box) of a 10-column ray set: merged depths strictly inside the interval become far_box
+    (onerf_sample_pdf_merge_clip)."""
     z_coarse, weights = _f32(z_coarse), _f32(weights.detach())
     n, s = z_coarse.shape
     if out is None:
         out = torch.empty(n, s + n_importance, dtype=torch.float32, device=z_coarse.device)
     assert out.is_contiguous() and out.shape == (n, s + n_importance)
     u = _f32(u) if u is not None else None
-    _lib.check(_lib.load().onerf_sample_pdf_merge(_lib.ctx(z_coarse.device), z_coarse.data_ptr(),
-                                                  weights.data_ptr(), n, s, n_importance, int(bool(det)),
-                                                  _lib.ptr(u), seed, out.data_ptr(), _lib.stream()))
+    lib = _lib.load()
+    args = (_lib.ctx(z_coarse.device), z_coarse.data_ptr(), weights.data_ptr(), n, s, n_importance, int(bool(det)),
+            _lib.ptr(u), seed)
+    if clip is None:
+        _lib.check(lib.onerf_sample_pdf_merge(*args, out.data_ptr(), _lib.stream()))
+    else:
+        clip = _f32(clip)
+        assert clip.shape == (n, 2)
+        _lib.check(lib.onerf_sample_pdf_merge_clip(*args, clip.data_ptr(), out.data_ptr(), _lib.stream()))
     return out
 
 
@@ -351,9 +359,12 @@ def composite_bwd(z, scene, obj, depth_scene, grads, noise_std=0.0, white_back=F
 
 
 @_on_device
-def composite_multi(z_all, field_all, white_back=False, want_ids=False, want_unsorted=False, merge=False):
+def composite_multi(z_all, field_all, white_back=False, want_ids=False, want_unsorted=False, merge=False, noise_std=0.0,
+                    noise=None, seed=0, fine=False):
     """z_all (n_obj, N, S), field_all (n_obj, N, S, 4) -> sorted-order outputs (N, n_obj*S).  Any n_obj * S: the bitonic
-    kernel up to 4096 samples per ray, the rank-merge path above (or always, with merge=True)."""
+    kernel up to 4096 samples per ray, the rank-merge path above (or always, with merge=True).
+    noise_std != 0: sigma noise by sorted position, from `noise` (N, n_obj*S) or else Philox stream 7 (coarse) / 8
+    (fine=True) keyed by `seed` (onerf_composite_multi_noise_ws / _merge)."""
     n_obj, n, s = z_all.shape
     t = n_obj * s
     dev = z_all.device
@@ -365,10 +376,16 @@ def composite_multi(z_all, field_all, white_back=False, want_ids=False, want_uns
     ws = None
     if merge or t > 4096:
         ws = torch.empty(max(lib.onerf_composite_multi_workspace_bytes(n, n_obj, s), 256), dtype=torch.uint8, device=dev)
-    entry = lib.onerf_composite_multi_merge if merge else lib.onerf_composite_multi_ws
+    head = (_lib.ctx(dev), z_all.data_ptr(), field_all.data_ptr(), n, n_obj, s, int(bool(white_back)))
+    if noise_std != 0 or noise is not None:
+        noise = _f32(noise) if noise is not None else None
+        assert noise is None or noise.shape == (n, t)
+        entry = lib.onerf_composite_multi_noise_merge if merge else lib.onerf_composite_multi_noise_ws
+        head += (float(noise_std), _lib.ptr(noise), seed, int(bool(fine)))
+    else:
+        entry = lib.onerf_composite_multi_merge if merge else lib.onerf_composite_multi_ws
     _lib.check(entry(
-        _lib.ctx(dev), z_all.data_ptr(), field_all.data_ptr(), n, n_obj, s, int(bool(white_back)),
-        out["z_vals"].data_ptr(), out["weights"].data_ptr(), _lib.ptr(ids), _lib.ptr(unsorted),
+        *head, out["z_vals"].data_ptr(), out["weights"].data_ptr(), _lib.ptr(ids), _lib.ptr(unsorted),
         out["opacity"].data_ptr(), out["rgb"].data_ptr(), out["depth"].data_ptr(), _lib.ptr(ws),
         ws.numel() if ws is not None else 0, _lib.stream()))
     if want_ids:

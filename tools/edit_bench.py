@@ -10,6 +10,7 @@ EditableRenderer.  The scene set carries two removed-object boxes.  A configurat
   python tools/edit_bench.py                      # 320x240 and 640x480: [0,4,4] with bench.py's random near / far
                                                   # (30 % misses), and [0] + [4] * k with boxes, k in 2 8 24 40
   python tools/edit_bench.py --bench-leg          # only bench.py's edit leg configuration (640x480, [0,4,4], 30 % misses)
+  python tools/edit_bench.py --bench-leg --noise-std 1   # the same with sigma noise drawn in the compositing kernels
   python tools/edit_bench.py --frame [--reps 5]   # a camera frame, three routes (below)
   torchrun --nproc-per-node N tools/edit_bench.py --frame    # ... plus the frame sharded over N GPUs
 
@@ -100,7 +101,7 @@ def bench_sets(rays, rng):
     return sets, hit_frac
 
 
-def time_frame(models, emb, lib, sets, ids, reps):
+def time_frame(models, emb, lib, sets, ids, reps, noise_std=0.0):
     from object_nerf_b200.multi_rendering import render_rays_multi
     boxes = {"4": Box(0), "6": Box(1)}
     n = sets[0].shape[0]
@@ -109,7 +110,8 @@ def time_frame(models, emb, lib, sets, ids, reps):
         with torch.no_grad():
             for i in range(0, n, CHUNK):
                 render_rays_multi(models, emb, lib, [s[i:i + CHUNK] for s in sets], ids, N_samples=64, N_importance=64,
-                                  chunk=CHUNK, white_back=False, background_skip_bbox=boxes, precision="bf16")
+                                  noise_std=noise_std, chunk=CHUNK, white_back=False, background_skip_bbox=boxes,
+                                  precision="bf16")
 
     frame()
     torch.cuda.synchronize()
@@ -241,6 +243,8 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--bench-leg", action="store_true")
     ap.add_argument("--frame", action="store_true")
+    ap.add_argument("--noise-std", type=float, default=0.0,
+                    help="sigma noise of render_rays_multi (drawn in the compositing kernels); 0 = the editing renderer's call")
     args = ap.parse_args()
     if args.frame:
         return frame_mode(args)
@@ -251,9 +255,9 @@ def main():
     if args.bench_leg:
         rays = S.pinhole_rays(480, 640).to(dev)
         sets, hf = bench_sets(rays, np.random.default_rng(7))
-        ms = time_frame(models, emb, lib, [rays] + sets, [0, 4, 4], args.reps)
+        ms = time_frame(models, emb, lib, [rays] + sets, [0, 4, 4], args.reps, args.noise_std)
         print(json.dumps({"config": "bench edit leg", "size": "640x480", "ids": [0, 4, 4], "ms_per_frame": ms,
-                          "object_rows_evaluated": statistics.mean(hf), "gpu": gpu}))
+                          "noise_std": args.noise_std, "object_rows_evaluated": statistics.mean(hf), "gpu": gpu}))
         return
     for size in args.sizes.split(","):
         w, h = (int(x) for x in size.split("x"))
@@ -264,7 +268,7 @@ def main():
             sets, hf = bench_sets(rays, rng) if name == "[0,4,4]" else box_sets(rays, k, rng)
             row = {"size": size, "ids": name, "n_sets": k + 1, "object_rows_evaluated": statistics.mean(hf), "gpu": gpu}
             try:
-                row["ms_per_frame"] = time_frame(models, emb, lib, [rays] + sets, [0] + [4] * k, args.reps)
+                row["ms_per_frame"] = time_frame(models, emb, lib, [rays] + sets, [0] + [4] * k, args.reps, args.noise_std)
             except RuntimeError as ex:
                 row["error"] = str(ex)[:160]
             print(json.dumps(row), flush=True)

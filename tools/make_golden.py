@@ -159,33 +159,58 @@ def gen_render_cases():
         save("render_" + name, **out)
 
 
+def _ref_multi_inputs(inp):
+    """The reference's models, embeddings, code library and removed-object box helpers of a multi case."""
+    models = {"coarse": ref_model(inp["weights"]["coarse"], True), "fine": ref_model(inp["weights"]["fine"], True)}
+    embeddings = {"xyz": ref_voxel_embedding(inp["grid"]), "dir": Embedding(3, 4)}
+
+    class Lib(torch.nn.Module):
+        def __init__(self, table):
+            super().__init__()
+            self.embedding_instance = torch.nn.Embedding.from_pretrained(table)
+
+    boxes = None
+    if inp["boxes"]:
+        boxes = {}
+        for k, b in enumerate(inp["boxes"]):
+            h = object.__new__(BBoxRayHelper)   # bypass the file-reading ctor (utils/bbox_utils.py:10-24)
+            h.scale_factor = b["scale_factor"]
+            h.pose_avg = b["pose_avg"]
+            h.axis_align_mat = b["axis_align_mat"]
+            h.bbox_bounds = b["bbox_bounds"]
+            boxes[k] = h
+    return models, embeddings, Lib(inp["code_table"]), boxes
+
+
 def gen_multi_cases():
     for name, c in cases.MULTI_CASES.items():
         inp = cases.build_multi_case(c)
-        models = {"coarse": ref_model(inp["weights"]["coarse"], True),
-                  "fine": ref_model(inp["weights"]["fine"], True)}
-        embeddings = {"xyz": ref_voxel_embedding(inp["grid"]), "dir": Embedding(3, 4)}
-
-        class Lib(torch.nn.Module):
-            def __init__(self, table):
-                super().__init__()
-                self.embedding_instance = torch.nn.Embedding.from_pretrained(table)
-
-        boxes = None
-        if inp["boxes"]:
-            boxes = {}
-            for k, b in enumerate(inp["boxes"]):
-                h = object.__new__(BBoxRayHelper)   # bypass the file-reading ctor (utils/bbox_utils.py:10-24)
-                h.scale_factor = b["scale_factor"]
-                h.pose_avg = b["pose_avg"]
-                h.axis_align_mat = b["axis_align_mat"]
-                h.bbox_bounds = b["bbox_bounds"]
-                boxes[k] = h
+        models, embeddings, lib, boxes = _ref_multi_inputs(inp)
         with torch.no_grad():
-            out = ref_render_rays_multi(models, embeddings, Lib(inp["code_table"]), inp["rays_list"],
+            out = ref_render_rays_multi(models, embeddings, lib, inp["rays_list"],
                                         c["obj_ids"], N_samples=c["n_samples"], use_disp=False, perturb=0,
                                         noise_std=0, N_importance=c["n_importance"], chunk=c.get("chunk", 32768),
                                         white_back=c["white_back"], background_skip_bbox=boxes)
+        save("multi_" + name, **out)
+
+
+def gen_multi_noise_clip_cases():
+    """render_rays_multi with sigma noise, perturbed importance sampling and 10-column ray sets
+    (tests/multi_noise_cases.py).  The reference draws randn_like over the sorted sigmas once per pass
+    (render_tools/multi_rendering.py:131) and torch.rand (N, K) once per set in sample_pdf (models/rendering.py:40);
+    InjectRandom hands it the case's buffers in that order."""
+    from tests import multi_noise_cases as M
+    for name, c in M.NOISE_CLIP_CASES.items():
+        inp = M.build_noise_clip_case(c)
+        models, embeddings, lib, boxes = _ref_multi_inputs(inp)
+        r = inp["rand"]
+        rand = list(r["u"]) if c["perturb"] != 0 else []
+        with torch.no_grad(), InjectRandom([], rand, [r["noise_coarse"], r["noise_fine"]]) as inj:
+            out = ref_render_rays_multi(models, embeddings, lib, inp["rays_list"], c["obj_ids"],
+                                        N_samples=c["n_samples"], use_disp=False, perturb=c["perturb"],
+                                        noise_std=c["noise_std"], N_importance=c["n_importance"], chunk=32768,
+                                        white_back=c["white_back"], background_skip_bbox=boxes)
+        assert not any(inj.seqs.values()), "the reference drew fewer random tensors than the case injects"
         save("multi_" + name, **out)
 
 
@@ -346,7 +371,7 @@ def gen_maint_cases():
 
 
 GENERATORS = ("ray_cases", "maint_cases", "loss_cases", "gridbuild", "grad_case", "grad_case_plain", "stage_cases",
-              "render_cases", "multi_cases")
+              "render_cases", "multi_cases", "multi_noise_clip_cases")
 
 if __name__ == "__main__":
     torch.set_num_threads(8)
@@ -366,3 +391,4 @@ if __name__ == "__main__":
     gen_stage_cases()
     gen_render_cases()
     gen_multi_cases()
+    gen_multi_noise_clip_cases()
