@@ -339,6 +339,48 @@ int onerf_prune_measure(onerf_ctx* ctx, const onerf_prune_args* args, void* stre
 int onerf_prune_apply(onerf_ctx* ctx, const int64_t* cells, int64_t n_cells, const float* max_alpha, float max_alpha_th,
                       int64_t dim_y, int64_t dim_z, uint8_t* occupancy, int64_t* idx_map, int64_t* n_pruned, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Backward of one field evaluation: ObjectNeRF.forward / forward_instance and inference_model under autograd
+ * (models/nerf_model.py:97-152, models/rendering.py:85-137).  A point query is a ray of one sample: rays[:, 3:6] = its
+ * direction, z = 0, xyz (B,1,3) = the points, codes (B,64) one row per point.
+ *   fwd      the onerf_field_fwd arguments of the forward: want_scene set, dense z and outputs (z_stride = out_stride =
+ *            n_samples), no editing extras, per-ray `codes` (not code_row) with want_object, xyz optional.
+ *            ONERF_PREC_BF16: the forward ran with train_ws (its dump) and its scene_out / obj_out still hold the fields;
+ *            ONERF_PREC_FP32: the backward re-runs the FFMA forward chunk by chunk with its activation dump.
+ *   d_scene, d_obj  (n_rays * n_samples, 4) d(r, g, b, sigma) of scene_out / obj_out (the float4 field layout); NULL = 0.
+ *            d_obj needs want_object.
+ *   grads    W: the 20 reference weight tensors (onerf_pack_weights order); dW / db: their gradients, ACCUMULATED (as
+ *            in onerf_render_bwd_args), all 20 pairs required, also without want_object; d_codes (n_rays,64)
+ *            accumulated, or NULL; table_grad (n_rows,24) accumulated, or
+ *            NULL (must be NULL for the plain-PE model); workspace >= onerf_field_bwd_workspace_bytes(precision,
+ *            grid != NULL, n_rays, n_samples) bytes, 1024-byte aligned.
+ * The stages are those of onerf_render_rays_bwd after its compositing backward: head -> input-gradient chain -> weight
+ * gradients -> per-ray-constant columns and d(code) -> encoding gradient, with each sample's position read from xyz when
+ * it is given.  Without want_object the object layers' dW / db keep their values (bf16 adds zeros to them, fp32 does not
+ * touch them).  No gradient flows to rays, z or xyz.
+ * Refusals: ONERF_ERR_BAD_ARG for the conditions above, ONERF_ERR_WORKSPACE for a small workspace.
+ *
+ * onerf_bwd_dx_xyz / onerf_encode_bwd_xyz: onerf_bwd_dx / onerf_encode_bwd with sample e at xyz[3 e .. 3 e + 2] instead
+ * of o + d z (stage entries).
+ * ------------------------------------------------------------------------------------------- */
+typedef struct onerf_field_bwd_args {
+  const float* const* W;
+  float* const* dW;
+  float* const* db;
+  float* d_codes;
+  float* table_grad;
+  void* workspace;
+  size_t workspace_bytes;
+} onerf_field_bwd_args;
+
+size_t onerf_field_bwd_workspace_bytes(int precision, int use_voxel, int n_rays, int n_samples);
+int onerf_field_bwd(onerf_ctx* ctx, const onerf_field_args* fwd, const float* d_scene, const float* d_obj,
+                    const onerf_field_bwd_args* grads, void* stream);
+int onerf_bwd_dx_xyz(onerf_ctx* ctx, int want_object, const void* packed, const void* ws, const float* xyz, int64_t n_samples,
+                     const onerf_grid* grid, float* table_grad, void* stream);
+int onerf_encode_bwd_xyz(onerf_ctx* ctx, const onerf_grid* grid, const float* xyz, const float* X, const float* dX, int ldx,
+                         int64_t sample0, int64_t n_chunk, float* table_grad, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -42,7 +42,8 @@ EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_w
                "onerf_validate_workspace_bytes", "onerf_validate_frame", "onerf_validate_finalize",
                "onerf_prune_workspace_bytes", "onerf_prune_measure", "onerf_prune_apply",
                "onerf_composite_multi_noise_ws", "onerf_composite_multi_noise_merge", "onerf_sample_pdf_merge_clip",
-               "onerf_render_multi_fwd_ext"]
+               "onerf_render_multi_fwd_ext", "onerf_field_bwd_workspace_bytes", "onerf_field_bwd", "onerf_bwd_dx_xyz",
+               "onerf_encode_bwd_xyz"]
 VALIDATE_RECORD_DOUBLES = 18
 PRUNE_SAMPLES = 4096
 PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
@@ -189,6 +190,11 @@ class RenderBwdArgs(C.Structure):
                 ("db_fine", C.POINTER(_p)), ("d_codes", _p), ("table_grad", _p)]
 
 
+class FieldBwdArgs(C.Structure):
+    _fields_ = [("W", C.POINTER(_p)), ("dW", C.POINTER(_p)), ("db", C.POINTER(_p)), ("d_codes", _p), ("table_grad", _p),
+                ("workspace", _p), ("workspace_bytes", C.c_size_t)]
+
+
 def build(verbose: bool = False) -> str:
     """Compile the CUDA sources for sm_90a into libonerf_sm90.so (nvcc cross-compiles without a GPU)."""
     r = subprocess.run(["make", "-C", CSRC, "-j8"], capture_output=True, text=True)
@@ -304,6 +310,11 @@ def load() -> C.CDLL:
         lib.onerf_prune_workspace_bytes.restype = C.c_size_t
         lib.onerf_prune_measure.argtypes = [_p, C.POINTER(PruneArgs), _p]
         lib.onerf_prune_apply.argtypes = [_p, _p, C.c_int64, _p, C.c_float, C.c_int64, C.c_int64, _p, _p, _p, _p]
+        lib.onerf_field_bwd_workspace_bytes.argtypes = [C.c_int] * 4
+        lib.onerf_field_bwd_workspace_bytes.restype = C.c_size_t
+        lib.onerf_field_bwd.argtypes = [_p, C.POINTER(FieldArgs), _p, _p, C.POINTER(FieldBwdArgs), _p]
+        lib.onerf_bwd_dx_xyz.argtypes = [_p, C.c_int, _p, _p, _p, C.c_int64, C.POINTER(Grid), _p, _p]
+        lib.onerf_encode_bwd_xyz.argtypes = [_p, C.POINTER(Grid), _p, _p, _p, C.c_int, C.c_int64, C.c_int64, _p, _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

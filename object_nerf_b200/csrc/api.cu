@@ -107,7 +107,7 @@ static int field_fwd(onerf_ctx* ctx, const onerf_field_args* a, const int* n_liv
   if (a->train_ws) {
     ONERF_UNSUPPORTED(a->precision != ONERF_PREC_BF16, "the training dump is written by the tensor-core (bf16) kernel");
     ONERF_UNSUPPORTED(!a->want_scene, "the training dump needs the scene branch");
-    ONERF_UNSUPPORTED(a->z_stride != a->n_samples || a->out_stride != a->n_samples || a->xyz, "training dump needs dense z / outputs and no explicit xyz");
+    ONERF_UNSUPPORTED(a->z_stride != a->n_samples || a->out_stride != a->n_samples, "training dump needs dense z / outputs");
     ONERF_UNSUPPORTED(a->mute_zero_rays || a->n_boxes > 0, "editing extras have no backward");
     ONERF_CHECK_ARG((reinterpret_cast<uintptr_t>(a->train_ws) & 1023u) == 0, "train_ws must be 1024-byte aligned");
     p.train_ws = a->train_ws;

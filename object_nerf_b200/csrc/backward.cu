@@ -9,6 +9,7 @@
 #include "composite_core.cuh"
 #include "encode.cuh"
 #include "field_common.cuh"
+#include "../../include/onerf_ext.h"
 
 namespace {
 
@@ -197,6 +198,8 @@ __global__ void dir_encode_kernel(const float* __restrict__ rays, int n, float* 
 //   d f_c = dX[f_c] + sum_k 2^k ( cos(2^k f_c) dX[sin_k c] - sin(2^k f_c) dX[cos_k c] ),  sin / cos taken from X itself;
 //   table_grad[row_corner][c] += trilinear weight * d f_c   (reference: embedding_helper.py:354-409 under autograd)
 // One thread per (sample, group of 8 channels): groups 0,1 = scene channels 0-7, 8-15; group 2 = object channels.
+// The sample's position is o + d z of its ray, or with XYZ row `gs` of p.xyz.
+template <bool XYZ>
 __global__ void __launch_bounds__(256)
 encode_bwd_kernel(FieldParams p, const float* __restrict__ X, const float* __restrict__ dX, int ldx, int64_t sample0,
                   int64_t n_samples, float* __restrict__ table_grad) {
@@ -205,12 +208,18 @@ encode_bwd_kernel(FieldParams p, const float* __restrict__ X, const float* __res
     const int64_t sl = e / 3;              // sample index inside the chunk
     const int grp = (int)(e - sl * 3);
     const int64_t gs = sample0 + sl;       // global sample index
-    const int ray = (int)(gs / p.S), si = (int)(gs - (int64_t)ray * p.S);
-    const float* rr = p.rays + (int64_t)ray * 8;
-    const float zz = __ldg(p.z + (int64_t)ray * p.z_stride + si);
-    const float x = __fadd_rn(__ldg(rr + 0), __fmul_rn(__ldg(rr + 3), zz));
-    const float y = __fadd_rn(__ldg(rr + 1), __fmul_rn(__ldg(rr + 4), zz));
-    const float z = __fadd_rn(__ldg(rr + 2), __fmul_rn(__ldg(rr + 5), zz));
+    float x, y, z;
+    if (XYZ) {
+      const float* q = p.xyz + gs * 3;
+      x = __ldg(q); y = __ldg(q + 1); z = __ldg(q + 2);
+    } else {
+      const int ray = (int)(gs / p.S), si = (int)(gs - (int64_t)ray * p.S);
+      const float* rr = p.rays + (int64_t)ray * 8;
+      const float zz = __ldg(p.z + (int64_t)ray * p.z_stride + si);
+      x = __fadd_rn(__ldg(rr + 0), __fmul_rn(__ldg(rr + 3), zz));
+      y = __fadd_rn(__ldg(rr + 1), __fmul_rn(__ldg(rr + 4), zz));
+      z = __fadd_rn(__ldg(rr + 2), __fmul_rn(__ldg(rr + 5), zz));
+    }
     const int base = (grp < 2) ? 0 : 272, width = (grp < 2) ? 16 : 8, ch0 = (grp == 1) ? 8 : 0;
     const float* xr = X + sl * ldx + base;
     const float* dr = dX + sl * ldx + base;
@@ -362,7 +371,20 @@ extern "C" int onerf_encode_bwd(onerf_ctx* ctx, const onerf_grid* grid, const fl
   memset(&p, 0, sizeof(p));
   p.rays = rays; p.z = z; p.z_stride = n_samples; p.n_rays = n_rays; p.S = n_samples; p.grid = *grid;
   int blocks = (int)((n_chunk * 3 + 255) / 256 < (int64_t)ctx->num_sms * 16 ? (n_chunk * 3 + 255) / 256 : (int64_t)ctx->num_sms * 16);
-  encode_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(p, X, dX, ldx, sample0, n_chunk, table_grad);
+  encode_bwd_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, X, dX, ldx, sample0, n_chunk, table_grad);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
+extern "C" int onerf_encode_bwd_xyz(onerf_ctx* ctx, const onerf_grid* grid, const float* xyz, const float* X, const float* dX,
+                                    int ldx, int64_t sample0, int64_t n_chunk, float* table_grad, void* stream) {
+  ONERF_CHECK_ARG(ctx && grid && xyz && X && dX && table_grad, "null argument");
+  if (n_chunk == 0) return ONERF_OK;
+  FieldParams p;
+  memset(&p, 0, sizeof(p));
+  p.xyz = xyz; p.grid = *grid;
+  int blocks = (int)((n_chunk * 3 + 255) / 256 < (int64_t)ctx->num_sms * 16 ? (n_chunk * 3 + 255) / 256 : (int64_t)ctx->num_sms * 16);
+  encode_bwd_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, X, dX, ldx, sample0, n_chunk, table_grad);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

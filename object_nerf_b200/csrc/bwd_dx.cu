@@ -38,6 +38,7 @@ struct DxParams {
   float* table_grad;      // (n_rows, 24)
   int want_object;
   uint32_t* diag;         // mbarrier timeout record (onerf_ctx)
+  const float* xyz;       // (total,3) explicit positions (XYZ instance); appended so the fields above keep their offsets
 };
 
 __device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
@@ -70,14 +71,21 @@ __device__ __forceinline__ void pe_chain(const float (&acc)[NACC], int r, int j0
   }
 }
 
-// trilinear scatter of NP channel pairs (d[2 p], d[2 p + 1] into table channels ch[p], ch[p] + 1) of sample e
-template <int NP>
+// trilinear scatter of NP channel pairs (d[2 p], d[2 p + 1] into table channels ch[p], ch[p] + 1) of sample e, whose
+// position is o + d z of its ray (the forward's fmaf) or, with XYZ, row e of P.xyz
+template <bool XYZ, int NP>
 __device__ __forceinline__ void scatter(const DxParams& P, const GridView& g, int64_t e, const int* ch, const float* d) {
-  const int ray = (int)(e / P.S), si = (int)(e - (int64_t)ray * P.S);
-  const float* rr = P.rays + (int64_t)ray * 8;
-  const float zz = __ldg(P.z + (int64_t)ray * P.S + si);
-  const float x = fmaf(__ldg(rr + 3), zz, __ldg(rr + 0)), y = fmaf(__ldg(rr + 4), zz, __ldg(rr + 1)),
-              z = fmaf(__ldg(rr + 5), zz, __ldg(rr + 2));
+  float x, y, z;
+  if (XYZ) {
+    const float* q = P.xyz + e * 3;
+    x = __ldg(q); y = __ldg(q + 1); z = __ldg(q + 2);
+  } else {
+    const int ray = (int)(e / P.S), si = (int)(e - (int64_t)ray * P.S);
+    const float* rr = P.rays + (int64_t)ray * 8;
+    const float zz = __ldg(P.z + (int64_t)ray * P.S + si);
+    x = fmaf(__ldg(rr + 3), zz, __ldg(rr + 0)); y = fmaf(__ldg(rr + 4), zz, __ldg(rr + 1));
+    z = fmaf(__ldg(rr + 5), zz, __ldg(rr + 2));
+  }
   const float px = __fdiv_rn(__fadd_rn(x, g.off[0]), g.vsize), py = __fdiv_rn(__fadd_rn(y, g.off[1]), g.vsize),
               pz = __fdiv_rn(__fadd_rn(z, g.off[2]), g.vsize);
   const float fx = floorf(px), fy = floorf(py), fz = floorf(pz);
@@ -98,6 +106,7 @@ __device__ __forceinline__ void scatter(const DxParams& P, const GridView& g, in
   }
 }
 
+template <bool XYZ>
 __global__ void __launch_bounds__(DX_THREADS, 1) bwd_dx_kernel(const __grid_constant__ DxParams P) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -194,7 +203,7 @@ __global__ void __launch_bounds__(DX_THREADS, 1) bwd_dx_kernel(const __grid_cons
       pe_chain(acc, r, 0, 2, xrow, 0, row[r] & 7, d[0], d[1]);
       pe_chain(acc, r, 1, 2, xrow, 0, row[r] & 7, d[2], d[3]);
       const int ch[2] = {2 * q, 8 + 2 * q};
-      if (e < P.total) scatter<2>(P, g, e, ch, d);
+      if (e < P.total) scatter<XYZ, 2>(P, g, e, ch, d);
     }
     if (!P.want_object) continue;
     // pass 1: object channels.  Column 272 + 8 b + c = local column 16 + 8 b + c: channels 2 q, 2 q + 1, block j = 2 + b
@@ -206,16 +215,17 @@ __global__ void __launch_bounds__(DX_THREADS, 1) bwd_dx_kernel(const __grid_cons
       float d[2];
       pe_chain(acc, r, 2, 1, xrow, 4, row[r] & 7, d[0], d[1]);
       const int ch[1] = {16 + 2 * q};
-      if (e < P.total) scatter<1>(P, g, e, ch, d);
+      if (e < P.total) scatter<XYZ, 1>(P, g, e, ch, d);
     }
   }
 }
 
 }  // namespace
 
+// xyz != NULL: sample e sits at xyz[3 e] (rays / z unused)
 int onerf_launch_bwd_dx(onerf_ctx* ctx, int want_object, const void* packed, const void* ws, int64_t n_samples,
-                        const float* rays, const float* z, int n_samples_per_ray, const onerf_grid* grid, float* table_grad,
-                        cudaStream_t stream) {
+                        const float* rays, const float* z, int n_samples_per_ray, const float* xyz, const onerf_grid* grid,
+                        float* table_grad, cudaStream_t stream) {
   DxParams P;
   memset(&P, 0, sizeof(P));
   P.diag = ctx->tc_diag;
@@ -224,15 +234,16 @@ int onerf_launch_bwd_dx(onerf_ctx* ctx, int want_object, const void* packed, con
   P.ximg_off = L.ximg_off;
   P.ws = reinterpret_cast<const uint8_t*>(ws);
   P.TL = onerf_make_train_layout(1, n_samples);
-  P.rays = rays; P.z = z; P.S = n_samples_per_ray; P.total = n_samples;
+  P.rays = rays; P.z = z; P.S = n_samples_per_ray; P.total = n_samples; P.xyz = xyz;
   P.grid = *grid;
   P.table_grad = table_grad;
   P.want_object = want_object;
   const int64_t tiles = (n_samples + TM - 1) / TM;
   const int blocks = (int)(tiles < ctx->num_sms ? tiles : ctx->num_sms);
   const size_t smem = 1024 + DX_STAGES * DX_STAGE_BYTES + 256;
-  ONERF_CUDA(cudaFuncSetAttribute(bwd_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  bwd_dx_kernel<<<blocks, DX_THREADS, smem, stream>>>(P);
+  const auto kernel = xyz ? bwd_dx_kernel<true> : bwd_dx_kernel<false>;
+  ONERF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<blocks, DX_THREADS, smem, stream>>>(P);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

@@ -33,7 +33,10 @@ struct TrainWs {
   int64_t total;
 };
 
-static inline TrainWs onerf_make_train_ws(int precision, int use_voxel, int n_rays, int n_samples, int n_importance) {
+// field_only: the workspace of onerf_field_bwd (one evaluation, n_importance 0), whose caller owns the forward's training
+// dump, fields and their gradients: the tl_*, scene_*, obj_*, dscene and dobj regions are empty.
+static inline TrainWs onerf_make_train_ws(int precision, int use_voxel, int n_rays, int n_samples, int n_importance,
+                                          bool field_only = false) {
   TrainWs W = {};
   int64_t o = 0;
   auto take = [&](int64_t bytes) { int64_t r = o; o += (bytes + 1023) & ~1023ll; return r; };
@@ -43,11 +46,13 @@ static inline TrainWs onerf_make_train_ws(int precision, int use_voxel, int n_ra
   const int rc = onerf_fp32_chunk_rays(n_rays, n_samples), rf = onerf_fp32_chunk_rays(n_rays, sf);
   const int R = tc ? 0 : (rc > rf ? rc : rf);                                      // fp32 chunk: rays, samples
   const int64_t B = tc ? 0 : ((int64_t)rc * n_samples > (int64_t)rf * sf ? (int64_t)rc * n_samples : (int64_t)rf * sf);
-  W.tl_coarse = take(tc ? onerf_make_train_layout(use_voxel, Bc).total_bytes : 0);
-  W.tl_fine = take(tc && n_importance > 0 ? onerf_make_train_layout(use_voxel, Bf).total_bytes : 0);
-  W.scene_c = take(Bc * 16); W.obj_c = take(Bc * 16);
-  W.scene_f = take(Bf * 16); W.obj_f = take(Bf * 16);
-  W.dscene = take(Bf * 16); W.dobj = take(Bf * 16); W.dA_s = take(tc ? Bf * 16 : 0); W.dA_o = take(tc ? Bf * 16 : 0);
+  const int64_t kept = field_only ? 0 : 1;                                         // scales the caller-owned regions
+  W.tl_coarse = take(tc ? kept * onerf_make_train_layout(use_voxel, Bc).total_bytes : 0);
+  W.tl_fine = take(tc && n_importance > 0 ? kept * onerf_make_train_layout(use_voxel, Bf).total_bytes : 0);
+  W.scene_c = take(kept * Bc * 16); W.obj_c = take(kept * Bc * 16);
+  W.scene_f = take(kept * Bf * 16); W.obj_f = take(kept * Bf * 16);
+  W.dscene = take(kept * Bf * 16); W.dobj = take(kept * Bf * 16);
+  W.dA_s = take(tc ? Bf * 16 : 0); W.dA_o = take(tc ? Bf * 16 : 0);
   W.rs = take(tc ? (int64_t)n_rays * ONERF_RAY_CONST_FLOATS * 4 : (int64_t)R * 128 * 4);
   W.pe = take((int64_t)n_rays * 27 * 4);
   W.gk = take(tc ? onerf_make_grad_layout(use_voxel).total_floats * 4 : 0);

@@ -28,10 +28,20 @@ class Embedding(nn.Module):
         self.out_channels = in_channels * (2 * N_freqs + 1)
 
     def forward(self, x):
-        if self.in_channels == 3 and self.N_freqs == 10 and x.is_cuda:
-            return engine.encode(x.reshape(-1, 3), None)[0].reshape(*x.shape[:-1], 63)
-        raise NotImplementedError("stand-alone Embedding.forward is only built for PE10 of CUDA xyz; "
-                                  "direction encoding happens inside the fused field kernel")
+        """(..., 3) CUDA -> (..., 63) for PE10 (positions) or (..., 27) for PE4 (directions).  The output remembers its
+        source (`_onerf_src` = (points (B,3), self)), so that ObjectNeRF.forward / forward_instance on it run the fused
+        kernel on the points / directions."""
+        if self.in_channels == 3 and self.N_freqs in (10, 4) and x.is_cuda:
+            pts = x.reshape(-1, 3)
+            if self.N_freqs == 10:
+                out = engine.encode(pts, None)[0]
+            else:
+                out = engine.dir_encode(pts)
+            out = out.reshape(*x.shape[:-1], self.out_channels)
+            out._onerf_src = (pts, self)
+            return out
+        raise NotImplementedError("stand-alone Embedding.forward is built for in_channels=3 with 10 (positions) or 4 "
+                                  "(directions) octaves, on CUDA tensors")
 
 
 class EmbeddingVoxel(nn.Module):

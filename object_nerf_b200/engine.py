@@ -237,6 +237,17 @@ def encode(xyz, grid: Optional[GridBuffers]):
 
 
 @_on_device
+def dir_encode(dirs):
+    """PE4 of directions (B,3) -> (B,27) (onerf_dir_encode, the encoding the field kernel applies to rays[:, 3:6])."""
+    n = dirs.shape[0]
+    rays = torch.zeros(n, 8, dtype=torch.float32, device=dirs.device)
+    rays[:, 3:6] = dirs
+    out = torch.empty(n, 27, dtype=torch.float32, device=dirs.device)
+    _lib.check(_lib.load().onerf_dir_encode(_lib.ctx(dirs.device), rays.data_ptr(), n, out.data_ptr(), _lib.stream()))
+    return out
+
+
+@_on_device
 def voxel_features(xyz, grid: GridBuffers):
     """Raw trilinear features (B,24) of the sparse voxel grid at xyz (no positional encoding)."""
     xyz = _f32(xyz).reshape(-1, 3)
@@ -249,9 +260,12 @@ def voxel_features(xyz, grid: GridBuffers):
 @_on_device
 def field(rays, z, packed, grid: Optional[GridBuffers], codes=None, code_row=None, want_scene=True,
           want_object=True, precision=None, xyz=None, mute_zero_rays=False, boxes=None, scene_out=None,
-          obj_out=None, z_stride=None, out_stride=None, n_samples=None, activations=None):
+          obj_out=None, z_stride=None, out_stride=None, n_samples=None, activations=None, train_ws=None,
+          _args_out=None):
     """Fused encode + MLP.  Returns (scene_out, obj_out), each (N,S,4) = rgb,sigma (or None).
-    z / outputs may be column blocks of wider arrays (z_stride / out_stride, in samples)."""
+    z / outputs may be column blocks of wider arrays (z_stride / out_stride, in samples).
+    train_ws: a 1024-byte aligned uint8 tensor of onerf_field_train_bytes bytes receiving the tensor-core training dump.
+    _args_out: a list that receives the argument block and the tensors it points into (field_bwd takes both)."""
     rays = _f32(rays)
     n = rays.shape[0]
     s = n_samples if n_samples is not None else z.shape[1]
@@ -266,7 +280,8 @@ def field(rays, z, packed, grid: Optional[GridBuffers], codes=None, code_row=Non
     prec = PRECISIONS[precision or default_precision()]
     a = _lib.FieldArgs()
     a.rays = rays.data_ptr()
-    a.xyz = _lib.ptr(_f32(xyz)) if xyz is not None else None
+    xyz = _f32(xyz) if xyz is not None else None
+    a.xyz = _lib.ptr(xyz)
     a.z = z.data_ptr()
     a.z_stride = z_stride
     codes = _f32(codes) if codes is not None else None
@@ -284,6 +299,10 @@ def field(rays, z, packed, grid: Optional[GridBuffers], codes=None, code_row=Non
     a.out_stride = out_stride
     a.ray_const = ray_const.data_ptr()
     a.activations = activations      # (c_void_p * 17) array or None: FFMA kernel dumps per-layer activations (backward)
+    a.train_ws = train_ws.data_ptr() if train_ws is not None else None
+    if _args_out is not None:
+        # (not the outputs: a caller that keeps them alive for the backward saves them itself)
+        _args_out += [a, (rays, xyz, z, codes, code_row, boxes, ray_const, grid, packed, train_ws)]
     if PROFILE_EVENTS is not None:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -292,6 +311,48 @@ def field(rays, z, packed, grid: Optional[GridBuffers], codes=None, code_row=Non
         e1.record()
         PROFILE_EVENTS.append((e0, e1, n, s))
     return (scene_out if want_scene else None), (obj_out if want_object else None)
+
+
+@_on_device
+def field_bwd(args, d_scene, d_obj, linears, grads=None, d_codes=None, table_grad=None, workspace=None):
+    """onerf_field_bwd for the evaluation `args` (from field(..., _args_out=...)): accumulates the 20 (dW, db) gradient
+    pairs into `grads` (zeros shaped like `linears` if None) and returns them, ABI order; d_codes / table_grad are
+    accumulated in place.  workspace: a 1024-byte aligned uint8 tensor of at least onerf_field_bwd_workspace_bytes
+    (allocated if None)."""
+    lib = _lib.load()
+    dev = linears[0][0].device
+    if workspace is None:
+        workspace = aligned_bytes(field_bwd_workspace_bytes(args.precision, bool(args.grid), args.n_rays, args.n_samples), dev)
+    ws = [_f32(w.detach()) for w, _ in linears]
+    if grads is None:
+        flat = torch.zeros(sum(w.numel() + b.numel() for w, b in linears), dtype=torch.float32, device=dev)
+        grads, o = [], 0
+        for w, b in linears:
+            grads.append((flat[o:o + w.numel()].view_as(w), flat[o + w.numel():o + w.numel() + b.numel()].view_as(b)))
+            o += w.numel() + b.numel()
+    g = _lib.FieldBwdArgs()
+    g.W = (C.c_void_p * 20)(*[t.data_ptr() for t in ws])
+    g.dW = (C.c_void_p * 20)(*[t[0].data_ptr() for t in grads])
+    g.db = (C.c_void_p * 20)(*[t[1].data_ptr() for t in grads])
+    g.d_codes, g.table_grad = _lib.ptr(d_codes), _lib.ptr(table_grad)
+    g.workspace, g.workspace_bytes = workspace.data_ptr(), workspace.numel()
+    d_scene = _f32(d_scene) if d_scene is not None else None
+    d_obj = _f32(d_obj) if d_obj is not None else None
+    _lib.check(lib.onerf_field_bwd(_lib.ctx(dev), C.byref(args), _lib.ptr(d_scene), _lib.ptr(d_obj), C.byref(g),
+                                   _lib.stream()))
+    return grads
+
+
+def field_bwd_workspace_bytes(precision: int, use_voxel: bool, n_rays: int, n_samples: int) -> int:
+    return int(_lib.load().onerf_field_bwd_workspace_bytes(precision, int(use_voxel), n_rays, n_samples))
+
+
+def aligned_bytes(nbytes: int, dev) -> torch.Tensor:
+    """A uint8 tensor of nbytes (at least 1) starting on a 1024-byte boundary (training dumps and workspaces)."""
+    nbytes = max(int(nbytes), 1)
+    t = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
+    off = (-t.data_ptr()) % 1024
+    return t[off:off + nbytes]
 
 
 def _composite_args(z, scene, obj, noise_std, white_back, is_eval, zero_last_delta, rays_in_bbox, frustum_bound_th,

@@ -6,6 +6,7 @@ parameters (engine.packed_for) and runs the fused kernels.
 """
 from __future__ import annotations
 
+import torch
 from torch import nn
 
 
@@ -69,28 +70,78 @@ class ObjectNeRF(nn.Module):
         self.inst_dir_encoding = _act_linear(inst_W + self.in_channels_dir, inst_W // 2, act)
         self.inst_rgb = nn.Sequential(nn.Linear(inst_W // 2, 3), nn.Sigmoid())
 
-    def _density(self, inputs, obj_code):
-        src = getattr(inputs.get("emb_xyz"), "_onerf_src", None) if isinstance(inputs, dict) else None
+    def _source(self, inputs, key):
+        """(points, module) an embedding module of this package attached to inputs[key], or None."""
+        t = inputs.get(key) if isinstance(inputs, dict) else None
+        return getattr(t, "_onerf_src", None), t
+
+    def _query(self, inputs, sigma_only, obj_code):
+        """Reference :97-152 on inputs made by this package's embeddings: the positions (and directions) they were encoded
+        from run through the fused encode + MLP kernel.  Returns the branch's (..., 4) field (rgb, raw sigma)."""
+        from . import field_query, rendering
+        (src, emb) = self._source(inputs, "emb_xyz")
         if src is None:
             raise NotImplementedError(
-                "ObjectNeRF is a weight container: the MLP runs fused with the encoding inside render_rays() / "
-                "render_rays_multi() / query_sigma().  forward(..., sigma_only=True) is supported on inputs produced by "
-                "EmbeddingVoxel.forward(xyz) (they carry their positions); arbitrary pre-embedded features are not.")
-        from . import rendering
-        pts, emb = src
-        return rendering.query_sigma(self, emb, pts, obj_code=obj_code)[:, None]
+                "ObjectNeRF is a weight container: the MLP runs fused with the encoding.  forward / forward_instance take "
+                "inputs produced by this package's EmbeddingVoxel(xyz) / Embedding(3, 10)(xyz) and Embedding(3, 4)(dirs) "
+                "(they carry their positions); arbitrary pre-embedded features are not supported.")
+        pts, emb_mod = src
+        grid_module = emb_mod if rendering._is_voxel(emb_mod) else None
+        if (grid_module is not None) != self.use_voxel_embedding:
+            raise ValueError("emb_xyz was encoded for the other model kind (voxel / plain PE) than this ObjectNeRF's")
+        dirs = None
+        if not sigma_only:
+            dsrc, _ = self._source(inputs, "emb_dir")
+            if inputs.get("emb_dir") is None:
+                raise ValueError("sigma_only=False needs inputs['emb_dir'] (the reference would fail in torch.cat)")
+            if dsrc is None or getattr(dsrc[1], "N_freqs", None) != 4:
+                raise NotImplementedError("emb_dir must be produced by this package's Embedding(3, 4)(dirs)")
+            dirs = dsrc[0]
+            if dirs.shape[0] != pts.shape[0]:
+                raise ValueError(f"emb_dir holds {dirs.shape[0]} directions for {pts.shape[0]} points")
+        fi = obj_code is not None
+        codes = None
+        if fi:
+            codes = obj_code.reshape(1, -1).expand(pts.shape[0], -1) if obj_code.dim() == 1 else obj_code
+            if codes.shape != (pts.shape[0], 64):
+                raise ValueError(f"obj_code must be (64,) or ({pts.shape[0]}, 64); got {tuple(obj_code.shape)}")
+        if torch.is_grad_enabled() and (pts.requires_grad or (dirs is not None and dirs.requires_grad)):
+            raise ValueError("positions and directions get no gradient here: detach them (the field backward stops at "
+                             "the encoding, as render_rays' does)")
+        table = field_query.table_of(grid_module)
+        grad = rendering._needs_grad(self, codes, table)
+        shape = emb.shape[:-1]
+        n = pts.shape[0]
+        if not grad and sigma_only and n > 0 and (not fi or bool((codes == codes[:1]).all())):
+            # the density-only route of mesh extraction and pruning, one code for every point
+            sigma = rendering.query_sigma(self, emb_mod, pts, obj_code=codes[0] if fi else None)
+            return torch.cat([torch.zeros(sigma.shape[0], 3, device=sigma.device), sigma[:, None]], 1).reshape(*shape, 4)
+        rays = torch.zeros(n, 8, dtype=torch.float32, device=pts.device)
+        if dirs is not None:
+            rays[:, 3:6] = dirs.detach()
+        z = torch.zeros(n, 1, dtype=torch.float32, device=pts.device)
+        xyz = pts.detach().float().reshape(n, 1, 3).contiguous()
+        prec = field_query.precision_name(None)
+        if grad:
+            reached = (field_query.OBJECT_SIGMA if sigma_only else field_query.OBJECT) if fi else (
+                field_query.SCENE_SIGMA if sigma_only else field_query.SCENE)
+            scene, obj = field_query.field_eval(self, grid_module, rays, z, xyz, codes, fi, prec, reached)
+        else:
+            from . import engine
+            packed = engine.packed_for(self, grid_module is not None)
+            grid = engine.GridBuffers.from_module(grid_module) if grid_module is not None else None
+            scene, obj = engine.field(rays, z, packed, grid, codes=codes.contiguous() if fi else None, want_scene=not fi,
+                                      want_object=fi, precision=prec, xyz=xyz)
+        return (obj if fi else scene).reshape(*shape, 4)
 
     def forward(self, inputs, sigma_only=False):
-        """Reference :97-121.  Only the density query (`sigma_only=True`: tools/extract_mesh.py:104-107, the voxel pruning
-        of embedding_helper.py:219-225) is served here, through the fused kernel; colours come from render_rays()."""
-        if not sigma_only:
-            raise NotImplementedError("per-sample colours are produced inside render_rays() / render_rays_multi()")
-        return {"sigma": self._density(inputs, None)}
+        """Reference :97-121: {"sigma" (..., 1)[, "rgb" (..., 3)]} of the scene branch at the points emb_xyz was encoded
+        from (and, without sigma_only, the directions of emb_dir).  Differentiable under grad (field_query)."""
+        f = self._query(inputs, sigma_only, None)
+        return {"sigma": f[..., 3:]} if sigma_only else {"sigma": f[..., 3:], "rgb": f[..., :3]}
 
     def forward_instance(self, inputs, sigma_only=False):
-        """Reference :123-152, density only (tools/extract_mesh.py:95-103): inputs["obj_code"] holds one code per point,
-        all rows equal (the reference looks the same id up for every point)."""
-        if not sigma_only:
-            raise NotImplementedError("per-sample colours are produced inside render_rays() / render_rays_multi()")
-        code = inputs["obj_code"]
-        return {"inst_sigma": self._density(inputs, code[0] if code.dim() == 2 else code)}
+        """Reference :123-152: {"inst_sigma"[, "inst_rgb"]} of the object branch, inputs["obj_code"] (B,64) one code per
+        point (any rows) or (64,)."""
+        f = self._query(inputs, sigma_only, inputs["obj_code"])
+        return {"inst_sigma": f[..., 3:]} if sigma_only else {"inst_sigma": f[..., 3:], "inst_rgb": f[..., :3]}

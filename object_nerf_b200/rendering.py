@@ -50,13 +50,19 @@ def inference_model(results: Dict[str, Any], model, embeddings: Dict[str, Any], 
                     precision: Optional[str] = None, _rand: Optional[dict] = None, _rays=None, _seed=None,
                     **dummy_kwargs):
     """Encode + two-branch MLP + compositing for one pass; fills `results` in place with the reference's
-    keys (models/rendering.py:64-230).  `chunk` is accepted and ignored: the kernels tile internally."""
-    if _needs_grad(model, embedding_instance):
-        raise NotImplementedError("inference_model() is the no-grad call surface; gradients flow through "
-                                  "render_rays() (backward.RenderRaysFn)")
+    keys (models/rendering.py:64-230).  `chunk` is accepted and ignored: the kernels tile internally.
+    Under grad (parameters, codes or the voxel table requiring it) the maps carry autograd to the model's Linear
+    tensors, embedding_instance and the voxel table (field_query); weights_* and z_vals_* are non-differentiable and
+    xyz, rays_d and z_vals get no gradient."""
     n, s = z_vals.shape
     emb_xyz = embeddings["xyz"]
     use_voxel = _is_voxel(emb_xyz)
+    table = emb_xyz.embedding_space_ftr.weight if use_voxel else None
+    if _needs_grad(model, embedding_instance if forward_instance else None, table):
+        return _inference_model_grad(results, model, emb_xyz if use_voxel else None, typ, xyz, rays_d, z_vals,
+                                     noise_std, white_back, is_eval, use_zero_as_last_delta, forward_instance,
+                                     embedding_instance, frustum_bound_th, pass_through_mask, rays_in_bbox, precision,
+                                     _rand, _rays, _seed)
     packed = engine.packed_for(model, use_voxel)
     grid = _grid_of(emb_xyz)
     if _rays is None:  # explicit-xyz call surface: only the direction columns of `rays` are used
@@ -86,6 +92,40 @@ def inference_model(results: Dict[str, Any], model, embeddings: Dict[str, Any], 
         results[f"opacity_instance_{typ}"] = out["opacity_instance"]
     return
 
+
+def _inference_model_grad(results, model, grid_module, typ, xyz, rays_d, z_vals, noise_std, white_back, is_eval,
+                          zero_last_delta, forward_instance, codes, frustum_bound_th, pass_through_mask, rays_in_bbox,
+                          precision, _rand, _rays, _seed):
+    from . import field_query
+    n, s = z_vals.shape
+    if any(t is not None and t.requires_grad for t in (xyz, rays_d, z_vals)):
+        raise ValueError("inference_model() gives no gradient to xyz, rays_d or z_vals: detach them")
+    if forward_instance and codes is None:
+        raise ValueError("forward_instance needs embedding_instance")
+    z = z_vals.detach().float().contiguous()
+    if _rays is None:   # explicit positions: only the direction columns of the rays are read
+        rays = torch.zeros(n, 8, dtype=torch.float32, device=z.device)
+        rays[:, 3:6] = rays_d.detach().reshape(n, 3)
+        pos = xyz.detach().float().reshape(n, s, 3).contiguous()
+    else:
+        rays, pos = _rays.detach().float().contiguous(), None
+    reached = field_query.SCENE + (field_query.OBJECT if forward_instance else ())
+    scene, obj = field_query.field_eval(model, grid_module, rays, z, pos, codes if forward_instance else None,
+                                        forward_instance, field_query.precision_name(precision), reached)
+    rand = _rand or {}
+    seed = _seed if _seed is not None else (engine.new_seed() if noise_std > 0 else 0)
+    cfg = dict(noise_std=float(noise_std), white_back=white_back, is_eval=is_eval, zero_last_delta=zero_last_delta,
+               rays_in_bbox=rays_in_bbox, frustum_bound_th=float(frustum_bound_th), pass_through_mask=pass_through_mask,
+               noise_scene=rand.get(f"noise_scene_{typ}"), noise_obj=rand.get(f"noise_obj_{typ}"), seed=seed)
+    out = dict(zip(field_query.CompositeFn.KEYS, field_query.CompositeFn.apply(cfg, z, scene, obj)))
+    results[f"weights_{typ}"] = out["weights"]
+    results[f"opacity_{typ}"] = out["opacity"]
+    results[f"z_vals_{typ}"] = z_vals
+    results[f"rgb_{typ}"] = out["rgb"]
+    results[f"depth_{typ}"] = out["depth"]
+    if forward_instance:
+        for k in ("rgb_instance", "depth_instance", "opacity_instance"):
+            results[f"{k}_{typ}"] = out[k]
 
 
 def query_sigma(model, embedding_xyz, xyz: torch.Tensor, obj_code: Optional[torch.Tensor] = None,
