@@ -344,13 +344,22 @@ def ctx(device: torch.device):
     idx = device.index if device.index is not None else torch.cuda.current_device()
     if idx not in _ctx:
         h = _p()
-        check(load().onerf_ctx_create(idx, C.byref(h)))
+        with torch.cuda.device(idx):        # onerf_ctx_create makes its device current
+            check(load().onerf_ctx_create(idx, C.byref(h)))
         _ctx[idx] = h
     return _ctx[idx]
 
 
 def stream():
     return torch.cuda.current_stream().cuda_stream
+
+
+def call(name: str, device: torch.device, *args) -> None:
+    """Run entry point `name` as onerf_<...>(ctx, *args, stream) with `device` current, so that the kernels and the
+    stream they are enqueued on belong to the tensors' GPU whichever device is current; raises on a failed call."""
+    c = ctx(device)
+    with torch.cuda.device(device):
+        check(getattr(load(), name)(c, *args, stream()))
 
 
 def launch_count(device: torch.device) -> int:

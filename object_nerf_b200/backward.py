@@ -37,11 +37,7 @@ class _WsPool:
 
     def take(self, nbytes, dev):
         lst = self.free.setdefault((nbytes, dev), [])
-        if lst:
-            return lst.pop()
-        t = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
-        off = (-t.data_ptr()) % 1024
-        return t[off:off + nbytes]
+        return lst.pop() if lst else engine.aligned_bytes(nbytes, dev)
 
     def give(self, t):
         lst = self.free.setdefault((t.numel(), t.device), [])
@@ -106,7 +102,6 @@ class RenderRaysFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *gouts):
-        lib = _lib.load()
         a, cfg = ctx.args, ctx.cfg
         _alive = ctx.saved_tensors  # noqa: F841
         dev = ctx.keep[1].device
@@ -119,29 +114,20 @@ class RenderRaysFn(torch.autograd.Function):
                 setattr(mg, name, _lib.ptr(g.get(f"{name}_{typ}")))
         grads = {}
         for typ in cfg["model_order"]:
-            lin = ctx.lins[typ]
-            ws = [engine._f32(w.detach()) for w, _ in lin]
-            sizes = [t.numel() for pair in lin for t in pair]
-            flat = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)   # one fill for the 40 gradient tensors
-            views, o = [], 0
-            for (w, bb) in lin:
-                views.append((flat[o:o + w.numel()].view_as(w), flat[o + w.numel():o + w.numel() + bb.numel()].view_as(bb)))
-                o += w.numel() + bb.numel()
-            grads[typ] = views
-            Wp = (C.c_void_p * 20)(*[t.data_ptr() for t in ws])
-            dWp = (C.c_void_p * 20)(*[v[0].data_ptr() for v in views])
-            dbp = (C.c_void_p * 20)(*[v[1].data_ptr() for v in views])
-            keep += [ws, Wp, dWp, dbp]
-            setattr(b, "W_" + typ, Wp)
-            setattr(b, "dW_" + typ, dWp)
-            setattr(b, "db_" + typ, dbp)
+            lin = [(engine._f32(w.detach()), bb) for w, bb in ctx.lins[typ]]
+            views = engine.grad_buffer([t for pair in lin for t in pair], dev)[1]    # one fill for the 40 tensors
+            grads[typ] = list(zip(views[0::2], views[1::2]))
+            keep.append(lin)
+            setattr(b, "W_" + typ, engine.pointer_tables(lin)[0])
+            dW, db = engine.pointer_tables(grads[typ])
+            setattr(b, "dW_" + typ, dW)
+            setattr(b, "db_" + typ, db)
         d_codes = torch.zeros(a.n_rays, 64, dtype=torch.float32, device=dev) if ctx.has_codes else None
         table_grad = None
         if cfg["has_table"]:
             table_grad = torch.zeros_like(cfg["embeddings"]["xyz"].embedding_space_ftr.weight, dtype=torch.float32)
         b.d_codes, b.table_grad = _lib.ptr(d_codes), _lib.ptr(table_grad)
-        with torch.cuda.device(dev):
-            _lib.check(lib.onerf_render_rays_bwd(_lib.ctx(dev), C.byref(a), C.byref(b), _lib.stream()))
+        _lib.call("onerf_render_rays_bwd", dev, C.byref(a), C.byref(b))
         flat_out: List[Optional[torch.Tensor]] = []
         if cfg["has_table"]:
             flat_out.append(table_grad)

@@ -161,9 +161,7 @@ class RaySampler:
 
     def next(self) -> Dict[str, torch.Tensor]:
         """Draw the batch of the device step counter and advance the counter by one (kernels only: capturable)."""
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().onerf_draw_batch_dstep(_lib.ctx(self.device), C.byref(self._args),
-                                                          self._step.data_ptr(), _lib.stream()))
+        _lib.call("onerf_draw_batch_dstep", self.device, C.byref(self._args), self._step.data_ptr())
         return dict(self._batch)
 
     @property

@@ -16,9 +16,7 @@ class _CodeLookup(torch.autograd.Function):
         ids = ids.reshape(-1).to(torch.int64).contiguous()
         t = table.detach().contiguous().float()
         out = torch.empty(ids.numel(), t.shape[1], dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().onerf_code_gather(_lib.ctx(dev), t.data_ptr(), ids.data_ptr(), ids.numel(), t.shape[0],
-                                                     out.data_ptr(), _lib.stream()))
+        _lib.call("onerf_code_gather", dev, t.data_ptr(), ids.data_ptr(), ids.numel(), t.shape[0], out.data_ptr())
         ctx.save_for_backward(ids)
         ctx.shape = tuple(t.shape)
         return out
@@ -28,9 +26,8 @@ class _CodeLookup(torch.autograd.Function):
         (ids,) = ctx.saved_tensors
         g = g.contiguous().float()
         grad = torch.zeros(ctx.shape, dtype=torch.float32, device=g.device)
-        with torch.cuda.device(g.device):
-            _lib.check(_lib.load().onerf_code_scatter_add(_lib.ctx(g.device), g.data_ptr(), ids.data_ptr(), ids.numel(),
-                                                          ctx.shape[0], grad.data_ptr(), _lib.stream()))
+        _lib.call("onerf_code_scatter_add", g.device, g.data_ptr(), ids.data_ptr(), ids.numel(), ctx.shape[0],
+                  grad.data_ptr())
         return grad, None
 
 

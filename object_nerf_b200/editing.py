@@ -95,7 +95,6 @@ def render_tile(models: Dict[str, Any], embeddings: Dict[str, Any], code_library
     dev = code_table.device
     begin, end = int(pixel_begin), int(pixel_end)
     n, n_obj = max(end - begin, 0), len(sets)
-    lib = _lib.load()
     a = _lib.RenderEditArgs()
     sets_c = (_lib.EditSet * max(n_obj, 1))()
     keep = []                                  # host structs the call reads
@@ -132,10 +131,9 @@ def render_tile(models: Dict[str, Any], embeddings: Dict[str, Any], code_library
                 w = widths.get(k, n_obj * s)
                 out[key] = torch.empty((n, w) if w != 1 else (n,), dtype=torch.float32, device=dev)
                 setattr(getattr(a, typ), k, out[key].data_ptr())
-    ws = _workspace(lib.onerf_render_edit_workspace_bytes(a.chunk_rays, n_obj, a.n_samples, a.n_importance), dev)
+    ws = _workspace(_lib.load().onerf_render_edit_workspace_bytes(a.chunk_rays, n_obj, a.n_samples, a.n_importance), dev)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-    with torch.cuda.device(dev):
-        _lib.check(lib.onerf_render_edit_frame(_lib.ctx(dev), C.byref(a), _lib.stream()))
+    _lib.call("onerf_render_edit_frame", dev, C.byref(a))
     return {k: out[k] for k in all_keys if k in out}
 
 

@@ -184,23 +184,19 @@ class EmbeddingVoxel(nn.Module):
         grid = self.grid_buffers()
         packed = engine.packed_for(model, True)
         prec = engine.PRECISIONS[precision or engine.default_precision()]
-        lib = _lib.load()
-        with torch.cuda.device(dev):
-            ctx = _lib.ctx(dev)
-            ws = torch.empty(lib.onerf_prune_workspace_bytes(prec), dtype=torch.uint8, device=dev)
-            a = _lib.PruneArgs()
-            a.grid, a.packed, a.precision = C.pointer(grid.c), packed.data_ptr(), prec
-            a.cells, a.n_cells, a.cell_begin, a.cell_end = _lib.ptr(cells), n_cells, begin, end
-            a.jitter, a.seed = _lib.ptr(jitter), seed
-            a.max_alpha_out = _lib.ptr(max_alpha)
-            a.workspace, a.workspace_bytes = (ws.data_ptr() if ws.numel() else None), ws.numel()
-            _lib.check(lib.onerf_prune_measure(ctx, C.byref(a), _lib.stream()))
-            if group is not None:
-                max_alpha = parallel.gather_tiles(max_alpha, n_cells, group)
-            n_pruned = torch.zeros(1, dtype=torch.int64, device=dev)
-            _lib.check(lib.onerf_prune_apply(ctx, _lib.ptr(cells), n_cells, _lib.ptr(max_alpha), float(max_alpha_th),
-                                             occ.shape[1], occ.shape[2], _lib.ptr(occ), _lib.ptr(self.voxel_idx_map),
-                                             n_pruned.data_ptr(), _lib.stream()))
+        ws = torch.empty(_lib.load().onerf_prune_workspace_bytes(prec), dtype=torch.uint8, device=dev)
+        a = _lib.PruneArgs()
+        a.grid, a.packed, a.precision = C.pointer(grid.c), packed.data_ptr(), prec
+        a.cells, a.n_cells, a.cell_begin, a.cell_end = _lib.ptr(cells), n_cells, begin, end
+        a.jitter, a.seed = _lib.ptr(jitter), seed
+        a.max_alpha_out = _lib.ptr(max_alpha)
+        a.workspace, a.workspace_bytes = (ws.data_ptr() if ws.numel() else None), ws.numel()
+        _lib.call("onerf_prune_measure", dev, C.byref(a))
+        if group is not None:
+            max_alpha = parallel.gather_tiles(max_alpha, n_cells, group)
+        n_pruned = torch.zeros(1, dtype=torch.int64, device=dev)
+        _lib.call("onerf_prune_apply", dev, _lib.ptr(cells), n_cells, _lib.ptr(max_alpha), float(max_alpha_th), occ.shape[1],
+                  occ.shape[2], _lib.ptr(occ), _lib.ptr(self.voxel_idx_map), n_pruned.data_ptr())
         # the library wrote the buffers in place: count it as an in-place change (training._grid_stamp)
         torch.autograd.graph.increment_version(occ)
         torch.autograd.graph.increment_version(self.voxel_idx_map)

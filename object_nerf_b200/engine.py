@@ -26,24 +26,15 @@ def default_precision() -> str:
     return os.environ.get("ONERF_PRECISION", "bf16")
 
 
+def train_precision(precision: Optional[str]) -> str:
+    """The arithmetic of a differentiable call: bf16 (None = the default) is the tensor-core forward and backward;
+    anything else selects the fp32 verification arithmetic end to end."""
+    return "bf16" if (precision or default_precision()) == "bf16" else "fp32"
+
+
 def new_seed() -> int:
     """A fresh 63-bit seed from torch's CPU generator (so torch.manual_seed controls the render RNG)."""
     return int(torch.randint(0, 2 ** 62, (1,), dtype=torch.int64).item())
-
-
-def _on_device(fn):
-    """Run an ABI wrapper with the device of its first tensor argument current, so that kernels and the stream they are
-    enqueued on (torch.cuda.current_stream()) belong to the tensors' GPU even when another device is current."""
-    import functools
-
-    @functools.wraps(fn)
-    def wrapped(*args, **kwargs):
-        dev = next((a.device for a in args if isinstance(a, torch.Tensor)), None)
-        if dev is None or dev.type != "cuda" or dev.index is None or dev.index == torch.cuda.current_device():
-            return fn(*args, **kwargs)
-        with torch.cuda.device(dev):
-            return fn(*args, **kwargs)
-    return wrapped
 
 
 def _f32(t: torch.Tensor) -> torch.Tensor:
@@ -90,25 +81,41 @@ def check_architecture(model, use_voxel: bool):
     return lin
 
 
-def pack_weights(linears: Sequence, use_voxel: bool) -> torch.Tensor:
-    """Run the pack kernel; returns the packed blob (uint8 tensor, 1024-byte aligned)."""
-    lib = _lib.load()
+def pointer_tables(pairs: Sequence):
+    """The two ABI pointer tables (c_void_p * 20) of 20 tensor pairs: (W, b) -> (W table, b table), and likewise
+    (dW, db)."""
+    return tuple((C.c_void_p * _lib.N_LINEAR)(*[t.data_ptr() for t in col]) for col in zip(*pairs))
+
+
+def grad_buffer(tensors: Sequence, dev):
+    """One zero-filled fp32 buffer with a gradient view shaped like each of `tensors`, each offset rounded up to 4 floats
+    (16 bytes).  Returns (buffer, views, offsets in floats)."""
+    offsets, off = [], 0
+    for t in tensors:
+        offsets.append(off)
+        off += -(-t.numel() // 4) * 4
+    flat = torch.zeros(off, dtype=torch.float32, device=dev)
+    return flat, [flat[o:o + t.numel()].view(t.shape) for t, o in zip(tensors, offsets)], offsets
+
+
+def aligned_bytes(nbytes: int, dev) -> torch.Tensor:
+    """A uint8 tensor of nbytes (at least 1) starting on a 1024-byte boundary (packed weights, training dumps and
+    workspaces)."""
+    nbytes = max(int(nbytes), 1)
+    t = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
+    off = (-t.data_ptr()) % 1024
+    return t[off:off + nbytes]
+
+
+def pack_weights(linears: Sequence, use_voxel: bool, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Run the pack kernel into `out` (a new blob if None); returns the packed blob (uint8 tensor, 1024-byte aligned)."""
     dev = linears[0][0].device
-    if dev.type == "cuda" and dev.index is not None and dev.index != torch.cuda.current_device():
-        with torch.cuda.device(dev):
-            return pack_weights(linears, use_voxel)
-    ws = [_f32(w.detach()) for w, _ in linears]
-    bs = [_f32(b.detach()) for _, b in linears]
-    nbytes = lib.onerf_packed_weights_bytes(1 if use_voxel else 0)
-    blob = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
-    off = (-blob.data_ptr()) % 1024
-    blob = blob[off:off + nbytes]
-    Wp = (C.c_void_p * 20)(*[w.data_ptr() for w in ws])
-    Bp = (C.c_void_p * 20)(*[b.data_ptr() for b in bs])
-    _lib.check(lib.onerf_pack_weights(_lib.ctx(dev), 1 if use_voxel else 0, Wp, Bp, blob.data_ptr(), nbytes,
-                                      _lib.stream()))
-    blob._keepalive = (ws, bs)  # sources must outlive the async pack kernels
-    return blob
+    lin = [(_f32(w.detach()), _f32(b.detach())) for w, b in linears]
+    if out is None:
+        out = aligned_bytes(_lib.load().onerf_packed_weights_bytes(int(use_voxel)), dev)
+    _lib.call("onerf_pack_weights", dev, int(use_voxel), *pointer_tables(lin), out.data_ptr(), out.numel())
+    out._keepalive = lin  # sources must outlive the async pack kernels
+    return out
 
 
 _pack_cache = {}   # id(model) -> (weakref to the model, content fingerprint, blob)
@@ -177,20 +184,17 @@ class GridBuffers:
 # ------------------------------------------------------------------------------------------------
 # stage kernels
 # ------------------------------------------------------------------------------------------------
-@_on_device
 def sample_coarse(rays, n_samples, use_disp=False, perturb=0.0, jitter=None, seed=0, out=None):
     rays = _f32(rays)
     n = rays.shape[0]
     z = out if out is not None else torch.empty(n, n_samples, dtype=torch.float32, device=rays.device)
     assert z.is_contiguous() and z.shape == (n, n_samples)
     jitter = _f32(jitter) if jitter is not None else None
-    _lib.check(_lib.load().onerf_sample_coarse(_lib.ctx(rays.device), rays.data_ptr(), n, n_samples,
-                                               int(bool(use_disp)), float(perturb), _lib.ptr(jitter), seed,
-                                               z.data_ptr(), _lib.stream()))
+    _lib.call("onerf_sample_coarse", rays.device, rays.data_ptr(), n, n_samples, int(bool(use_disp)), float(perturb),
+              _lib.ptr(jitter), seed, z.data_ptr())
     return z
 
 
-@_on_device
 def sample_pdf_merge(z_coarse, weights, n_importance, det, u=None, seed=0, out=None, clip=None):
     """clip (N,2) = (near_box, far_box) of a 10-column ray set: merged depths strictly inside the interval become far_box
     (onerf_sample_pdf_merge_clip)."""
@@ -200,64 +204,55 @@ def sample_pdf_merge(z_coarse, weights, n_importance, det, u=None, seed=0, out=N
         out = torch.empty(n, s + n_importance, dtype=torch.float32, device=z_coarse.device)
     assert out.is_contiguous() and out.shape == (n, s + n_importance)
     u = _f32(u) if u is not None else None
-    lib = _lib.load()
-    args = (_lib.ctx(z_coarse.device), z_coarse.data_ptr(), weights.data_ptr(), n, s, n_importance, int(bool(det)),
-            _lib.ptr(u), seed)
+    args = (z_coarse.data_ptr(), weights.data_ptr(), n, s, n_importance, int(bool(det)), _lib.ptr(u), seed)
     if clip is None:
-        _lib.check(lib.onerf_sample_pdf_merge(*args, out.data_ptr(), _lib.stream()))
+        _lib.call("onerf_sample_pdf_merge", z_coarse.device, *args, out.data_ptr())
     else:
         clip = _f32(clip)
         assert clip.shape == (n, 2)
-        _lib.check(lib.onerf_sample_pdf_merge_clip(*args, clip.data_ptr(), out.data_ptr(), _lib.stream()))
+        _lib.call("onerf_sample_pdf_merge_clip", z_coarse.device, *args, clip.data_ptr(), out.data_ptr())
     return out
 
 
-@_on_device
 def sample_pdf(bins, weights, n_importance, det, u=None, seed=0):
     bins, weights = _f32(bins), _f32(weights.detach())
     n, nb = bins.shape
     assert weights.shape == (n, nb - 1)
     out = torch.empty(n, n_importance, dtype=torch.float32, device=bins.device)
     u = _f32(u) if u is not None else None
-    _lib.check(_lib.load().onerf_sample_pdf(_lib.ctx(bins.device), bins.data_ptr(), weights.data_ptr(), n, nb,
-                                            n_importance, int(bool(det)), _lib.ptr(u), seed, out.data_ptr(),
-                                            _lib.stream()))
+    _lib.call("onerf_sample_pdf", bins.device, bins.data_ptr(), weights.data_ptr(), n, nb, n_importance, int(bool(det)),
+              _lib.ptr(u), seed, out.data_ptr())
     return out
 
 
-@_on_device
 def encode(xyz, grid: Optional[GridBuffers]):
     xyz = _f32(xyz)
     n = xyz.shape[0]
     scene = torch.empty(n, 271 if grid is not None else 63, dtype=torch.float32, device=xyz.device)
     obj = torch.empty(n, 104, dtype=torch.float32, device=xyz.device) if grid is not None else None
-    _lib.check(_lib.load().onerf_encode(_lib.ctx(xyz.device), C.byref(grid.c) if grid is not None else None,
-                                        xyz.data_ptr(), n, scene.data_ptr(), _lib.ptr(obj), _lib.stream()))
+    _lib.call("onerf_encode", xyz.device, C.byref(grid.c) if grid is not None else None, xyz.data_ptr(), n,
+              scene.data_ptr(), _lib.ptr(obj))
     return scene, obj
 
 
-@_on_device
 def dir_encode(dirs):
     """PE4 of directions (B,3) -> (B,27) (onerf_dir_encode, the encoding the field kernel applies to rays[:, 3:6])."""
     n = dirs.shape[0]
     rays = torch.zeros(n, 8, dtype=torch.float32, device=dirs.device)
     rays[:, 3:6] = dirs
     out = torch.empty(n, 27, dtype=torch.float32, device=dirs.device)
-    _lib.check(_lib.load().onerf_dir_encode(_lib.ctx(dirs.device), rays.data_ptr(), n, out.data_ptr(), _lib.stream()))
+    _lib.call("onerf_dir_encode", dirs.device, rays.data_ptr(), n, out.data_ptr())
     return out
 
 
-@_on_device
 def voxel_features(xyz, grid: GridBuffers):
     """Raw trilinear features (B,24) of the sparse voxel grid at xyz (no positional encoding)."""
     xyz = _f32(xyz).reshape(-1, 3)
     out = torch.empty(xyz.shape[0], 24, dtype=torch.float32, device=xyz.device)
-    _lib.check(_lib.load().onerf_voxel_features(_lib.ctx(xyz.device), C.byref(grid.c), xyz.data_ptr(), xyz.shape[0],
-                                                out.data_ptr(), _lib.stream()))
+    _lib.call("onerf_voxel_features", xyz.device, C.byref(grid.c), xyz.data_ptr(), xyz.shape[0], out.data_ptr())
     return out
 
 
-@_on_device
 def field(rays, z, packed, grid: Optional[GridBuffers], codes=None, code_row=None, want_scene=True,
           want_object=True, precision=None, xyz=None, mute_zero_rays=False, boxes=None, scene_out=None,
           obj_out=None, z_stride=None, out_stride=None, n_samples=None, activations=None, train_ws=None,
@@ -304,55 +299,41 @@ def field(rays, z, packed, grid: Optional[GridBuffers], codes=None, code_row=Non
         # (not the outputs: a caller that keeps them alive for the backward saves them itself)
         _args_out += [a, (rays, xyz, z, codes, code_row, boxes, ray_const, grid, packed, train_ws)]
     if PROFILE_EVENTS is not None:
+        launch_stream = torch.cuda.current_stream(dev)      # the stream _lib.call enqueues the field kernel on
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-    _lib.check(_lib.load().onerf_field_fwd(_lib.ctx(dev), C.byref(a), _lib.stream()))
+        e0.record(launch_stream)
+    _lib.call("onerf_field_fwd", dev, C.byref(a))
     if PROFILE_EVENTS is not None:
-        e1.record()
+        e1.record(launch_stream)
         PROFILE_EVENTS.append((e0, e1, n, s))
     return (scene_out if want_scene else None), (obj_out if want_object else None)
 
 
-@_on_device
 def field_bwd(args, d_scene, d_obj, linears, grads=None, d_codes=None, table_grad=None, workspace=None):
     """onerf_field_bwd for the evaluation `args` (from field(..., _args_out=...)): accumulates the 20 (dW, db) gradient
     pairs into `grads` (zeros shaped like `linears` if None) and returns them, ABI order; d_codes / table_grad are
     accumulated in place.  workspace: a 1024-byte aligned uint8 tensor of at least onerf_field_bwd_workspace_bytes
     (allocated if None)."""
-    lib = _lib.load()
     dev = linears[0][0].device
     if workspace is None:
         workspace = aligned_bytes(field_bwd_workspace_bytes(args.precision, bool(args.grid), args.n_rays, args.n_samples), dev)
-    ws = [_f32(w.detach()) for w, _ in linears]
+    lin = [(_f32(w.detach()), b) for w, b in linears]
     if grads is None:
-        flat = torch.zeros(sum(w.numel() + b.numel() for w, b in linears), dtype=torch.float32, device=dev)
-        grads, o = [], 0
-        for w, b in linears:
-            grads.append((flat[o:o + w.numel()].view_as(w), flat[o + w.numel():o + w.numel() + b.numel()].view_as(b)))
-            o += w.numel() + b.numel()
+        views = grad_buffer([t for pair in linears for t in pair], dev)[1]
+        grads = list(zip(views[0::2], views[1::2]))
     g = _lib.FieldBwdArgs()
-    g.W = (C.c_void_p * 20)(*[t.data_ptr() for t in ws])
-    g.dW = (C.c_void_p * 20)(*[t[0].data_ptr() for t in grads])
-    g.db = (C.c_void_p * 20)(*[t[1].data_ptr() for t in grads])
+    g.W = pointer_tables(lin)[0]
+    g.dW, g.db = pointer_tables(grads)
     g.d_codes, g.table_grad = _lib.ptr(d_codes), _lib.ptr(table_grad)
     g.workspace, g.workspace_bytes = workspace.data_ptr(), workspace.numel()
     d_scene = _f32(d_scene) if d_scene is not None else None
     d_obj = _f32(d_obj) if d_obj is not None else None
-    _lib.check(lib.onerf_field_bwd(_lib.ctx(dev), C.byref(args), _lib.ptr(d_scene), _lib.ptr(d_obj), C.byref(g),
-                                   _lib.stream()))
+    _lib.call("onerf_field_bwd", dev, C.byref(args), _lib.ptr(d_scene), _lib.ptr(d_obj), C.byref(g))
     return grads
 
 
 def field_bwd_workspace_bytes(precision: int, use_voxel: bool, n_rays: int, n_samples: int) -> int:
     return int(_lib.load().onerf_field_bwd_workspace_bytes(precision, int(use_voxel), n_rays, n_samples))
-
-
-def aligned_bytes(nbytes: int, dev) -> torch.Tensor:
-    """A uint8 tensor of nbytes (at least 1) starting on a 1024-byte boundary (training dumps and workspaces)."""
-    nbytes = max(int(nbytes), 1)
-    t = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
-    off = (-t.data_ptr()) % 1024
-    return t[off:off + nbytes]
 
 
 def _composite_args(z, scene, obj, noise_std, white_back, is_eval, zero_last_delta, rays_in_bbox, frustum_bound_th,
@@ -376,7 +357,6 @@ def _composite_args(z, scene, obj, noise_std, white_back, is_eval, zero_last_del
     return a, (noise_scene, noise_obj, ptm)
 
 
-@_on_device
 def composite(z, scene, obj, noise_std=0.0, white_back=False, is_eval=False, zero_last_delta=False,
               rays_in_bbox=False, frustum_bound_th=0.0, pass_through_mask=None, noise_scene=None,
               noise_obj=None, seed=0):
@@ -394,11 +374,10 @@ def composite(z, scene, obj, noise_std=0.0, white_back=False, is_eval=False, zer
         a.rgb_instance = out["rgb_instance"].data_ptr()
         a.depth_instance = out["depth_instance"].data_ptr()
         a.opacity_instance = out["opacity_instance"].data_ptr()
-    _lib.check(_lib.load().onerf_composite(_lib.ctx(dev), C.byref(a), _lib.stream()))
+    _lib.call("onerf_composite", dev, C.byref(a))
     return out
 
 
-@_on_device
 def composite_bwd(z, scene, obj, depth_scene, grads, noise_std=0.0, white_back=False, is_eval=False,
                   zero_last_delta=False, frustum_bound_th=0.0, pass_through_mask=None, noise_scene=None,
                   noise_obj=None, seed=0):
@@ -412,14 +391,12 @@ def composite_bwd(z, scene, obj, depth_scene, grads, noise_std=0.0, white_back=F
     a, _keep = _composite_args(z, scene, obj, noise_std, white_back, is_eval, zero_last_delta, False,
                                frustum_bound_th, pass_through_mask, noise_scene, noise_obj, seed)
     g = {k: (v.contiguous().float() if v is not None else None) for k, v in grads.items()}
-    _lib.check(_lib.load().onerf_composite_bwd(
-        _lib.ctx(dev), C.byref(a), _lib.ptr(depth_scene), _lib.ptr(g.get("rgb")), _lib.ptr(g.get("depth")),
-        _lib.ptr(g.get("opacity")), _lib.ptr(g.get("rgb_instance")), _lib.ptr(g.get("depth_instance")),
-        _lib.ptr(g.get("opacity_instance")), dscene.data_ptr(), _lib.ptr(dobj), _lib.stream()))
+    _lib.call("onerf_composite_bwd", dev, C.byref(a), _lib.ptr(depth_scene), _lib.ptr(g.get("rgb")),
+              _lib.ptr(g.get("depth")), _lib.ptr(g.get("opacity")), _lib.ptr(g.get("rgb_instance")),
+              _lib.ptr(g.get("depth_instance")), _lib.ptr(g.get("opacity_instance")), dscene.data_ptr(), _lib.ptr(dobj))
     return dscene, dobj
 
 
-@_on_device
 def composite_multi(z_all, field_all, white_back=False, want_ids=False, want_unsorted=False, merge=False, noise_std=0.0,
                     noise=None, seed=0, fine=False):
     """z_all (n_obj, N, S), field_all (n_obj, N, S, 4) -> sorted-order outputs (N, n_obj*S).  Any n_obj * S: the bitonic
@@ -429,26 +406,24 @@ def composite_multi(z_all, field_all, white_back=False, want_ids=False, want_uns
     n_obj, n, s = z_all.shape
     t = n_obj * s
     dev = z_all.device
-    lib = _lib.load()
     f = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
     out = {"z_vals": f(n, t), "weights": f(n, t), "opacity": f(n), "rgb": f(n, 3), "depth": f(n)}
     ids = f(n, t) if want_ids else None
     unsorted = f(n_obj, n, s) if want_unsorted else None
     ws = None
     if merge or t > 4096:
-        ws = torch.empty(max(lib.onerf_composite_multi_workspace_bytes(n, n_obj, s), 256), dtype=torch.uint8, device=dev)
-    head = (_lib.ctx(dev), z_all.data_ptr(), field_all.data_ptr(), n, n_obj, s, int(bool(white_back)))
+        ws = torch.empty(max(_lib.load().onerf_composite_multi_workspace_bytes(n, n_obj, s), 256), dtype=torch.uint8, device=dev)
+    head = (z_all.data_ptr(), field_all.data_ptr(), n, n_obj, s, int(bool(white_back)))
     if noise_std != 0 or noise is not None:
         noise = _f32(noise) if noise is not None else None
         assert noise is None or noise.shape == (n, t)
-        entry = lib.onerf_composite_multi_noise_merge if merge else lib.onerf_composite_multi_noise_ws
+        entry = "onerf_composite_multi_noise_merge" if merge else "onerf_composite_multi_noise_ws"
         head += (float(noise_std), _lib.ptr(noise), seed, int(bool(fine)))
     else:
-        entry = lib.onerf_composite_multi_merge if merge else lib.onerf_composite_multi_ws
-    _lib.check(entry(
-        *head, out["z_vals"].data_ptr(), out["weights"].data_ptr(), _lib.ptr(ids), _lib.ptr(unsorted),
-        out["opacity"].data_ptr(), out["rgb"].data_ptr(), out["depth"].data_ptr(), _lib.ptr(ws),
-        ws.numel() if ws is not None else 0, _lib.stream()))
+        entry = "onerf_composite_multi_merge" if merge else "onerf_composite_multi_ws"
+    _lib.call(entry, dev, *head, out["z_vals"].data_ptr(), out["weights"].data_ptr(), _lib.ptr(ids), _lib.ptr(unsorted),
+              out["opacity"].data_ptr(), out["rgb"].data_ptr(), out["depth"].data_ptr(), _lib.ptr(ws),
+              ws.numel() if ws is not None else 0)
     if want_ids:
         out["obj_ids"] = ids
     if want_unsorted:
@@ -521,12 +496,10 @@ class RenderPlan:
         seed_dev: a one-element int64 tensor on the plan's device holding the Philox seed; the draws then use the value it
         holds when the kernels run instead of args.seed, and the call adds 4 to it (onerf_render_rays_fwd_dseed), so
         every replay of a captured run draws fresh numbers."""
-        with torch.cuda.device(self.rays.device):
-            ctx, lib = _lib.ctx(self.rays.device), _lib.load()
-            if seed_dev is None:
-                _lib.check(lib.onerf_render_rays_fwd(ctx, C.byref(self.args), _lib.stream()))
-            else:
-                if seed_dev.dtype != torch.int64 or seed_dev.numel() != 1 or seed_dev.device != self.rays.device:
-                    raise ValueError("seed_dev must be a one-element int64 tensor on the plan's device")
-                _lib.check(lib.onerf_render_rays_fwd_dseed(ctx, C.byref(self.args), seed_dev.data_ptr(), _lib.stream()))
+        if seed_dev is None:
+            _lib.call("onerf_render_rays_fwd", self.rays.device, C.byref(self.args))
+        else:
+            if seed_dev.dtype != torch.int64 or seed_dev.numel() != 1 or seed_dev.device != self.rays.device:
+                raise ValueError("seed_dev must be a one-element int64 tensor on the plan's device")
+            _lib.call("onerf_render_rays_fwd_dseed", self.rays.device, C.byref(self.args), seed_dev.data_ptr())
         return {f"{k}_{typ}": v for typ, m in self.maps.items() for k, v in m.items()}

@@ -10,8 +10,6 @@ trunk and the sigma head), the voxel table and the object codes.  Positions, dir
 """
 from __future__ import annotations
 
-from typing import Optional
-
 import torch
 
 from . import _lib, engine
@@ -128,8 +126,3 @@ class CompositeFn(torch.autograd.Function):
         grads = {k: g for k, g in zip(CompositeFn.KEYS, gouts) if g is not None}
         dscene, dobj = engine.composite_bwd(z, scene, obj, depth, grads, **cfg)
         return None, None, dscene, dobj
-
-
-def precision_name(precision: Optional[str]) -> str:
-    """bf16: the tensor-core training dump; anything else: the fp32 verification arithmetic (as render_rays trains)."""
-    return "bf16" if (precision or engine.default_precision()) == "bf16" else "fp32"

@@ -19,6 +19,13 @@ TERMS = ("color_loss", "depth_loss", "opacity_loss", "instance_color_loss", "ins
 MAPS = ("rgb", "depth", "opacity_instance", "rgb_instance", "depth_instance")
 
 
+def fill_loss_args(a, weights, out: torch.Tensor, present: torch.Tensor) -> None:
+    """Set onerf_loss_args' five term weights (TERMS order) and its outputs: out (6,) = loss_sum then the five terms,
+    present (5,) int32."""
+    (a.color_weight, a.depth_weight, a.opacity_weight, a.instance_color_weight, a.instance_depth_weight) = weights
+    a.loss_sum_out, a.terms_out, a.present_out = out.data_ptr(), out[1:].data_ptr(), present.data_ptr()
+
+
 class _TotalLossFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, weights, batch, has_fine, *maps):
@@ -28,8 +35,7 @@ class _TotalLossFn(torch.autograd.Function):
         grads = [torch.empty_like(m) for m in maps]
         out = torch.empty(1 + 5, dtype=torch.float32, device=dev)          # loss_sum, 5 terms
         present = torch.empty(5, dtype=torch.int32, device=dev)
-        lib = _lib.load()
-        ws = torch.empty(lib.onerf_total_loss_workspace_bytes() // 8, dtype=torch.float64, device=dev)
+        ws = torch.empty(_lib.load().onerf_total_loss_workspace_bytes() // 8, dtype=torch.float64, device=dev)
         keep = [batch["rgbs"].reshape(n, 3).contiguous().float(), batch["depths"].reshape(n).contiguous().float(),
                 batch["valid_mask"].reshape(n).to(torch.uint8).contiguous(),
                 batch["instance_mask"].reshape(n).to(torch.uint8).contiguous(),
@@ -41,11 +47,9 @@ class _TotalLossFn(torch.autograd.Function):
                 setattr(getattr(a, typ), k, maps[5 * i + j].data_ptr())
                 setattr(getattr(a, "grad_" + typ), k, grads[5 * i + j].data_ptr())
         a.rgbs, a.depths, a.valid_mask, a.instance_mask, a.instance_mask_weight = (t.data_ptr() for t in keep)
-        (a.color_weight, a.depth_weight, a.opacity_weight, a.instance_color_weight, a.instance_depth_weight) = weights
-        a.loss_sum_out, a.terms_out, a.present_out = out.data_ptr(), out[1:].data_ptr(), present.data_ptr()
+        fill_loss_args(a, weights, out, present)
         a.workspace = ws.data_ptr()
-        with torch.cuda.device(dev):
-            _lib.check(lib.onerf_total_loss(_lib.ctx(dev), C.byref(a), _lib.stream()))
+        _lib.call("onerf_total_loss", dev, C.byref(a))
         ctx.grads = grads
         ctx.mark_non_differentiable(present)
         return out[0], out[1:].detach(), present

@@ -145,7 +145,6 @@ def _check_rand(rand: dict, n_obj: int, n: int, n_samples: int, n_importance: in
 def _render_multi_one_call(models, grid, code_table, rays_list, obj_ids, n_samples, use_disp, perturb, n_importance,
                            white_back, boxes, precision, noise_std=0.0, seed=0, clips=None, u_list=None, noise_c=None,
                            noise_f=None):
-    lib = _lib.load()
     dev = rays_list[0].device
     n_obj, n = len(rays_list), rays_list[0].shape[0]
     f = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
@@ -187,9 +186,8 @@ def _render_multi_one_call(models, grid, code_table, rays_list, obj_ids, n_sampl
         for k, v in m.items():
             setattr(cm, k, v.data_ptr())
             results[f"{k}_{typ}"] = v
-    ws = torch.empty(max(lib.onerf_render_multi_workspace_bytes(n, n_obj, n_samples, n_importance), 256), dtype=torch.uint8,
-                     device=dev)
+    ws = torch.empty(max(_lib.load().onerf_render_multi_workspace_bytes(n, n_obj, n_samples, n_importance), 256),
+                     dtype=torch.uint8, device=dev)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-    with torch.cuda.device(dev):
-        _lib.check(lib.onerf_render_multi_fwd_ext(_lib.ctx(dev), C.byref(a), C.byref(x), _lib.stream()))
+    _lib.call("onerf_render_multi_fwd_ext", dev, C.byref(a), C.byref(x))
     return results

@@ -78,7 +78,7 @@ class ObjectNeRF(nn.Module):
     def _query(self, inputs, sigma_only, obj_code):
         """Reference :97-152 on inputs made by this package's embeddings: the positions (and directions) they were encoded
         from run through the fused encode + MLP kernel.  Returns the branch's (..., 4) field (rgb, raw sigma)."""
-        from . import field_query, rendering
+        from . import engine, field_query, rendering
         (src, emb) = self._source(inputs, "emb_xyz")
         if src is None:
             raise NotImplementedError(
@@ -121,13 +121,12 @@ class ObjectNeRF(nn.Module):
             rays[:, 3:6] = dirs.detach()
         z = torch.zeros(n, 1, dtype=torch.float32, device=pts.device)
         xyz = pts.detach().float().reshape(n, 1, 3).contiguous()
-        prec = field_query.precision_name(None)
+        prec = engine.train_precision(None)
         if grad:
             reached = (field_query.OBJECT_SIGMA if sigma_only else field_query.OBJECT) if fi else (
                 field_query.SCENE_SIGMA if sigma_only else field_query.SCENE)
             scene, obj = field_query.field_eval(self, grid_module, rays, z, xyz, codes, fi, prec, reached)
         else:
-            from . import engine
             packed = engine.packed_for(self, grid_module is not None)
             grid = engine.GridBuffers.from_module(grid_module) if grid_module is not None else None
             scene, obj = engine.field(rays, z, packed, grid, codes=codes.contiguous() if fi else None, want_scene=not fi,

@@ -48,8 +48,7 @@ def get_ray_directions(H: int, W: int, focal: float, device=None) -> torch.Tenso
     """(H, W, 3) camera-space directions, datasets/ray_utils.py:5-25 (returned on the GPU)."""
     dev = _device(device)
     out = torch.empty(H, W, 3, dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().onerf_ray_directions(_lib.ctx(dev), H, W, float(focal), out.data_ptr(), _lib.stream()))
+    _lib.call("onerf_ray_directions", dev, H, W, float(focal), out.data_ptr())
     return out
 
 
@@ -59,9 +58,7 @@ def get_rays(directions: torch.Tensor, c2w):
     n = d.numel() // 3
     rays_o = torch.empty(n, 3, dtype=torch.float32, device=d.device)
     rays_d = torch.empty(n, 3, dtype=torch.float32, device=d.device)
-    with torch.cuda.device(d.device):
-        _lib.check(_lib.load().onerf_get_rays(_lib.ctx(d.device), d.data_ptr(), n, _c2w_host(c2w), rays_o.data_ptr(),
-                                              rays_d.data_ptr(), _lib.stream()))
+    _lib.call("onerf_get_rays", d.device, d.data_ptr(), n, _c2w_host(c2w), rays_o.data_ptr(), rays_d.data_ptr())
     return rays_o, rays_d
 
 
@@ -78,10 +75,8 @@ def generate_rays(obj_id: int, rays_o: torch.Tensor, rays_d: torch.Tensor, near:
         if box is None:
             raise ValueError("generate_rays: an object (obj_id != 0) needs its bounding-box helper")
         bh = C.byref(_box_host(box, bbox_enlarge))
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().onerf_generate_rays(_lib.ctx(dev), rays_o.data_ptr(), rays_d.data_ptr(), n, bh,
-                                                   float(scale_factor), float(near), float(far), out.data_ptr(),
-                                                   _lib.ptr(hit), _lib.stream()))
+    _lib.call("onerf_generate_rays", dev, rays_o.data_ptr(), rays_d.data_ptr(), n, bh, float(scale_factor), float(near),
+              float(far), out.data_ptr(), _lib.ptr(hit))
     return (out, hit.bool()) if return_mask else out
 
 
@@ -101,7 +96,6 @@ def camera_rays(H: int, W: int, focal: float, c2w, near: float, far: float, scal
     out = torch.empty(H * W, 8, dtype=torch.float32, device=dev)
     hit = torch.empty(H * W, dtype=torch.uint8, device=dev) if return_mask else None
     bh = C.byref(_box_host(box, bbox_enlarge)) if box is not None else None
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().onerf_camera_rays(_lib.ctx(dev), H, W, float(focal), _c2w_host(c2w), bh, float(scale_factor),
-                                                 float(near), float(far), out.data_ptr(), _lib.ptr(hit), _lib.stream()))
+    _lib.call("onerf_camera_rays", dev, H, W, float(focal), _c2w_host(c2w), bh, float(scale_factor), float(near),
+              float(far), out.data_ptr(), _lib.ptr(hit))
     return (out, hit.bool()) if return_mask else out

@@ -26,6 +26,14 @@ def _grid_of(embedding_xyz):
     return engine.GridBuffers.from_module(embedding_xyz) if _is_voxel(embedding_xyz) else None
 
 
+def _store_pass(results: Dict[str, Any], typ: str, out: Dict[str, torch.Tensor], z_vals, forward_instance: bool):
+    """One pass's maps into the result dict under the reference's keys (models/rendering.py:210-230)."""
+    for k in ("weights", "opacity", "rgb", "depth") + (("rgb_instance", "depth_instance", "opacity_instance")
+                                                          if forward_instance else ()):
+        results[f"{k}_{typ}"] = out[k]
+    results[f"z_vals_{typ}"] = z_vals
+
+
 def _needs_grad(model, *tensors) -> bool:
     if not torch.is_grad_enabled():
         return False
@@ -81,16 +89,7 @@ def inference_model(results: Dict[str, Any], model, embeddings: Dict[str, Any], 
                            frustum_bound_th=frustum_bound_th, pass_through_mask=pass_through_mask,
                            noise_scene=rand.get(f"noise_scene_{typ}"), noise_obj=rand.get(f"noise_obj_{typ}"),
                            seed=seed)
-    results[f"weights_{typ}"] = out["weights"]
-    results[f"opacity_{typ}"] = out["opacity"]
-    results[f"z_vals_{typ}"] = z_vals
-    results[f"rgb_{typ}"] = out["rgb"]
-    results[f"depth_{typ}"] = out["depth"]
-    if forward_instance:
-        results[f"rgb_instance_{typ}"] = out["rgb_instance"]
-        results[f"depth_instance_{typ}"] = out["depth_instance"]
-        results[f"opacity_instance_{typ}"] = out["opacity_instance"]
-    return
+    _store_pass(results, typ, out, z_vals, forward_instance)
 
 
 def _inference_model_grad(results, model, grid_module, typ, xyz, rays_d, z_vals, noise_std, white_back, is_eval,
@@ -111,21 +110,14 @@ def _inference_model_grad(results, model, grid_module, typ, xyz, rays_d, z_vals,
         rays, pos = _rays.detach().float().contiguous(), None
     reached = field_query.SCENE + (field_query.OBJECT if forward_instance else ())
     scene, obj = field_query.field_eval(model, grid_module, rays, z, pos, codes if forward_instance else None,
-                                        forward_instance, field_query.precision_name(precision), reached)
+                                        forward_instance, engine.train_precision(precision), reached)
     rand = _rand or {}
     seed = _seed if _seed is not None else (engine.new_seed() if noise_std > 0 else 0)
     cfg = dict(noise_std=float(noise_std), white_back=white_back, is_eval=is_eval, zero_last_delta=zero_last_delta,
                rays_in_bbox=rays_in_bbox, frustum_bound_th=float(frustum_bound_th), pass_through_mask=pass_through_mask,
                noise_scene=rand.get(f"noise_scene_{typ}"), noise_obj=rand.get(f"noise_obj_{typ}"), seed=seed)
     out = dict(zip(field_query.CompositeFn.KEYS, field_query.CompositeFn.apply(cfg, z, scene, obj)))
-    results[f"weights_{typ}"] = out["weights"]
-    results[f"opacity_{typ}"] = out["opacity"]
-    results[f"z_vals_{typ}"] = z_vals
-    results[f"rgb_{typ}"] = out["rgb"]
-    results[f"depth_{typ}"] = out["depth"]
-    if forward_instance:
-        for k in ("rgb_instance", "depth_instance", "opacity_instance"):
-            results[f"{k}_{typ}"] = out[k]
+    _store_pass(results, typ, out, z_vals, forward_instance)
 
 
 def query_sigma(model, embedding_xyz, xyz: torch.Tensor, obj_code: Optional[torch.Tensor] = None,
@@ -174,15 +166,7 @@ def _render_forward(cfg, rays, codes):
                                rays_in_bbox=cfg["rays_in_bbox"], frustum_bound_th=cfg["frustum_bound_th"],
                                pass_through_mask=cfg["pass_through_mask"], noise_scene=rand.get(f"noise_scene_{typ}"),
                                noise_obj=rand.get(f"noise_obj_{typ}"), seed=seed + seed_off)
-        results[f"weights_{typ}"] = out["weights"]
-        results[f"opacity_{typ}"] = out["opacity"]
-        results[f"z_vals_{typ}"] = z_vals
-        results[f"rgb_{typ}"] = out["rgb"]
-        results[f"depth_{typ}"] = out["depth"]
-        if fi:
-            results[f"rgb_instance_{typ}"] = out["rgb_instance"]
-            results[f"depth_instance_{typ}"] = out["depth_instance"]
-            results[f"opacity_instance_{typ}"] = out["opacity_instance"]
+        _store_pass(results, typ, out, z_vals, fi)
 
     one_pass("coarse", z, 1)
     if cfg["N_importance"] > 0:
@@ -223,8 +207,7 @@ def render_rays(models: Dict[str, Any], embeddings: Dict[str, Any], rays: torch.
     # weights_* (models/rendering.py:228-229, :307): the gradients are unaffected.
     from . import backward
     cfg["has_table"], cfg["model_order"] = has_table, model_order
-    # bf16: tensor-core forward + backward; anything else selects the fp32 verification arithmetic end to end
-    cfg["precision"] = "bf16" if (cfg["precision"] or engine.default_precision()) == "bf16" else "fp32"
+    cfg["precision"] = engine.train_precision(cfg["precision"])
     params = ([emb_xyz.embedding_space_ftr.weight] if has_table else [])
     for typ in model_order:
         for w, b in engine.model_linears(models[typ]):

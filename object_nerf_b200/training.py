@@ -73,7 +73,8 @@ from typing import Any, Dict
 import torch
 
 from . import _lib, backward, editing, engine, parallel
-from .losses import TERMS
+from .losses import TERMS, fill_loss_args
+from .rendering import _is_voxel
 
 __all__ = ["train_step", "step_seed", "sync_replicas", "TrainStepFn", "install_training", "validate_frame",
            "install_validation"]
@@ -86,10 +87,6 @@ _synced: "weakref.WeakKeyDictionary[Any, tuple]" = weakref.WeakKeyDictionary()
 RANK_SEED_STRIDE = 1 << 52
 # EmbeddingVoxel's grid state besides the table (voxel_occupancy and voxel_count are absent from bare grid modules)
 GRID_BUFFERS = ("voxel_shape", "voxel_size", "voxel_offset", "voxel_count", "voxel_idx_map", "voxel_occupancy")
-
-
-def _is_voxel(emb) -> bool:
-    return hasattr(emb, "voxel_idx_map")
 
 
 def _grid_stamp(emb) -> tuple:
@@ -121,15 +118,10 @@ class _GradBucket:
     all-reduce, or it is the step's own gradient sink (train_step(grad_sink=True))."""
 
     def __init__(self, tensors, has_table, dev):
-        self.offsets, off = [], 0
-        for t in tensors:
-            self.offsets.append(off)
-            off += -(-t.numel() // 4) * 4
-        self.flat = torch.zeros(off, dtype=torch.float32, device=dev)
+        self.flat, self.views, self.offsets = engine.grad_buffer(tensors, dev)
         self.table_offset = self.offsets[-1] if has_table else None
         self.table_row = tensors[-1].shape[1] if has_table else 0
         self.shapes = [tuple(t.shape) for t in tensors]
-        self.views = [self.flat[o:o + t.numel()].view(t.shape) for t, o in zip(tensors, self.offsets)]
         self.ptrs = None
 
     def adopt(self, tensors) -> "_GradBucket":
@@ -166,13 +158,7 @@ class _StepPlan:
         self.rgbs, self.depths, self.weight = f(n, 3), f(n), f(n)
         self.valid, self.inst, self.ptm = (f(n, dtype=torch.uint8) for _ in range(3))
         self.out, self.present, self.psnr = f(1 + len(TERMS)), f(len(TERMS), dtype=torch.int32), f(1)
-        nbytes = lib.onerf_packed_weights_bytes(int(self.use_voxel))
-        self.packed = {}
-        for typ in self.model_order:
-            engine.check_architecture(models[typ], self.use_voxel)
-            blob = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
-            off = (-blob.data_ptr()) % 1024
-            self.packed[typ] = blob[off:off + nbytes]
+        self.packed = _packed_blobs(models, self.model_order, self.use_voxel, dev)
         prec = engine.PRECISIONS[cfg["precision"]]
         self.ws = backward._pool.take(lib.onerf_train_step_workspace_bytes(
             prec, int(self.use_voxel), n, cfg["N_samples"], cfg["N_importance"]), dev)
@@ -188,10 +174,23 @@ class _StepPlan:
         la.n_rays, la.has_fine = n, int(len(self.model_order) == 2)
         la.rgbs, la.depths, la.valid_mask = self.rgbs.data_ptr(), self.depths.data_ptr(), self.valid.data_ptr()
         la.instance_mask, la.instance_mask_weight = self.inst.data_ptr(), self.weight.data_ptr()
-        (la.color_weight, la.depth_weight, la.opacity_weight, la.instance_color_weight,
-         la.instance_depth_weight) = cfg["loss_weights"]
-        la.loss_sum_out, la.terms_out, la.present_out = self.out.data_ptr(), self.out[1:].data_ptr(), self.present.data_ptr()
+        fill_loss_args(la, cfg["loss_weights"], self.out, self.present)
         self.loss_args = la
+
+
+def _packed_blobs(models, model_order, use_voxel, dev) -> dict:
+    """One packed-weights blob per model of a plan, filled by every call (a captured graph replays their addresses)."""
+    nbytes = _lib.load().onerf_packed_weights_bytes(int(use_voxel))
+    for typ in model_order:
+        engine.check_architecture(models[typ], use_voxel)
+    return {typ: engine.aligned_bytes(nbytes, dev) for typ in model_order}
+
+
+def _pack(models, typ, use_voxel, packed) -> list:
+    """Re-pack model `typ`'s current weights into the plan's blob; returns its (W, b) pairs."""
+    lin = [(_f32_param(w), _f32_param(b)) for w, b in engine.model_linears(models[typ])]
+    engine.pack_weights(lin, use_voxel, out=packed[typ])
+    return lin
 
 
 def _capturing(dev) -> bool:
@@ -290,18 +289,16 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
     if grad_sink and group is not None:
         raise ValueError("train_step: grad_sink returns the gradients for the caller to reduce (DDP does it through "
                          "autograd); group= reduces .grad itself: choose one")
-    lib = _lib.load()
     rays = batch["rays"].reshape(-1, 8)
     dev = rays.device
     n = rays.shape[0]
     emb_xyz = embeddings["xyz"]
-    precision = render_kwargs.get("precision") or engine.default_precision()
     rand = render_kwargs.get("_rand") or {}
     cfg = dict(N_samples=int(N_samples), N_importance=int(N_importance), use_disp=bool(use_disp), perturb=float(perturb),
                noise_std=float(noise_std), white_back=bool(white_back), is_eval=bool(render_kwargs.get("is_eval", False)),
                zero_last_delta=bool(render_kwargs.get("use_zero_as_last_delta", False)),
                rays_in_bbox=bool(rays_in_bbox), frustum_bound_th=float(frustum_bound_th),
-               has_ptm=pass_through_mask is not None, precision="bf16" if precision == "bf16" else "fp32",
+               has_ptm=pass_through_mask is not None, precision=engine.train_precision(render_kwargs.get("precision")),
                loss_weights=tuple(float(loss_conf[f"{t}_weight"]) for t in TERMS))
     use_voxel = _is_voxel(emb_xyz)
     table = emb_xyz.embedding_space_ftr.weight if use_voxel else None
@@ -369,41 +366,30 @@ def train_step(models: Dict[str, Any], embeddings: Dict[str, Any], code_library,
     if pass_through_mask is not None:
         plan.ptm.copy_(pass_through_mask.reshape(n))
     plan.d_codes.zero_()
-    ctx, stream = _lib.ctx(dev), _lib.stream()
-    keep = []
-    with torch.cuda.device(dev):
-        _lib.check(lib.onerf_code_gather(ctx, _f32_param(code_table).data_ptr(), plan.ids.data_ptr(), n,
-                                         code_table.shape[0], plan.codes.data_ptr(), stream))
-        b = _lib.RenderBwdArgs()
-        for typ in plan.model_order:
-            lin = engine.model_linears(models[typ])
-            Wp = (C.c_void_p * 20)(*[_f32_param(w).data_ptr() for w, _ in lin])
-            Bp = (C.c_void_p * 20)(*[_f32_param(bb).data_ptr() for _, bb in lin])
-            g = grads[first[typ]:first[typ] + 40]
-            dWp = (C.c_void_p * 20)(*[d.data_ptr() for d in g[0::2]])
-            dbp = (C.c_void_p * 20)(*[d.data_ptr() for d in g[1::2]])
-            keep += [Wp, Bp, dWp, dbp]
-            _lib.check(lib.onerf_pack_weights(ctx, int(plan.use_voxel), Wp, Bp, plan.packed[typ].data_ptr(),
-                                              plan.packed[typ].numel(), stream))
-            setattr(b, "W_" + typ, Wp)
-            setattr(b, "dW_" + typ, dWp)
-            setattr(b, "db_" + typ, dbp)
-        b.d_codes = plan.d_codes.data_ptr()
-        b.table_grad = grads[-1].data_ptr() if table is not None else None
-        a = plan.render.args
-        if capturing:
-            _lib.check(lib.onerf_train_step_dseed(ctx, C.byref(a), C.byref(plan.loss_args), C.byref(b),
-                                                  plan.psnr.data_ptr(), plan.seed_dev.data_ptr(), stream))
-        else:
-            a.seed = seed
-            _lib.check(lib.onerf_train_step(ctx, C.byref(a), C.byref(plan.loss_args), C.byref(b), plan.psnr.data_ptr(),
-                                            stream))
-        _lib.check(lib.onerf_code_scatter_add(ctx, plan.d_codes.data_ptr(), plan.ids.data_ptr(), n, code_table.shape[0],
-                                              grads[40 * len(plan.model_order)].data_ptr(), stream))
-        if group is not None:
-            reduced = plan.bucket.flat[:plan.bucket.prefix(synced[1])]
-            dist.all_reduce(reduced, op=dist.ReduceOp.SUM, group=group)     # gloo has no AVG
-            reduced.mul_(1.0 / world)
+    _lib.call("onerf_code_gather", dev, _f32_param(code_table).data_ptr(), plan.ids.data_ptr(), n, code_table.shape[0],
+              plan.codes.data_ptr())
+    b = _lib.RenderBwdArgs()
+    for typ in plan.model_order:
+        g = grads[first[typ]:first[typ] + 40]
+        setattr(b, "W_" + typ, engine.pointer_tables(_pack(models, typ, plan.use_voxel, plan.packed))[0])
+        dW, db = engine.pointer_tables(zip(g[0::2], g[1::2]))
+        setattr(b, "dW_" + typ, dW)
+        setattr(b, "db_" + typ, db)
+    b.d_codes = plan.d_codes.data_ptr()
+    b.table_grad = grads[-1].data_ptr() if table is not None else None
+    a = plan.render.args
+    if capturing:
+        _lib.call("onerf_train_step_dseed", dev, C.byref(a), C.byref(plan.loss_args), C.byref(b), plan.psnr.data_ptr(),
+                  plan.seed_dev.data_ptr())
+    else:
+        a.seed = seed
+        _lib.call("onerf_train_step", dev, C.byref(a), C.byref(plan.loss_args), C.byref(b), plan.psnr.data_ptr())
+    _lib.call("onerf_code_scatter_add", dev, plan.d_codes.data_ptr(), plan.ids.data_ptr(), n, code_table.shape[0],
+              grads[40 * len(plan.model_order)].data_ptr())
+    if group is not None:
+        reduced = plan.bucket.flat[:plan.bucket.prefix(synced[1])]
+        dist.all_reduce(reduced, op=dist.ReduceOp.SUM, group=group)     # gloo has no AVG
+        reduced.mul_(1.0 / world)
     if grad_sink:
         return plan.out[0], plan.out[1:], plan.present, plan.psnr[0], grads
     return plan.out[0], plan.out[1:], plan.present, plan.psnr[0]
@@ -504,7 +490,6 @@ class _ValPlan:
     maps and, for a batch without instance_mask, the all-zero mask and weight."""
 
     def __init__(self, models, n, tile, cfg, keys, dev, use_voxel):
-        lib = _lib.load()
         self.model_order = ["coarse"] + (["fine"] if cfg["N_importance"] > 0 else [])
         self.typ = self.model_order[-1]
         f = lambda *shape, dtype=torch.float32: torch.empty(*shape, dtype=dtype, device=dev)
@@ -514,13 +499,7 @@ class _ValPlan:
         if not cfg["has_instance_mask"]:
             self.no_inst = torch.zeros(n, dtype=torch.uint8, device=dev)
             self.no_weight = torch.zeros(n, dtype=torch.float32, device=dev)
-        nbytes = lib.onerf_packed_weights_bytes(int(use_voxel))
-        self.packed = {}
-        for typ in self.model_order:
-            engine.check_architecture(models[typ], use_voxel)
-            blob = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
-            off = (-blob.data_ptr()) % 1024
-            self.packed[typ] = blob[off:off + nbytes]
+        self.packed = _packed_blobs(models, self.model_order, use_voxel, dev)
         self.maps = {f"{k}_{self.typ}": f(tile, 3) if _VAL_WIDTHS[k] == 3 else f(tile) for k in keys}
         self.weights = (C.c_float * len(TERMS))(*cfg["loss_weights"])
         a = self.args = _lib.ValidateArgs()
@@ -534,9 +513,7 @@ class _ValPlan:
         for k in keys:
             setattr(getattr(r, self.typ), k, self.maps[f"{k}_{self.typ}"].data_ptr())
         la.n_rays, la.has_fine = n, int(self.typ == "fine")
-        (la.color_weight, la.depth_weight, la.opacity_weight, la.instance_color_weight,
-         la.instance_depth_weight) = cfg["loss_weights"]
-        la.loss_sum_out, la.terms_out, la.present_out = self.out.data_ptr(), self.out[1:].data_ptr(), self.present.data_ptr()
+        fill_loss_args(la, cfg["loss_weights"], self.out, self.present)
         a.chunk_rays = cfg["chunk"]
         a.psnr_mask = _lib.PSNR_VALID_INSTANCE if cfg["has_instance_mask"] else _lib.PSNR_ALL_RAYS
         a.record, a.psnr_out = self.record.data_ptr(), self.psnr.data_ptr()
@@ -575,14 +552,12 @@ def validate_frame(models: Dict[str, Any], embeddings: Dict[str, Any], code_libr
         raise ValueError(f"validate_frame: rays need 8 columns (o, d, near, far), got {rays.shape[-1]}")
     rays = rays.reshape(-1, rays.shape[-1])[:, :8]
     n, dev = rays.shape[0], rays.device
-    lib = _lib.load()
-    ctx = _lib.ctx(dev)
     emb_xyz = embeddings["xyz"]
     use_voxel = _is_voxel(emb_xyz)
     has_mask = "instance_mask" in batch
     cfg = dict(N_samples=int(N_samples), N_importance=int(N_importance), use_disp=bool(use_disp),
                white_back=bool(white_back), rays_in_bbox=bool(rays_in_bbox), chunk=int(chunk),
-               precision="bf16" if precision == "bf16" else "fp32", has_instance_mask=has_mask,
+               precision=engine.train_precision(precision), has_instance_mask=has_mask,
                loss_weights=tuple(float(loss_conf[f"{t}_weight"]) for t in TERMS))
     begin, end = 0, n
     if group is not None:
@@ -607,24 +582,18 @@ def validate_frame(models: Dict[str, Any], embeddings: Dict[str, Any], code_libr
     grid = engine.GridBuffers.from_module(emb_xyz) if use_voxel else None
     a.render.grid = C.pointer(grid.c) if use_voxel else None
     a.ray_begin, a.ray_end, a.finalize = begin, end, int(group is None)
-    ws = editing._workspace(lib.onerf_validate_workspace_bytes(cfg["chunk"], cfg["N_samples"], cfg["N_importance"]), dev)
+    ws = editing._workspace(_lib.load().onerf_validate_workspace_bytes(cfg["chunk"], cfg["N_samples"],
+                                                                       cfg["N_importance"]), dev)
     a.render.workspace, a.render.workspace_bytes = ws.data_ptr(), ws.numel()
-    stream = _lib.stream()
-    with torch.cuda.device(dev):
-        for typ in plan.model_order:
-            lin = engine.model_linears(models[typ])
-            Wp = (C.c_void_p * 20)(*[_f32_param(w).data_ptr() for w, _ in lin])
-            Bp = (C.c_void_p * 20)(*[_f32_param(b).data_ptr() for _, b in lin])
-            _lib.check(lib.onerf_pack_weights(ctx, int(use_voxel), Wp, Bp, plan.packed[typ].data_ptr(),
-                                              plan.packed[typ].numel(), stream))
-        _lib.check(lib.onerf_validate_frame(ctx, C.byref(a), stream))
-        maps = dict(plan.maps)
-        if group is not None:
-            dist.all_reduce(plan.record, op=dist.ReduceOp.SUM, group=group)
-            _lib.check(lib.onerf_validate_finalize(ctx, plan.record.data_ptr(), plan.weights, a.loss.has_fine,
-                                                   plan.out.data_ptr(), plan.out[1:].data_ptr(), plan.present.data_ptr(),
-                                                   plan.psnr.data_ptr(), stream))
-            maps = {k: parallel.gather_tiles(v, n, group) for k, v in maps.items()}
+    for typ in plan.model_order:
+        _pack(models, typ, use_voxel, plan.packed)
+    _lib.call("onerf_validate_frame", dev, C.byref(a))
+    maps = dict(plan.maps)
+    if group is not None:
+        dist.all_reduce(plan.record, op=dist.ReduceOp.SUM, group=group)
+        _lib.call("onerf_validate_finalize", dev, plan.record.data_ptr(), plan.weights, a.loss.has_fine,
+                  plan.out.data_ptr(), plan.out[1:].data_ptr(), plan.present.data_ptr(), plan.psnr.data_ptr())
+        maps = {k: parallel.gather_tiles(v, n, group) for k, v in maps.items()}
     return {"loss_sum": plan.out[0], "terms": plan.out[1:], "present": plan.present, "psnr": plan.psnr[0], **maps}
 
 

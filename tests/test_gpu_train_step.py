@@ -294,3 +294,42 @@ def test_step_follows_voxel_subdivision():
         assert torch.equal(maps_f[k], v.detach()), k
     assert embs[1].embedding_space_ftr.weight.grad.norm() > 0      # the rays do reach the grid
     _assert_same_grads(named_f, named_e, 1e-5, 0.99999)
+
+
+def _step_and_validation(dev, precision):
+    """One train_step and one validate_frame on the voxel case with every tensor on `dev`: their outputs, the gradients
+    and the step's maps, copied to the host."""
+    from object_nerf_b200 import Embedding, training
+    torch.manual_seed(0)
+    inp = cases.build_grad_case()
+    models = {k: helpers.make_model(w, True, dev).train() for k, w in inp["weights"].items()}
+    embeddings = {"xyz": helpers.GridModule(inp["grid"]).to(dev), "dir": Embedding(3, 4)}
+    lib = helpers.CodeLib(inp["code_table"]).to(dev)
+    batch = {k: v.to(dev) for k, v in inp["batch"].items()}
+    batch["rays"], batch["instance_ids"] = inp["rays"].to(dev), inp["instance_ids"].to(dev)
+    kw = _kwargs(cases.GRAD_CASE, inp, precision, {k: v.to(dev) for k, v in inp["rand"].items()},
+                 pass_through_mask=inp["pass_through_mask"].to(dev))
+    step = training.train_step(models, embeddings, lib, batch, cases.LOSS_CONF, **kw)
+    (plan,) = training._plans[models["coarse"]].values()
+    maps = [v for m in plan.render.maps.values() for v in m.values()]
+    val = training.validate_frame(models, embeddings, lib, {k: v[None] for k, v in batch.items()}, cases.LOSS_CONF,
+                                  N_samples=kw["N_samples"], N_importance=kw["N_importance"], use_disp=False,
+                                  white_back=False, precision=precision)
+    torch.cuda.synchronize(dev)
+    grads = [p.grad for _, p in _named(models, embeddings, lib)]
+    return [t.cpu() for t in list(step) + maps + grads + list(val.values())]
+
+
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
+@pytest.mark.parametrize("precision", ["bf16", "fp32"])
+def test_step_and_validation_on_a_device_that_is_not_current(precision):
+    """train_step and validate_frame on tensors of cuda:1 while cuda:0 is current compute bit for bit what they compute
+    with cuda:1 current: every launch goes to the tensors' device and that device's current stream."""
+    with torch.cuda.device(1):
+        want = _step_and_validation("cuda:1", precision)
+    assert torch.cuda.current_device() == 0
+    got = _step_and_validation("cuda:1", precision)
+    assert torch.cuda.current_device() == 0
+    assert len(got) == len(want)
+    bits = lambda t: t.reshape(-1).view(torch.uint8)
+    assert all(torch.equal(bits(g), bits(w)) for g, w in zip(got, want))
