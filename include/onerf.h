@@ -103,7 +103,8 @@ int onerf_sample_pdf(onerf_ctx* ctx, const float* bins, const float* weights, in
                      int n_importance, int det, const float* u, uint64_t seed, float* out, void* stream);
 
 /* Encoding only (test / ncu entry): xyz (B,3) -> scene_in (B,271|63), obj_in (B,104) (null for plain
- * PE).  models/embedding_helper.py:57-74, :325-411.  grid == NULL selects plain PE(10). */
+ * PE).  models/embedding_helper.py:57-74, :325-411.  grid == NULL selects plain PE(10); a grid's table
+ * must be 16-byte aligned (rows are read as float4). */
 int onerf_encode(onerf_ctx* ctx, const onerf_grid* grid, const float* xyz, int64_t n_points,
                  float* scene_in, float* obj_in, void* stream);
 

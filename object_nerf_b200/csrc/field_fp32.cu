@@ -400,9 +400,10 @@ int onerf_launch_field_fp32(onerf_ctx* ctx, const FieldParams& p, cudaStream_t s
 
 extern "C" int onerf_encode(onerf_ctx* ctx, const onerf_grid* grid, const float* xyz, int64_t n_points,
                             float* scene_in, float* obj_in, void* stream) {
-  ONERF_CHECK_ARG(ctx && xyz && scene_in, "null argument");
+  ONERF_CHECK_ARG(ctx && (n_points == 0 || (xyz && scene_in)), "null argument");   // (empty tensors have no data)
   ONERF_CHECK_ARG(n_points >= 0, "bad shape");
-  if (grid) ONERF_CHECK_ARG(obj_in && grid->table && grid->idx_map && grid->voxel_offset && grid->voxel_size && grid->voxel_shape, "null grid buffer");
+  if (grid) ONERF_CHECK_ARG((n_points == 0 || obj_in) && grid->table && grid->idx_map && grid->voxel_offset && grid->voxel_size && grid->voxel_shape, "null grid buffer");
+  if (grid) ONERF_CHECK_ARG(onerf_aligned16(grid->table), "misaligned grid table (rows are read as float4)");
   if (n_points == 0) return ONERF_OK;
   onerf_grid g = grid ? *grid : onerf_grid{nullptr, nullptr, nullptr, nullptr, nullptr};
   int blocks = (int)((n_points + 255) / 256);
@@ -431,7 +432,7 @@ voxel_features_kernel(onerf_grid grid, const float* __restrict__ xyz, int64_t n,
 
 extern "C" int onerf_voxel_features(onerf_ctx* ctx, const onerf_grid* grid, const float* xyz, int64_t n_points, float* out,
                                     void* stream) {
-  ONERF_CHECK_ARG(ctx && grid && xyz && out, "null argument");
+  ONERF_CHECK_ARG(ctx && grid && (n_points == 0 || (xyz && out)), "null argument");   // (empty tensors have no data)
   ONERF_CHECK_ARG(grid->table && grid->idx_map && grid->voxel_offset && grid->voxel_size && grid->voxel_shape, "null grid buffer");
   ONERF_CHECK_ARG(n_points >= 0 && onerf_aligned16(out) && onerf_aligned16(grid->table), "bad count or misaligned buffer");
   if (n_points == 0) return ONERF_OK;

@@ -206,7 +206,8 @@ class EmbeddingVoxel(nn.Module):
         """Reference :247-302: halve the voxel size.  Every occupied voxel spawns its 8 children
         (itertools.product([0, 1], repeat=3) order), whose features are the trilinear samples of the OLD grid at the
         child positions (raw features, no positional encoding: `onerf_voxel_features`); occupancy / index map are
-        rebuilt at twice the resolution and the children's rows written into the feature table."""
+        rebuilt at twice the resolution and the children's rows written into the feature table.  More children than
+        table rows raises RuntimeError with every buffer and the table unchanged."""
         idx_occu, voxel_xyz = self._occupied()
         dev = voxel_xyz.device
         target = self.voxel_size / 2
@@ -220,11 +221,13 @@ class EmbeddingVoxel(nn.Module):
         features_fn = _features_fn or (lambda pts: engine.voxel_features(pts, self.grid_buffers()))
         with torch.no_grad():
             new_ftrs = features_fn(new_xyz)
+        occ = torch.zeros([2 * int(v) for v in self.voxel_shape], dtype=torch.bool, device=dev)
+        occ[new_coord[:, 0], new_coord[:, 1], new_coord[:, 2]] = True
+        # refuse before touching any buffer: a failed call leaves the old grid whole (the index map matches the shape)
+        if int(occ.sum()) > self.embedding_space_ftr.num_embeddings:
+            raise RuntimeError("more occupied voxels than N_max_voxels")
         self.voxel_size = target
         self.voxel_shape *= 2
-        shape = [int(v) for v in self.voxel_shape]
-        occ = torch.zeros(shape, dtype=torch.bool, device=dev)
-        occ[new_coord[:, 0], new_coord[:, 1], new_coord[:, 2]] = True
         self.voxel_occupancy = occ
         self.voxel_count = self.voxel_shape[0] * self.voxel_shape[1] * self.voxel_shape[2]
         self.generate_voxel_idx_map()

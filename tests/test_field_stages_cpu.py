@@ -14,6 +14,7 @@ import torch
 from oracle import onerf_oracle as O
 from tests import synth
 from tests.test_gpu_train_stages import _wgrad_inputs
+from tests.voxel_grid_cases import voxel_features32  # noqa: F401  (the kernels' trilinear blend, re-exported)
 
 # GEMM layers in GemmId order (csrc/layout.h); the output of GEMMS[i] is activation slot i + 1
 GEMMS = ("S0", "S1", "S2", "S3", "S4", "S5", "S6", "S7", "SFIN", "SDIR", "O0", "O1", "O2", "O3", "OFIN", "ODIR")
@@ -168,38 +169,6 @@ def positions(rays, z, fused):
     d = rays[:, None, 3:6].expand(n, S, 3).reshape(-1, 3)
     zz = z.reshape(-1, 1).expand(-1, 3)
     return fma32(d, zz, o) if fused else o + d * zz
-
-
-def voxel_features32(x, g):
-    """Trilinear features at float32 positions x (B, 3) with the kernels' fp32 voxel coordinates and corner weights
-    (encode.cuh voxel_trilinear): -> (float64 sum of the fp32-weighted corners, sum of |weighted corners|, the
-    individually rounded fp32 sum of the FFMA kernel)."""
-    dev = x.device
-    off, vs = g["offset"].to(dev).float(), g["voxel_size"].to(dev).float()
-    p = (x + off) / vs
-    q = torch.floor(p)
-    u = p - q
-    lu = 1.0 - u
-    q = q.long()
-    shape = g["shape"].to(dev)
-    idx_map, table = g["idx_map"].to(dev), g["table"].to(dev)
-    f64 = torch.zeros(x.shape[0], 24, dtype=torch.float64, device=dev)
-    bound = torch.zeros_like(f64)
-    f32 = torch.zeros(x.shape[0], 24, dtype=torch.float32, device=dev)
-    for corner in range(8):
-        cc = [(corner >> 2) & 1, (corner >> 1) & 1, corner & 1]
-        ix = q + torch.tensor(cc, device=dev)
-        ok = ((ix >= 0) & (ix < shape)).all(1)
-        ixc = torch.where(ok[:, None], ix, torch.zeros_like(ix))
-        row = idx_map[ixc[:, 0], ixc[:, 1], ixc[:, 2]]
-        ok &= row >= 0
-        wt = ((u[:, 0] if cc[0] else lu[:, 0]) * (u[:, 1] if cc[1] else lu[:, 1])) * (u[:, 2] if cc[2] else lu[:, 2])
-        t = torch.where(ok[:, None], table[row.clamp(min=0)], torch.zeros(1, device=dev))
-        term = t * wt[:, None]
-        f32 = torch.where(ok[:, None], f32 + term, f32)
-        f64 += t.double() * wt.double()[:, None]
-        bound += (t.double() * wt.double()[:, None]).abs()
-    return f64, bound, f32
 
 
 def pe_budget(v, dv, e0, n_freq):
