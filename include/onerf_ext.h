@@ -234,6 +234,51 @@ int onerf_draw_batch(onerf_ctx* ctx, const onerf_batch_args* args, void* stream)
 int onerf_draw_batch_dstep(onerf_ctx* ctx, const onerf_batch_args* args, uint64_t* step_dev, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Training batches drawn from a frame store: onerf_draw_batch over the R = F*H*W rays GenericDataset would expand the
+ * frames into, each drawn row rebuilt from its pixel instead of read from per-ray buffers.  Ray i = f*H*W + p (frame f,
+ * pixel p = y*W + x row-major) and column c are drawn exactly as onerf_draw_batch draws them (same seed, step, rank and
+ * world give the same (i, c)); the row's fields are
+ *   rays           (o, d, near_s, far_s): o = poses[f] translation, d = directions[p] rotated by poses[f] and normalised
+ *                  with onerf_get_rays' arithmetic;
+ *   rgbs           rgb[f,p,k] / 255 (IEEE division, as torchvision's ToTensor);
+ *   depths         depths[f,p];
+ *   valid_mask     1 iff border <= x < W - border and border <= y < H - border;
+ *   frame_idx      frame_idx[f];
+ *   instance_ids   ids[c];
+ *   instance_mask, instance_mask_weight, pass_through_mask
+ *                  mask_all_ones[c]: 1, weights[f,c,1], 1; otherwise with l = labels[f,p]: m = (l == ids[c]),
+ *                  weights[f,c,m], and 1 iff l is one of pass_ids[c, 0..n_pass) (-1 pads a row: it matches no label).
+ * Outputs, seed, step, rank, world and index_out are those of onerf_batch_args; args->data is not read.
+ * Refusals (ONERF_ERR_BAD_ARG): those of onerf_draw_batch with R = F*H*W, and a null frame store, a null table, a null
+ * labels buffer with a column whose mask is not all ones, F, H or W < 1, border < 0, n_pass outside [1,
+ * ONERF_FRAME_MAX_PASS].  Kernels only, no host read: CUDA-graph capturable; onerf_draw_frames_dstep steps as
+ * onerf_draw_batch_dstep does.
+ * ------------------------------------------------------------------------------------------- */
+#define ONERF_FRAME_MAX_PASS 16
+
+typedef struct onerf_frame_dataset {
+  int n_frames, H, W;                   /* F, H, W */
+  int n_instances;                      /* I */
+  const float* poses;                   /* (F,12) row-major (3,4) c2w */
+  const float* directions;              /* (H*W,3) from onerf_ray_directions */
+  const uint8_t* rgb;                   /* (F,H*W,3) */
+  const float* depths;                  /* (F,H*W) */
+  const uint16_t* labels;               /* (F,H*W), or NULL when every column's mask is all ones */
+  const int64_t* frame_idx;             /* (F,) */
+  float near_s, far_s;                  /* near / scale_factor, far / scale_factor */
+  int border;
+  const int64_t* ids;                   /* (I,) */
+  const uint8_t* mask_all_ones;         /* (I,) 0 / 1 */
+  const float* weights;                 /* (F,I,2): [background, foreground] */
+  const int32_t* pass_ids;              /* (I,n_pass) */
+  int n_pass;
+} onerf_frame_dataset;
+
+int onerf_draw_frames(onerf_ctx* ctx, const onerf_frame_dataset* frames, const onerf_batch_args* args, void* stream);
+int onerf_draw_frames_dstep(onerf_ctx* ctx, const onerf_frame_dataset* frames, const onerf_batch_args* args,
+                            uint64_t* step_dev, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * One validation image, or a contiguous tile of it, in one call (train.py:73-105, 182-223: ObjectNeRFSystem.forward over
  * the image, TotalLoss, psnr).  Rays [ray_begin, ray_end) of the image's batch are rendered in chunks of chunk_rays rays
  * through onerf_render_rays_fwd's passes (is_eval, nothing random); the compositing kernel of each pass also adds the

@@ -5,3 +5,4 @@ from .nerf_model import ObjectNeRF  # noqa: F401
 from .embedding_helper import Embedding, EmbeddingVoxel  # noqa: F401
 from .code_library import CodeLibrary  # noqa: F401
 from .batches import RaySampler  # noqa: F401
+from .frames import FrameSet  # noqa: F401

@@ -43,10 +43,11 @@ EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_w
                "onerf_prune_workspace_bytes", "onerf_prune_measure", "onerf_prune_apply",
                "onerf_composite_multi_noise_ws", "onerf_composite_multi_noise_merge", "onerf_sample_pdf_merge_clip",
                "onerf_render_multi_fwd_ext", "onerf_field_bwd_workspace_bytes", "onerf_field_bwd", "onerf_bwd_dx_xyz",
-               "onerf_encode_bwd_xyz"]
+               "onerf_encode_bwd_xyz", "onerf_draw_frames", "onerf_draw_frames_dstep"]
 VALIDATE_RECORD_DOUBLES = 18
 PRUNE_SAMPLES = 4096
 PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
+FRAME_MAX_PASS = 16                                          # label values one instance column lets pass through
 STREAM_MULTI_NOISE_COARSE, STREAM_MULTI_NOISE_FINE = 7, 8   # Philox streams of the joint compositing's sigma noise
 
 _p = C.c_void_p
@@ -161,6 +162,13 @@ class BatchArgs(C.Structure):
         ("instance_mask", _p), ("instance_mask_weight", _p), ("instance_ids", _p), ("pass_through_mask", _p),
         ("index_out", _p),
     ]
+
+
+class FrameDataset(C.Structure):
+    _fields_ = [("n_frames", C.c_int), ("H", C.c_int), ("W", C.c_int), ("n_instances", C.c_int), ("poses", _p),
+                ("directions", _p), ("rgb", _p), ("depths", _p), ("labels", _p), ("frame_idx", _p),
+                ("near_s", C.c_float), ("far_s", C.c_float), ("border", C.c_int), ("ids", _p), ("mask_all_ones", _p),
+                ("weights", _p), ("pass_ids", _p), ("n_pass", C.c_int)]
 
 
 class ValidateArgs(C.Structure):
@@ -302,6 +310,8 @@ def load() -> C.CDLL:
         lib.onerf_render_edit_frame.argtypes = [_p, C.POINTER(RenderEditArgs), _p]
         lib.onerf_draw_batch.argtypes = [_p, C.POINTER(BatchArgs), _p]
         lib.onerf_draw_batch_dstep.argtypes = [_p, C.POINTER(BatchArgs), _p, _p]
+        lib.onerf_draw_frames.argtypes = [_p, C.POINTER(FrameDataset), C.POINTER(BatchArgs), _p]
+        lib.onerf_draw_frames_dstep.argtypes = [_p, C.POINTER(FrameDataset), C.POINTER(BatchArgs), _p, _p]
         lib.onerf_validate_workspace_bytes.argtypes = [C.c_int] * 3
         lib.onerf_validate_workspace_bytes.restype = C.c_size_t
         lib.onerf_validate_frame.argtypes = [_p, C.POINTER(ValidateArgs), _p]

@@ -1,8 +1,10 @@
 """Training batches drawn on the device (GenericDataset.__getitem__ through DataLoader(shuffle=True) in the reference,
 datasets/generic_dataset.py:475-490 and train.py:121-129).
 
-`RaySampler` uploads a training dataset's ray buffers once.  Each `next()` is one kernel (onerf_draw_batch_dstep) that
-draws the batch of the sampler's device step counter into fixed output buffers and advances the counter.  It reads
+`RaySampler` uploads a training dataset's ray buffers once (or, with `from_frames`, draws from a frames.FrameSet and
+rebuilds each row from its pixel: onerf_draw_frames_dstep, the same batches bit for bit).  Each `next()` is one kernel
+(onerf_draw_batch_dstep) that draws the batch of the sampler's device step counter into fixed output buffers and
+advances the counter.  It reads
 nothing back to the host, so `next()` + `training.train_step` + `Adam(capturable=True)` capture in one CUDA graph, and
 each replay trains on the next batch.
 
@@ -42,6 +44,28 @@ def _column_fields(t: torch.Tensor, n: int, name: str):
     return t
 
 
+def _group_rank(rank, world_size, group):
+    """(rank, world_size), taken from `group` when one is given."""
+    if group is None:
+        return rank, world_size
+    import torch.distributed as dist
+    g_rank, g_world = dist.get_rank(group), dist.get_world_size(group)
+    if (rank, world_size) not in ((0, 1), (g_rank, g_world)):
+        raise ValueError(f"RaySampler: rank {rank} / world_size {world_size} disagree with the group's "
+                         f"{g_rank} / {g_world}")
+    return g_rank, g_world
+
+
+def _check_batch(R, batch_size, rank, world_size):
+    B, W = int(batch_size), int(world_size)
+    if B < 1 or W < 1 or not 0 <= rank < W:
+        raise ValueError(f"RaySampler: bad batch_size {B}, world_size {W} or rank {rank}")
+    if R < B * W:
+        raise ValueError(f"RaySampler: {R} rays hold no full batch of {B} rays on each of {W} ranks")
+    if R >= MAX_RAYS:
+        raise ValueError(f"RaySampler: {R} rays; at most 2^40 - 1 are supported")
+
+
 class RaySampler:
     """Device-resident training batches of a GenericDataset's ray buffers.
 
@@ -61,13 +85,7 @@ class RaySampler:
         missing = [k for k in DATASET_KEYS if k not in tensors]
         if missing:
             raise ValueError(f"RaySampler: missing dataset buffers {missing}")
-        if group is not None:
-            import torch.distributed as dist
-            g_rank, g_world = dist.get_rank(group), dist.get_world_size(group)
-            if (rank, world_size) not in ((0, 1), (g_rank, g_world)):
-                raise ValueError(f"RaySampler: rank {rank} / world_size {world_size} disagree with the group's "
-                                 f"{g_rank} / {g_world}")
-            rank, world_size = g_rank, g_world
+        rank, world_size = _group_rank(rank, world_size, group)
         rays = tensors["all_rays"].reshape(-1, 8)
         R = rays.shape[0]
         src = {"rays": rays}
@@ -90,20 +108,12 @@ class RaySampler:
                              + ", ".join(f"{k} {src[k].shape[1]}" for k in COLUMN_KEYS))
         if I < 1:
             raise ValueError("RaySampler: the dataset has no instance column (I = 0)")
-        B, W = int(batch_size), int(world_size)
-        if B < 1 or W < 1 or not 0 <= rank < W:
-            raise ValueError(f"RaySampler: bad batch_size {B}, world_size {W} or rank {rank}")
-        if R < B * W:
-            raise ValueError(f"RaySampler: {R} rays hold no full batch of {B} rays on each of {W} ranks")
-        if R >= MAX_RAYS:
-            raise ValueError(f"RaySampler: {R} rays; at most 2^40 - 1 are supported")
+        _check_batch(R, batch_size, rank, world_size)
 
         dev = torch.device(device)
         if dev.type == "cuda" and dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
-        self.device, self.batch_size, self.rank, self.world_size = dev, B, int(rank), W
-        self.n_rays, self.n_instances = R, I
-        self.batches_per_epoch = R // (B * W)
+        self._setup(dev, R, I, batch_size, rank, world_size, seed, group)
 
         def up(t, kind):
             t = t.to(dev)
@@ -115,6 +125,18 @@ class RaySampler:
                  "instance_mask": "mask", "instance_mask_weight": "float", "instance_ids": "int",
                  "pass_through_mask": "mask"}
         self.buffers = {k: up(t, kinds[k]) for k, t in src.items()}
+        d = self._args.data
+        d.n_rays, d.n_instances = R, I
+        for k in kinds:
+            setattr(d, k, self.buffers[k].data_ptr() if k in self.buffers else None)
+
+    def _setup(self, dev, R, I, batch_size, rank, world_size, seed, group):
+        """Counters, seed and the fixed output buffers; the dataset part of the argument block is the caller's."""
+        B, W = int(batch_size), int(world_size)
+        self.device, self.batch_size, self.rank, self.world_size = dev, B, int(rank), W
+        self.n_rays, self.n_instances = R, I
+        self.batches_per_epoch = R // (B * W)
+        self.frames = None
 
         if seed is None:
             seed = engine.new_seed()
@@ -141,14 +163,8 @@ class RaySampler:
                        "instance_mask_weight": o["instance_mask_weight"].view(B, 1),
                        "instance_ids": o["instance_ids"].view(B, 1),
                        "pass_through_mask": o["pass_through_mask"].view(torch.bool).view(B, 1)}
-
-        buf = self.buffers
-        d = _lib.RayDataset()
-        d.n_rays, d.n_instances = R, I
-        for k in kinds:
-            setattr(d, k, buf[k].data_ptr() if k in buf else None)
         a = _lib.BatchArgs()
-        a.data, a.batch, a.rank, a.world, a.seed = d, B, self.rank, W, self.seed
+        a.batch, a.rank, a.world, a.seed = B, self.rank, W, self.seed
         for k, t in o.items():
             setattr(a, k, t.data_ptr())
         self._args = a
@@ -159,9 +175,29 @@ class RaySampler:
         names = list(DATASET_KEYS) + ["all_frame_indices"]
         return cls({k: getattr(dataset, k) for k in names if getattr(dataset, k, None) is not None}, **kw)
 
+    @classmethod
+    def from_frames(cls, frame_set, batch_size: int = 2048, device=None, seed=None, rank: int = 0,
+                    world_size: int = 1, group=None) -> "RaySampler":
+        """A sampler over a frames.FrameSet: the same batches as RaySampler(frame_set.expand(), ...) with the same
+        seed, bit for bit, each row rebuilt from the frame store on the device (onerf_draw_frames_dstep) instead of
+        read from per-ray buffers.  device: the frame set's (the default); another one is refused."""
+        rank, world_size = _group_rank(rank, world_size, group)
+        _check_batch(frame_set.n_rays, batch_size, rank, world_size)
+        if device is not None and torch.device(device) not in (frame_set.device, torch.device(frame_set.device.type)):
+            raise ValueError(f"RaySampler.from_frames: the frame set lives on {frame_set.device}, not {device}")
+        self = cls.__new__(cls)
+        self._setup(frame_set.device, frame_set.n_rays, frame_set.n_instances, batch_size, rank, world_size, seed,
+                    group)
+        self.frames, self.buffers = frame_set, {}
+        return self
+
     def next(self) -> Dict[str, torch.Tensor]:
         """Draw the batch of the device step counter and advance the counter by one (kernels only: capturable)."""
-        _lib.call("onerf_draw_batch_dstep", self.device, C.byref(self._args), self._step.data_ptr())
+        if self.frames is None:
+            _lib.call("onerf_draw_batch_dstep", self.device, C.byref(self._args), self._step.data_ptr())
+        else:
+            _lib.call("onerf_draw_frames_dstep", self.device, C.byref(self.frames.args), C.byref(self._args),
+                      self._step.data_ptr())
         return dict(self._batch)
 
     @property
