@@ -178,6 +178,37 @@ size_t onerf_render_edit_workspace_bytes(int chunk_rays, int n_obj, int n_sample
 int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_args* args, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * onerf_render_edit_frame plus, per pass, how much of each pixel each ray set shows.  For ray r, set position i (the
+ * list position, as obj_ids numbers the sets: duplicates of one object are separate columns) and the pass's weights w
+ * (those written to maps.weights: the joint compositing's, with the removed-object boxes and the box culling as there),
+ * summed over set i's samples:
+ *   opacity  (N, n_obj)     sum w
+ *   depth    (N, n_obj)     sum w z
+ *   rgb      (N, n_obj, 3)  sum w rgb, with no white background (white_back applies to maps.rgb only)
+ * For the coarse pass this is weights summed by obj_ids; summed over i the maps give the pass's opacity, depth and rgb
+ * (without the white background) up to float32 reassociation.  Each (ray, set) is a fixed-order sum over the set's
+ * weights in sample order, so every value is bit-identical whatever chunk_rays, the tile bounds or the sort path.  A set
+ * whose ray misses its box and a sample muted by a removed-object box add exactly 0.
+ *   coarse, fine   NULL, or tile-sized outputs (rows as maps); any NULL array is not written.  A fine array needs
+ *                  n_importance > 0.  Arrays 4-byte aligned.
+ *   workspace      >= onerf_render_edit_sets_workspace_bytes(chunk_rays, n_obj, n_samples, n_importance) bytes when any
+ *                  array is given (the fine pass's weights in set order need one more chunk-sized buffer; the same as
+ *                  onerf_render_edit_workspace_bytes without a fine pass), else as onerf_render_edit_frame.
+ * onerf_render_edit_frame is this call with coarse = fine = NULL, and the other outputs do not change with the set maps.
+ * Refusals (ONERF_ERR_BAD_ARG), before any launch, besides those of onerf_render_edit_frame: a fine array without a fine
+ * pass, an array not 4-byte aligned.  Kernels only, no host read: CUDA-graph capturable.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct onerf_set_maps {
+  float* opacity;                     /* (N, n_obj) or NULL */
+  float* depth;                       /* (N, n_obj) or NULL */
+  float* rgb;                         /* (N, n_obj, 3) or NULL */
+} onerf_set_maps;
+
+size_t onerf_render_edit_sets_workspace_bytes(int chunk_rays, int n_obj, int n_samples, int n_importance);
+int onerf_render_edit_frame_sets(onerf_ctx* ctx, const onerf_render_edit_args* args, const onerf_set_maps* coarse,
+                                 const onerf_set_maps* fine, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Training batches drawn on the device (GenericDataset.__getitem__ through DataLoader(shuffle=True), and under DDP
  * DistributedSampler; datasets/generic_dataset.py:475-490, train.py:121-129).  The dataset's R rays stay in device
  * memory; one launch draws batch `step` of rank `rank` into B-row outputs:

@@ -43,7 +43,8 @@ EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_w
                "onerf_prune_workspace_bytes", "onerf_prune_measure", "onerf_prune_apply",
                "onerf_composite_multi_noise_ws", "onerf_composite_multi_noise_merge", "onerf_sample_pdf_merge_clip",
                "onerf_render_multi_fwd_ext", "onerf_field_bwd_workspace_bytes", "onerf_field_bwd", "onerf_bwd_dx_xyz",
-               "onerf_encode_bwd_xyz", "onerf_draw_frames", "onerf_draw_frames_dstep"]
+               "onerf_encode_bwd_xyz", "onerf_draw_frames", "onerf_draw_frames_dstep",
+               "onerf_render_edit_sets_workspace_bytes", "onerf_render_edit_frame_sets"]
 VALIDATE_RECORD_DOUBLES = 18
 PRUNE_SAMPLES = 4096
 PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
@@ -147,6 +148,10 @@ class RenderEditArgs(C.Structure):
         ("use_disp", C.c_int), ("white_back", C.c_int), ("boxes", _p), ("n_boxes", C.c_int), ("chunk_rays", C.c_int),
         ("coarse", RenderMultiMaps), ("fine", RenderMultiMaps), ("workspace", _p), ("workspace_bytes", C.c_size_t),
     ]
+
+
+class SetMaps(C.Structure):
+    _fields_ = [("opacity", _p), ("depth", _p), ("rgb", _p)]
 
 
 class RayDataset(C.Structure):
@@ -308,6 +313,9 @@ def load() -> C.CDLL:
         lib.onerf_render_edit_workspace_bytes.argtypes = [C.c_int] * 4
         lib.onerf_render_edit_workspace_bytes.restype = C.c_size_t
         lib.onerf_render_edit_frame.argtypes = [_p, C.POINTER(RenderEditArgs), _p]
+        lib.onerf_render_edit_sets_workspace_bytes.argtypes = [C.c_int] * 4
+        lib.onerf_render_edit_sets_workspace_bytes.restype = C.c_size_t
+        lib.onerf_render_edit_frame_sets.argtypes = [_p, C.POINTER(RenderEditArgs), C.POINTER(SetMaps), C.POINTER(SetMaps), _p]
         lib.onerf_draw_batch.argtypes = [_p, C.POINTER(BatchArgs), _p]
         lib.onerf_draw_batch_dstep.argtypes = [_p, C.POINTER(BatchArgs), _p, _p]
         lib.onerf_draw_frames.argtypes = [_p, C.POINTER(FrameDataset), C.POINTER(BatchArgs), _p]

@@ -395,10 +395,17 @@ static int check_multi_ext(const char* fn, const onerf_render_multi_args* a, con
   }
   return ONERF_OK;
 }
-#undef FN_CHECK_ARG
-#undef FN_UNSUPPORTED
+// The per-set maps multi_forward writes (onerf_render_edit_frame_sets): the chunk's rows of each pass's outputs, and
+// where the fine pass's weights go in set order ((n_obj, N, S + K), the edit workspace's extension).
+struct SetMapsOut {
+  onerf_set_maps coarse, fine;
+  float* w_fine;
+};
 
-static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const onerf_render_multi_ext& x, void* stream);
+static bool any_set_map(const onerf_set_maps& m) { return m.opacity || m.depth || m.rgb; }
+
+static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const onerf_render_multi_ext& x, void* stream,
+                         const SetMapsOut* sets = nullptr);
 
 static int render_multi_fwd(const char* fn, onerf_ctx* ctx, const onerf_render_multi_args* a,
                             const onerf_render_multi_ext* ext, void* stream) {
@@ -433,10 +440,13 @@ extern "C" int onerf_render_multi_fwd_ext(onerf_ctx* ctx, const onerf_render_mul
 }
 
 // The forward of onerf_render_multi_fwd_ext on checked arguments: n_rays rays of every set in a->rays_list_host, maps
-// written to a->coarse / a->fine, scratch in a->workspace.
-static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const onerf_render_multi_ext& x, void* stream) {
+// written to a->coarse / a->fine, scratch in a->workspace; with `sets`, each pass's per-set maps too, from its weights
+// in set order while the pass's depths and fields are still in the workspace.
+static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const onerf_render_multi_ext& x, void* stream,
+                         const SetMapsOut* sets) {
   const onerf_render_multi_maps& c = a->coarse;
   if (a->n_rays == 0) return ONERF_OK;
+  const bool sets_c = sets && any_set_map(sets->coarse), sets_f = sets && any_set_map(sets->fine);
   const int S = a->n_samples, SF = a->n_samples + a->n_importance, N = a->n_rays, NO = a->n_obj;
   const MultiWs w = multi_ws_layout(reinterpret_cast<char*>(a->workspace), N, NO, S, a->n_importance);
   int rc;
@@ -447,8 +457,12 @@ static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const
   rc = multi_fields(ctx, a, a->packed_coarse, w.z_all, S, w, stream);
   if (rc != ONERF_OK) return rc;
   rc = onerf_composite_multi_noise_ws(ctx, w.z_all, w.field_all, N, NO, S, a->white_back, x.noise_std, x.noise_coarse, a->seed,
-                                      0, c.z_vals, c.weights, c.obj_ids, a->n_importance > 0 ? w.w_unsorted : nullptr,
-                                      c.opacity, c.rgb, c.depth, w.sort, w.sort_bytes, stream);
+                                      0, c.z_vals, c.weights, c.obj_ids,
+                                      (a->n_importance > 0 || sets_c) ? w.w_unsorted : nullptr, c.opacity, c.rgb, c.depth,
+                                      w.sort, w.sort_bytes, stream);
+  if (rc == ONERF_OK && sets_c)
+    rc = onerf_launch_set_maps(ctx, w.z_all, w.field_all, w.w_unsorted, N, NO, S, sets->coarse.opacity, sets->coarse.depth,
+                               sets->coarse.rgb, (cudaStream_t)stream);
   if (rc != ONERF_OK || a->n_importance == 0) return rc;
   const int det = a->perturb == 0.0f ? 1 : 0;
   for (int i = 0; i < NO; ++i) {
@@ -461,9 +475,12 @@ static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const
   }
   rc = multi_fields(ctx, a, a->packed_fine, w.z_fine, SF, w, stream);
   if (rc != ONERF_OK) return rc;
-  return onerf_composite_multi_noise_ws(ctx, w.z_fine, w.field_all, N, NO, SF, a->white_back, x.noise_std, x.noise_fine,
-                                        a->seed, 1, a->fine.z_vals, a->fine.weights, nullptr, nullptr, a->fine.opacity,
-                                        a->fine.rgb, a->fine.depth, w.sort, w.sort_bytes, stream);
+  rc = onerf_composite_multi_noise_ws(ctx, w.z_fine, w.field_all, N, NO, SF, a->white_back, x.noise_std, x.noise_fine,
+                                      a->seed, 1, a->fine.z_vals, a->fine.weights, nullptr, sets_f ? sets->w_fine : nullptr,
+                                      a->fine.opacity, a->fine.rgb, a->fine.depth, w.sort, w.sort_bytes, stream);
+  if (rc != ONERF_OK || !sets_f) return rc;
+  return onerf_launch_set_maps(ctx, w.z_fine, w.field_all, sets->w_fine, N, NO, SF, sets->fine.opacity, sets->fine.depth,
+                               sets->fine.rgb, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -477,6 +494,8 @@ struct EditWs {
   void* multi;                            // workspace of multi_forward for one chunk
   size_t multi_bytes;
   size_t total;
+  float* w_fine;                          // onerf_render_edit_frame_sets: the fine pass's weights in set order (SetMapsOut)
+  size_t total_sets;
 };
 
 static EditWs edit_ws_layout(char* base, int chunk, int n_obj, int n_samples, int n_importance) {
@@ -494,6 +513,8 @@ static EditWs edit_ws_layout(char* base, int chunk, int n_obj, int n_samples, in
   w.multi = base + off;
   off += align256(w.multi_bytes);
   w.total = off;
+  w.w_fine = take(no * nf * (n_samples + n_importance));   // past everything onerf_render_edit_frame uses; 0 bytes without
+  w.total_sets = off;                                       // a fine pass
   return w;
 }
 
@@ -516,20 +537,33 @@ extern "C" size_t onerf_render_edit_workspace_bytes(int chunk_rays, int n_obj, i
   return edit_ws_layout(nullptr, chunk_rays, n_obj, n_samples, n_importance).total;
 }
 
-extern "C" int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_args* a, void* stream) {
-  ONERF_CHECK_ARG(ctx && a && a->sets_host, "null argument");
-  ONERF_CHECK_ARG(a->n_obj >= 1, "bad shape");
-  ONERF_CHECK_ARG(a->H > 0 && a->W > 0 && a->focal > 0, "bad camera");
+extern "C" size_t onerf_render_edit_sets_workspace_bytes(int chunk_rays, int n_obj, int n_samples, int n_importance) {
+  if (onerf_render_edit_workspace_bytes(chunk_rays, n_obj, n_samples, n_importance) == 0) return 0;
+  return edit_ws_layout(nullptr, chunk_rays, n_obj, n_samples, n_importance).total_sets;
+}
+
+// rows [r0, r0 + chunk) of tile-sized per-set maps (n_obj columns), NULL where the caller's array is NULL
+static onerf_set_maps chunk_set_maps(const onerf_set_maps& out, int64_t r0, int64_t n_obj) {
+  auto at = [&](float* o, int64_t width) { return o ? o + r0 * width : nullptr; };
+  return onerf_set_maps{at(out.opacity, n_obj), at(out.depth, n_obj), at(out.rgb, n_obj * 3)};
+}
+
+// onerf_render_edit_frame(_sets), refusals reported under the entry `fn`
+static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_edit_args* a, const onerf_set_maps* sets_c,
+                             const onerf_set_maps* sets_f, void* stream) {
+  FN_CHECK_ARG(ctx && a && a->sets_host, "null argument");
+  FN_CHECK_ARG(a->n_obj >= 1, "bad shape");
+  FN_CHECK_ARG(a->H > 0 && a->W > 0 && a->focal > 0, "bad camera");
   const int64_t n_tile = a->pixel_end - a->pixel_begin;
-  ONERF_CHECK_ARG(a->pixel_begin >= 0 && n_tile >= 0 && a->pixel_end <= (int64_t)a->H * a->W, "tile outside the frame");
-  ONERF_CHECK_ARG(a->chunk_rays >= 1, "chunk_rays < 1");
-  ONERF_CHECK_ARG(a->scale_factor > 0, "scale_factor must be positive");
+  FN_CHECK_ARG(a->pixel_begin >= 0 && n_tile >= 0 && a->pixel_end <= (int64_t)a->H * a->W, "tile outside the frame");
+  FN_CHECK_ARG(a->chunk_rays >= 1, "chunk_rays < 1");
+  FN_CHECK_ARG(a->scale_factor > 0, "scale_factor must be positive");
   const int NO = a->n_obj;
   std::vector<int> ids(NO);
   for (int i = 0; i < NO; ++i) {
     const onerf_edit_set& s = a->sets_host[i];
-    ONERF_CHECK_ARG(s.obj_id == 0 || s.box, "an object set needs its box");
-    ONERF_CHECK_ARG(s.obj_id != 0 || !s.box, "the scene set takes no box");
+    FN_CHECK_ARG(s.obj_id == 0 || s.box, "an object set needs its box");
+    FN_CHECK_ARG(s.obj_id != 0 || !s.box, "the scene set takes no box");
     ids[i] = s.obj_id;
   }
   const int chunk = a->chunk_rays;
@@ -544,12 +578,21 @@ extern "C" int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_a
   m.code_table = a->code_table; m.n_codes = a->n_codes;
   m.precision = a->precision; m.use_disp = a->use_disp; m.perturb = 0.0f; m.seed = 0; m.white_back = a->white_back;
   m.boxes = a->boxes; m.n_boxes = a->n_boxes;
-  int rc = check_multi_args(__func__, &m, false);
+  int rc = check_multi_args(fn, &m, false);
   if (rc != ONERF_OK) return rc;
-  const size_t need = onerf_render_edit_workspace_bytes(chunk, NO, a->n_samples, a->n_importance);
-  ONERF_CHECK_ARG(a->workspace && (reinterpret_cast<uintptr_t>(a->workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
+  const onerf_set_maps none = {nullptr, nullptr, nullptr};
+  const onerf_set_maps& sc = sets_c ? *sets_c : none;
+  const onerf_set_maps& sf = sets_f ? *sets_f : none;
+  const bool with_sets = any_set_map(sc) || any_set_map(sf);
+  FN_CHECK_ARG(!any_set_map(sf) || a->n_importance > 0, "fine set maps without a fine pass");
+  for (const onerf_set_maps* p : {&sc, &sf})
+    FN_CHECK_ARG(onerf_aligned4(p->opacity) && onerf_aligned4(p->depth) && onerf_aligned4(p->rgb),
+                 "set maps must be 4-byte aligned");
+  const size_t need = with_sets ? onerf_render_edit_sets_workspace_bytes(chunk, NO, a->n_samples, a->n_importance)
+                                : onerf_render_edit_workspace_bytes(chunk, NO, a->n_samples, a->n_importance);
+  FN_CHECK_ARG(a->workspace && (reinterpret_cast<uintptr_t>(a->workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
   if (a->workspace_bytes < need) {
-    onerf_set_error("onerf_render_edit_frame: workspace too small (%zu < %zu)", a->workspace_bytes, need);
+    onerf_set_error("%s: workspace too small (%zu < %zu)", fn, a->workspace_bytes, need);
     return ONERF_ERR_WORKSPACE;
   }
   const EditWs w = edit_ws_layout(reinterpret_cast<char*>(a->workspace), chunk, NO, a->n_samples, a->n_importance);
@@ -570,10 +613,22 @@ extern "C" int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_a
     m.n_rays = n;
     m.coarse = chunk_maps(a->coarse, w.coarse, r0, TC);
     if (a->n_importance > 0) m.fine = chunk_maps(a->fine, w.fine, r0, TF);
-    rc = multi_forward(ctx, &m, no_ext, stream);
+    const SetMapsOut so = {chunk_set_maps(sc, r0, NO), chunk_set_maps(sf, r0, NO), w.w_fine};
+    rc = multi_forward(ctx, &m, no_ext, stream, with_sets ? &so : nullptr);
     if (rc != ONERF_OK) return rc;
   }
   return ONERF_OK;
+}
+#undef FN_CHECK_ARG
+#undef FN_UNSUPPORTED
+
+extern "C" int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_args* a, void* stream) {
+  return render_edit_frame(__func__, ctx, a, nullptr, nullptr, stream);
+}
+
+extern "C" int onerf_render_edit_frame_sets(onerf_ctx* ctx, const onerf_render_edit_args* a, const onerf_set_maps* coarse,
+                                            const onerf_set_maps* fine, void* stream) {
+  return render_edit_frame(__func__, ctx, a, coarse, fine, stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -26,6 +26,12 @@ int onerf_launch_camera_rays(onerf_ctx* ctx, int H, int W, float focal, const fl
                              double scale_factor, double near, double far, int64_t p0, int64_t n, float* rays_out,
                              uint8_t* hit_out, cudaStream_t stream);
 
+// composite.cu: the per-set maps of one joint compositing from its weights in set order (weights_unsorted of
+// onerf_composite_multi_ws), depths z_all (n_obj,N,S) and fields field_all (n_obj,N,S,4); NULL outputs are skipped.
+int onerf_launch_set_maps(onerf_ctx* ctx, const float* z_all, const float* field_all, const float* weights_unsorted,
+                          int n_rays, int n_obj, int n_samples, float* opacity, float* depth, float* rgb,
+                          cudaStream_t stream);
+
 #define ONERF_CHECK_ARG(cond, msg)                       \
   do {                                                   \
     if (!(cond)) {                                       \

@@ -370,7 +370,63 @@ merge_composite_kernel(const float4* __restrict__ field_all, int n_rays, int n_o
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Per-set maps of a joint compositing: for ray r and set i, the sums over set i's own samples of w, w z and w rgb, read in
+// sample order from the weights scattered back to the sets (weights_unsorted, [obj][ray][s]) next to the set's depths
+// and fields.  One warp per (ray, set): lane l sums samples l, l + 32, ... then warp_sum, an order fixed by S alone, so
+// the maps do not depend on the sort path, the chunking or the tiling.  A zero weight adds nothing: a culled or muted
+// sample's field value never reaches the maps (0 * inf would be NaN).  Outputs (n_rays, n_obj) / (n_rays, n_obj, 3),
+// each skipped when NULL; no white background.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128)
+set_maps_kernel(const float* __restrict__ z_all, const float4* __restrict__ field_all, const float* __restrict__ w_all,
+                int n_rays, int n_obj, int S, float* __restrict__ opacity, float* __restrict__ depth,
+                float* __restrict__ rgb) {
+  const int warps_per_block = blockDim.x >> 5;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t n_lists = (int64_t)n_rays * n_obj;
+  for (int64_t l = (int64_t)blockIdx.x * warps_per_block + warp; l < n_lists; l += (int64_t)gridDim.x * warps_per_block) {
+    const int r = (int)(l / n_obj), obj = (int)(l % n_obj);
+    const int64_t base = ((int64_t)obj * n_rays + r) * S;
+    Acc acc = {0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int s = lane; s < S; s += 32) {
+      const float w = __ldg(w_all + base + s);
+      if (w != 0.0f) {
+        const float4 f = __ldg(field_all + base + s);
+        acc.opacity += w;
+        acc.r += w * f.x;
+        acc.g += w * f.y;
+        acc.b += w * f.z;
+        acc.depth += w * __ldg(z_all + base + s);
+      }
+    }
+    acc = warp_sum(acc);
+    if (lane == 0) {
+      if (opacity) opacity[l] = acc.opacity;
+      if (depth) depth[l] = acc.depth;
+      if (rgb) {
+        rgb[l * 3 + 0] = acc.r;
+        rgb[l * 3 + 1] = acc.g;
+        rgb[l * 3 + 2] = acc.b;
+      }
+    }
+  }
+}
+
 }  // namespace
+
+int onerf_launch_set_maps(onerf_ctx* ctx, const float* z_all, const float* field_all, const float* weights_unsorted,
+                          int n_rays, int n_obj, int n_samples, float* opacity, float* depth, float* rgb,
+                          cudaStream_t stream) {
+  if (n_rays == 0 || !(opacity || depth || rgb)) return ONERF_OK;
+  const int warps = 4;
+  const int64_t lists = (int64_t)n_rays * n_obj;
+  const int blocks = (int)std::min((lists + warps - 1) / warps, (int64_t)ctx->num_sms * 16);
+  set_maps_kernel<<<blocks, warps * 32, 0, stream>>>(z_all, reinterpret_cast<const float4*>(field_all), weights_unsorted,
+                                                     n_rays, n_obj, n_samples, opacity, depth, rgb);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
 
 extern "C" int onerf_composite(onerf_ctx* ctx, const onerf_composite_args* a, void* stream) {
   return onerf_launch_composite(ctx, a, nullptr, (cudaStream_t)stream);

@@ -6,6 +6,9 @@
         and the maps are written straight into frame-sized buffers (onerf_render_edit_frame, include/onerf_ext.h).
     render_tile(..., pixel_begin, pixel_end, ...)
         The same for a contiguous range of pixels only.
+    keys= may also name the per-set maps of set_keys(N_importance): opacity_sets_{typ}, depth_sets_{typ} (H*W, n_obj)
+        and rgb_sets_{typ} (H*W, n_obj, 3), how much of each pixel each ray set shows in pass typ
+        (onerf_render_edit_frame_sets).  They are never part of the default result.
     render_edit(renderer, ...), render_origin(renderer, ...)
         EditableRenderer.render_edit / render_origin (render_tools/editable_renderer.py:183-294) for an instance of the
         reference's class: the same poses, duplicate counting, boxes and side effects, then one render_frame call.
@@ -32,6 +35,7 @@ from .ray_utils import _box_host, _c2w_host
 from .rendering import _grid_of, _is_voxel
 
 _MAPS = ("weights", "opacity", "z_vals", "rgb", "depth", "obj_ids")
+_SET_MAPS = ("opacity_sets", "depth_sets", "rgb_sets")
 _workspaces: Dict[Any, torch.Tensor] = {}
 
 
@@ -41,6 +45,14 @@ def result_keys(N_importance: int):
     if N_importance > 0:
         keys += [f"{k}_fine" for k in _MAPS[:-1]]
     return keys
+
+
+def set_keys(N_importance: int):
+    """The per-set map keys render_frame computes on request (keys=), for each pass: for pixel r and set position i,
+    the sums over set i's samples of the pass's weights w, w * z and w * rgb (no white background).  Summed over the sets
+    they give opacity_{typ}, depth_{typ} and rgb_{typ} without the white background."""
+    typs = ("coarse", "fine") if N_importance > 0 else ("coarse",)
+    return [f"{k}_{typ}" for typ in typs for k in _SET_MAPS]
 
 
 def _workspace(nbytes: int, dev: torch.device) -> torch.Tensor:
@@ -84,6 +96,7 @@ def render_tile(models: Dict[str, Any], embeddings: Dict[str, Any], code_library
     results, row for row those of the whole frame."""
     all_keys = result_keys(N_importance)
     keys = all_keys if keys is None else list(keys)
+    all_keys = all_keys + set_keys(N_importance)
     unknown = [k for k in keys if k not in all_keys]
     if unknown:
         raise KeyError(f"render_frame: no such result key {unknown} (N_importance = {N_importance})")
@@ -131,9 +144,21 @@ def render_tile(models: Dict[str, Any], embeddings: Dict[str, Any], code_library
                 w = widths.get(k, n_obj * s)
                 out[key] = torch.empty((n, w) if w != 1 else (n,), dtype=torch.float32, device=dev)
                 setattr(getattr(a, typ), k, out[key].data_ptr())
-    ws = _workspace(_lib.load().onerf_render_edit_workspace_bytes(a.chunk_rays, n_obj, a.n_samples, a.n_importance), dev)
+    set_maps = {"coarse": _lib.SetMaps(), "fine": _lib.SetMaps()}
+    for key in set_keys(N_importance):
+        if key in keys:
+            k, typ = key.rsplit("_", 1)
+            out[key] = torch.empty((n, n_obj, 3) if k == "rgb_sets" else (n, n_obj), dtype=torch.float32, device=dev)
+            setattr(set_maps[typ], k.split("_")[0], out[key].data_ptr())
+    lib = _lib.load()
+    with_sets = any(k in keys for k in set_keys(N_importance))
+    ws_bytes = lib.onerf_render_edit_sets_workspace_bytes if with_sets else lib.onerf_render_edit_workspace_bytes
+    ws = _workspace(ws_bytes(a.chunk_rays, n_obj, a.n_samples, a.n_importance), dev)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-    _lib.call("onerf_render_edit_frame", dev, C.byref(a))
+    if with_sets:
+        _lib.call("onerf_render_edit_frame_sets", dev, C.byref(a), C.byref(set_maps["coarse"]), C.byref(set_maps["fine"]))
+    else:
+        _lib.call("onerf_render_edit_frame", dev, C.byref(a))
     return {k: out[k] for k in all_keys if k in out}
 
 
@@ -209,7 +234,8 @@ def render_origin(renderer, h: int, w: int, camera_pose_Twc, fovx_deg: float = 7
 
 def install(editable_renderer_cls, keys=None, group=None):
     """Make `editable_renderer_cls` (the reference's EditableRenderer) render through render_edit / render_origin above.
-    keys: what render_edit computes and returns (None: every key); group: the process group whose ranks share each frame
+    keys: what render_edit computes and returns (None: every key of the reference's dict; the per-set maps of set_keys
+    only when named here); group: the process group whose ranks share each frame
     (None: one process renders it)."""
     def _render_edit(self, h, w, camera_pose_Twc, fovx_deg=70, show_progress=True, render_bg_only=False,
                      render_obj_only=False, white_back=False):
