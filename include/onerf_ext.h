@@ -209,6 +209,52 @@ int onerf_render_edit_frame_sets(onerf_ctx* ctx, const onerf_render_edit_args* a
                                  const onerf_set_maps* fine, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * onerf_render_edit_frame_sets with objects from other trained scenes.  The frame's BASE scene is the one args describes
+ * (grid, packed weights, code_table, scale_factor s_base).  Set i with set_scene_host[i] = j >= 0 comes from SOURCE scene
+ * scenes_host[j] instead, with its own voxel grid, packed weights (same architecture and precision as the frame), code
+ * table and scale_factor s_src, and is evaluated exactly as a native object set of that scene:
+ *   - its rays from its Toc, whose translation is at the source's NeRF scale (divided by s_src), and its box slab test
+ *     un-scaled with s_src;
+ *   - its coarse depths, fields (its grid, weights and code row), importance sampling and fine depths in the source's
+ *     units, from its own weights.
+ * The joint compositing of each pass then takes, with k = float32(s_src / s_base) computed in double, the set's depths
+ * as z * k (on the base scene's axis) and its densities as sigma / k (each interval keeps its optical depth).  This is
+ * render_rays_multi (multi_rendering.py:160-325) run per set in the set's own units, with volume_rendering_multi given
+ * [z_i * k_i] and [sigma_i / k_i].  Every output is in base-scene units: z_vals, depth and the per-set depth maps.  A
+ * frame whose sets all have k == 1 converts nothing: such a set's outputs are bit-identical to the same set rendered
+ * natively from a base scene with its values.
+ * Source scenes contribute object sets only (obj_id > 0); the removed-object boxes mute the base scene set only.
+ *   scenes_host     n_scenes source scenes (host array; NULL when n_scenes = 0).
+ *   set_scene_host  n_obj ints (host array): -1 = base scene, else an index into scenes_host.  NULL: every set is of
+ *                   the base scene.
+ *   coarse, fine    per-set maps as for onerf_render_edit_frame_sets (NULL: none).
+ *   workspace       >= onerf_render_edit_scenes_workspace_bytes(chunk_rays, n_obj, n_samples, n_importance) bytes when
+ *                   any set comes from a source scene (the sets entry's, plus one (n_obj, chunk, S + K) float buffer for
+ *                   a pass's depths on the base axis), else as onerf_render_edit_frame_sets.
+ * onerf_render_edit_frame_sets (and so onerf_render_edit_frame) is this call with no source scenes.  Refusals before any
+ * launch, besides those of onerf_render_edit_frame_sets (ONERF_ERR_BAD_ARG unless noted): a negative n_scenes or a NULL
+ * scenes_host with n_scenes > 0; in a scene a NULL grid, grid buffer, packed_coarse or code_table, a misaligned grid
+ * table, a NULL packed_fine when n_importance > 0, a scale_factor that is not positive and finite (or whose ratio k is
+ * not a positive finite float); a set scene index outside [-1, n_scenes); an object id outside its source scene's code
+ * table; a source scene set with obj_id 0 (ONERF_ERR_UNSUPPORTED).  Kernels and device copies only, no host read:
+ * CUDA-graph capturable.  Each pass with a set of k != 1 adds one device copy of its depths and one rescale launch per
+ * such set.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct onerf_edit_scene {
+  const onerf_grid* grid;
+  const void* packed_coarse;
+  const void* packed_fine;            /* required iff n_importance > 0 */
+  const float* code_table;            /* (n_codes,64) */
+  int n_codes;
+  double scale_factor;
+} onerf_edit_scene;
+
+size_t onerf_render_edit_scenes_workspace_bytes(int chunk_rays, int n_obj, int n_samples, int n_importance);
+int onerf_render_edit_frame_scenes(onerf_ctx* ctx, const onerf_render_edit_args* args, const onerf_edit_scene* scenes_host,
+                                   int n_scenes, const int* set_scene_host, const onerf_set_maps* coarse,
+                                   const onerf_set_maps* fine, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Training batches drawn on the device (GenericDataset.__getitem__ through DataLoader(shuffle=True), and under DDP
  * DistributedSampler; datasets/generic_dataset.py:475-490, train.py:121-129).  The dataset's R rays stay in device
  * memory; one launch draws batch `step` of rank `rank` into B-row outputs:

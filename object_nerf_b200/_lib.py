@@ -44,7 +44,8 @@ EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_w
                "onerf_composite_multi_noise_ws", "onerf_composite_multi_noise_merge", "onerf_sample_pdf_merge_clip",
                "onerf_render_multi_fwd_ext", "onerf_field_bwd_workspace_bytes", "onerf_field_bwd", "onerf_bwd_dx_xyz",
                "onerf_encode_bwd_xyz", "onerf_draw_frames", "onerf_draw_frames_dstep",
-               "onerf_render_edit_sets_workspace_bytes", "onerf_render_edit_frame_sets"]
+               "onerf_render_edit_sets_workspace_bytes", "onerf_render_edit_frame_sets",
+               "onerf_render_edit_scenes_workspace_bytes", "onerf_render_edit_frame_scenes"]
 VALIDATE_RECORD_DOUBLES = 18
 PRUNE_SAMPLES = 4096
 PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
@@ -152,6 +153,11 @@ class RenderEditArgs(C.Structure):
 
 class SetMaps(C.Structure):
     _fields_ = [("opacity", _p), ("depth", _p), ("rgb", _p)]
+
+
+class EditScene(C.Structure):
+    _fields_ = [("grid", C.POINTER(Grid)), ("packed_coarse", _p), ("packed_fine", _p), ("code_table", _p),
+                ("n_codes", C.c_int), ("scale_factor", C.c_double)]
 
 
 class RayDataset(C.Structure):
@@ -316,6 +322,10 @@ def load() -> C.CDLL:
         lib.onerf_render_edit_sets_workspace_bytes.argtypes = [C.c_int] * 4
         lib.onerf_render_edit_sets_workspace_bytes.restype = C.c_size_t
         lib.onerf_render_edit_frame_sets.argtypes = [_p, C.POINTER(RenderEditArgs), C.POINTER(SetMaps), C.POINTER(SetMaps), _p]
+        lib.onerf_render_edit_scenes_workspace_bytes.argtypes = [C.c_int] * 4
+        lib.onerf_render_edit_scenes_workspace_bytes.restype = C.c_size_t
+        lib.onerf_render_edit_frame_scenes.argtypes = [_p, C.POINTER(RenderEditArgs), C.POINTER(EditScene), C.c_int,
+                                                       C.POINTER(C.c_int), C.POINTER(SetMaps), C.POINTER(SetMaps), _p]
         lib.onerf_draw_batch.argtypes = [_p, C.POINTER(BatchArgs), _p]
         lib.onerf_draw_batch_dstep.argtypes = [_p, C.POINTER(BatchArgs), _p, _p]
         lib.onerf_draw_frames.argtypes = [_p, C.POINTER(FrameDataset), C.POINTER(BatchArgs), _p]

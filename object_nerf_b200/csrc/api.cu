@@ -306,21 +306,35 @@ extern "C" size_t onerf_render_multi_workspace_bytes(int n_rays, int n_obj, int 
   return multi_ws_layout(nullptr, n_rays, n_obj, n_samples, n_importance).total;
 }
 
+// Where each set of an edited frame comes from (onerf_render_edit_frame_scenes): its scene's grid, weights and code table,
+// and k = float(s_src / s_base), the factor that puts the set's depths on the frame's axis (1 for the base scene).
+struct SetSource {
+  const onerf_grid* grid;
+  const void* packed_coarse;
+  const void* packed_fine;
+  const float* code_table;
+  float k;
+};
+
+// The sets of one pass (pass 0 coarse, 1 fine); with `src`, set i reads its grid, weights and code row from src[i]
+// instead of from `a` and `packed`.
 static int multi_fields(onerf_ctx* ctx, const onerf_render_multi_args* a, const void* packed, const float* z_all, int S,
-                        const MultiWs& w, void* stream) {
+                        const MultiWs& w, void* stream, const SetSource* src = nullptr, int pass = 0) {
   const int N = a->n_rays;
   for (int i = 0; i < a->n_obj; ++i) {
     const int id = a->obj_ids_host[i];
     const float* z = z_all + (size_t)i * N * S;
     float* out = w.field_all + (size_t)i * N * S * 4;
+    const float* code_table = src ? src[i].code_table : a->code_table;
     onerf_field_args f;
     memset(&f, 0, sizeof(f));
     f.rays = a->rays_list_host[i];
     f.z = z;
     f.z_stride = S;
-    f.code_row = id > 0 ? a->code_table + (size_t)id * ONERF_NCODE : nullptr;
+    f.code_row = id > 0 ? code_table + (size_t)id * ONERF_NCODE : nullptr;
     f.n_rays = N; f.n_samples = S;
-    f.grid = a->grid; f.packed = packed;
+    f.grid = src ? src[i].grid : a->grid;
+    f.packed = src ? (pass ? src[i].packed_fine : src[i].packed_coarse) : packed;
     f.want_scene = id > 0 ? 0 : 1; f.want_object = id > 0 ? 1 : 0;
     f.precision = a->precision;
     f.mute_zero_rays = 1;
@@ -360,7 +374,9 @@ static int multi_fields(onerf_ctx* ctx, const onerf_render_multi_args* a, const 
     if (cond) { onerf_set_error("%s: unsupported: %s", fn, msg); return ONERF_ERR_UNSUPPORTED; }  \
   } while (0)
 
-static int check_multi_args(const char* fn, const onerf_render_multi_args* a, bool with_rays_and_maps) {
+// set_scene: NULL, or per set -1 (base scene) or the index of its source scene, whose ids the caller checks.
+static int check_multi_args(const char* fn, const onerf_render_multi_args* a, bool with_rays_and_maps,
+                            const int* set_scene = nullptr) {
   FN_CHECK_ARG((a->rays_list_host || !with_rays_and_maps) && a->obj_ids_host && a->packed_coarse && a->grid && a->code_table,
                "null input");
   FN_CHECK_ARG(a->n_rays >= 0 && a->n_obj >= 1 && a->n_samples >= 2 && a->n_importance >= 0, "bad shape");
@@ -370,7 +386,8 @@ static int check_multi_args(const char* fn, const onerf_render_multi_args* a, bo
   FN_CHECK_ARG(a->n_boxes == 0 || a->boxes, "n_boxes > 0 with null boxes");
   for (int i = 0; i < a->n_obj; ++i) {
     if (with_rays_and_maps) FN_CHECK_ARG(a->rays_list_host[i], "null ray set");
-    FN_CHECK_ARG(a->obj_ids_host[i] >= 0 && a->obj_ids_host[i] < a->n_codes, "object id outside the code table");
+    if (!set_scene || set_scene[i] < 0)
+      FN_CHECK_ARG(a->obj_ids_host[i] >= 0 && a->obj_ids_host[i] < a->n_codes, "object id outside the code table");
   }
   if (!with_rays_and_maps) return ONERF_OK;
   const onerf_render_multi_maps& c = a->coarse;
@@ -404,8 +421,17 @@ struct SetMapsOut {
 
 static bool any_set_map(const onerf_set_maps& m) { return m.opacity || m.depth || m.rgb; }
 
+// The sets' sources of an edited frame with source scenes (multi_forward): per set its SetSource; with `rescale` (some
+// set has k != 1) each pass composites a frame-axis copy of its depths, z_frame ((n_obj, N, S + K), the edit
+// workspace's extension).
+struct FrameScenes {
+  const SetSource* set;
+  bool rescale;
+  float* z_frame;
+};
+
 static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const onerf_render_multi_ext& x, void* stream,
-                         const SetMapsOut* sets = nullptr);
+                         const SetMapsOut* sets = nullptr, const FrameScenes* scenes = nullptr);
 
 static int render_multi_fwd(const char* fn, onerf_ctx* ctx, const onerf_render_multi_args* a,
                             const onerf_render_multi_ext* ext, void* stream) {
@@ -439,11 +465,28 @@ extern "C" int onerf_render_multi_fwd_ext(onerf_ctx* ctx, const onerf_render_mul
   return render_multi_fwd(__func__, ctx, a, ext, stream);
 }
 
+// One pass's depths z_all (n_obj, N, S) on the frame's axis, in fs.z_frame: copied, then each set with k != 1 rewritten
+// as z k, with its sigmas in field_all divided by k.  z_all keeps the sets' own units for their importance sampling.
+static int to_frame_axis(onerf_ctx* ctx, const FrameScenes& fs, int n_obj, const float* z_all, float* field_all, int N,
+                         int S, void* stream) {
+  const size_t per_set = (size_t)N * S;
+  ONERF_CUDA(cudaMemcpyAsync(fs.z_frame, z_all, n_obj * per_set * sizeof(float), cudaMemcpyDeviceToDevice,
+                             (cudaStream_t)stream));
+  for (int i = 0; i < n_obj; ++i) {
+    if (fs.set[i].k == 1.0f) continue;
+    const int rc = onerf_launch_rescale_set(ctx, z_all + i * per_set, fs.z_frame + i * per_set, field_all + i * per_set * 4,
+                                            (int64_t)per_set, fs.set[i].k, (cudaStream_t)stream);
+    if (rc != ONERF_OK) return rc;
+  }
+  return ONERF_OK;
+}
+
 // The forward of onerf_render_multi_fwd_ext on checked arguments: n_rays rays of every set in a->rays_list_host, maps
 // written to a->coarse / a->fine, scratch in a->workspace; with `sets`, each pass's per-set maps too, from its weights
-// in set order while the pass's depths and fields are still in the workspace.
+// in set order while the pass's depths and fields are still in the workspace; with `scenes`, each set's field from its
+// own scene, composited on the frame's depth axis.
 static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const onerf_render_multi_ext& x, void* stream,
-                         const SetMapsOut* sets) {
+                         const SetMapsOut* sets, const FrameScenes* scenes) {
   const onerf_render_multi_maps& c = a->coarse;
   if (a->n_rays == 0) return ONERF_OK;
   const bool sets_c = sets && any_set_map(sets->coarse), sets_f = sets && any_set_map(sets->fine);
@@ -454,14 +497,21 @@ static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const
     rc = onerf_sample_coarse(ctx, a->rays_list_host[i], N, S, a->use_disp, 0.0f, nullptr, 0, w.z_all + (size_t)i * N * S, stream);
     if (rc != ONERF_OK) return rc;
   }
-  rc = multi_fields(ctx, a, a->packed_coarse, w.z_all, S, w, stream);
+  const SetSource* src = scenes ? scenes->set : nullptr;
+  rc = multi_fields(ctx, a, a->packed_coarse, w.z_all, S, w, stream, src, 0);
   if (rc != ONERF_OK) return rc;
-  rc = onerf_composite_multi_noise_ws(ctx, w.z_all, w.field_all, N, NO, S, a->white_back, x.noise_std, x.noise_coarse, a->seed,
+  const float* z_c = w.z_all;   // the depths the compositing and the set maps see
+  if (scenes && scenes->rescale) {
+    rc = to_frame_axis(ctx, *scenes, NO, w.z_all, w.field_all, N, S, stream);
+    if (rc != ONERF_OK) return rc;
+    z_c = scenes->z_frame;
+  }
+  rc = onerf_composite_multi_noise_ws(ctx, z_c, w.field_all, N, NO, S, a->white_back, x.noise_std, x.noise_coarse, a->seed,
                                       0, c.z_vals, c.weights, c.obj_ids,
                                       (a->n_importance > 0 || sets_c) ? w.w_unsorted : nullptr, c.opacity, c.rgb, c.depth,
                                       w.sort, w.sort_bytes, stream);
   if (rc == ONERF_OK && sets_c)
-    rc = onerf_launch_set_maps(ctx, w.z_all, w.field_all, w.w_unsorted, N, NO, S, sets->coarse.opacity, sets->coarse.depth,
+    rc = onerf_launch_set_maps(ctx, z_c, w.field_all, w.w_unsorted, N, NO, S, sets->coarse.opacity, sets->coarse.depth,
                                sets->coarse.rgb, (cudaStream_t)stream);
   if (rc != ONERF_OK || a->n_importance == 0) return rc;
   const int det = a->perturb == 0.0f ? 1 : 0;
@@ -473,13 +523,19 @@ static int multi_forward(onerf_ctx* ctx, const onerf_render_multi_args* a, const
                                        w.z_fine + (size_t)i * N * SF, stream, clip);
     if (rc != ONERF_OK) return rc;
   }
-  rc = multi_fields(ctx, a, a->packed_fine, w.z_fine, SF, w, stream);
+  rc = multi_fields(ctx, a, a->packed_fine, w.z_fine, SF, w, stream, src, 1);
   if (rc != ONERF_OK) return rc;
-  rc = onerf_composite_multi_noise_ws(ctx, w.z_fine, w.field_all, N, NO, SF, a->white_back, x.noise_std, x.noise_fine,
+  const float* z_f = w.z_fine;
+  if (scenes && scenes->rescale) {
+    rc = to_frame_axis(ctx, *scenes, NO, w.z_fine, w.field_all, N, SF, stream);
+    if (rc != ONERF_OK) return rc;
+    z_f = scenes->z_frame;
+  }
+  rc = onerf_composite_multi_noise_ws(ctx, z_f, w.field_all, N, NO, SF, a->white_back, x.noise_std, x.noise_fine,
                                       a->seed, 1, a->fine.z_vals, a->fine.weights, nullptr, sets_f ? sets->w_fine : nullptr,
                                       a->fine.opacity, a->fine.rgb, a->fine.depth, w.sort, w.sort_bytes, stream);
   if (rc != ONERF_OK || !sets_f) return rc;
-  return onerf_launch_set_maps(ctx, w.z_fine, w.field_all, sets->w_fine, N, NO, SF, sets->fine.opacity, sets->fine.depth,
+  return onerf_launch_set_maps(ctx, z_f, w.field_all, sets->w_fine, N, NO, SF, sets->fine.opacity, sets->fine.depth,
                                sets->fine.rgb, (cudaStream_t)stream);
 }
 
@@ -496,6 +552,8 @@ struct EditWs {
   size_t total;
   float* w_fine;                          // onerf_render_edit_frame_sets: the fine pass's weights in set order (SetMapsOut)
   size_t total_sets;
+  float* z_frame;                         // onerf_render_edit_frame_scenes: a pass's depths on the frame's axis (FrameScenes)
+  size_t total_scenes;
 };
 
 static EditWs edit_ws_layout(char* base, int chunk, int n_obj, int n_samples, int n_importance) {
@@ -515,6 +573,8 @@ static EditWs edit_ws_layout(char* base, int chunk, int n_obj, int n_samples, in
   w.total = off;
   w.w_fine = take(no * nf * (n_samples + n_importance));   // past everything onerf_render_edit_frame uses; 0 bytes without
   w.total_sets = off;                                       // a fine pass
+  w.z_frame = take(no * n * (n_samples + n_importance));
+  w.total_scenes = off;
   return w;
 }
 
@@ -542,15 +602,21 @@ extern "C" size_t onerf_render_edit_sets_workspace_bytes(int chunk_rays, int n_o
   return edit_ws_layout(nullptr, chunk_rays, n_obj, n_samples, n_importance).total_sets;
 }
 
+extern "C" size_t onerf_render_edit_scenes_workspace_bytes(int chunk_rays, int n_obj, int n_samples, int n_importance) {
+  if (onerf_render_edit_workspace_bytes(chunk_rays, n_obj, n_samples, n_importance) == 0) return 0;
+  return edit_ws_layout(nullptr, chunk_rays, n_obj, n_samples, n_importance).total_scenes;
+}
+
 // rows [r0, r0 + chunk) of tile-sized per-set maps (n_obj columns), NULL where the caller's array is NULL
 static onerf_set_maps chunk_set_maps(const onerf_set_maps& out, int64_t r0, int64_t n_obj) {
   auto at = [&](float* o, int64_t width) { return o ? o + r0 * width : nullptr; };
   return onerf_set_maps{at(out.opacity, n_obj), at(out.depth, n_obj), at(out.rgb, n_obj * 3)};
 }
 
-// onerf_render_edit_frame(_sets), refusals reported under the entry `fn`
+// onerf_render_edit_frame(_sets, _scenes), refusals reported under the entry `fn`
 static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_edit_args* a, const onerf_set_maps* sets_c,
-                             const onerf_set_maps* sets_f, void* stream) {
+                             const onerf_set_maps* sets_f, const onerf_edit_scene* scenes, int n_scenes,
+                             const int* set_scene, void* stream) {
   FN_CHECK_ARG(ctx && a && a->sets_host, "null argument");
   FN_CHECK_ARG(a->n_obj >= 1, "bad shape");
   FN_CHECK_ARG(a->H > 0 && a->W > 0 && a->focal > 0, "bad camera");
@@ -558,10 +624,30 @@ static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_
   FN_CHECK_ARG(a->pixel_begin >= 0 && n_tile >= 0 && a->pixel_end <= (int64_t)a->H * a->W, "tile outside the frame");
   FN_CHECK_ARG(a->chunk_rays >= 1, "chunk_rays < 1");
   FN_CHECK_ARG(a->scale_factor > 0, "scale_factor must be positive");
+  FN_CHECK_ARG(n_scenes >= 0 && (n_scenes == 0 || scenes), "null or negative source scene list");
+  for (int j = 0; j < n_scenes; ++j) {
+    const onerf_edit_scene& sc = scenes[j];
+    FN_CHECK_ARG(sc.grid && sc.packed_coarse && sc.code_table, "a source scene needs its grid, packed_coarse and code_table");
+    FN_CHECK_ARG(sc.grid->table && sc.grid->idx_map && sc.grid->voxel_offset && sc.grid->voxel_size &&
+                     sc.grid->voxel_shape && onerf_aligned16(sc.grid->table),
+                 "null / misaligned grid buffer in a source scene");
+    FN_CHECK_ARG(a->n_importance == 0 || sc.packed_fine, "n_importance > 0 needs a source scene's packed_fine");
+    const double k = sc.scale_factor / a->scale_factor;
+    FN_CHECK_ARG(sc.scale_factor > 0 && sc.scale_factor <= DBL_MAX && (float)k > 0 && (float)k <= FLT_MAX,
+                 "a source scene's scale_factor must be positive and finite");
+  }
   const int NO = a->n_obj;
   std::vector<int> ids(NO);
+  bool any_source = false;
   for (int i = 0; i < NO; ++i) {
     const onerf_edit_set& s = a->sets_host[i];
+    const int j = set_scene ? set_scene[i] : -1;
+    FN_CHECK_ARG(j >= -1 && j < n_scenes, "set scene index outside [-1, n_scenes)");
+    if (j >= 0) {
+      FN_UNSUPPORTED(s.obj_id == 0, "a set of a source scene must be an object set (obj_id > 0)");
+      FN_CHECK_ARG(s.obj_id > 0 && s.obj_id < scenes[j].n_codes, "object id outside its source scene's code table");
+      any_source = true;
+    }
     FN_CHECK_ARG(s.obj_id == 0 || s.box, "an object set needs its box");
     FN_CHECK_ARG(s.obj_id != 0 || !s.box, "the scene set takes no box");
     ids[i] = s.obj_id;
@@ -578,7 +664,7 @@ static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_
   m.code_table = a->code_table; m.n_codes = a->n_codes;
   m.precision = a->precision; m.use_disp = a->use_disp; m.perturb = 0.0f; m.seed = 0; m.white_back = a->white_back;
   m.boxes = a->boxes; m.n_boxes = a->n_boxes;
-  int rc = check_multi_args(fn, &m, false);
+  int rc = check_multi_args(fn, &m, false, set_scene);
   if (rc != ONERF_OK) return rc;
   const onerf_set_maps none = {nullptr, nullptr, nullptr};
   const onerf_set_maps& sc = sets_c ? *sets_c : none;
@@ -588,14 +674,31 @@ static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_
   for (const onerf_set_maps* p : {&sc, &sf})
     FN_CHECK_ARG(onerf_aligned4(p->opacity) && onerf_aligned4(p->depth) && onerf_aligned4(p->rgb),
                  "set maps must be 4-byte aligned");
-  const size_t need = with_sets ? onerf_render_edit_sets_workspace_bytes(chunk, NO, a->n_samples, a->n_importance)
-                                : onerf_render_edit_workspace_bytes(chunk, NO, a->n_samples, a->n_importance);
+  const size_t need = any_source ? onerf_render_edit_scenes_workspace_bytes(chunk, NO, a->n_samples, a->n_importance)
+                     : with_sets  ? onerf_render_edit_sets_workspace_bytes(chunk, NO, a->n_samples, a->n_importance)
+                                  : onerf_render_edit_workspace_bytes(chunk, NO, a->n_samples, a->n_importance);
   FN_CHECK_ARG(a->workspace && (reinterpret_cast<uintptr_t>(a->workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
   if (a->workspace_bytes < need) {
     onerf_set_error("%s: workspace too small (%zu < %zu)", fn, a->workspace_bytes, need);
     return ONERF_ERR_WORKSPACE;
   }
   const EditWs w = edit_ws_layout(reinterpret_cast<char*>(a->workspace), chunk, NO, a->n_samples, a->n_importance);
+  // sets of source scenes: every set's source (the base scene's for the others), k in float32 of the double ratio
+  std::vector<SetSource> src;
+  std::vector<double> set_scale(NO, a->scale_factor);
+  FrameScenes fs = {nullptr, false, w.z_frame};
+  if (any_source) {
+    src.resize(NO);
+    for (int i = 0; i < NO; ++i) {
+      const int j = set_scene[i];
+      src[i] = j < 0 ? SetSource{a->grid, a->packed_coarse, a->packed_fine, a->code_table, 1.0f}
+                     : SetSource{scenes[j].grid, scenes[j].packed_coarse, scenes[j].packed_fine, scenes[j].code_table,
+                                 (float)(scenes[j].scale_factor / a->scale_factor)};
+      if (j >= 0) set_scale[i] = scenes[j].scale_factor;
+      fs.rescale = fs.rescale || src[i].k != 1.0f;
+    }
+    fs.set = src.data();
+  }
   std::vector<const float*> rays(NO);
   for (int i = 0; i < NO; ++i) rays[i] = w.rays + (size_t)i * chunk * 8;
   m.rays_list_host = rays.data();
@@ -606,7 +709,7 @@ static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_
     const int n = (int)(n_tile - r0 < chunk ? n_tile - r0 : chunk);
     for (int i = 0; i < NO; ++i) {
       const onerf_edit_set& s = a->sets_host[i];
-      rc = onerf_launch_camera_rays(ctx, a->H, a->W, a->focal, s.Toc, s.box, a->scale_factor, a->near, a->far,
+      rc = onerf_launch_camera_rays(ctx, a->H, a->W, a->focal, s.Toc, s.box, set_scale[i], a->near, a->far,
                                     a->pixel_begin + r0, n, const_cast<float*>(rays[i]), nullptr, (cudaStream_t)stream);
       if (rc != ONERF_OK) return rc;
     }
@@ -614,7 +717,7 @@ static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_
     m.coarse = chunk_maps(a->coarse, w.coarse, r0, TC);
     if (a->n_importance > 0) m.fine = chunk_maps(a->fine, w.fine, r0, TF);
     const SetMapsOut so = {chunk_set_maps(sc, r0, NO), chunk_set_maps(sf, r0, NO), w.w_fine};
-    rc = multi_forward(ctx, &m, no_ext, stream, with_sets ? &so : nullptr);
+    rc = multi_forward(ctx, &m, no_ext, stream, with_sets ? &so : nullptr, any_source ? &fs : nullptr);
     if (rc != ONERF_OK) return rc;
   }
   return ONERF_OK;
@@ -623,12 +726,18 @@ static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_
 #undef FN_UNSUPPORTED
 
 extern "C" int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_args* a, void* stream) {
-  return render_edit_frame(__func__, ctx, a, nullptr, nullptr, stream);
+  return render_edit_frame(__func__, ctx, a, nullptr, nullptr, nullptr, 0, nullptr, stream);
 }
 
 extern "C" int onerf_render_edit_frame_sets(onerf_ctx* ctx, const onerf_render_edit_args* a, const onerf_set_maps* coarse,
                                             const onerf_set_maps* fine, void* stream) {
-  return render_edit_frame(__func__, ctx, a, coarse, fine, stream);
+  return render_edit_frame(__func__, ctx, a, coarse, fine, nullptr, 0, nullptr, stream);
+}
+
+extern "C" int onerf_render_edit_frame_scenes(onerf_ctx* ctx, const onerf_render_edit_args* a,
+                                              const onerf_edit_scene* scenes_host, int n_scenes, const int* set_scene_host,
+                                              const onerf_set_maps* coarse, const onerf_set_maps* fine, void* stream) {
+  return render_edit_frame(__func__, ctx, a, coarse, fine, scenes_host, n_scenes, set_scene_host, stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -32,6 +32,11 @@ int onerf_launch_set_maps(onerf_ctx* ctx, const float* z_all, const float* field
                           int n_rays, int n_obj, int n_samples, float* opacity, float* depth, float* rgb,
                           cudaStream_t stream);
 
+// composite.cu: n samples of one set of a source scene onto the frame's depth axis: z_out = z * k, field sigma /= k in
+// place (field: n float4).
+int onerf_launch_rescale_set(onerf_ctx* ctx, const float* z, float* z_out, float* field, int64_t n, float k,
+                             cudaStream_t stream);
+
 #define ONERF_CHECK_ARG(cond, msg)                       \
   do {                                                   \
     if (!(cond)) {                                       \

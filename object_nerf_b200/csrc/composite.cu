@@ -413,7 +413,30 @@ set_maps_kernel(const float* __restrict__ z_all, const float4* __restrict__ fiel
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// One set of a source scene onto the frame's depth axis (k = s_src / s_base): z_out = z k for the joint compositing and
+// the set maps, and the field's sigma / k in place, so that each interval keeps its optical depth sigma * delta.  z
+// itself stays in the source's units for the set's importance sampling.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+rescale_set_kernel(const float* __restrict__ z, float* __restrict__ z_out, float4* __restrict__ field, int64_t n, float k) {
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+    z_out[e] = z[e] * k;
+    field[e].w = field[e].w / k;
+  }
+}
+
 }  // namespace
+
+int onerf_launch_rescale_set(onerf_ctx* ctx, const float* z, float* z_out, float* field, int64_t n, float k,
+                             cudaStream_t stream) {
+  if (n == 0) return ONERF_OK;
+  const int threads = 256;
+  const int blocks = (int)std::min((n + threads - 1) / threads, (int64_t)ctx->num_sms * 8);
+  rescale_set_kernel<<<blocks, threads, 0, stream>>>(z, z_out, reinterpret_cast<float4*>(field), n, k);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
 
 int onerf_launch_set_maps(onerf_ctx* ctx, const float* z_all, const float* field_all, const float* weights_unsorted,
                           int n_rays, int n_obj, int n_samples, float* opacity, float* depth, float* rgb,

@@ -9,9 +9,14 @@
     keys= may also name the per-set maps of set_keys(N_importance): opacity_sets_{typ}, depth_sets_{typ} (H*W, n_obj)
         and rgb_sets_{typ} (H*W, n_obj, 3), how much of each pixel each ray set shows in pass typ
         (onerf_render_edit_frame_sets).  They are never part of the default result.
-    render_edit(renderer, ...), render_origin(renderer, ...)
+    Scene(models, embeddings, code_library, scale_factor)
+        Another trained scene.  A set (obj_id, Toc, box, bbox_enlarge, scene) renders object obj_id of that scene into
+        the frame (onerf_render_edit_frame_scenes): its rays, fields and importance samples in the scene's own units,
+        composited on the frame's depth axis.
+    render_edit(renderer, ..., imports=None), render_origin(renderer, ...)
         EditableRenderer.render_edit / render_origin (render_tools/editable_renderer.py:183-294) for an instance of the
         reference's class: the same poses, duplicate counting, boxes and side effects, then one render_frame call.
+        imports= adds objects of other EditableRenderer instances, each placed by a rigid transform in metres.
     install(EditableRenderer, keys=None, group=None)
         Binds those two as the class's methods, so the reference's demo loop renders through them unchanged.
 
@@ -55,6 +60,20 @@ def set_keys(N_importance: int):
     return [f"{k}_{typ}" for typ in typs for k in _SET_MAPS]
 
 
+class Scene:
+    """A trained scene that edited frames take objects from: its models ("coarse", "fine"), embeddings (the voxel
+    embedding under "xyz"), code library and scale_factor (world units per NeRF unit).  Its weights must have the frame's
+    architecture; they are packed as engine.packed_for packs them."""
+
+    def __init__(self, models: Dict[str, Any], embeddings: Dict[str, Any], code_library, scale_factor: float):
+        if not _is_voxel(embeddings["xyz"]):
+            raise RuntimeError("editing.Scene requires the voxel embedding, as render_frame does")
+        scale_factor = float(scale_factor)
+        if not (np.isfinite(scale_factor) and scale_factor > 0):
+            raise ValueError(f"editing.Scene: scale_factor must be positive and finite, got {scale_factor}")
+        self.models, self.embeddings, self.code_library, self.scale_factor = models, embeddings, code_library, scale_factor
+
+
 def _workspace(nbytes: int, dev: torch.device) -> torch.Tensor:
     """One workspace per (device, size), kept across frames (calls on one stream are ordered)."""
     key = (dev.index, nbytes)
@@ -71,7 +90,10 @@ def render_frame(models: Dict[str, Any], embeddings: Dict[str, Any], code_librar
                  precision: Optional[str] = None) -> Dict[str, torch.Tensor]:
     """Render the H x W frame of `sets`, a list of (obj_id, Toc, box_helper_or_None, bbox_enlarge): obj_id 0 is the scene
     set (no box), Toc its (3,4) or (4,4) camera-to-set pose at NeRF scale; an object set's box helper has BBoxRayHelper's
-    pose_avg, axis_align_mat and bbox_bounds.  background_skip_bbox: the removed objects' helpers (as render_rays_multi).
+    pose_avg, axis_align_mat and bbox_bounds.  An object set may carry a fifth element, a Scene (None: this frame's
+    scene): the set is then that scene's object, its Toc translation at that scene's NeRF scale and its box in that
+    scene's frame; its depths are reported on this frame's axis.  background_skip_bbox: the removed objects' helpers
+    (as render_rays_multi).
     Returns render_rays_multi's keys for the whole frame ((H*W, T) per-sample arrays, (H*W, ...) maps) on the device of
     the code table; `keys` restricts what is kept and returned (the rest goes to scratch).  perturb = 0 and noise_std = 0,
     as EditableRenderer renders."""
@@ -111,7 +133,17 @@ def render_tile(models: Dict[str, Any], embeddings: Dict[str, Any], code_library
     a = _lib.RenderEditArgs()
     sets_c = (_lib.EditSet * max(n_obj, 1))()
     keep = []                                  # host structs the call reads
-    for i, (obj_id, Toc, box, bbox_enlarge) in enumerate(sets):
+    scenes: list = []                          # the distinct source scenes, in order of first use
+    set_scene = (C.c_int * max(n_obj, 1))()
+    for i, s in enumerate(sets):
+        obj_id, Toc, box, bbox_enlarge = s[:4]
+        scene = s[4] if len(s) > 4 else None
+        set_scene[i] = -1
+        if scene is not None:
+            j = next((j for j, sc in enumerate(scenes) if sc is scene), len(scenes))
+            if j == len(scenes):
+                scenes.append(scene)
+            set_scene[i] = j
         sets_c[i].obj_id = int(obj_id)
         sets_c[i].Toc = _c2w_host(Toc)
         if box is not None:
@@ -127,6 +159,19 @@ def render_tile(models: Dict[str, Any], embeddings: Dict[str, Any], code_library
     with torch.no_grad():          # inference: the cached packed weights (held until the call has been enqueued)
         packed_c = engine.packed_for(models["coarse"], True)
         packed_f = engine.packed_for(models["fine"], True) if N_importance > 0 else None
+        scenes_c = (_lib.EditScene * max(len(scenes), 1))()
+        for j, sc in enumerate(scenes):
+            g = _grid_of(sc.embeddings["xyz"])
+            ct = engine._f32(sc.code_library.embedding_instance.weight.detach())
+            if ct.device != dev:
+                raise RuntimeError(f"render_frame: a source scene's code table is on {ct.device}, the frame on {dev}")
+            pc = engine.packed_for(sc.models["coarse"], True)
+            pf = engine.packed_for(sc.models["fine"], True) if N_importance > 0 else None
+            keep += [g, ct, pc, pf]
+            scenes_c[j].grid = C.pointer(g.c)
+            scenes_c[j].packed_coarse, scenes_c[j].packed_fine = pc.data_ptr(), (pf.data_ptr() if pf is not None else None)
+            scenes_c[j].code_table, scenes_c[j].n_codes = ct.data_ptr(), ct.shape[0]
+            scenes_c[j].scale_factor = sc.scale_factor
     a.packed_coarse = packed_c.data_ptr()
     a.packed_fine = packed_f.data_ptr() if packed_f is not None else None
     a.code_table, a.n_codes = code_table.data_ptr(), code_table.shape[0]
@@ -152,10 +197,14 @@ def render_tile(models: Dict[str, Any], embeddings: Dict[str, Any], code_library
             setattr(set_maps[typ], k.split("_")[0], out[key].data_ptr())
     lib = _lib.load()
     with_sets = any(k in keys for k in set_keys(N_importance))
-    ws_bytes = lib.onerf_render_edit_sets_workspace_bytes if with_sets else lib.onerf_render_edit_workspace_bytes
+    ws_bytes = (lib.onerf_render_edit_scenes_workspace_bytes if scenes else
+                lib.onerf_render_edit_sets_workspace_bytes if with_sets else lib.onerf_render_edit_workspace_bytes)
     ws = _workspace(ws_bytes(a.chunk_rays, n_obj, a.n_samples, a.n_importance), dev)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-    if with_sets:
+    if scenes:
+        _lib.call("onerf_render_edit_frame_scenes", dev, C.byref(a), scenes_c, len(scenes), set_scene,
+                  C.byref(set_maps["coarse"]), C.byref(set_maps["fine"]))
+    elif with_sets:
         _lib.call("onerf_render_edit_frame_sets", dev, C.byref(a), C.byref(set_maps["coarse"]), C.byref(set_maps["fine"]))
     else:
         _lib.call("onerf_render_edit_frame", dev, C.byref(a))
@@ -207,12 +256,41 @@ def edit_sets(renderer, camera_pose_Twc, render_bg_only: bool = False, render_ob
     return sets
 
 
+def scene_of(renderer) -> Scene:
+    """The trained scene an EditableRenderer instance holds, as a Scene."""
+    s = renderer.system
+    return Scene(s.models, s.embeddings, s.code_library, renderer.scale_factor)
+
+
+def import_sets(camera_pose_Twc, imports, bbox_enlarge: float):
+    """The ray sets of objects taken from other scenes: for each (source, obj_id, place) of `imports`, with source an
+    EditableRenderer instance of the other scene and place the 4x4 rigid transform (metres) from the source's world (its
+    transforms_full.json / bbox frame) to this frame's world, the set (obj_id, Toc, box, bbox_enlarge, Scene of source)
+    with Toc = C_src @ inv(place) @ Twc and its translation divided by the source's scale_factor (C_src: the source's
+    scene_center centring, center_pose_from_avg) and box = source.get_object_bbox_helper(obj_id)."""
+    Twc = np.eye(4)
+    Twc[:3] = np.asarray(camera_pose_Twc, dtype=np.float64)[:3]
+    sets, scenes = [], {}
+    for source, obj_id, place in imports:
+        scene = scenes.setdefault(id(source), scene_of(source))
+        Toc = _center_pose_from_avg(source)(source.pose_avg, np.linalg.inv(np.asarray(place, dtype=np.float64)) @ Twc)
+        Toc[:, 3] /= source.scale_factor
+        sets.append((int(obj_id), torch.from_numpy(Toc).float()[:3, :4], source.get_object_bbox_helper(obj_id),
+                     bbox_enlarge, scene))
+    return sets
+
+
 def render_edit(renderer, h: int, w: int, camera_pose_Twc, fovx_deg: float = 70, show_progress: bool = True,
                 render_bg_only: bool = False, render_obj_only: bool = False, white_back: bool = False, *, keys=None,
-                group=None) -> Dict[str, torch.Tensor]:
+                group=None, imports=None) -> Dict[str, torch.Tensor]:
     """EditableRenderer.render_edit (editable_renderer.py:203-294) in one render_frame call; CPU tensors as the
-    reference returns them.  show_progress is accepted and unused (there is no chunk loop to report on)."""
+    reference returns them.  show_progress is accepted and unused (there is no chunk loop to report on).
+    imports: [(source_renderer, obj_id, place)] objects of other scenes added after the renderer's own sets (see
+    import_sets; the renderer's bbox_enlarge applies), except with render_bg_only."""
+    raw_Twc = np.array(camera_pose_Twc, dtype=np.float64)
     sets = edit_sets(renderer, camera_pose_Twc, render_bg_only, render_obj_only)
+    if imports and not render_bg_only:
+        sets += import_sets(raw_Twc, imports, renderer.bbox_enlarge)
     res = _frame_of(renderer, h, w, _focal(w, fovx_deg), sets, renderer.get_skipping_bbox_helper(), white_back, keys,
                     group)
     return {k: v.cpu() for k, v in res.items()}
