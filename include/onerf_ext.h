@@ -503,6 +503,54 @@ int onerf_bwd_dx_xyz(onerf_ctx* ctx, int want_object, const void* packed, const 
 int onerf_encode_bwd_xyz(onerf_ctx* ctx, const onerf_grid* grid, const float* xyz, const float* X, const float* dX, int ldx,
                          int64_t sample0, int64_t n_chunk, float* table_grad, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Masked PSNR and SSIM of a held-out frame, for the scene and for each of K objects (utils/metrics.py:14-23 with a mask).
+ * Column 0 is the scene: mask m = valid, prediction pred_scene.  Column k >= 1 is object ids_host[k-1]: m = valid &
+ * (labels == ids_host[k-1]), prediction pred_object.  Per column, with both images set to 0 outside m:
+ *   - each channel filtered with g = outer(g1, g1), g1[i] = exp(-(i - w/2)^2 / (2 * 1.5^2)) normalised to sum 1
+ *     (w = window), reflect padding of w/2 (F.pad(mode="reflect"): mirror without repeating the edge), H x W output;
+ *   - mu_p, mu_g, s_pp = E[p^2] - mu_p^2, s_gg, s_pg from those window sums, and
+ *     ssim_map = ((2 mu_p mu_g + C1)(2 s_pg + C2)) / ((mu_p^2 + mu_g^2 + C1)(s_pp + s_gg + C2)), C1 = 0.01^2, C2 = 0.03^2;
+ *   - SSIM = mean of clamp(ssim_map, 0, 1) over the 3 channels of the pixels in m;
+ *   - PSNR = -10 log10(mean squared error over the 3 channels of the pixels in m).
+ * An empty mask gives NaN for both.  With m all ones, SSIM is kornia 0.4.1's losses.ssim(pred, gt, w) read as
+ * 1 - 2 * dssim.  Window sums, ssim_map and the error sums are fp64.
+ *
+ * onerf_image_metrics: adds one frame's sums to `record` ((K+1) x 3 doubles: squared-error sum, clamped ssim_map sum,
+ * pixel count of m, per column), which must hold zeros (or an earlier part of the same frame) before the call.
+ * onerf_image_metrics_finalize: one launch that writes psnr_out[slot, :] and ssim_out[slot, :] ((F, K+1) row-major
+ * float32; either may be NULL: not written) from the record and zeroes it.  Only window, n_ids, record, psnr_out and
+ * ssim_out are read.
+ *   pred_scene, gt  (H*W, 3) float32, row-major pixels; pred_object (H*W, 3), NULL when K = 0
+ *   valid           (H*W) uint8 0 / 1, or NULL: every pixel
+ *   labels          (H*W) uint16, NULL when K = 0
+ *   ids_host        K ints in [0, 65535] (host array), 0 <= K <= ONERF_METRICS_MAX_IDS
+ * Refusals (ONERF_ERR_BAD_ARG): an even window or one outside [1, ONERF_METRICS_MAX_WINDOW], H or W <= window / 2 (reflect
+ * padding is undefined there), H > 1048560, K outside [0, ONERF_METRICS_MAX_IDS], an id outside [0, 65535], a NULL image, record or
+ * (with K > 0) pred_object, labels or ids_host, misaligned buffers.  Kernels only, no allocation and no host read:
+ * CUDA-graph capturable.  The record's fp64 sums are added with atomics, so their last bits may depend on the CTA order.
+ * ------------------------------------------------------------------------------------------- */
+#define ONERF_METRICS_MAX_WINDOW 11
+#define ONERF_METRICS_MAX_IDS 64
+
+typedef struct onerf_metrics_args {
+  int H, W;
+  const float* pred_scene;              /* (H*W,3) */
+  const float* pred_object;             /* (H*W,3), or NULL when n_ids = 0 */
+  const float* gt;                      /* (H*W,3) */
+  const uint8_t* valid;                 /* (H*W) or NULL */
+  const uint16_t* labels;               /* (H*W), or NULL when n_ids = 0 */
+  const int* ids_host;                  /* (n_ids,) host array */
+  int n_ids;                            /* K */
+  int window;                           /* odd, 1 .. ONERF_METRICS_MAX_WINDOW */
+  double* record;                       /* ((K+1),3) */
+  float* psnr_out;                      /* (F,K+1), finalize only */
+  float* ssim_out;                      /* (F,K+1), finalize only */
+} onerf_metrics_args;
+
+int onerf_image_metrics(onerf_ctx* ctx, const onerf_metrics_args* args, void* stream);
+int onerf_image_metrics_finalize(onerf_ctx* ctx, const onerf_metrics_args* args, int slot, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

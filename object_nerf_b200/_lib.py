@@ -45,12 +45,14 @@ EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_w
                "onerf_render_multi_fwd_ext", "onerf_field_bwd_workspace_bytes", "onerf_field_bwd", "onerf_bwd_dx_xyz",
                "onerf_encode_bwd_xyz", "onerf_draw_frames", "onerf_draw_frames_dstep",
                "onerf_render_edit_sets_workspace_bytes", "onerf_render_edit_frame_sets",
-               "onerf_render_edit_scenes_workspace_bytes", "onerf_render_edit_frame_scenes"]
+               "onerf_render_edit_scenes_workspace_bytes", "onerf_render_edit_frame_scenes",
+               "onerf_image_metrics", "onerf_image_metrics_finalize"]
 VALIDATE_RECORD_DOUBLES = 18
 PRUNE_SAMPLES = 4096
 PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
 FRAME_MAX_PASS = 16                                          # label values one instance column lets pass through
 STREAM_MULTI_NOISE_COARSE, STREAM_MULTI_NOISE_FINE = 7, 8   # Philox streams of the joint compositing's sigma noise
+METRICS_MAX_WINDOW, METRICS_MAX_IDS = 11, 64                 # onerf_image_metrics: largest window, most object columns
 
 _p = C.c_void_p
 
@@ -188,6 +190,12 @@ class ValidateArgs(C.Structure):
         ("ray_begin", C.c_int64), ("ray_end", C.c_int64), ("chunk_rays", C.c_int), ("psnr_mask", C.c_int),
         ("record", _p), ("finalize", C.c_int), ("psnr_out", _p),
     ]
+
+
+class MetricsArgs(C.Structure):
+    _fields_ = [("H", C.c_int), ("W", C.c_int), ("pred_scene", _p), ("pred_object", _p), ("gt", _p), ("valid", _p),
+                ("labels", _p), ("ids_host", C.POINTER(C.c_int)), ("n_ids", C.c_int), ("window", C.c_int),
+                ("record", _p), ("psnr_out", _p), ("ssim_out", _p)]
 
 
 class PruneArgs(C.Structure):
@@ -343,6 +351,8 @@ def load() -> C.CDLL:
         lib.onerf_field_bwd.argtypes = [_p, C.POINTER(FieldArgs), _p, _p, C.POINTER(FieldBwdArgs), _p]
         lib.onerf_bwd_dx_xyz.argtypes = [_p, C.c_int, _p, _p, _p, C.c_int64, C.POINTER(Grid), _p, _p]
         lib.onerf_encode_bwd_xyz.argtypes = [_p, C.POINTER(Grid), _p, _p, _p, C.c_int, C.c_int64, C.c_int64, _p, _p]
+        lib.onerf_image_metrics.argtypes = [_p, C.POINTER(MetricsArgs), _p]
+        lib.onerf_image_metrics_finalize.argtypes = [_p, C.POINTER(MetricsArgs), C.c_int, _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

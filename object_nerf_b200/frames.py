@@ -11,8 +11,13 @@ expanded buffers with the same seed.
 Decoding stays on the host, as in the reference: PNG reads, PIL LANCZOS for colour, cv2 INTER_NEAREST for depth and
 labels, and the depth arithmetic with the reference's own torch ops.
 
+`read_frames(..., split="test")` / `FrameSet.load(..., split="test")` keep the held-out frames instead: those whose idx
+split/test.txt lists, in transforms_full.json order, without the frames whose pose is not finite, decoded exactly as the
+training frames (evaluation.evaluate_frames renders and scores them).
+
 Refused rather than approximated (ValueError, before any device work):
-  - training rays clipped to a box (use_bbox without use_bbox_only_for_test);
+  - training rays clipped to a box (use_bbox without use_bbox_only_for_test), and for the test split any use_bbox (its
+    rays would be clipped to the object box);
   - mask_rebalance_strategy other than fg_bg_reweight (distance_transform crashes in the reference itself);
   - a frame whose RGB image is missing (the reference then misaligns its per-instance buffers against all_rays);
   - label images wider than 16 bits, and more than FRAME_MAX_PASS pass-through labels per instance column.
@@ -80,13 +85,19 @@ def _columns(conf):
     return [ids[0]] + [i for i in ids[1:] if i != 0]
 
 
-def read_frames(conf, img_wh) -> Dict[str, object]:
+def read_frames(conf, img_wh, split: str = "train") -> Dict[str, object]:
     """Decode GenericDataset's train split on the host: the FrameSet constructor's keyword arguments (arrays on the
-    host, frames in GenericDataset's order)."""
+    host, frames in GenericDataset's order).  split="test": the frames split/test.txt lists instead, in
+    transforms_full.json order, dropping only those whose pose is not finite (no train_start_idx, validate_idx,
+    observation check, train_skip_step or train_max_size), decoded the same way."""
     import cv2
     from PIL import Image
 
     w, h = img_wh
+    if split not in ("train", "test"):
+        raise ValueError(f"FrameSet: unknown split {split!r} (train or test)")
+    if split == "test" and conf["use_bbox"]:
+        raise ValueError("FrameSet: test rays clipped to the object box (use_bbox) are not supported")
     if conf["use_bbox"] and not conf["use_bbox_only_for_test"]:
         raise ValueError("FrameSet: training rays clipped to the object box (use_bbox with use_bbox_only_for_test "
                          "false) are not supported")
@@ -110,14 +121,20 @@ def read_frames(conf, img_wh) -> Dict[str, object]:
     scale = conf["scale_factor"]
     pose_avg = np.concatenate([np.eye(3), np.array(conf["scene_center"])[:, None]], 1)
 
-    split_inds = np.loadtxt(os.path.join(conf["split"], "train.txt")).tolist()
+    split_inds = np.loadtxt(os.path.join(conf["split"], f"{split}.txt"))
+    split_inds = (split_inds.reshape(-1) if split == "test" else split_inds).tolist()    # a one-line test.txt
     frames = [x for x in meta["frames"] if x["idx"] in split_inds]
-    frames = [x for x in frames if x["idx"] >= conf["train_start_idx"] and x["idx"] != conf["validate_idx"]]
-    frames = [x for x in frames if _obs_check(x, conf, pose_avg[:3, 3])]
-    frames = [frames[i] for i in np.arange(0, len(frames), conf["train_skip_step"])]
-    frames = frames[:min(conf["train_max_size"], len(frames))]
-    if not frames:
-        raise ValueError("FrameSet: no training frame passes the split and observation filters")
+    if split == "test":
+        frames = [x for x in frames if np.isfinite(np.array(x["transform_matrix"], dtype=np.float64)).all()]
+        if not frames:
+            raise ValueError("FrameSet: split/test.txt lists no frame with a finite pose")
+    else:
+        frames = [x for x in frames if x["idx"] >= conf["train_start_idx"] and x["idx"] != conf["validate_idx"]]
+        frames = [x for x in frames if _obs_check(x, conf, pose_avg[:3, 3])]
+        frames = [frames[i] for i in np.arange(0, len(frames), conf["train_skip_step"])]
+        frames = frames[:min(conf["train_max_size"], len(frames))]
+        if not frames:
+            raise ValueError("FrameSet: no training frame passes the split and observation filters")
     for fr in frames:
         p = os.path.join(root, f"{fr['file_path']}.png")
         if not os.path.exists(p):
@@ -277,9 +294,10 @@ class FrameSet:
         self.args = a
 
     @classmethod
-    def load(cls, dataset_extra, img_wh=(640, 480), device="cuda") -> "FrameSet":
-        """GenericDataset(split="train", img_wh, dataset_extra)'s training frames, kept as pixels (read_frames)."""
-        return cls(**read_frames(dataset_extra, tuple(img_wh)), device=device)
+    def load(cls, dataset_extra, img_wh=(640, 480), device="cuda", split: str = "train") -> "FrameSet":
+        """GenericDataset(split="train", img_wh, dataset_extra)'s training frames, kept as pixels (read_frames);
+        split="test": the held-out frames of split/test.txt."""
+        return cls(**read_frames(dataset_extra, tuple(img_wh), split), device=device)
 
     @property
     def nbytes(self) -> int:
