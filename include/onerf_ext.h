@@ -551,6 +551,90 @@ typedef struct onerf_metrics_args {
 int onerf_image_metrics(onerf_ctx* ctx, const onerf_metrics_args* args, void* stream);
 int onerf_image_metrics_finalize(onerf_ctx* ctx, const onerf_metrics_args* args, int slot, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Depth errors of a held-out frame, for the scene and for each of K objects.  Inputs are float32, every sum is fp64.
+ * s = scale.  A pixel is in column 0 when valid and gt > 0; it is also in column k >= 1 when labelled ids_host[k-1].
+ * Column 0 reads pred_scene, column k reads pred_object (depth_instance).  Per pixel of a column:
+ *   g = gt * s, d = clamp(pred * s, d_min, d_max) (a NaN pred stays NaN),
+ * and the column's record row holds the eight sums
+ *   n, sum |d - g| / g, sum (d - g)^2 / g, sum (d - g)^2, sum (ln d - ln g)^2,
+ *   and the counts of max(d / g, g / d) < 1.25, < 1.25^2, < 1.25^3 (a NaN ratio adds NaN to each count).
+ * The seven outputs (ONERF_DEPTH_METRICS order) are
+ *   abs_rel = sum |d - g| / g / n, sq_rel = sum (d - g)^2 / g / n, rmse = sqrt(sum (d - g)^2 / n),
+ *   rmse_log = sqrt(sum (ln d - ln g)^2 / n), delta_i = count_i / n.
+ * An empty column gives NaN for all seven; a NaN prediction in a column makes all seven NaN.
+ *
+ * onerf_depth_metrics: adds one frame's sums to `record` ((K+1) x 8 doubles in the order above), which must hold zeros
+ * (or an earlier part of the same frame) before the call.
+ * onerf_depth_metrics_finalize: one launch that writes out[slot, :, :] ((F, K+1, 7) row-major float32; NULL: not
+ * written) from the record and zeroes it.  Only n_ids, record and out are read.
+ *   pred_scene, gt  (H*W) float32; pred_object (H*W) float32, NULL when K = 0
+ *   valid           (H*W) uint8 0 / 1, or NULL: every pixel
+ *   labels          (H*W) uint16, NULL when K = 0
+ *   ids_host        K distinct ints in [0, 65535] (host array), 0 <= K <= ONERF_METRICS_MAX_IDS
+ *   scale           finite and > 0; d_min, d_max finite with 0 < d_min < d_max
+ * Refusals (ONERF_ERR_BAD_ARG): a NULL ctx or args, H or W < 1, H * W >= 2^40, K outside [0, ONERF_METRICS_MAX_IDS], an
+ * id outside [0, 65535] or repeated, d_min <= 0 or d_min >= d_max, a non-finite or non-positive scale or depth bound, a
+ * NULL pred_scene, gt or record or (with K > 0) pred_object, labels or ids_host, misaligned buffers.
+ *
+ * Instance-mask agreement of one object's opacity map (the object branch's OpacityLoss target), over the valid pixels:
+ *   G = (labels == id), P = (opacity >= threshold) (float32 comparison),
+ *   iou = |P & G| / |P | G| (NaN when P | G is empty), opacity_l1 = sum |opacity - [G]| / n_valid (NaN when no pixel
+ *   is valid).
+ * onerf_mask_metrics: adds the four sums |P & G|, |P | G|, sum |opacity - [G]| and n_valid (fp64) to row `column` of
+ * `record` (K x 4 doubles, K = n_ids), which must hold zeros (or an earlier part of the same frame) there.
+ * onerf_mask_metrics_finalize: one launch that writes iou_out[slot, :] and opacity_l1_out[slot, :] ((F, K) row-major
+ * float32; either may be NULL: not written) from the record and zeroes it.  Only n_ids, record and the outputs are
+ * read.
+ *   opacity         (H*W) float32 (opacity_instance rendered with object id's code)
+ *   valid           (H*W) uint8 0 / 1, or NULL: every pixel
+ *   labels          (H*W) uint16
+ *   id              in [0, 65535]; column in [0, K), 1 <= K <= ONERF_METRICS_MAX_IDS; threshold finite
+ * Refusals (ONERF_ERR_BAD_ARG): a NULL ctx or args, H or W < 1, H * W >= 2^40, K outside [1, ONERF_METRICS_MAX_IDS],
+ * column outside [0, K), an id outside [0, 65535], a non-finite threshold, a NULL opacity, labels or record, misaligned
+ * buffers.
+ *
+ * All four are kernels only, with no allocation and no host read: CUDA-graph capturable.  Counts are exact (integers
+ * below 2^53); the other fp64 sums are added with atomics, so their last bits may depend on the CTA order.
+ * ------------------------------------------------------------------------------------------- */
+#define ONERF_DEPTH_METRICS 7
+#define ONERF_DEPTH_RECORD 8
+#define ONERF_MASK_RECORD 4
+
+typedef struct onerf_depth_metrics_args {
+  int H, W;
+  const float* pred_scene;              /* (H*W) */
+  const float* pred_object;             /* (H*W), or NULL when n_ids = 0 */
+  const float* gt;                      /* (H*W) */
+  const uint8_t* valid;                 /* (H*W) or NULL */
+  const uint16_t* labels;               /* (H*W), or NULL when n_ids = 0 */
+  const int* ids_host;                  /* (n_ids,) host array */
+  int n_ids;                            /* K */
+  double scale;                         /* s: metres per stored depth unit */
+  double d_min, d_max;                  /* clamp of the prediction, metres */
+  double* record;                       /* ((K+1),8) */
+  float* out;                           /* (F,K+1,7), finalize only */
+} onerf_depth_metrics_args;
+
+typedef struct onerf_mask_metrics_args {
+  int H, W;
+  const float* opacity;                 /* (H*W) */
+  const uint8_t* valid;                 /* (H*W) or NULL */
+  const uint16_t* labels;               /* (H*W) */
+  int id;                               /* the object's label */
+  int column;                           /* its row of the record, 0 .. n_ids-1 */
+  int n_ids;                            /* K */
+  float threshold;                      /* tau */
+  double* record;                       /* (K,4) */
+  float* iou_out;                       /* (F,K), finalize only */
+  float* opacity_l1_out;                /* (F,K), finalize only */
+} onerf_mask_metrics_args;
+
+int onerf_depth_metrics(onerf_ctx* ctx, const onerf_depth_metrics_args* args, void* stream);
+int onerf_depth_metrics_finalize(onerf_ctx* ctx, const onerf_depth_metrics_args* args, int slot, void* stream);
+int onerf_mask_metrics(onerf_ctx* ctx, const onerf_mask_metrics_args* args, void* stream);
+int onerf_mask_metrics_finalize(onerf_ctx* ctx, const onerf_mask_metrics_args* args, int slot, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -46,13 +46,15 @@ EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_w
                "onerf_encode_bwd_xyz", "onerf_draw_frames", "onerf_draw_frames_dstep",
                "onerf_render_edit_sets_workspace_bytes", "onerf_render_edit_frame_sets",
                "onerf_render_edit_scenes_workspace_bytes", "onerf_render_edit_frame_scenes",
-               "onerf_image_metrics", "onerf_image_metrics_finalize"]
+               "onerf_image_metrics", "onerf_image_metrics_finalize", "onerf_depth_metrics",
+               "onerf_depth_metrics_finalize", "onerf_mask_metrics", "onerf_mask_metrics_finalize"]
 VALIDATE_RECORD_DOUBLES = 18
 PRUNE_SAMPLES = 4096
 PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
 FRAME_MAX_PASS = 16                                          # label values one instance column lets pass through
 STREAM_MULTI_NOISE_COARSE, STREAM_MULTI_NOISE_FINE = 7, 8   # Philox streams of the joint compositing's sigma noise
 METRICS_MAX_WINDOW, METRICS_MAX_IDS = 11, 64                 # onerf_image_metrics: largest window, most object columns
+DEPTH_METRICS, DEPTH_RECORD, MASK_RECORD = 7, 8, 4           # outputs and record sums per column: depth; sums: mask
 
 _p = C.c_void_p
 
@@ -196,6 +198,18 @@ class MetricsArgs(C.Structure):
     _fields_ = [("H", C.c_int), ("W", C.c_int), ("pred_scene", _p), ("pred_object", _p), ("gt", _p), ("valid", _p),
                 ("labels", _p), ("ids_host", C.POINTER(C.c_int)), ("n_ids", C.c_int), ("window", C.c_int),
                 ("record", _p), ("psnr_out", _p), ("ssim_out", _p)]
+
+
+class DepthMetricsArgs(C.Structure):
+    _fields_ = [("H", C.c_int), ("W", C.c_int), ("pred_scene", _p), ("pred_object", _p), ("gt", _p), ("valid", _p),
+                ("labels", _p), ("ids_host", C.POINTER(C.c_int)), ("n_ids", C.c_int), ("scale", C.c_double),
+                ("d_min", C.c_double), ("d_max", C.c_double), ("record", _p), ("out", _p)]
+
+
+class MaskMetricsArgs(C.Structure):
+    _fields_ = [("H", C.c_int), ("W", C.c_int), ("opacity", _p), ("valid", _p), ("labels", _p), ("id", C.c_int),
+                ("column", C.c_int), ("n_ids", C.c_int), ("threshold", C.c_float), ("record", _p), ("iou_out", _p),
+                ("opacity_l1_out", _p)]
 
 
 class PruneArgs(C.Structure):
@@ -353,6 +367,10 @@ def load() -> C.CDLL:
         lib.onerf_encode_bwd_xyz.argtypes = [_p, C.POINTER(Grid), _p, _p, _p, C.c_int, C.c_int64, C.c_int64, _p, _p]
         lib.onerf_image_metrics.argtypes = [_p, C.POINTER(MetricsArgs), _p]
         lib.onerf_image_metrics_finalize.argtypes = [_p, C.POINTER(MetricsArgs), C.c_int, _p]
+        lib.onerf_depth_metrics.argtypes = [_p, C.POINTER(DepthMetricsArgs), _p]
+        lib.onerf_depth_metrics_finalize.argtypes = [_p, C.POINTER(DepthMetricsArgs), C.c_int, _p]
+        lib.onerf_mask_metrics.argtypes = [_p, C.POINTER(MaskMetricsArgs), _p]
+        lib.onerf_mask_metrics_finalize.argtypes = [_p, C.POINTER(MaskMetricsArgs), C.c_int, _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

@@ -1,5 +1,6 @@
 """Held-out views scored on the device: per-frame PSNR and SSIM of the scene and of each object over a frame store
-(frames.FrameSet, typically `FrameSet.load(conf.dataset_extra, img_wh, split="test")`).
+(frames.FrameSet, typically `FrameSet.load(conf.dataset_extra, img_wh, split="test")`), and on request their depth
+errors and each object's mask agreement.
 
 For each frame, `evaluate_frames`
   - builds the frame's (H*W, 8) rays on the device with the arithmetic of onerf_draw_frames' training rows
@@ -10,6 +11,12 @@ For each frame, `evaluate_frames`
     column k reads only pixels labelled object_ids[k-1], and each of those was rendered with that object's code;
   - scores the maps with onerf_image_metrics (metrics.py's definition; column 0 the scene over the valid pixels, column k
     the object prediction over the valid pixels labelled object_ids[k-1]) and finalises row f of the outputs.
+With depth=True the one render also gives the last pass's depth and depth_instance, scored with onerf_depth_metrics
+(metrics.py's definition) against the store's processed depths at scale frames.scale_factor: column 0 the scene over
+the valid pixels with a depth, column k the object depth over those labelled object_ids[k-1].  The same argument as for
+the colours makes the one render exact for every object column.  With masks=True each object is rendered once more per
+frame with its own code at every pixel (frame_batch(frames, f, [k]), keys ("opacity_instance",)): its opacity_instance
+is scored against the pixels labelled k by onerf_mask_metrics.  Neither flag changes the colour render or its scores.
 Valid pixels are those frames.BORDER or more pixels from every edge, the training split's valid_mask.  The loop reads
 nothing back to the host; the per-frame outputs stay on the device.
 
@@ -65,7 +72,8 @@ def frame_batch(frames, f: int, object_ids: Sequence[int] = (), rays=None) -> Di
 
 def evaluate_frames(models: Dict[str, Any], embeddings: Dict[str, Any], code_library, frames, conf, *,
                     object_ids: Sequence[int] = (), window: int = 3, chunk: int = 65536, precision: str = "bf16",
-                    group=None) -> Dict[str, torch.Tensor]:
+                    group=None, depth: bool = False, masks: bool = False, mask_threshold: float = 0.5,
+                    depth_range=(1e-3, 10.0)) -> Dict[str, torch.Tensor]:
     """PSNR and SSIM of every frame of `frames` (a frames.FrameSet) rendered by the trained model (module docstring).
     conf: the reference's config (conf.model's N_samples, N_importance and use_disp), or that model section itself.
     object_ids: up to 64 object ids to score, each a label of the store's label images and a row of the code table.
@@ -74,7 +82,13 @@ def evaluate_frames(models: Dict[str, Any], embeddings: Dict[str, Any], code_lib
 
     Returns device tensors: "psnr", "ssim" (F,) of the scene; "psnr_objects", "ssim_objects" (F, K); "mean_psnr",
     "mean_ssim" () and "mean_psnr_objects", "mean_ssim_objects" (K,), the means over frames ignoring NaN (a frame in
-    which an object has no valid pixel scores NaN for it)."""
+    which an object has no valid pixel scores NaN for it).
+
+    depth=True adds "depth_metrics" (F, 7) of the scene and "depth_metrics_objects" (F, K, 7), columns in
+    metrics.DEPTH_METRICS order, and their NaN-ignoring means over frames "mean_depth_metrics" (7,) and
+    "mean_depth_metrics_objects" (K, 7).  depth_range: the (d_min, d_max) clamp of the predictions in metres.
+    masks=True adds "iou_objects" and "opacity_l1_objects" (F, K) and "mean_iou_objects", "mean_opacity_l1_objects"
+    (K,); it costs K more renders per frame.  mask_threshold: the opacity at which a pixel counts as covered."""
     ids = [int(i) for i in object_ids]
     K = len(ids)
     if K > _lib.METRICS_MAX_IDS:
@@ -92,18 +106,40 @@ def evaluate_frames(models: Dict[str, Any], embeddings: Dict[str, Any], code_lib
     F, H, W, dev = frames.n_frames, frames.H, frames.W, frames.device
     HW, typ = H * W, "fine" if N_importance > 0 else "coarse"
     keys = ("rgb", "rgb_instance") if K else ("rgb",)
+    if depth:
+        keys += ("depth", "depth_instance") if K else ("depth",)
+    render = dict(N_samples=N_samples, N_importance=N_importance, use_disp=use_disp, white_back=False, chunk=chunk,
+                  precision=precision, group=group)
 
     plan = metrics.MetricsPlan(H, W, ids, window, F, dev)
+    dplan = metrics.DepthMetricsPlan(H, W, ids, frames.scale_factor, depth_range, F, dev) if depth else None
+    mplan = metrics.MaskMetricsPlan(H, W, ids, mask_threshold, F, dev) if masks else None
     rays = torch.empty(HW, 8, dtype=torch.float32, device=dev)
     for f in range(F):
         batch = frame_batch(frames, f, ids, rays)
-        out = training.validate_frame(models, embeddings, code_library, batch, _NO_LOSS, N_samples=N_samples,
-                                      N_importance=N_importance, use_disp=use_disp, white_back=False, chunk=chunk,
-                                      keys=keys, precision=precision, group=group)
-        plan.accumulate(out[f"rgb_{typ}"], batch["rgbs"], batch["valid_mask"], out.get(f"rgb_instance_{typ}"),
-                        t["labels"][f] if K else None)
+        out = training.validate_frame(models, embeddings, code_library, batch, _NO_LOSS, keys=keys, **render)
+        labels = t["labels"][f] if K else None
+        plan.accumulate(out[f"rgb_{typ}"], batch["rgbs"], batch["valid_mask"], out.get(f"rgb_instance_{typ}"), labels)
         plan.finalize(f)
+        if depth:
+            dplan.accumulate(out[f"depth_{typ}"], t["depths"][f], batch["valid_mask"], out.get(f"depth_instance_{typ}"),
+                             labels)
+            dplan.finalize(f)
+        if masks and K:
+            for k, i in enumerate(ids):
+                out = training.validate_frame(models, embeddings, code_library, frame_batch(frames, f, [i], rays),
+                                              _NO_LOSS, keys=("opacity_instance",), **render)
+                mplan.accumulate(k, out[f"opacity_instance_{typ}"], labels, batch["valid_mask"])
+            mplan.finalize(f)
     P, S = plan.psnr, plan.ssim
-    return {"psnr": P[:, 0], "ssim": S[:, 0], "psnr_objects": P[:, 1:], "ssim_objects": S[:, 1:],
-            "mean_psnr": P[:, 0].nanmean(), "mean_ssim": S[:, 0].nanmean(),
-            "mean_psnr_objects": P[:, 1:].nanmean(0), "mean_ssim_objects": S[:, 1:].nanmean(0)}
+    res = {"psnr": P[:, 0], "ssim": S[:, 0], "psnr_objects": P[:, 1:], "ssim_objects": S[:, 1:],
+           "mean_psnr": P[:, 0].nanmean(), "mean_ssim": S[:, 0].nanmean(),
+           "mean_psnr_objects": P[:, 1:].nanmean(0), "mean_ssim_objects": S[:, 1:].nanmean(0)}
+    if depth:
+        D = dplan.out
+        res.update({"depth_metrics": D[:, 0], "depth_metrics_objects": D[:, 1:],
+                    "mean_depth_metrics": D[:, 0].nanmean(0), "mean_depth_metrics_objects": D[:, 1:].nanmean(0)})
+    if masks:
+        res.update({"iou_objects": mplan.iou, "opacity_l1_objects": mplan.opacity_l1,
+                    "mean_iou_objects": mplan.iou.nanmean(0), "mean_opacity_l1_objects": mplan.opacity_l1.nanmean(0)})
+    return res
