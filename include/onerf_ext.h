@@ -635,6 +635,66 @@ int onerf_depth_metrics_finalize(onerf_ctx* ctx, const onerf_depth_metrics_args*
 int onerf_mask_metrics(onerf_ctx* ctx, const onerf_mask_metrics_args* args, void* stream);
 int onerf_mask_metrics_finalize(onerf_ctx* ctx, const onerf_mask_metrics_args* args, int slot, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Every object's own maps of a set of rays in one render: the object branch's decomposition (opacity, depth and colour of
+ * each object, what OpacityLoss trains) for K object codes at once.  For K codes code_table[ids_host[k]], column k of
+ * each object map is bit for bit the opacity_instance / depth_instance / rgb_instance that onerf_render_rays_fwd writes
+ * when every ray carries that code (is_eval, perturb = 0, noise_std = 0, rays_in_bbox = 0: models/rendering.py's
+ * render_rays(..., forward_instance=True, is_eval=True, perturb=0, noise_std=0, rays_in_bbox=False)), at the same
+ * precision, and the scene maps are that render's scene maps.  In such a render the coarse depths, the scene branch,
+ * its weights, the importance samples and each sample's encoding do not depend on the code, so per chunk and pass they
+ * are computed once: ONERF_PREC_BF16 runs one tensor-core field launch that encodes each sample once and runs the
+ * object branch once per code, then the scene branch; ONERF_PREC_FP32 runs the FFMA field once for the scene and once
+ * per code for the object branch.  One compositing launch gives the scene maps, one more every object map.  A pass
+ * runs the object branch only when one of its object maps is given, and the scene branch only when one of its scene
+ * maps is given or its weights feed the fine samples (the coarse pass of a render with n_importance > 0); what runs
+ * gives the same bits either way.
+ *   render     rays (n_rays,8), n_rays, grid, packed_coarse / packed_fine, precision, n_samples, n_importance, use_disp,
+ *              white_back, zero_last_delta; is_eval must be set, perturb and noise_std 0, rays_in_bbox 0, train_ws NULL.
+ *              codes, forward_instance, the random buffers and the maps of onerf_render_args are not read.  workspace:
+ *              >= onerf_render_instances_workspace_bytes(chunk_rays, n_ids, n_samples, n_importance) bytes, 256-byte
+ *              aligned (0 for a bad shape): per chunk the field rows of the K codes and the scene, K per-ray-constant
+ *              blocks, depths and weights.  Its size does not depend on the image.
+ *   code_table (n_codes_table,64); ids_host: n_ids ints (host array), 1 <= n_ids <= ONERF_INSTANCES_MAX_CODES, each a
+ *              row of the table; repeats are allowed (each is its own column).
+ *   ray_begin, ray_end  the tile [ray_begin, ray_end) of the rays rendered, in chunks of chunk_rays rays.
+ *   coarse, fine  tile-sized maps (N = ray_end - ray_begin rows): scene rgb (N,3), depth (N,), opacity (N,); object
+ *              opacity and depth (N,K), rgb (N,K,3), K = n_ids.  Any may be NULL: it is not written.  fine maps need
+ *              n_importance > 0.  4-byte aligned.
+ * Every row depends on its ray only, never on chunk_rays or the tile bounds.  Refusals before any launch: a NULL ctx or
+ * args, n_ids outside [1, 64], a NULL ids_host or code_table, an id outside the code table, is_eval off, perturb or
+ * noise_std non-zero, a training workspace, a bad shape, a tile outside [0, n_rays], chunk_rays < 1, NULL rays or packed
+ * weights, a NULL or misaligned grid buffer, an unknown precision, fine maps without a fine pass, a misaligned map, a
+ * misaligned or undersized workspace (ONERF_ERR_BAD_ARG); rays_in_bbox set (the fine depths would then follow the
+ * object's weights) and n_samples + n_importance > 2048 (ONERF_ERR_UNSUPPORTED).  Kernels only, no allocation and no
+ * host read: CUDA-graph capturable.
+ * ------------------------------------------------------------------------------------------- */
+#define ONERF_INSTANCES_MAX_CODES 64
+
+typedef struct onerf_instance_maps {
+  float* rgb;                           /* (N,3) scene */
+  float* depth;                         /* (N,) scene */
+  float* opacity;                       /* (N,) scene */
+  float* opacity_instance;              /* (N,K) */
+  float* depth_instance;                /* (N,K) */
+  float* rgb_instance;                  /* (N,K,3) */
+} onerf_instance_maps;
+
+typedef struct onerf_instances_args {
+  onerf_render_args render;
+  const float* code_table;              /* (n_codes_table,64) */
+  int n_codes_table;
+  const int* ids_host;                  /* (n_ids,) host array */
+  int n_ids;                            /* K */
+  int64_t ray_begin, ray_end;
+  int chunk_rays;
+  onerf_instance_maps coarse;
+  onerf_instance_maps fine;             /* n_importance > 0 only */
+} onerf_instances_args;
+
+size_t onerf_render_instances_workspace_bytes(int chunk_rays, int n_codes, int n_samples, int n_importance);
+int onerf_render_instances(onerf_ctx* ctx, const onerf_instances_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

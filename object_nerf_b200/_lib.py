@@ -47,7 +47,8 @@ EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_w
                "onerf_render_edit_sets_workspace_bytes", "onerf_render_edit_frame_sets",
                "onerf_render_edit_scenes_workspace_bytes", "onerf_render_edit_frame_scenes",
                "onerf_image_metrics", "onerf_image_metrics_finalize", "onerf_depth_metrics",
-               "onerf_depth_metrics_finalize", "onerf_mask_metrics", "onerf_mask_metrics_finalize"]
+               "onerf_depth_metrics_finalize", "onerf_mask_metrics", "onerf_mask_metrics_finalize",
+               "onerf_render_instances_workspace_bytes", "onerf_render_instances"]
 VALIDATE_RECORD_DOUBLES = 18
 PRUNE_SAMPLES = 4096
 PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
@@ -55,6 +56,7 @@ FRAME_MAX_PASS = 16                                          # label values one 
 STREAM_MULTI_NOISE_COARSE, STREAM_MULTI_NOISE_FINE = 7, 8   # Philox streams of the joint compositing's sigma noise
 METRICS_MAX_WINDOW, METRICS_MAX_IDS = 11, 64                 # onerf_image_metrics: largest window, most object columns
 DEPTH_METRICS, DEPTH_RECORD, MASK_RECORD = 7, 8, 4           # outputs and record sums per column: depth; sums: mask
+INSTANCES_MAX_CODES = 64                                     # onerf_render_instances: most object codes per render
 
 _p = C.c_void_p
 
@@ -210,6 +212,17 @@ class MaskMetricsArgs(C.Structure):
     _fields_ = [("H", C.c_int), ("W", C.c_int), ("opacity", _p), ("valid", _p), ("labels", _p), ("id", C.c_int),
                 ("column", C.c_int), ("n_ids", C.c_int), ("threshold", C.c_float), ("record", _p), ("iou_out", _p),
                 ("opacity_l1_out", _p)]
+
+
+class InstanceMaps(C.Structure):
+    _fields_ = [("rgb", _p), ("depth", _p), ("opacity", _p), ("opacity_instance", _p), ("depth_instance", _p),
+                ("rgb_instance", _p)]
+
+
+class InstancesArgs(C.Structure):
+    _fields_ = [("render", RenderArgs), ("code_table", _p), ("n_codes_table", C.c_int), ("ids_host", C.POINTER(C.c_int)),
+                ("n_ids", C.c_int), ("ray_begin", C.c_int64), ("ray_end", C.c_int64), ("chunk_rays", C.c_int),
+                ("coarse", InstanceMaps), ("fine", InstanceMaps)]
 
 
 class PruneArgs(C.Structure):
@@ -371,6 +384,9 @@ def load() -> C.CDLL:
         lib.onerf_depth_metrics_finalize.argtypes = [_p, C.POINTER(DepthMetricsArgs), C.c_int, _p]
         lib.onerf_mask_metrics.argtypes = [_p, C.POINTER(MaskMetricsArgs), _p]
         lib.onerf_mask_metrics_finalize.argtypes = [_p, C.POINTER(MaskMetricsArgs), C.c_int, _p]
+        lib.onerf_render_instances_workspace_bytes.argtypes = [C.c_int] * 4
+        lib.onerf_render_instances_workspace_bytes.restype = C.c_size_t
+        lib.onerf_render_instances.argtypes = [_p, C.POINTER(InstancesArgs), _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

@@ -858,3 +858,177 @@ extern "C" int onerf_validate_frame(onerf_ctx* ctx, const onerf_validate_args* v
   return onerf_validate_finalize(ctx, v->record, wt, ra.n_importance > 0, la.loss_sum_out, la.terms_out, la.present_out,
                                  v->psnr_out, stream);
 }
+
+// ------------------------------------------------------------------------------------------------
+// Every object's maps of a tile of rays in one render (onerf_render_instances): per chunk the coarse depths, the K
+// codes' per-ray constants, one field evaluation of the scene and every code, the scene compositing (whose weights
+// feed the importance sampler) and one compositing launch of every object column, then the same for the fine pass.
+// Same kernels, arguments and order of arithmetic as onerf_render_rays_fwd with is_eval and nothing random, so every
+// column is bit-identical to that call with the column's code on every ray.
+// ------------------------------------------------------------------------------------------------
+struct InstancesWs {
+  float *ray_const, *scene, *obj, *z_c, *w_c, *z_f, *w_f;
+  onerf_instance_maps scratch;      // scene maps of one chunk, for those the caller leaves NULL
+  int64_t rc_stride, obj_stride;    // floats between two codes' blocks of ray_const / obj
+  size_t total;
+};
+
+static InstancesWs instances_ws_layout(char* base, int chunk, int n_codes, int n_samples, int n_importance) {
+  const size_t n = chunk, K = n_codes, S = n_samples, SF = (size_t)n_samples + n_importance;
+  const size_t nf = n_importance > 0 ? n : 0;
+  InstancesWs w;
+  size_t off = 0;
+  auto take = [&](size_t floats) { float* p = reinterpret_cast<float*>(base + off); off += align256(floats * sizeof(float)); return p; };
+  w.rc_stride = (int64_t)(n * ONERF_RAY_CONST_FLOATS);
+  w.obj_stride = (int64_t)(n * SF * 4);
+  w.ray_const = take(K * n * ONERF_RAY_CONST_FLOATS);
+  w.scene = take(n * SF * 4);
+  w.obj = take(K * n * SF * 4);
+  w.z_c = take(n * S); w.w_c = take(n * S);
+  w.z_f = take(nf * SF); w.w_f = take(nf * SF);
+  w.scratch = onerf_instance_maps{take(n * 3), take(n), take(n), nullptr, nullptr, nullptr};
+  w.total = off;
+  return w;
+}
+
+extern "C" size_t onerf_render_instances_workspace_bytes(int chunk_rays, int n_codes, int n_samples, int n_importance) {
+  if (chunk_rays < 1 || n_codes < 1 || n_codes > ONERF_INSTANCES_MAX_CODES || n_samples < 2 || n_importance < 0) return 0;
+  return instances_ws_layout(nullptr, chunk_rays, n_codes, n_samples, n_importance).total;
+}
+
+static bool instance_maps_aligned(const onerf_instance_maps& m) {
+  return onerf_aligned4(m.rgb) && onerf_aligned4(m.depth) && onerf_aligned4(m.opacity) &&
+         onerf_aligned4(m.opacity_instance) && onerf_aligned4(m.depth_instance) && onerf_aligned4(m.rgb_instance);
+}
+
+static bool any_instance_map(const onerf_instance_maps& m) {
+  return m.rgb || m.depth || m.opacity || m.opacity_instance || m.depth_instance || m.rgb_instance;
+}
+
+// One pass of one chunk of n rays (rows r0.. of the tile's maps) on depths z (n,S).  Only what the pass's maps need runs:
+// the object branch (per-code ray constants, field, object compositing) when the pass has an object map, the scene
+// branch (field and compositing, weights to w_out) when it has a scene map or its weights feed the fine samples
+// (feeds_fine).  Neither changes the other's bits.
+static int instances_pass(onerf_ctx* ctx, const onerf_instances_args* a, const InstancesWs& w, const float* rays, int n,
+                          const void* packed, const float* z, int S, float* w_out, const onerf_instance_maps& m,
+                          bool feeds_fine, int64_t r0, cudaStream_t stream) {
+  const onerf_render_args& ra = a->render;
+  const int K = a->n_ids;
+  const bool want_obj = m.opacity_instance || m.depth_instance || m.rgb_instance;
+  const bool want_scene = feeds_fine || m.rgb || m.depth || m.opacity;
+  if (!want_obj && !want_scene) return ONERF_OK;
+  FieldParams base;
+  memset(&base, 0, sizeof(base));
+  base.rays = rays; base.z = z; base.z_stride = S;
+  base.n_rays = n; base.S = S;
+  if (ra.grid) base.grid = *ra.grid;
+  base.packed = packed;
+  base.L = onerf_make_layout(ra.grid ? 1 : 0);
+  base.out_stride = S;
+  base.scene_out = w.scene;
+  int rc;
+  // code k's per-ray constants (the direction terms are the same in every block); the scene alone needs block 0's
+  for (int k = 0; k < (want_obj ? K : 1); ++k) {
+    FieldParams p = base;
+    p.want_object = want_obj ? 1 : 0;
+    p.code_row = a->code_table + (size_t)a->ids_host[k] * ONERF_NCODE;
+    p.ray_const = w.ray_const + k * w.rc_stride;
+    rc = onerf_launch_ray_const(ctx, p, stream);
+    if (rc != ONERF_OK) return rc;
+  }
+  if (ra.precision == ONERF_PREC_BF16) {
+    FieldParams p = base;
+    p.want_scene = want_scene ? 1 : 0; p.want_object = want_obj ? 1 : 0;
+    p.obj_out = want_obj ? w.obj : nullptr;
+    p.ray_const = w.ray_const;
+    rc = want_obj ? onerf_launch_field_bf16_codes(ctx, p, K, w.rc_stride, w.obj_stride, stream)
+                  : onerf_launch_field_bf16(ctx, p, stream);
+    if (rc != ONERF_OK) return rc;
+  } else {   // ONERF_PREC_FP32: the FFMA field once for the scene, once per code for the object branch
+    FieldParams p = base;
+    if (want_scene) {
+      p.want_scene = 1;
+      p.ray_const = w.ray_const;
+      rc = onerf_launch_field_fp32(ctx, p, stream);
+      if (rc != ONERF_OK) return rc;
+    }
+    for (int k = 0; k < (want_obj ? K : 0); ++k) {
+      p = base;
+      p.want_object = 1;
+      p.ray_const = w.ray_const + k * w.rc_stride;
+      p.obj_out = w.obj + k * w.obj_stride;
+      rc = onerf_launch_field_fp32(ctx, p, stream);
+      if (rc != ONERF_OK) return rc;
+    }
+  }
+  if (want_scene) {
+    onerf_composite_args c;
+    memset(&c, 0, sizeof(c));
+    c.z = z; c.scene = w.scene; c.obj = nullptr;
+    c.n_rays = n; c.n_samples = S;
+    c.white_back = ra.white_back; c.is_eval = 1; c.zero_last_delta = ra.zero_last_delta;
+    c.weights = w_out;
+    c.opacity = m.opacity ? m.opacity + r0 : w.scratch.opacity;
+    c.rgb = m.rgb ? m.rgb + r0 * 3 : w.scratch.rgb;
+    c.depth = m.depth ? m.depth + r0 : w.scratch.depth;
+    rc = onerf_launch_composite(ctx, &c, nullptr, stream);
+    if (rc != ONERF_OK) return rc;
+  }
+  auto col = [&](float* o, int64_t width) { return o ? o + r0 * K * width : nullptr; };
+  return onerf_launch_composite_instances(ctx, z, w.obj, w.obj_stride, n, S, K, col(m.opacity_instance, 1),
+                                          col(m.depth_instance, 1), col(m.rgb_instance, 3), stream);
+}
+
+extern "C" int onerf_render_instances(onerf_ctx* ctx, const onerf_instances_args* a, void* stream_) {
+  ONERF_CHECK_ARG(ctx && a, "null argument");
+  const onerf_render_args& ra = a->render;
+  const int64_t n_tile = a->ray_end - a->ray_begin;
+  ONERF_CHECK_ARG(a->n_ids >= 1 && a->n_ids <= ONERF_INSTANCES_MAX_CODES, "n_ids outside [1, 64]");
+  ONERF_CHECK_ARG(a->ids_host && a->code_table, "null ids_host / code_table");
+  for (int k = 0; k < a->n_ids; ++k)
+    ONERF_CHECK_ARG(a->ids_host[k] >= 0 && a->ids_host[k] < a->n_codes_table, "object id outside the code table");
+  ONERF_CHECK_ARG(ra.is_eval, "the object maps are those of an evaluation render: is_eval must be set");
+  ONERF_UNSUPPORTED(ra.rays_in_bbox, "rays_in_bbox (the fine depths would follow each object's weights)");
+  ONERF_CHECK_ARG(ra.perturb == 0.0f && ra.noise_std == 0.0f, "perturb and noise_std must be 0");
+  ONERF_CHECK_ARG(!ra.train_ws, "a training workspace is refused: nothing is kept for a backward");
+  ONERF_CHECK_ARG(ra.n_rays >= 0 && ra.n_samples >= 2 && ra.n_importance >= 0, "bad shape");
+  ONERF_UNSUPPORTED((int64_t)ra.n_samples + ra.n_importance > 2048, "S + K > 2048");
+  ONERF_CHECK_ARG(a->ray_begin >= 0 && n_tile >= 0 && a->ray_end <= ra.n_rays, "tile outside the rays");
+  ONERF_CHECK_ARG(a->chunk_rays >= 1, "chunk_rays < 1");
+  ONERF_CHECK_ARG(ra.rays && ra.packed_coarse, "null rays / packed_coarse");
+  ONERF_CHECK_ARG(ra.n_importance == 0 || ra.packed_fine, "n_importance > 0 needs packed_fine");
+  if (ra.grid)
+    ONERF_CHECK_ARG(ra.grid->table && ra.grid->idx_map && ra.grid->voxel_offset && ra.grid->voxel_size &&
+                        ra.grid->voxel_shape && onerf_aligned16(ra.grid->table),
+                    "null / misaligned grid buffer");
+  ONERF_CHECK_ARG(ra.precision == ONERF_PREC_FP32 || ra.precision == ONERF_PREC_BF16, "unknown precision");
+  ONERF_CHECK_ARG(ra.n_importance > 0 || !any_instance_map(a->fine), "fine maps without a fine pass");
+  ONERF_CHECK_ARG(instance_maps_aligned(a->coarse) && instance_maps_aligned(a->fine), "maps must be 4-byte aligned");
+  const int chunk = a->chunk_rays;
+  const size_t need = onerf_render_instances_workspace_bytes(chunk, a->n_ids, ra.n_samples, ra.n_importance);
+  ONERF_CHECK_ARG(ra.workspace && (reinterpret_cast<uintptr_t>(ra.workspace) & 255u) == 0,
+                  "workspace null or not 256-byte aligned");
+  if (ra.workspace_bytes < need) {
+    onerf_set_error("onerf_render_instances: workspace too small (%zu < %zu)", ra.workspace_bytes, need);
+    return ONERF_ERR_BAD_ARG;
+  }
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const InstancesWs w = instances_ws_layout(reinterpret_cast<char*>(ra.workspace), chunk, a->n_ids, ra.n_samples,
+                                            ra.n_importance);
+  const int S = ra.n_samples, SF = ra.n_samples + ra.n_importance;
+  for (int64_t r0 = 0; r0 < n_tile; r0 += chunk) {
+    const int n = (int)(n_tile - r0 < chunk ? n_tile - r0 : chunk);
+    const float* rays = ra.rays + (a->ray_begin + r0) * 8;
+    int rc = onerf_launch_sample_coarse(ctx, rays, n, S, ra.use_disp, 0.0f, nullptr, 0, nullptr, w.z_c, stream);
+    if (rc != ONERF_OK) return rc;
+    rc = instances_pass(ctx, a, w, rays, n, ra.packed_coarse, w.z_c, S, w.w_c, a->coarse, ra.n_importance > 0, r0,
+                        stream);
+    if (rc != ONERF_OK) return rc;
+    if (ra.n_importance == 0) continue;
+    rc = onerf_launch_sample_pdf_merge(ctx, w.z_c, w.w_c, n, S, ra.n_importance, 1, nullptr, 0, nullptr, w.z_f, stream);
+    if (rc != ONERF_OK) return rc;
+    rc = instances_pass(ctx, a, w, rays, n, ra.packed_fine, w.z_f, SF, w.w_f, a->fine, false, r0, stream);
+    if (rc != ONERF_OK) return rc;
+  }
+  return ONERF_OK;
+}

@@ -32,6 +32,13 @@ int onerf_launch_set_maps(onerf_ctx* ctx, const float* z_all, const float* field
                           int n_rays, int n_obj, int n_samples, float* opacity, float* depth, float* rgb,
                           cudaStream_t stream);
 
+// composite.cu: the object maps of n_codes object fields of the same rays and depths z (n_rays,S): field k is the
+// (n_rays,S,4) block at obj + k * obj_stride floats, composited as onerf_composite composites the object branch with
+// is_eval set.  opacity / depth (n_rays,n_codes), rgb (n_rays,n_codes,3); NULL outputs are skipped.
+int onerf_launch_composite_instances(onerf_ctx* ctx, const float* z, const float* obj, int64_t obj_stride, int n_rays,
+                                     int n_samples, int n_codes, float* opacity, float* depth, float* rgb,
+                                     cudaStream_t stream);
+
 // composite.cu: n samples of one set of a source scene onto the frame's depth axis: z_out = z * k, field sigma /= k in
 // place (field: n float4).
 int onerf_launch_rescale_set(onerf_ctx* ctx, const float* z, float* z_out, float* field, int64_t n, float k,

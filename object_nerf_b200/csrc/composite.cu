@@ -160,6 +160,32 @@ __global__ void __launch_bounds__(256) composite_kernel(onerf_composite_args a, 
   if (seed_dev) *seed_dev += ONERF_SEED_ADVANCE;
 }
 
+// One warp per (ray, code): code k's object field of ray r composited with exactly what composite_kernel passes for
+// the object branch with is_eval set and no noise (last delta 0, no occlusion mask, no weights kept, on white), so
+// column k is bit for bit that kernel's opacity_instance / depth_instance / rgb_instance of a render with code k.
+__global__ void __launch_bounds__(256)
+composite_instances_kernel(const float* __restrict__ z_all, const float* __restrict__ obj, int64_t obj_stride, int n_rays,
+                           int S, int K, float* __restrict__ opacity, float* __restrict__ depth, float* __restrict__ rgb) {
+  const int warps_per_block = blockDim.x >> 5;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t n_lists = (int64_t)n_rays * K;
+  for (int64_t l = (int64_t)blockIdx.x * warps_per_block + warp; l < n_lists; l += (int64_t)gridDim.x * warps_per_block) {
+    const int r = (int)(l / K), k = (int)(l % K);
+    const float* z = z_all + (int64_t)r * S;
+    const float4* f = reinterpret_cast<const float4*>(obj + k * obj_stride) + (int64_t)r * S;
+    const Acc ob = warp_sum(composite_branch(z, f, S, 0.0f, 0.0f, nullptr, 0, 3u, r, false, 0.0f, nullptr, lane));
+    if (lane == 0) {
+      if (opacity) opacity[l] = ob.opacity;
+      if (depth) depth[l] = ob.depth;
+      if (rgb) {
+        rgb[l * 3 + 0] = __fadd_rn(__fadd_rn(ob.r, 1.0f), -ob.opacity);
+        rgb[l * 3 + 1] = __fadd_rn(__fadd_rn(ob.g, 1.0f), -ob.opacity);
+        rgb[l * 3 + 2] = __fadd_rn(__fadd_rn(ob.b, 1.0f), -ob.opacity);
+      }
+    }
+  }
+}
+
 // The forward-only call's last device work (onerf_render_rays_fwd_dseed).
 __global__ void seed_advance_kernel(uint64_t* seed_dev) { *seed_dev += ONERF_SEED_ADVANCE; }
 
@@ -447,6 +473,19 @@ int onerf_launch_set_maps(onerf_ctx* ctx, const float* z_all, const float* field
   const int blocks = (int)std::min((lists + warps - 1) / warps, (int64_t)ctx->num_sms * 16);
   set_maps_kernel<<<blocks, warps * 32, 0, stream>>>(z_all, reinterpret_cast<const float4*>(field_all), weights_unsorted,
                                                      n_rays, n_obj, n_samples, opacity, depth, rgb);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
+int onerf_launch_composite_instances(onerf_ctx* ctx, const float* z, const float* obj, int64_t obj_stride, int n_rays,
+                                     int n_samples, int n_codes, float* opacity, float* depth, float* rgb,
+                                     cudaStream_t stream) {
+  if (n_rays == 0 || !(opacity || depth || rgb)) return ONERF_OK;
+  const int warps = 8;
+  const int64_t lists = (int64_t)n_rays * n_codes;
+  const int blocks = (int)std::min((lists + warps - 1) / warps, (int64_t)ctx->num_sms * 8);
+  composite_instances_kernel<<<blocks, warps * 32, 0, stream>>>(z, obj, obj_stride, n_rays, n_samples, n_codes, opacity,
+                                                                depth, rgb);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

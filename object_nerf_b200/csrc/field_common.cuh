@@ -64,6 +64,11 @@ __device__ __forceinline__ bool point_in_boxes(const float* __restrict__ boxes, 
 int onerf_launch_ray_const(onerf_ctx* ctx, const FieldParams& p, cudaStream_t stream);
 int onerf_launch_field_fp32(onerf_ctx* ctx, const FieldParams& p, cudaStream_t stream);
 int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& p, cudaStream_t stream);
+// The tensor-core field with the object branch once per code c in [0, n_codes) on one encoding of each sample: code c's
+// per-ray constants at p.ray_const + c * rc_stride, its outputs at p.obj_out + c * obj_stride (floats), then the scene
+// branch when p.want_scene.  Needs want_object, no training dump.
+int onerf_launch_field_bf16_codes(onerf_ctx* ctx, const FieldParams& p, int n_codes, int64_t rc_stride,
+                                  int64_t obj_stride, cudaStream_t stream);
 
 // box culling of an (N,8) ray set with depths z (N,S) (cull.cu): live[0, *count) = rays whose last depth is not 0, in ray
 // order, slot[r] = position of ray r in that list or -1; rays_c / z_c = the listed rays' rows.  uncull writes the field

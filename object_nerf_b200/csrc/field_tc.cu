@@ -185,8 +185,9 @@ __device__ __forceinline__ float row_sum(float part) {
   return part;
 }
 
-// finish the heads of one branch: sum the four lanes of each row, add the head biases, write (rgb, sigma)
-__device__ __forceinline__ void write_heads(const FieldParams& p, const Rows& R, int branch, float (&part)[2][4]) {
+// finish the heads of one branch: sum the four lanes of each row, add the head biases, write (rgb, sigma) to outp
+__device__ __forceinline__ void write_heads(const FieldParams& p, const Rows& R, int branch, float (&part)[2][4],
+                                            float* outp) {
   const float* Pf = reinterpret_cast<const float*>(p.packed);
   const float* hb = Pf + (branch ? p.L.orgb_b : p.L.rgb_b);
   const float sb = __ldg(Pf + (branch ? p.L.osigma_b : p.L.sigma_b));
@@ -200,7 +201,6 @@ __device__ __forceinline__ void write_heads(const FieldParams& p, const Rows& R,
       const float cg = 1.0f / (1.0f + __expf(-(part[r][2] + __ldg(hb + 1))));
       const float cb = 1.0f / (1.0f + __expf(-(part[r][3] + __ldg(hb + 2))));
       if (R.mute[r] & (branch ? 2 : 1)) sg = -1e5f;
-      float* outp = branch ? p.obj_out : p.scene_out;
       reinterpret_cast<float4*>(outp)[(int64_t)R.ray[r] * p.out_stride + R.si[r]] = make_float4(cr, cg, cb, sg);
     }
   }
@@ -399,8 +399,18 @@ __device__ __forceinline__ Ring cta_prologue(const FieldSmem& S, const TcParams&
   return ring;
 }
 
-template <bool VOXEL, bool DUMP>
-__global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_constant__ TcParams P) {
+// The code loop of the multi-code instance (field_tc_multi_kernel): the object branch runs once per code c in [0, n),
+// with that code's per-ray constants at ray_const + c * rc_stride and its outputs at obj_out + c * obj_stride (floats).
+// Every code's block carries the same direction terms (RC_SDIR, RC_ODIR).  The single-code instances run {1, 0, 0}.
+struct CodeLoop {
+  int n;
+  int64_t rc_stride, obj_stride;
+};
+
+// Body of the field kernels.  MULTI: the object branch once per code of `cl` on the tile's one encoding X, then the
+// scene branch; X is released after S4, or after the last code's O2 in an object-only launch.
+template <bool VOXEL, bool DUMP, bool MULTI>
+__device__ __forceinline__ void field_tc_body(const TcParams& P, const CodeLoop& cl) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const FieldParams& p = P.f;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -420,9 +430,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
 
   if (warp >= PRODUCER_WARP) {
     setmaxnreg_dec<PRODUCER_REGS>();
-    if (warp == PRODUCER_WARP)
-      tc_producer_loop(P.layers, P.n_layers, reinterpret_cast<const uint8_t*>(p.packed), ring, n_tiles);
-    else
+    if (warp == PRODUCER_WARP) {
+      // a multi-code program leads with the six object layers, streamed once per code
+      if constexpr (MULTI)
+        tc_producer_loop(P.layers, P.n_layers, reinterpret_cast<const uint8_t*>(p.packed), ring, n_tiles,
+                         G_ODIR - G_O0 + 1, cl.n);
+      else
+        tc_producer_loop(P.layers, P.n_layers, reinterpret_cast<const uint8_t*>(p.packed), ring, n_tiles);
+    } else
       encoder_loop<VOXEL>(P, sX, meta, x_full, x_free, n_tiles, total);
     return;
   }
@@ -463,24 +478,36 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
     TL_AT(R.tl, 2);
 
     if (p.want_object) {
-      float acc[64];
-      uint32_t h[32];
-      float part[2][4] = {};
-      run_layer<128, XO, 0, EPI_HIDDEN_RC, DUMP>(P, R, ring, sXw, acc, h, h, nullptr, RC_OL0, nullptr, part, 11,
-                                                 onerf_mask_word0(11), x_free, false);
-      run_layer<128, 0, 4, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_O1 * 256, 0, nullptr, part, 12,
-                                             onerf_mask_word0(12));
-      // [X | h1], object code through ray_const
-      run_layer<128, XO, 4, EPI_HIDDEN_RC, DUMP>(P, R, ring, sXw, acc, h, h, nullptr, RC_OL2, nullptr, part, 13,
-                                                 onerf_mask_word0(13), x_free, free_after_o2);
-      run_layer<128, 0, 4, EPI_HIDDEN_SIGMA, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_O3 * 256, 0,
-                                                   Pf + p.L.osigma_w, part, 14, onerf_mask_word0(14));
-      run_layer<128, 0, 4, EPI_FINAL, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_OFIN * 256, 0, nullptr, part, 15, -1);
-      float accd[32];
-      uint32_t hd[16];
-      run_layer<64, 0, 4, EPI_DIR, DUMP>(P, R, ring, sXw, accd, h, hd, nullptr, RC_ODIR, Pf + p.L.orgb_w, part, 16,
-                                         onerf_mask_word0(16));
-      write_heads(p, R, 1, part);
+      // one pass of the object branch per code (one in the single-code instances) on the tile's X
+      const float* rc0[2] = {R.rc[0], R.rc[1]};
+      for (int c = 0; c < (MULTI ? cl.n : 1); ++c) {
+        if constexpr (MULTI) {
+          R.rc[0] = rc0[0] + c * cl.rc_stride;
+          R.rc[1] = rc0[1] + c * cl.rc_stride;
+        }
+        float acc[64];
+        uint32_t h[32];
+        float part[2][4] = {};
+        run_layer<128, XO, 0, EPI_HIDDEN_RC, DUMP>(P, R, ring, sXw, acc, h, h, nullptr, RC_OL0, nullptr, part, 11,
+                                                   onerf_mask_word0(11), x_free, false);
+        run_layer<128, 0, 4, EPI_HIDDEN, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_O1 * 256, 0, nullptr, part, 12,
+                                               onerf_mask_word0(12));
+        // [X | h1], object code through ray_const
+        run_layer<128, XO, 4, EPI_HIDDEN_RC, DUMP>(P, R, ring, sXw, acc, h, h, nullptr, RC_OL2, nullptr, part, 13,
+                                                   onerf_mask_word0(13), x_free, MULTI ? free_after_o2 && c == cl.n - 1 : free_after_o2);
+        run_layer<128, 0, 4, EPI_HIDDEN_SIGMA, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_O3 * 256, 0,
+                                                     Pf + p.L.osigma_w, part, 14, onerf_mask_word0(14));
+        run_layer<128, 0, 4, EPI_FINAL, DUMP>(P, R, ring, sXw, acc, h, h, bias_tab + G_OFIN * 256, 0, nullptr, part, 15, -1);
+        float accd[32];
+        uint32_t hd[16];
+        run_layer<64, 0, 4, EPI_DIR, DUMP>(P, R, ring, sXw, accd, h, hd, nullptr, RC_ODIR, Pf + p.L.orgb_w, part, 16,
+                                           onerf_mask_word0(16));
+        write_heads(p, R, 1, part, MULTI ? p.obj_out + c * cl.obj_stride : p.obj_out);
+      }
+      if constexpr (MULTI) {
+        R.rc[0] = rc0[0];
+        R.rc[1] = rc0[1];
+      }
     }
     if (p.want_scene) {
       float acc[128];
@@ -492,11 +519,28 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_c
       uint32_t hd[32];
       run_layer<128, 0, 8, EPI_DIR, DUMP>(P, R, ring, sXw, accd, h, hd, nullptr, RC_SDIR, Pf + p.L.rgb_w, part, 10,
                                           onerf_mask_word0(10));
-      write_heads(p, R, 0, part);
+      write_heads(p, R, 0, part, p.scene_out);
     }
     TL_AT(R.tl, 51);
     TL_AT(R.tl, 52);
   }
+}
+
+template <bool VOXEL, bool DUMP>
+__global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_kernel(const __grid_constant__ TcParams P) {
+  field_tc_body<VOXEL, DUMP, false>(P, CodeLoop{1, 0, 0});
+}
+
+// Every object code of a render in one pass over the samples (onerf_render_instances): X is encoded once per tile and
+// the object branch runs once per code.  Inference only.
+struct MultiTcParams {
+  TcParams t;
+  CodeLoop codes;
+};
+
+template <bool VOXEL>
+__global__ void __launch_bounds__(NUM_THREADS, 1) field_tc_multi_kernel(const __grid_constant__ MultiTcParams Q) {
+  field_tc_body<VOXEL, false, true>(Q.t, Q.codes);
 }
 
 // =============================== pruning pass (sigma only, voxel model) ===============================
@@ -624,6 +668,25 @@ int onerf_launch_field_bf16(onerf_ctx* ctx, const FieldParams& fp, cudaStream_t 
   auto* kernel = voxel ? (train ? field_tc_kernel<true, true> : field_tc_kernel<true, false>)
                        : (train ? field_tc_kernel<false, true> : field_tc_kernel<false, false>);
   return launch_persistent(ctx, kernel, P, (total + TM - 1) / TM, field_smem(voxel ? 6 : 1, true).bytes, stream);
+}
+
+int onerf_launch_field_bf16_codes(onerf_ctx* ctx, const FieldParams& fp, int n_codes, int64_t rc_stride,
+                                  int64_t obj_stride, cudaStream_t stream) {
+  ONERF_CHECK_ARG(fp.want_object && !fp.train_ws && n_codes >= 1, "a multi-code launch is an object-branch inference");
+  MultiTcParams Q;
+  memset(&Q, 0, sizeof(Q));
+  Q.t.f = fp;
+  add_layers(Q.t, G_O0, G_ODIR);
+  if (fp.want_scene) add_layers(Q.t, G_S0, G_SDIR);
+  Q.t.diag = ctx->tc_diag;
+#ifdef ONERF_FIELD_TIMELINE
+  Q.t.tl = g_timeline;
+#endif
+  Q.codes = CodeLoop{n_codes, rc_stride, obj_stride};
+  const bool voxel = fp.L.use_voxel;
+  const int64_t total = (int64_t)fp.n_rays * fp.S;
+  return launch_persistent(ctx, voxel ? field_tc_multi_kernel<true> : field_tc_multi_kernel<false>, Q,
+                           (total + TM - 1) / TM, field_smem(voxel ? 6 : 1, true).bytes, stream);
 }
 
 int onerf_launch_prune_bf16(onerf_ctx* ctx, const FieldParams& fp, const PruneSource& src, int64_t cell_begin,

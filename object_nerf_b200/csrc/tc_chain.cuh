@@ -51,11 +51,13 @@ __device__ __forceinline__ void ring_init_bars(uint32_t full, uint32_t empty) {
 }
 
 // =============================== weight producer (bulk copies) ===============================
-// The whole warp runs the (uniform) loop; one elected lane talks to the barriers.
+// The whole warp runs the (uniform) loop; one elected lane talks to the barriers.  Per tile the program is layers
+// [0, lead) lead_repeat times, then the rest of the list (the multi-code field kernel repeats its object layers once
+// per code; MAX_LAYERS leaves no room to list them again).
 __device__ __forceinline__ void tc_producer_loop(const WLayer* layers, int n_layers, const uint8_t* blob, Ring r,
-                                                 int64_t n_tiles) {
+                                                 int64_t n_tiles, int lead = 0, int lead_repeat = 1) {
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    for (int l = 0; l < n_layers; ++l) {
+    for (int l = 0, rep = 1; l < n_layers; ++l) {
       const WLayer& Ly = layers[l];
       const int spp = 256 / Ly.N;
       const uint32_t slab_bytes = (uint32_t)Ly.N * 64u;
@@ -69,6 +71,10 @@ __device__ __forceinline__ void tc_producer_loop(const WLayer* layers, int n_lay
         }
         __syncwarp();
         if (++r.stage == NSTAGE) { r.stage = 0; r.phase ^= 1; }
+      }
+      if (rep < lead_repeat && l == lead - 1) {   // the leading group again, from layer 0
+        ++rep;
+        l = -1;
       }
     }
   }

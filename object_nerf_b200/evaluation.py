@@ -14,9 +14,10 @@ For each frame, `evaluate_frames`
 With depth=True the one render also gives the last pass's depth and depth_instance, scored with onerf_depth_metrics
 (metrics.py's definition) against the store's processed depths at scale frames.scale_factor: column 0 the scene over
 the valid pixels with a depth, column k the object depth over those labelled object_ids[k-1].  The same argument as for
-the colours makes the one render exact for every object column.  With masks=True each object is rendered once more per
-frame with its own code at every pixel (frame_batch(frames, f, [k]), keys ("opacity_instance",)): its opacity_instance
-is scored against the pixels labelled k by onerf_mask_metrics.  Neither flag changes the colour render or its scores.
+the colours makes the one render exact for every object column.  With masks=True one more render per frame,
+rendering.render_instances over object_ids, gives every object's opacity_instance with its own code at every pixel
+(what validate_frame gives for frame_batch(frames, f, [k]), bit for bit); column k is scored against the pixels
+labelled object_ids[k] by onerf_mask_metrics.  Neither flag changes the colour render or its scores.
 Valid pixels are those frames.BORDER or more pixels from every edge, the training split's valid_mask.  The loop reads
 nothing back to the host; the per-frame outputs stay on the device.
 
@@ -29,7 +30,7 @@ from typing import Any, Dict, Sequence
 
 import torch
 
-from . import _lib, metrics, training
+from . import _lib, metrics, rendering, training
 from .losses import TERMS
 from .ray_utils import _c2w_host
 
@@ -88,7 +89,8 @@ def evaluate_frames(models: Dict[str, Any], embeddings: Dict[str, Any], code_lib
     metrics.DEPTH_METRICS order, and their NaN-ignoring means over frames "mean_depth_metrics" (7,) and
     "mean_depth_metrics_objects" (K, 7).  depth_range: the (d_min, d_max) clamp of the predictions in metres.
     masks=True adds "iou_objects" and "opacity_l1_objects" (F, K) and "mean_iou_objects", "mean_opacity_l1_objects"
-    (K,); it costs K more renders per frame.  mask_threshold: the opacity at which a pixel counts as covered."""
+    (K,); it costs one more render per frame, whose object branch runs once per object.  mask_threshold: the opacity
+    at which a pixel counts as covered."""
     ids = [int(i) for i in object_ids]
     K = len(ids)
     if K > _lib.METRICS_MAX_IDS:
@@ -126,10 +128,10 @@ def evaluate_frames(models: Dict[str, Any], embeddings: Dict[str, Any], code_lib
                              labels)
             dplan.finalize(f)
         if masks and K:
-            for k, i in enumerate(ids):
-                out = training.validate_frame(models, embeddings, code_library, frame_batch(frames, f, [i], rays),
-                                              _NO_LOSS, keys=("opacity_instance",), **render)
-                mplan.accumulate(k, out[f"opacity_instance_{typ}"], labels, batch["valid_mask"])
+            out = rendering.render_instances(models, embeddings, code_library, rays, ids, keys=("opacity_instance",),
+                                             **render)
+            for k in range(K):
+                mplan.accumulate(k, out[f"opacity_instance_{typ}"][:, k], labels, batch["valid_mask"])
             mplan.finalize(f)
     P, S = plan.psnr, plan.ssim
     res = {"psnr": P[:, 0], "ssim": S[:, 0], "psnr_objects": P[:, 1:], "ssim_objects": S[:, 1:],

@@ -9,13 +9,15 @@ Extra keyword-only knobs (absorbed by **dummy_kwargs in the reference, so call s
 """
 from __future__ import annotations
 
-from typing import Any, Dict, Optional
+import ctypes as C
+import weakref
+from typing import Any, Dict, Optional, Sequence
 
 import torch
 
-from . import engine
+from . import _lib, engine
 
-__all__ = ["render_rays", "sample_pdf", "inference_model"]
+__all__ = ["render_rays", "sample_pdf", "inference_model", "render_instances"]
 
 
 def _is_voxel(embedding_xyz) -> bool:
@@ -221,3 +223,120 @@ def _result_keys(model_order, forward_instance):
     base = ["weights", "opacity", "z_vals", "rgb", "depth"] + (
         ["rgb_instance", "depth_instance", "opacity_instance"] if forward_instance else [])
     return [f"{k}_{typ}" for typ in model_order for k in base]
+
+
+# ------------------------------------------------------------------------------------------------
+# every object's maps in one render
+# ------------------------------------------------------------------------------------------------
+INSTANCE_KEYS = ("rgb", "depth", "opacity", "opacity_instance", "depth_instance", "rgb_instance")
+# render_instances keeps its per-chunk workspace (the field rows of K codes) within this many bytes by shrinking chunk
+INSTANCES_WORKSPACE_BUDGET = 1 << 30
+_instance_plans: "weakref.WeakKeyDictionary[Any, Dict[tuple, _InstancesPlan]]" = weakref.WeakKeyDictionary()
+
+
+def _instances_chunk(chunk: int, K: int, n_samples: int, n_importance: int) -> int:
+    """The largest chunk <= `chunk` whose onerf_render_instances workspace fits INSTANCES_WORKSPACE_BUDGET, or 1."""
+    ws = _lib.load().onerf_render_instances_workspace_bytes
+    while chunk > 1 and ws(chunk, K, n_samples, n_importance) > INSTANCES_WORKSPACE_BUDGET:
+        chunk = max(1, min(chunk - 1, chunk * INSTANCES_WORKSPACE_BUDGET // ws(chunk, K, n_samples, n_importance)))
+    return chunk
+
+
+class _InstancesPlan:
+    """Every buffer one configuration of render_instances owns: the packed weights, the tile's maps and the argument
+    block."""
+
+    def __init__(self, models, n, tile, cfg, maps, ids, dev, use_voxel):
+        from . import training
+        self.model_order = ["coarse"] + (["fine"] if cfg["N_importance"] > 0 else [])
+        self.packed = training._packed_blobs(models, self.model_order, use_voxel, dev)
+        K = len(ids)
+        widths = {"rgb": (3,), "depth": (), "opacity": (), "opacity_instance": (K,), "depth_instance": (K,),
+                  "rgb_instance": (K, 3)}
+        self.maps = {f"{k}_{typ}": torch.empty((tile,) + widths[k], dtype=torch.float32, device=dev) for k, typ in maps}
+        self.ids = (C.c_int * K)(*ids)
+        a = self.args = _lib.InstancesArgs()
+        r = a.render
+        r.n_rays, r.n_samples, r.n_importance = n, cfg["N_samples"], cfg["N_importance"]
+        r.precision = engine.PRECISIONS[cfg["precision"]]
+        r.use_disp, r.white_back, r.is_eval = int(cfg["use_disp"]), int(cfg["white_back"]), 1
+        r.packed_coarse = self.packed["coarse"].data_ptr()
+        r.packed_fine = self.packed["fine"].data_ptr() if "fine" in self.packed else None
+        for k, typ in maps:
+            setattr(getattr(a, typ), k, self.maps[f"{k}_{typ}"].data_ptr())
+        a.ids_host, a.n_ids = C.cast(self.ids, C.POINTER(C.c_int)), K
+        a.chunk_rays = _instances_chunk(cfg["chunk"], K, cfg["N_samples"], cfg["N_importance"])
+
+
+def render_instances(models: Dict[str, Any], embeddings: Dict[str, Any], code_library, rays: torch.Tensor,
+                     ids: Sequence[int], *, N_samples: int, N_importance: int, use_disp: bool, white_back: bool = False,
+                     chunk: int = 65536, keys: Sequence[str] = INSTANCE_KEYS, precision: str = "bf16", group=None):
+    """Every object's own maps of `rays` (N, 8) in one render (onerf_render_instances).  Not a reference function:
+    it returns, for K = len(ids) object codes code_library rows ids[k] (1 <= K <= 64, repeats allowed), what the
+    reference's render_rays(..., embedding_instance=code of ids[k] on every ray, forward_instance=True, is_eval=True,
+    perturb=0, noise_std=0, rays_in_bbox=False) returns, in one pass: the samples, the scene branch and each sample's
+    encoding, which do not depend on the code, are computed once, and only the object branch runs per code.
+    Column k of each object map is bit for bit that render's map at the same precision, and the scene maps are its
+    scene maps.
+
+    keys: of INSTANCE_KEYS, for the last pass (f"{key}_fine", or f"{key}_coarse" without a fine pass); a key written
+    f"{key}_coarse" (or "_fine") selects that pass, so both passes' maps can be asked for.  Only the branches the asked
+    maps need run: a pass without an object map skips the object branch, the fine pass without a scene map the scene
+    branch.  Returns {name: device tensor}: rgb (N, 3), depth and opacity (N,), opacity_instance and depth_instance
+    (N, K), rgb_instance (N, K, 3).  The tensors belong to a plan cached per configuration and are overwritten by the
+    next call with it.
+    chunk: rays per kernel chunk, lowered so that the workspace stays within INSTANCES_WORKSPACE_BUDGET bytes.  The
+    workspace is cached per (device, size) for the life of the process, as validate_frame's and render_frame's are, so
+    that a captured call keeps valid addresses: each distinct (K, chunk, samples) configuration holds up to
+    INSTANCES_WORKSPACE_BUDGET bytes (1 GiB) of device memory.  Lower the budget (or chunk) to hold less.
+    group: a torch.distributed process group; rank r renders parallel.shard_bounds(N, W, r) and the maps are
+    all-gathered, so every rank returns the whole of them."""
+    from . import editing, parallel, training
+    ids = [int(i) for i in ids]
+    K = len(ids)
+    if not 1 <= K <= _lib.INSTANCES_MAX_CODES:
+        raise ValueError(f"render_instances: 1 to {_lib.INSTANCES_MAX_CODES} object ids, got {K}")
+    if int(chunk) < 1:
+        raise ValueError("render_instances: chunk must be at least 1 ray")
+    last = "fine" if N_importance > 0 else "coarse"
+    maps = []
+    for key in keys:
+        base, _, typ = key.rpartition("_")
+        base, typ = (base, typ) if typ in ("coarse", "fine") else (key, last)
+        if base not in INSTANCE_KEYS or (typ == "fine" and N_importance == 0):
+            raise KeyError(f"render_instances: no such map {key!r} (choose from {INSTANCE_KEYS}, optionally with "
+                           f"_coarse or _fine)")
+        maps.append((base, typ))
+    maps = tuple(dict.fromkeys(maps))
+    rays = rays.reshape(-1, rays.shape[-1])[:, :8].float().contiguous()
+    n, dev = rays.shape[0], rays.device
+    emb_xyz = embeddings["xyz"]
+    use_voxel = _is_voxel(emb_xyz)
+    cfg = dict(N_samples=int(N_samples), N_importance=int(N_importance), use_disp=bool(use_disp),
+               white_back=bool(white_back), chunk=int(chunk), precision=engine.train_precision(precision))
+    begin, end = 0, n
+    if group is not None:
+        import torch.distributed as dist
+        begin, end = parallel.shard_bounds(n, dist.get_world_size(group), dist.get_rank(group))
+    plans = _instance_plans.setdefault(models["coarse"], {})
+    key = (dev, n, begin, end, use_voxel, tuple(sorted(cfg.items())), maps, tuple(ids))
+    plan = plans.get(key)
+    if plan is None:
+        plan = plans[key] = _InstancesPlan(models, n, end - begin, cfg, maps, ids, dev, use_voxel)
+    a = plan.args
+    code_table = training._f32_param(code_library.embedding_instance.weight)
+    a.render.rays = rays.data_ptr()
+    a.code_table, a.n_codes_table = code_table.data_ptr(), code_table.shape[0]
+    grid = engine.GridBuffers.from_module(emb_xyz) if use_voxel else None
+    a.render.grid = C.pointer(grid.c) if use_voxel else None
+    a.ray_begin, a.ray_end = begin, end
+    ws = editing._workspace(_lib.load().onerf_render_instances_workspace_bytes(a.chunk_rays, K, cfg["N_samples"],
+                                                                              cfg["N_importance"]), dev)
+    a.render.workspace, a.render.workspace_bytes = ws.data_ptr(), ws.numel()
+    for typ in plan.model_order:
+        training._pack(models, typ, use_voxel, plan.packed)
+    if end > begin:                  # an empty tile renders nothing (and its rays may have no storage)
+        _lib.call("onerf_render_instances", dev, C.byref(a))
+    if group is None:
+        return dict(plan.maps)
+    return {k: parallel.gather_tiles(v, n, group) for k, v in plan.maps.items()}
