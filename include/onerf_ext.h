@@ -695,6 +695,79 @@ typedef struct onerf_instances_args {
 size_t onerf_render_instances_workspace_bytes(int chunk_rays, int n_codes, int n_samples, int n_importance);
 int onerf_render_instances(onerf_ctx* ctx, const onerf_instances_args* args, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Every object rendered inside its own box, from a camera, in one call: the object evaluation of a dataset with
+ * use_bbox (GenericDataset's test split clips each ray to the object's box and scores instance_mask * bbox_mask; the
+ * validation render runs with rays_in_bbox, so the object's weights drive the importance samples).
+ * For K boxes boxes_host[k] with code rows ids_host[k] (1 <= K <= 64, repeats allowed), object k's rays are
+ * onerf_camera_rays(H, W, focal, c2w_host, &boxes_host[k], scale_factor, near, far) and hit_k that call's hit_out:
+ *   hit pixel of object k: its opacity, depth and rgb (on white) of each pass are bit for bit the opacity_instance /
+ *     depth_instance / rgb_instance of onerf_render_rays_fwd over those rays with code_table[ids_host[k]] on every ray,
+ *     forward_instance, is_eval, rays_in_bbox = 1, perturb = 0, noise_std = 0, at the same precision;
+ *   missed pixel of object k: opacity +0, depth +0, rgb 1, what the editing path's muted field gives.  (The reference's
+ *     render evaluates such rays at z = 0 instead; its metrics exclude them through instance_mask * bbox_mask.)
+ * Every map given is first set to the missed values.  The rows are the (object, pixel) pairs of the tile, object-major (row k * T + p is pixel p_begin + p of object k,
+ * T = p_end - p_begin), processed chunk_rays rows at a time.  Per chunk: the rows' box-clipped rays and hit bits (the
+ * camera-ray kernel's pixel ray and float64 slab test); the hit rows listed in row order and their rays gathered; then,
+ * on the listed rows only and stopping at the device-side count, the coarse depths,
+ * the object branch and its compositing with rays_in_bbox semantics, whose weights feed the importance sampler, and
+ * the fine pass.  No scene branch runs.
+ *   grid (NULL: plain PE model), packed_coarse / packed_fine (the latter iff n_importance > 0), precision, n_samples,
+ *   n_importance, use_disp: as onerf_render_args.  H, W, focal, c2w_host (12 floats, host, row-major 3x4): the camera.
+ *   boxes_host: n_boxes boxes (host array).  scale_factor: as onerf_camera_rays.  near, far: not read (every ray takes
+ *   its near / far from its box, as onerf_camera_rays' rays with a box do); kept for the camera call's argument set.
+ *   ids_host: n_boxes ints
+ *   (host), each a row of code_table (n_codes_table,64), 16-byte aligned.
+ *   pixel_begin, pixel_end: the tile [pixel_begin, pixel_end) of the H*W pixels (row-major).
+ *   coarse, fine: tile-sized maps, T rows: opacity and depth (T,K), rgb (T,K,3); column k is object k.  Any may be NULL
+ *   (not written); fine maps need n_importance > 0.  hit: (T,K) u8 or NULL.  4-byte aligned (any alignment for hit).
+ *   workspace: >= onerf_render_boxes_workspace_bytes(chunk_rays, n_samples, n_importance) bytes, 256-byte aligned (0
+ *   for a bad shape).  Its size depends on neither K nor the image.
+ * Every row depends on its pixel and box only, never on chunk_rays or the tile.  Refusals before any launch: a NULL ctx
+ * or args; n_boxes outside [1, 64]; a NULL boxes_host, ids_host or code_table, an id outside the code table; a
+ * non-finite box entry, camera entry or scale_factor, H or W < 1, focal <= 0 or scale_factor <= 0; a tile
+ * outside [0, H*W]; chunk_rays < 1; a bad shape; NULL packed weights; a NULL or misaligned grid buffer; an unknown
+ * precision; fine maps without a fine pass; a misaligned code table or map; a misaligned or undersized workspace
+ * (ONERF_ERR_BAD_ARG); n_importance > 0 with n_samples + n_importance > 2048, as onerf_render_rays_fwd
+ * (ONERF_ERR_UNSUPPORTED).  Kernels only, no allocation and no
+ * host read: CUDA-graph capturable.
+ * ------------------------------------------------------------------------------------------- */
+#define ONERF_BOXES_MAX 64
+
+typedef struct onerf_box_maps {
+  float* opacity;                       /* (T,K) */
+  float* depth;                         /* (T,K) */
+  float* rgb;                           /* (T,K,3) */
+} onerf_box_maps;
+
+typedef struct onerf_render_boxes_args {
+  const onerf_grid* grid;               /* NULL -> plain PE model */
+  const void* packed_coarse;
+  const void* packed_fine;              /* required iff n_importance > 0 */
+  int precision;                        /* onerf_precision */
+  int n_samples, n_importance;
+  int use_disp;
+  int H, W;
+  float focal;
+  const float* c2w_host;                /* 12 floats (host) */
+  const onerf_box_host* boxes_host;     /* (n_boxes,) host array */
+  int n_boxes;                          /* K */
+  double scale_factor, near, far;
+  const int* ids_host;                  /* (n_boxes,) host array */
+  const float* code_table;              /* (n_codes_table,64) */
+  int n_codes_table;
+  int64_t pixel_begin, pixel_end;
+  int chunk_rays;
+  onerf_box_maps coarse;
+  onerf_box_maps fine;                  /* n_importance > 0 only */
+  uint8_t* hit;                         /* (T,K) or NULL */
+  void* workspace;
+  size_t workspace_bytes;
+} onerf_render_boxes_args;
+
+size_t onerf_render_boxes_workspace_bytes(int chunk_rays, int n_samples, int n_importance);
+int onerf_render_boxes(onerf_ctx* ctx, const onerf_render_boxes_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

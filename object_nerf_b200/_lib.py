@@ -48,7 +48,8 @@ EXPORTS_EXT = ["onerf_composite_multi_workspace_bytes", "onerf_composite_multi_w
                "onerf_render_edit_scenes_workspace_bytes", "onerf_render_edit_frame_scenes",
                "onerf_image_metrics", "onerf_image_metrics_finalize", "onerf_depth_metrics",
                "onerf_depth_metrics_finalize", "onerf_mask_metrics", "onerf_mask_metrics_finalize",
-               "onerf_render_instances_workspace_bytes", "onerf_render_instances"]
+               "onerf_render_instances_workspace_bytes", "onerf_render_instances",
+               "onerf_render_boxes_workspace_bytes", "onerf_render_boxes"]
 VALIDATE_RECORD_DOUBLES = 18
 PRUNE_SAMPLES = 4096
 PSNR_VALID_INSTANCE, PSNR_ALL_RAYS = 0, 1
@@ -57,6 +58,7 @@ STREAM_MULTI_NOISE_COARSE, STREAM_MULTI_NOISE_FINE = 7, 8   # Philox streams of 
 METRICS_MAX_WINDOW, METRICS_MAX_IDS = 11, 64                 # onerf_image_metrics: largest window, most object columns
 DEPTH_METRICS, DEPTH_RECORD, MASK_RECORD = 7, 8, 4           # outputs and record sums per column: depth; sums: mask
 INSTANCES_MAX_CODES = 64                                     # onerf_render_instances: most object codes per render
+BOXES_MAX = 64                                               # onerf_render_boxes: most object boxes per render
 
 _p = C.c_void_p
 
@@ -225,6 +227,20 @@ class InstancesArgs(C.Structure):
                 ("coarse", InstanceMaps), ("fine", InstanceMaps)]
 
 
+class BoxMaps(C.Structure):
+    _fields_ = [("opacity", _p), ("depth", _p), ("rgb", _p)]
+
+
+class RenderBoxesArgs(C.Structure):
+    _fields_ = [("grid", C.POINTER(Grid)), ("packed_coarse", _p), ("packed_fine", _p), ("precision", C.c_int),
+                ("n_samples", C.c_int), ("n_importance", C.c_int), ("use_disp", C.c_int), ("H", C.c_int), ("W", C.c_int),
+                ("focal", C.c_float), ("c2w_host", C.POINTER(C.c_float)), ("boxes_host", C.POINTER(BoxHost)),
+                ("n_boxes", C.c_int), ("scale_factor", C.c_double), ("near", C.c_double), ("far", C.c_double),
+                ("ids_host", C.POINTER(C.c_int)), ("code_table", _p), ("n_codes_table", C.c_int),
+                ("pixel_begin", C.c_int64), ("pixel_end", C.c_int64), ("chunk_rays", C.c_int), ("coarse", BoxMaps),
+                ("fine", BoxMaps), ("hit", _p), ("workspace", _p), ("workspace_bytes", C.c_size_t)]
+
+
 class PruneArgs(C.Structure):
     _fields_ = [
         ("grid", C.POINTER(Grid)), ("packed", _p), ("precision", C.c_int), ("cells", _p), ("n_cells", C.c_int64),
@@ -387,6 +403,9 @@ def load() -> C.CDLL:
         lib.onerf_render_instances_workspace_bytes.argtypes = [C.c_int] * 4
         lib.onerf_render_instances_workspace_bytes.restype = C.c_size_t
         lib.onerf_render_instances.argtypes = [_p, C.POINTER(InstancesArgs), _p]
+        lib.onerf_render_boxes_workspace_bytes.argtypes = [C.c_int] * 3
+        lib.onerf_render_boxes_workspace_bytes.restype = C.c_size_t
+        lib.onerf_render_boxes.argtypes = [_p, C.POINTER(RenderBoxesArgs), _p]
         if lib.onerf_abi_version() != ABI_VERSION:
             raise RuntimeError("libonerf_sm90.so ABI version mismatch")
         _lib = lib

@@ -25,6 +25,12 @@ void onerf_set_error(const char* fmt, ...);
 int onerf_launch_camera_rays(onerf_ctx* ctx, int H, int W, float focal, const float* c2w_host, const onerf_box_host* box,
                              double scale_factor, double near, double far, int64_t p0, int64_t n, float* rays_out,
                              uint8_t* hit_out, cudaStream_t stream);
+// rays.cu: rows [g0, g0 + n) of onerf_render_boxes' (object, pixel) rows of the tile of T pixels from p_begin (row g is
+// pixel p_begin + g % T clipped to boxes[g / T], K boxes): their rays to rays_out (n,8) and hit bits to hit_rows (n,), and
+// to hit_out[(g % T) * K + g / T] when hit_out is given.  The arguments are the caller's to check.
+int onerf_launch_box_rays(onerf_ctx* ctx, int H, int W, float focal, const float* c2w_host, const onerf_box_host* boxes,
+                          int K, double scale_factor, int64_t p_begin, int64_t T, int64_t g0, int n, float* rays_out,
+                          uint8_t* hit_rows, uint8_t* hit_out, cudaStream_t stream);
 
 // composite.cu: the per-set maps of one joint compositing from its weights in set order (weights_unsorted of
 // onerf_composite_multi_ws), depths z_all (n_obj,N,S) and fields field_all (n_obj,N,S,4); NULL outputs are skipped.

@@ -6,6 +6,7 @@
 #include <string.h>
 
 #include "camera.cuh"
+#include "../../include/onerf_ext.h"
 
 namespace {
 
@@ -108,6 +109,36 @@ __global__ void __launch_bounds__(256) camera_rays_kernel(Cam c, BoxParams b, in
   }
 }
 
+// onerf_render_boxes: rows [g0, g0 + n) of the (object, pixel) rows of a tile of T pixels, object-major (row g is pixel
+// p_begin + g % T of box g / T).  Row i of out / hit_rows is that row's ray as camera_rays_kernel writes it with the
+// row's box; hit_out, when given, gets the hit bit at [(g % T) * K + g / T] as well.
+struct BoxRaysParams {
+  Cam c;
+  BoxParams b[ONERF_BOXES_MAX];
+  int64_t p_begin, T, g0;
+  int n, K;
+};
+
+__global__ void __launch_bounds__(256) box_rays_kernel(const __grid_constant__ BoxRaysParams q, float* __restrict__ out,
+                                                       uint8_t* __restrict__ hit_rows, uint8_t* __restrict__ hit_out) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < q.n; i += gridDim.x * blockDim.x) {
+    const int64_t g = q.g0 + i;
+    const int k = (int)(g / q.T);
+    const int64_t t = g - (int64_t)k * q.T, p = q.p_begin + t;
+    const Cam& c = q.c;
+    const int y = (int)(p / c.W), x = (int)(p - (int64_t)y * c.W);
+    float dx, dy, dz, wx, wy, wz, near, far;
+    pixel_direction(c, x, y, dx, dy, dz);
+    rotate_normalise(c, dx, dy, dz, wx, wy, wz);
+    const bool hit = box_near_far(q.b[k], c.t[0], c.t[1], c.t[2], wx, wy, wz, near, far);
+    float4* o4 = reinterpret_cast<float4*>(out + (int64_t)i * 8);
+    o4[0] = make_float4(c.t[0], c.t[1], c.t[2], wx);
+    o4[1] = make_float4(wy, wz, near, far);
+    hit_rows[i] = hit ? 1 : 0;
+    if (hit_out) hit_out[t * q.K + k] = hit ? 1 : 0;
+  }
+}
+
 int grid_for(const onerf_ctx* ctx, int64_t n) {
   const int64_t want = (n + 255) / 256, cap = (int64_t)ctx->num_sms * 8;   // grid-stride: a multiple of the SM count
   return (int)(want < cap ? (want > 0 ? want : 1) : cap);
@@ -195,6 +226,23 @@ int onerf_launch_camera_rays(onerf_ctx* ctx, int H, int W, float focal, const fl
   if (n == 0) return ONERF_OK;
   const Cam c = make_cam(H, W, focal, c2w_host);
   camera_rays_kernel<<<grid_for(ctx, n), 256, 0, stream>>>(c, b, p0, n, rays_out, hit_out);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
+int onerf_launch_box_rays(onerf_ctx* ctx, int H, int W, float focal, const float* c2w_host, const onerf_box_host* boxes,
+                          int K, double scale_factor, int64_t p_begin, int64_t T, int64_t g0, int n, float* rays_out,
+                          uint8_t* hit_rows, uint8_t* hit_out, cudaStream_t stream) {
+  if (n == 0) return ONERF_OK;
+  BoxRaysParams q;
+  memset(&q, 0, sizeof(q));
+  q.c = make_cam(H, W, focal, c2w_host);
+  for (int k = 0; k < K; ++k) {
+    const int rc = make_box(&boxes[k], scale_factor, 0.0, 0.0, q.b[k]);
+    if (rc != ONERF_OK) return rc;
+  }
+  q.p_begin = p_begin; q.T = T; q.g0 = g0; q.n = n; q.K = K;
+  box_rays_kernel<<<grid_for(ctx, n), 256, 0, stream>>>(q, rays_out, hit_rows, hit_out);
   ONERF_LAUNCH_CHECK(ctx);
   return ONERF_OK;
 }

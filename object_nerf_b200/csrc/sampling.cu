@@ -2,6 +2,8 @@
 // the sorted merge.  HBM-bound, one pass over the data; see DESIGN.md §kernels.
 //
 // Reference behaviour: models/rendering.py:259-277 (stratified), :11-61 (sample_pdf), :301-313 (merge).
+#include <algorithm>
+
 #include "common.cuh"
 #include "train_ws.h"
 #include "../../include/onerf_ext.h"
@@ -27,9 +29,9 @@ __device__ __forceinline__ float coarse_depth(float near, float far, int i, int 
 }
 
 // seed_dev != null: the draws use seed + *seed_dev (the caller passes only the offset in `seed`); see onerf_ext.h
-__global__ void __launch_bounds__(256)
-sample_coarse_kernel(const float* __restrict__ rays, int n_rays, int S, int use_disp, float perturb,
-                     const float* __restrict__ jitter, uint64_t seed, const uint64_t* seed_dev, float* __restrict__ z_out) {
+__device__ __forceinline__ void sample_coarse_rows(const float* __restrict__ rays, int n_rays, int S, int use_disp,
+                                                   float perturb, const float* __restrict__ jitter, uint64_t seed,
+                                                   const uint64_t* seed_dev, float* __restrict__ z_out) {
   if (seed_dev && perturb > 0.0f && !jitter) seed += *seed_dev;
   const int64_t total = (int64_t)n_rays * S;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total;
@@ -47,6 +49,19 @@ sample_coarse_kernel(const float* __restrict__ rays, int n_rays, int S, int use_
     }
     z_out[e] = z;
   }
+}
+
+__global__ void __launch_bounds__(256)
+sample_coarse_kernel(const float* __restrict__ rays, int n_rays, int S, int use_disp, float perturb,
+                     const float* __restrict__ jitter, uint64_t seed, const uint64_t* seed_dev, float* __restrict__ z_out) {
+  sample_coarse_rows(rays, n_rays, S, use_disp, perturb, jitter, seed, seed_dev, z_out);
+}
+
+// The deterministic coarse depths of rows [0, min(*count, n_rays)) only (onerf_render_boxes' compacted rows).
+__global__ void __launch_bounds__(256)
+sample_coarse_live_kernel(const float* __restrict__ rays, const int* __restrict__ count, int n_rays, int S, int use_disp,
+                          float* __restrict__ z_out) {
+  sample_coarse_rows(rays, min(*count, n_rays), S, use_disp, 0.0f, nullptr, 0, nullptr, z_out);
 }
 
 // inclusive additive warp scan in double: torch's CPU cumsum accumulates fp32 rows in double and rounds
@@ -67,11 +82,11 @@ __device__ __forceinline__ double warp_scan_add(double v, int lane) {
 // (render_tools/multi_rendering.py:278-287): z with clip[r][0] < z < clip[r][1] (both strict) becomes clip[r][1].
 // The map is monotone, so the stored row stays sorted.
 template <bool kClip>
-__global__ void __launch_bounds__(256)
-sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restrict__ weights, int n_rays,
-                        int S, int K, int P, int det, const float* __restrict__ u_in, uint64_t seed,
-                        const uint64_t* seed_dev, float* __restrict__ z_out, const float* __restrict__ bins_in,
-                        const float* __restrict__ clip) {
+__device__ __forceinline__ void sample_pdf_merge_rows(const float* __restrict__ z_coarse, const float* __restrict__ weights,
+                                                      int n_rays, int S, int K, int P, int det,
+                                                      const float* __restrict__ u_in, uint64_t seed,
+                                                      const uint64_t* seed_dev, float* __restrict__ z_out,
+                                                      const float* __restrict__ bins_in, const float* __restrict__ clip) {
   // bins_in != null: stand-alone sample_pdf on explicit bins (N, S-1) and weights (N, S-2): no merge,
   // z_out (N, K) in draw order.  Otherwise the fused form on coarse depths / full coarse weights.
   // seed_dev != null: as in sample_coarse_kernel.
@@ -154,7 +169,49 @@ sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restr
   }
 }
 
+template <bool kClip>
+__global__ void __launch_bounds__(256)
+sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restrict__ weights, int n_rays,
+                        int S, int K, int P, int det, const float* __restrict__ u_in, uint64_t seed,
+                        const uint64_t* seed_dev, float* __restrict__ z_out, const float* __restrict__ bins_in,
+                        const float* __restrict__ clip) {
+  sample_pdf_merge_rows<kClip>(z_coarse, weights, n_rays, S, K, P, det, u_in, seed, seed_dev, z_out, bins_in, clip);
+}
+
+// The deterministic fused form on rows [0, min(*count, n_rays)) only (onerf_render_boxes' compacted rows).
+__global__ void __launch_bounds__(256)
+sample_pdf_merge_live_kernel(const float* __restrict__ z_coarse, const float* __restrict__ weights,
+                             const int* __restrict__ count, int n_rays, int S, int K, int P, float* __restrict__ z_out) {
+  sample_pdf_merge_rows<false>(z_coarse, weights, min(*count, n_rays), S, K, P, 1, nullptr, 0, nullptr, z_out, nullptr,
+                               nullptr);
+}
+
 }  // namespace
+
+int onerf_launch_sample_coarse_live(onerf_ctx* ctx, const float* rays, const int* count, int n_rays, int n_samples,
+                                    int use_disp, float* z_out, cudaStream_t stream) {
+  if (n_rays == 0) return ONERF_OK;
+  const int64_t total = (int64_t)n_rays * n_samples;
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, (int64_t)ctx->num_sms * 16);
+  sample_coarse_live_kernel<<<blocks, 256, 0, stream>>>(rays, count, n_rays, n_samples, use_disp, z_out);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
+
+int onerf_launch_sample_pdf_merge_live(onerf_ctx* ctx, const float* z_coarse, const float* weights, const int* count,
+                                       int n_rays, int n_samples, int n_importance, float* z_out, cudaStream_t stream) {
+  if (n_rays == 0) return ONERF_OK;
+  int P = 1;
+  while (P < n_samples + n_importance) P <<= 1;
+  const int warps = 8;
+  const size_t smem = (size_t)warps * (2 * n_samples + P) * sizeof(float);
+  ONERF_CUDA(cudaFuncSetAttribute(sample_pdf_merge_live_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int blocks = std::min((n_rays + warps - 1) / warps, ctx->num_sms * 8);
+  sample_pdf_merge_live_kernel<<<blocks, warps * 32, smem, stream>>>(z_coarse, weights, count, n_rays, n_samples,
+                                                                     n_importance, P, z_out);
+  ONERF_LAUNCH_CHECK(ctx);
+  return ONERF_OK;
+}
 
 int onerf_launch_sample_coarse(onerf_ctx* ctx, const float* rays, int n_rays, int n_samples, int use_disp, float perturb,
                                const float* jitter, uint64_t seed, const uint64_t* seed_dev, float* z_out, void* stream) {

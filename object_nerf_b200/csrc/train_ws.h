@@ -120,6 +120,12 @@ int onerf_launch_sample_coarse(onerf_ctx* ctx, const float* rays, int n_rays, in
 int onerf_launch_sample_pdf_merge(onerf_ctx* ctx, const float* z_coarse, const float* weights, int n_rays, int n_samples,
                                   int n_importance, int det, const float* u, uint64_t seed, const uint64_t* seed_dev,
                                   float* z_out, void* stream, const float* clip = nullptr);   // clip: onerf_sample_pdf_merge_clip
+// The deterministic samplers on rows [0, min(*count, n_rays)) only, count on the device (onerf_render_boxes): the same
+// depths, row for row, as onerf_launch_sample_coarse with perturb 0 and onerf_launch_sample_pdf_merge with det 1.
+int onerf_launch_sample_coarse_live(onerf_ctx* ctx, const float* rays, const int* count, int n_rays, int n_samples,
+                                    int use_disp, float* z_out, cudaStream_t stream);
+int onerf_launch_sample_pdf_merge_live(onerf_ctx* ctx, const float* z_coarse, const float* weights, const int* count,
+                                       int n_rays, int n_samples, int n_importance, float* z_out, cudaStream_t stream);
 int onerf_launch_batch_stats(onerf_ctx* ctx, const onerf_loss_args* a, double* acc, cudaStream_t stream);
 // onerf_render_rays_fwd with an optional training step: step == NULL is the plain forward; otherwise both passes'
 // compositing runs onerf_launch_composite_step with `step` (fine / finalize / dscene / dobj set per pass from ws_step),

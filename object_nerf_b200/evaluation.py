@@ -18,6 +18,11 @@ the colours makes the one render exact for every object column.  With masks=True
 rendering.render_instances over object_ids, gives every object's opacity_instance with its own code at every pixel
 (what validate_frame gives for frame_batch(frames, f, [k]), bit for bit); column k is scored against the pixels
 labelled object_ids[k] by onerf_mask_metrics.  Neither flag changes the colour render or its scores.
+With boxes (one per object id, e.g. frames.read_boxes of the dataset's own files), the object columns follow a
+use_bbox dataset's evaluation instead (GenericDataset's test split: rays clipped to the object's box, instance_mask *
+bbox_mask, rays_in_bbox): one rendering.render_boxes call per frame gives every object's maps over its box-clipped
+rays, and object k is scored over the valid pixels labelled object_ids[k] whose ray hits box k, for colour, depth and
+(masks=True: G = label object_ids[k] and hit_k, from the same call's opacity) masks.  The scene columns are unchanged.
 Valid pixels are those frames.BORDER or more pixels from every edge, the training split's valid_mask.  The loop reads
 nothing back to the host; the per-frame outputs stay on the device.
 
@@ -71,10 +76,21 @@ def frame_batch(frames, f: int, object_ids: Sequence[int] = (), rays=None) -> Di
             "instance_ids": inst}
 
 
+def _box_columns(labels, ids, hit, outside: int):
+    """Box mode's per-pixel inputs of the metrics kernels: the labels with every pixel whose object missed its box
+    relabelled `outside` (so object k reads the pixels labelled ids[k] with hit_k, GenericDataset's
+    instance_mask * bbox_mask), and each pixel's column: the position of its label in ids, else 0."""
+    lab = labels.to(torch.int32) & 0xFFFF
+    match = lab.view(-1, 1) == ids.view(1, -1)
+    pick = match.to(torch.uint8).argmax(1)
+    keep = (match & hit).any(1)
+    return metrics._labels16(torch.where(keep, lab, outside)), pick
+
+
 def evaluate_frames(models: Dict[str, Any], embeddings: Dict[str, Any], code_library, frames, conf, *,
                     object_ids: Sequence[int] = (), window: int = 3, chunk: int = 65536, precision: str = "bf16",
                     group=None, depth: bool = False, masks: bool = False, mask_threshold: float = 0.5,
-                    depth_range=(1e-3, 10.0)) -> Dict[str, torch.Tensor]:
+                    depth_range=(1e-3, 10.0), boxes=None) -> Dict[str, torch.Tensor]:
     """PSNR and SSIM of every frame of `frames` (a frames.FrameSet) rendered by the trained model (module docstring).
     conf: the reference's config (conf.model's N_samples, N_importance and use_disp), or that model section itself.
     object_ids: up to 64 object ids to score, each a label of the store's label images and a row of the code table.
@@ -90,7 +106,9 @@ def evaluate_frames(models: Dict[str, Any], embeddings: Dict[str, Any], code_lib
     "mean_depth_metrics_objects" (K, 7).  depth_range: the (d_min, d_max) clamp of the predictions in metres.
     masks=True adds "iou_objects" and "opacity_l1_objects" (F, K) and "mean_iou_objects", "mean_opacity_l1_objects"
     (K,); it costs one more render per frame, whose object branch runs once per object.  mask_threshold: the opacity
-    at which a pixel counts as covered."""
+    at which a pixel counts as covered.
+    boxes: None, or one box per object id (objects with BBoxRayHelper's pose_avg, axis_align_mat and bbox_bounds): the
+    object columns then come from one render_boxes call per frame (module docstring), masks=True included."""
     ids = [int(i) for i in object_ids]
     K = len(ids)
     if K > _lib.METRICS_MAX_IDS:
@@ -104,12 +122,16 @@ def evaluate_frames(models: Dict[str, Any], embeddings: Dict[str, Any], code_lib
     if K and "labels" not in t:
         raise ValueError("evaluate_frames: object columns need the store's label images (load it with an instance "
                          "column that reads a mask)")
+    if boxes is not None and len(boxes) != K:
+        raise ValueError(f"evaluate_frames: one box per object id, got {len(boxes)} boxes for {K} ids")
+    in_boxes = boxes is not None and K > 0
     N_samples, N_importance, use_disp = _model_conf(conf)
     F, H, W, dev = frames.n_frames, frames.H, frames.W, frames.device
     HW, typ = H * W, "fine" if N_importance > 0 else "coarse"
-    keys = ("rgb", "rgb_instance") if K else ("rgb",)
+    keys = ("rgb", "rgb_instance") if K and not in_boxes else ("rgb",)
     if depth:
-        keys += ("depth", "depth_instance") if K else ("depth",)
+        keys += ("depth", "depth_instance") if K and not in_boxes else ("depth",)
+    box_keys = ("rgb_instance",) + (("depth_instance",) if depth else ()) + (("opacity_instance",) if masks else ())
     render = dict(N_samples=N_samples, N_importance=N_importance, use_disp=use_disp, white_back=False, chunk=chunk,
                   precision=precision, group=group)
 
@@ -117,17 +139,35 @@ def evaluate_frames(models: Dict[str, Any], embeddings: Dict[str, Any], code_lib
     dplan = metrics.DepthMetricsPlan(H, W, ids, frames.scale_factor, depth_range, F, dev) if depth else None
     mplan = metrics.MaskMetricsPlan(H, W, ids, mask_threshold, F, dev) if masks else None
     rays = torch.empty(HW, 8, dtype=torch.float32, device=dev)
+    if in_boxes:
+        ids_dev = torch.tensor(ids, dtype=torch.int32, device=dev)
+        outside = min(set(range(K + 1)) - set(ids))        # a label no object column reads
     for f in range(F):
         batch = frame_batch(frames, f, ids, rays)
         out = training.validate_frame(models, embeddings, code_library, batch, _NO_LOSS, keys=keys, **render)
         labels = t["labels"][f] if K else None
+        if in_boxes:
+            out.update(rendering.render_boxes(models, embeddings, code_library, H, W, frames.focal,
+                                              torch.from_numpy(frames.poses_host[f].reshape(3, 4)), boxes, ids,
+                                              N_samples=N_samples, N_importance=N_importance, use_disp=use_disp,
+                                              scale_factor=frames.scale_factor, near=frames.near, far=frames.far,
+                                              chunk=chunk, keys=box_keys, precision=precision, group=group))
+            labels, pick = _box_columns(labels, ids_dev, out["hit"], outside)
+            for key in box_keys[:1 + depth]:         # colour and depth: each pixel's own object's column
+                v = out[f"{key}_{typ}"]
+                out[f"{key}_{typ}"] = v.gather(1, pick.view(HW, 1, *([1] * (v.dim() - 2))).expand(HW, 1, *v.shape[2:]))
         plan.accumulate(out[f"rgb_{typ}"], batch["rgbs"], batch["valid_mask"], out.get(f"rgb_instance_{typ}"), labels)
         plan.finalize(f)
         if depth:
             dplan.accumulate(out[f"depth_{typ}"], t["depths"][f], batch["valid_mask"], out.get(f"depth_instance_{typ}"),
                              labels)
             dplan.finalize(f)
-        if masks and K:
+        if masks and in_boxes:
+            o = out[f"opacity_instance_{typ}"]
+            for k in range(K):
+                mplan.accumulate(k, o[:, k], labels, batch["valid_mask"])
+            mplan.finalize(f)
+        elif masks and K:
             out = rendering.render_instances(models, embeddings, code_library, rays, ids, keys=("opacity_instance",),
                                              **render)
             for k in range(K):

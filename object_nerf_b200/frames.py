@@ -13,11 +13,13 @@ labels, and the depth arithmetic with the reference's own torch ops.
 
 `read_frames(..., split="test")` / `FrameSet.load(..., split="test")` keep the held-out frames instead: those whose idx
 split/test.txt lists, in transforms_full.json order, without the frames whose pose is not finite, decoded exactly as the
-training frames (evaluation.evaluate_frames renders and scores them).
+training frames (evaluation.evaluate_frames renders and scores them).  `FrameSet.load` takes a test split with use_bbox
+too: its frames decode exactly as without it, since the clipping to each object's box belongs to the render
+(rendering.render_boxes over the boxes `read_boxes` reads, evaluate_frames(boxes=...)).
 
 Refused rather than approximated (ValueError, before any device work):
-  - training rays clipped to a box (use_bbox without use_bbox_only_for_test), and for the test split any use_bbox (its
-    rays would be clipped to the object box);
+  - training rays clipped to a box (use_bbox without use_bbox_only_for_test), and read_frames of a test split with
+    use_bbox (its rays would be clipped to the object box; FrameSet.load leaves that clipping to the render);
   - mask_rebalance_strategy other than fg_bg_reweight (distance_transform crashes in the reference itself);
   - a frame whose RGB image is missing (the reference then misaligns its per-instance buffers against all_rays);
   - label images wider than 16 bits, and more than FRAME_MAX_PASS pass-through labels per instance column.
@@ -33,7 +35,7 @@ import torch
 
 from . import _lib, ray_utils
 
-__all__ = ["FrameSet", "read_frames", "BORDER"]
+__all__ = ["FrameSet", "read_frames", "read_boxes", "ObjectBox", "BORDER"]
 
 BORDER = 20                     # black border of undistorted images, masked out of training (generic_dataset.py:44-52)
 MAX_PASS = _lib.FRAME_MAX_PASS
@@ -296,7 +298,10 @@ class FrameSet:
     @classmethod
     def load(cls, dataset_extra, img_wh=(640, 480), device="cuda", split: str = "train") -> "FrameSet":
         """GenericDataset(split="train", img_wh, dataset_extra)'s training frames, kept as pixels (read_frames);
-        split="test": the held-out frames of split/test.txt."""
+        split="test": the held-out frames of split/test.txt.  A test split with use_bbox decodes exactly as without it:
+        GenericDataset clips its rays to the object's box, which render_boxes does at render time."""
+        if split == "test" and dataset_extra["use_bbox"]:
+            dataset_extra = dict(dataset_extra, use_bbox=False)
         return cls(**read_frames(dataset_extra, tuple(img_wh), split), device=device)
 
     @property
@@ -337,3 +342,80 @@ class FrameSet:
                 "all_frame_indices": t["frame_idx"][f_of], "all_instance_masks": torch.stack(masks, -1),
                 "all_instance_masks_weight": torch.stack(weights, -1), "all_instance_ids": torch.stack(ids, -1),
                 "all_pass_through_masks": torch.stack(passes, -1)}
+
+
+# ------------------------------------------------------------------------------------------------
+# object boxes
+# ------------------------------------------------------------------------------------------------
+class ObjectBox:
+    """One object's box with the attributes of the reference's BBoxRayHelper (utils/bbox_utils.py:9-99) that describe
+    it: dataset_name, conf (the dataset_extra section), scale_factor, instance_id, scene_id (scannet_base only),
+    axis_align_mat (4, 4), bbox_bounds (2, 3) = [lo, hi], bbox_c (3,) and pose_avg (4, 4), all float64.  What
+    ray_utils.camera_rays(box=...) and rendering.render_boxes take."""
+
+    def __init__(self, **attrs):
+        self.__dict__.update(attrs)
+
+
+def _scannet_box(conf, instance_id):
+    """BBoxRayHelper.read_bbox_info_scannet (utils/bbox_utils.py:64-84): the first axisAlignment line of
+    scans_dir/<scene_id>/<scene_id>.txt, parsed with the reference's str.strip("axisAlignment = ") (a character set),
+    and the last row of bbox_dir/<scene_id>_bbox.npy whose column 6 is the id."""
+    if "scene_id" not in conf:
+        raise ValueError("read_boxes: a scannet_base dataset_extra needs scene_id (BBoxRayHelper reads conf['scene_id'])")
+    scene_id = conf["scene_id"]
+    with open(os.path.join(conf["scans_dir"], f"{scene_id}/{scene_id}.txt")) as f:
+        lines = f.readlines()
+    align = None
+    for line in lines:
+        if "axisAlignment" in line:
+            align = [float(x) for x in line.rstrip().strip("axisAlignment = ").split(" ")]
+            break
+    if align is None:
+        raise ValueError(f"read_boxes: no axisAlignment line in {scene_id}.txt")
+    center = bounds = None
+    for b in np.load(os.path.join(conf["bbox_dir"], f"{scene_id}_bbox.npy")):
+        if b[6] != instance_id:
+            continue
+        length = np.array([b[3], b[4], b[5]]) * 0.5
+        center = np.array([b[0], b[1], b[2]])
+        bounds = np.array([center - length, center + length])
+    if bounds is None:
+        raise ValueError(f"read_boxes: {scene_id}_bbox.npy has no box for instance id {instance_id}")
+    return dict(scene_id=scene_id, axis_align_mat=np.array(align).reshape(4, 4), bbox_bounds=bounds, bbox_c=center)
+
+
+def _toydesk_box(conf, instance_id):
+    """BBoxRayHelper.read_bbox_info_desk (utils/bbox_utils.py:86-96): the first label of the bbox_dir JSON with this id
+    and a position; axis_align_mat = inv([R(quaternion) | position]), bbox_bounds = [-scale / 2, scale / 2]."""
+    from scipy.spatial.transform import Rotation
+
+    with open(conf["bbox_dir"]) as f:
+        labels = json.load(f)["labels"]
+    for lab in labels:
+        if int(lab["id"]) != instance_id or "position" not in lab["data"]:
+            continue
+        pos, scale = np.array(lab["data"]["position"]), np.array(lab["data"]["scale"])
+        align = np.eye(4)
+        align[:3, :3] = Rotation.from_quat(lab["data"]["quaternion"]).as_matrix()
+        align[:3, 3] = pos
+        return dict(axis_align_mat=np.linalg.inv(align), bbox_bounds=np.array([-scale / 2, scale / 2]), bbox_c=pos)
+    raise ValueError(f"read_boxes: the bbox JSON has no box with a position for instance id {instance_id}")
+
+
+def read_boxes(dataset_name: str, conf, ids: Sequence[int]):
+    """The boxes of objects `ids` as the reference's BBoxRayHelper(config, id) reads them from the dataset's own files
+    (utils/bbox_utils.py:41-99), for dataset_name "scannet_base" or "toydesk"; conf is the dataset_extra section.
+    pose_avg = [I | scene_center].  An id without a box raises ValueError (the reference would reuse a stale centre
+    or fail with a NameError).  Returns one ObjectBox per id, in order."""
+    if dataset_name not in ("scannet_base", "toydesk"):
+        raise ValueError(f"read_boxes: unknown dataset {dataset_name!r} (scannet_base or toydesk)")
+    out = []
+    for i in ids:
+        i = int(i)
+        attrs = _scannet_box(conf, i) if dataset_name == "scannet_base" else _toydesk_box(conf, i)
+        pose_avg = np.eye(4)
+        pose_avg[:3, 3] = np.array(conf["scene_center"])
+        out.append(ObjectBox(dataset_name=dataset_name, conf=conf, scale_factor=conf["scale_factor"], instance_id=i,
+                             pose_avg=pose_avg, **attrs))
+    return out

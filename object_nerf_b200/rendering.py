@@ -17,7 +17,7 @@ import torch
 
 from . import _lib, engine
 
-__all__ = ["render_rays", "sample_pdf", "inference_model", "render_instances"]
+__all__ = ["render_rays", "sample_pdf", "inference_model", "render_instances", "render_boxes"]
 
 
 def _is_voxel(embedding_xyz) -> bool:
@@ -340,3 +340,132 @@ def render_instances(models: Dict[str, Any], embeddings: Dict[str, Any], code_li
     if group is None:
         return dict(plan.maps)
     return {k: parallel.gather_tiles(v, n, group) for k, v in plan.maps.items()}
+
+
+# ------------------------------------------------------------------------------------------------
+# every object inside its own box
+# ------------------------------------------------------------------------------------------------
+BOX_KEYS = ("opacity_instance", "depth_instance", "rgb_instance")
+# render_boxes keeps its per-chunk workspace within this many bytes by shrinking chunk
+BOXES_WORKSPACE_BUDGET = 1 << 30
+_box_plans: "weakref.WeakKeyDictionary[Any, Dict[tuple, _BoxesPlan]]" = weakref.WeakKeyDictionary()
+
+
+def _boxes_chunk(chunk: int, n_samples: int, n_importance: int) -> int:
+    """The largest chunk <= `chunk` whose onerf_render_boxes workspace fits BOXES_WORKSPACE_BUDGET, or 1."""
+    ws = _lib.load().onerf_render_boxes_workspace_bytes
+    while chunk > 1 and ws(chunk, n_samples, n_importance) > BOXES_WORKSPACE_BUDGET:
+        chunk = max(1, min(chunk - 1, chunk * BOXES_WORKSPACE_BUDGET // ws(chunk, n_samples, n_importance)))
+    return chunk
+
+
+class _BoxesPlan:
+    """Every buffer one configuration of render_boxes owns: the packed weights, the tile's maps and hit mask, and the
+    argument block with its host arrays."""
+
+    def __init__(self, models, H, W, tile, cfg, maps, K, dev, use_voxel):
+        from . import training
+        self.model_order = ["coarse"] + (["fine"] if cfg["N_importance"] > 0 else [])
+        self.packed = training._packed_blobs(models, self.model_order, use_voxel, dev)
+        widths = {"opacity_instance": (K,), "depth_instance": (K,), "rgb_instance": (K, 3)}
+        self.maps = {f"{k}_{typ}": torch.empty((tile,) + widths[k], dtype=torch.float32, device=dev) for k, typ in maps}
+        self.hit = torch.empty(tile, K, dtype=torch.uint8, device=dev)
+        self.ids, self.boxes, self.c2w = (C.c_int * K)(), (_lib.BoxHost * K)(), (C.c_float * 12)()
+        a = self.args = _lib.RenderBoxesArgs()
+        a.packed_coarse = self.packed["coarse"].data_ptr()
+        a.packed_fine = self.packed["fine"].data_ptr() if "fine" in self.packed else None
+        a.precision = engine.PRECISIONS[cfg["precision"]]
+        a.n_samples, a.n_importance, a.use_disp = cfg["N_samples"], cfg["N_importance"], int(cfg["use_disp"])
+        a.H, a.W = H, W
+        a.c2w_host, a.boxes_host, a.n_boxes = self.c2w, self.boxes, K
+        a.ids_host = C.cast(self.ids, C.POINTER(C.c_int))
+        fields = {"opacity_instance": "opacity", "depth_instance": "depth", "rgb_instance": "rgb"}
+        for k, typ in maps:
+            setattr(getattr(a, typ), fields[k], self.maps[f"{k}_{typ}"].data_ptr())
+        a.hit = self.hit.data_ptr()
+        a.chunk_rays = _boxes_chunk(cfg["chunk"], cfg["N_samples"], cfg["N_importance"])
+
+
+def render_boxes(models: Dict[str, Any], embeddings: Dict[str, Any], code_library, H: int, W: int, focal: float, c2w,
+                 boxes: Sequence[Any], ids: Sequence[int], *, N_samples: int, N_importance: int, use_disp: bool,
+                 scale_factor: float, near: float, far: float, chunk: int = 65536, keys: Sequence[str] = BOX_KEYS,
+                 precision: str = "bf16", group=None):
+    """Every object rendered inside its own box from one camera (onerf_render_boxes): the object evaluation of a
+    dataset with use_bbox, where GenericDataset clips each test ray to the object's box (near = far = 0 where it misses)
+    and renders with rays_in_bbox, so the object's own weights drive the importance samples.  Not a reference function.
+
+    For K = len(boxes) boxes (1 <= K <= 64; objects with BBoxRayHelper's pose_avg, axis_align_mat and bbox_bounds, such
+    as frames.read_boxes returns) with code_library rows ids[k] (repeats allowed), object k's rays are
+    ray_utils.camera_rays(H, W, focal, c2w, near, far, scale_factor, box=boxes[k]) and hit_k its return_mask:
+      - at a hit pixel, column k of each map is bit for bit the opacity_instance / depth_instance / rgb_instance of the
+        evaluation render of those rays (render_rays / training.validate_frame with is_eval, forward_instance,
+        rays_in_bbox=True, perturb=0, noise_std=0) with code ids[k] on every ray, at the same precision;
+      - at a missed pixel it is opacity +0, depth +0, rgb 1.  The reference's render evaluates those rays at z = 0
+        instead; its metrics exclude them anyway (instance_mask * bbox_mask).
+    No scene branch runs, and the object branch runs only on the rows that hit their box, so the field work follows
+    the pixels the boxes cover.
+
+    keys: of BOX_KEYS, for the last pass, or with a "_coarse" / "_fine" suffix for that pass.  Returns {name: device
+    tensor}: opacity_instance and depth_instance (H*W, K), rgb_instance (H*W, K, 3), and "hit" (H*W, K) bool.  The
+    tensors belong to a plan cached per configuration and are overwritten by the next call with it.
+    chunk: (object, pixel) rows per kernel chunk, lowered so that the workspace stays within BOXES_WORKSPACE_BUDGET
+    bytes; the workspace depends on neither K nor the image and is cached per (device, size) for the life of the
+    process, as render_instances' is.
+    group: a torch.distributed process group; rank r renders the pixels parallel.shard_bounds(H*W, W, r) and the maps
+    are all-gathered, so every rank returns the whole of them."""
+    from . import editing, parallel, ray_utils, training
+    ids = [int(i) for i in ids]
+    K = len(ids)
+    if not 1 <= K <= _lib.BOXES_MAX or len(boxes) != K:
+        raise ValueError(f"render_boxes: 1 to {_lib.BOXES_MAX} boxes, one id each; got {len(boxes)} boxes, {K} ids")
+    if int(chunk) < 1:
+        raise ValueError("render_boxes: chunk must be at least 1 row")
+    last = "fine" if N_importance > 0 else "coarse"
+    maps = []
+    for key in keys:
+        base, _, typ = key.rpartition("_")
+        base, typ = (base, typ) if typ in ("coarse", "fine") else (key, last)
+        if base not in BOX_KEYS or (typ == "fine" and N_importance == 0):
+            raise KeyError(f"render_boxes: no such map {key!r} (choose from {BOX_KEYS}, optionally with _coarse or "
+                           f"_fine)")
+        maps.append((base, typ))
+    maps = tuple(dict.fromkeys(maps))
+    H, W = int(H), int(W)
+    n = H * W
+    table = training._f32_param(code_library.embedding_instance.weight)
+    dev = table.device
+    emb_xyz = embeddings["xyz"]
+    use_voxel = _is_voxel(emb_xyz)
+    cfg = dict(N_samples=int(N_samples), N_importance=int(N_importance), use_disp=bool(use_disp), chunk=int(chunk),
+               precision=engine.train_precision(precision))
+    begin, end = 0, n
+    if group is not None:
+        import torch.distributed as dist
+        begin, end = parallel.shard_bounds(n, dist.get_world_size(group), dist.get_rank(group))
+    plans = _box_plans.setdefault(models["coarse"], {})
+    key = (dev, H, W, begin, end, use_voxel, tuple(sorted(cfg.items())), maps, K)
+    plan = plans.get(key)
+    if plan is None:
+        plan = plans[key] = _BoxesPlan(models, H, W, end - begin, cfg, maps, K, dev, use_voxel)
+    a = plan.args
+    for k in range(K):
+        plan.ids[k] = ids[k]
+        plan.boxes[k] = ray_utils._box_host(boxes[k], 0.0)
+    C.memmove(plan.c2w, ray_utils._c2w_host(c2w), C.sizeof(plan.c2w))
+    a.focal, a.scale_factor, a.near, a.far = float(focal), float(scale_factor), float(near), float(far)
+    a.code_table, a.n_codes_table = table.data_ptr(), table.shape[0]
+    grid = engine.GridBuffers.from_module(emb_xyz) if use_voxel else None
+    a.grid = C.pointer(grid.c) if use_voxel else None
+    a.pixel_begin, a.pixel_end = begin, end
+    ws = editing._workspace(_lib.load().onerf_render_boxes_workspace_bytes(a.chunk_rays, cfg["N_samples"],
+                                                                          cfg["N_importance"]), dev)
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+    for typ in plan.model_order:
+        training._pack(models, typ, use_voxel, plan.packed)
+    if end > begin:
+        _lib.call("onerf_render_boxes", dev, C.byref(a))
+    out = dict(plan.maps, hit=plan.hit)
+    if group is not None:
+        out = {k: parallel.gather_tiles(v, n, group) for k, v in out.items()}
+    out["hit"] = out["hit"].bool()
+    return out
