@@ -76,20 +76,13 @@ static int field_fwd(onerf_ctx* ctx, const onerf_field_args* a, const int* n_liv
   }
   ONERF_CHECK_ARG(a->n_boxes == 0 || a->boxes, "n_boxes > 0 with null boxes");
   ONERF_CHECK_ARG(a->z_stride >= a->n_samples && a->out_stride >= a->n_samples, "bad strides");
-  if (a->grid)
-    ONERF_CHECK_ARG(a->grid->table && a->grid->idx_map && a->grid->voxel_offset && a->grid->voxel_size &&
-                        a->grid->voxel_shape && onerf_aligned16(a->grid->table),
-                    "null / misaligned grid buffer");
-  if (a->n_rays == 0) return ONERF_OK;
+  int rc = onerf_check_grid(__func__, a->grid);
+  if (rc != ONERF_OK || a->n_rays == 0) return rc;
   cudaStream_t stream = (cudaStream_t)stream_;
-  FieldParams p;
-  memset(&p, 0, sizeof(p));
+  FieldParams p = onerf_field_params(a->grid, a->packed);
   p.rays = a->rays; p.xyz = a->xyz; p.z = a->z; p.z_stride = a->z_stride;
   p.codes = a->codes; p.code_row = a->code_row;
   p.n_rays = a->n_rays; p.S = a->n_samples;
-  if (a->grid) p.grid = *a->grid;
-  p.packed = a->packed;
-  p.L = onerf_make_layout(a->grid ? 1 : 0);
   p.want_scene = a->want_scene; p.want_object = a->want_object;
   p.mute_zero_rays = a->mute_zero_rays;
   p.boxes = a->boxes; p.n_boxes = a->n_boxes;
@@ -112,7 +105,7 @@ static int field_fwd(onerf_ctx* ctx, const onerf_field_args* a, const int* n_liv
     ONERF_CHECK_ARG((reinterpret_cast<uintptr_t>(a->train_ws) & 1023u) == 0, "train_ws must be 1024-byte aligned");
     p.train_ws = a->train_ws;
   }
-  int rc = onerf_launch_ray_const(ctx, p, stream);
+  rc = onerf_launch_ray_const(ctx, p, stream);
   if (rc != ONERF_OK) return rc;
   if (a->precision == ONERF_PREC_FP32) return onerf_launch_field_fp32(ctx, p, stream);
   if (a->precision == ONERF_PREC_BF16) return onerf_launch_field_bf16(ctx, p, stream);
@@ -128,13 +121,25 @@ extern "C" int onerf_field_fwd(onerf_ctx* ctx, const onerf_field_args* a, void* 
 // render_rays() forward as one call: composition of the stage entry points (same kernels, same order and seeds as
 // object_nerf_b200/rendering.py::_render_forward, so both routes give bit-identical results).
 // ------------------------------------------------------------------------------------------------
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+struct RenderWs {
+  float *ray_const, *scene, *obj;   // per-ray hoisted terms, (rgb, sigma) of both branches
+  size_t total;
+};
+
+static RenderWs render_ws_layout(char* base, int n_rays, int n_samples, int n_importance) {
+  const size_t n = n_rays, sf = (size_t)n_samples + (size_t)n_importance;
+  WsCarver c{base};
+  RenderWs w;
+  w.ray_const = c.floats(n * ONERF_RAY_CONST_FLOATS);
+  w.scene = c.floats(n * sf * 4);
+  w.obj = c.floats(n * sf * 4);
+  w.total = c.off;
+  return w;
+}
 
 extern "C" size_t onerf_render_rays_workspace_bytes(int n_rays, int n_samples, int n_importance) {
   if (n_rays < 0 || n_samples < 1 || n_importance < 0) return 0;
-  const size_t s_max = (size_t)n_samples + (size_t)n_importance;
-  return align256((size_t)n_rays * ONERF_RAY_CONST_FLOATS * sizeof(float)) +   // per-ray hoisted terms
-         2 * align256((size_t)n_rays * s_max * 4 * sizeof(float));             // (rgb, sigma) of both branches
+  return render_ws_layout(nullptr, n_rays, n_samples, n_importance).total;
 }
 
 static int render_pass(onerf_ctx* ctx, const onerf_render_args* a, const void* packed, const float* z, int S,
@@ -198,23 +203,13 @@ int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const oner
   ONERF_CHECK_ARG(a->n_importance == 0 || a->packed_fine, "n_importance > 0 needs packed_fine");
   ONERF_CHECK_ARG(maps_ok(a->coarse, a->forward_instance), "null coarse output map");
   ONERF_CHECK_ARG(a->n_importance == 0 || maps_ok(a->fine, a->forward_instance), "null fine output map");
-  const size_t need = onerf_render_rays_workspace_bytes(a->n_rays, a->n_samples, a->n_importance);
-  ONERF_CHECK_ARG(a->workspace && (reinterpret_cast<uintptr_t>(a->workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
-  if (a->workspace_bytes < need) {
-    onerf_set_error("onerf_render_rays_fwd: workspace too small (%zu < %zu)", a->workspace_bytes, need);
-    return ONERF_ERR_WORKSPACE;
-  }
-  if (a->n_rays == 0) return ONERF_OK;
+  const RenderWs w = render_ws_layout(reinterpret_cast<char*>(a->workspace), a->n_rays, a->n_samples, a->n_importance);
+  int rc = onerf_check_workspace("onerf_render_rays_fwd", a->workspace, a->workspace_bytes, w.total, ONERF_ERR_WORKSPACE);
+  if (rc != ONERF_OK || a->n_rays == 0) return rc;
   const int S = a->n_samples, SF = a->n_samples + a->n_importance;
-  char* ws = reinterpret_cast<char*>(a->workspace);
-  float* ray_const = reinterpret_cast<float*>(ws);
-  ws += align256((size_t)a->n_rays * ONERF_RAY_CONST_FLOATS * sizeof(float));
-  float* scene = reinterpret_cast<float*>(ws);
-  ws += align256((size_t)a->n_rays * SF * 4 * sizeof(float));
-  float* obj = reinterpret_cast<float*>(ws);
   // training: both passes' fields are kept in the training workspace, and with bf16 the backward operands too (the fp32
   // backward re-runs the FFMA forward chunk by chunk instead)
-  float *scene_c = scene, *obj_c = obj, *scene_f = scene, *obj_f = obj;
+  float *scene_c = w.scene, *obj_c = w.obj, *scene_f = w.scene, *obj_f = w.obj;
   void *tl_c = nullptr, *tl_f = nullptr;
   if (a->train_ws) {
     ONERF_CHECK_ARG((reinterpret_cast<uintptr_t>(a->train_ws) & 1023u) == 0, "train_ws must be 1024-byte aligned");
@@ -250,17 +245,17 @@ int onerf_render_fwd_impl(onerf_ctx* ctx, const onerf_render_args* a, const oner
   // seeds: coarse depths, coarse noise, importance u, fine noise (rendering.py::_render_forward); with seed_dev the kernels
   // add *seed_dev to these offsets
   const uint64_t seed = seed_dev ? 0 : a->seed;
-  int rc = onerf_launch_sample_coarse(ctx, a->rays, a->n_rays, S, a->use_disp, a->perturb, a->jitter, seed, seed_dev,
-                                      a->coarse.z_vals, stream);
+  rc = onerf_launch_sample_coarse(ctx, a->rays, a->n_rays, S, a->use_disp, a->perturb, a->jitter, seed, seed_dev,
+                                  a->coarse.z_vals, stream);
   if (rc != ONERF_OK) return rc;
   rc = render_pass(ctx, a, a->packed_coarse, a->coarse.z_vals, S, a->coarse, a->noise_scene_coarse, a->noise_obj_coarse,
-                   seed + 1, ray_const, scene_c, obj_c, tl_c, step ? &step_c : nullptr, seed_dev, stream);
+                   seed + 1, w.ray_const, scene_c, obj_c, tl_c, step ? &step_c : nullptr, seed_dev, stream);
   if (rc != ONERF_OK || a->n_importance == 0) return rc;
   rc = onerf_launch_sample_pdf_merge(ctx, a->coarse.z_vals, a->coarse.weights, a->n_rays, S, a->n_importance,
                                      a->perturb == 0.0f ? 1 : 0, a->u, seed + 2, seed_dev, a->fine.z_vals, stream);
   if (rc != ONERF_OK) return rc;
   return render_pass(ctx, a, a->packed_fine, a->fine.z_vals, SF, a->fine, a->noise_scene_fine, a->noise_obj_fine, seed + 3,
-                     ray_const, scene_f, obj_f, tl_f, step ? &step_f : nullptr, seed_dev, stream);
+                     w.ray_const, scene_f, obj_f, tl_f, step ? &step_f : nullptr, seed_dev, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -282,22 +277,21 @@ struct MultiWs {
 static MultiWs multi_ws_layout(char* base, int n_rays, int n_obj, int n_samples, int n_importance) {
   const size_t sf = (size_t)n_samples + (size_t)n_importance, no = (size_t)n_obj, n = (size_t)n_rays;
   MultiWs w;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { void* p = base + off; off += align256(bytes); return p; };
-  w.ray_const = (float*)take(n * ONERF_RAY_CONST_FLOATS * sizeof(float));   // per-ray hoisted terms (one set at a time)
-  w.z_all = (float*)take(no * n * n_samples * sizeof(float));               // coarse depths of every set
-  w.z_fine = (float*)take(no * n * sf * sizeof(float));                     // fine depths
-  w.field_all = (float*)take(no * n * sf * 4 * sizeof(float));              // fields (rgb, sigma) of every set
-  w.w_unsorted = (float*)take(no * n * n_samples * sizeof(float));          // per-set coarse weights in sample order
-  w.live = (int*)take(n * sizeof(int));
-  w.slot = (int*)take(n * sizeof(int));
-  w.count = (int*)take(sizeof(int));
-  w.rays_c = (float*)take(n * 8 * sizeof(float));
-  w.z_c = (float*)take(n * sf * sizeof(float));
-  w.field_c = (float*)take(n * sf * 4 * sizeof(float));
+  WsCarver c{base};
+  w.ray_const = c.floats(n * ONERF_RAY_CONST_FLOATS);   // per-ray hoisted terms (one set at a time)
+  w.z_all = c.floats(no * n * n_samples);               // coarse depths of every set
+  w.z_fine = c.floats(no * n * sf);                     // fine depths
+  w.field_all = c.floats(no * n * sf * 4);              // fields (rgb, sigma) of every set
+  w.w_unsorted = c.floats(no * n * n_samples);          // per-set coarse weights in sample order
+  w.live = static_cast<int*>(c.take(n * sizeof(int)));
+  w.slot = static_cast<int*>(c.take(n * sizeof(int)));
+  w.count = static_cast<int*>(c.take(sizeof(int)));
+  w.rays_c = c.floats(n * 8);
+  w.z_c = c.floats(n * sf);
+  w.field_c = c.floats(n * sf * 4);
   w.sort_bytes = onerf_composite_multi_workspace_bytes(n_rays, n_obj, (int)sf);
-  w.sort = take(w.sort_bytes);
-  w.total = off;
+  w.sort = c.take(w.sort_bytes);
+  w.total = c.off;
   return w;
 }
 
@@ -365,15 +359,6 @@ static int multi_fields(onerf_ctx* ctx, const onerf_render_multi_args* a, const 
 
 // The argument checks of onerf_render_multi_fwd, reported under the entry `fn`.  with_rays_and_maps = 0 leaves out the ray
 // sets and the outputs (onerf_render_edit_frame makes both itself).
-#define FN_CHECK_ARG(cond, msg)                                                      \
-  do {                                                                               \
-    if (!(cond)) { onerf_set_error("%s: %s", fn, msg); return ONERF_ERR_BAD_ARG; }   \
-  } while (0)
-#define FN_UNSUPPORTED(cond, msg)                                                                 \
-  do {                                                                                            \
-    if (cond) { onerf_set_error("%s: unsupported: %s", fn, msg); return ONERF_ERR_UNSUPPORTED; }  \
-  } while (0)
-
 // set_scene: NULL, or per set -1 (base scene) or the index of its source scene, whose ids the caller checks.
 static int check_multi_args(const char* fn, const onerf_render_multi_args* a, bool with_rays_and_maps,
                             const int* set_scene = nullptr) {
@@ -442,15 +427,10 @@ static int render_multi_fwd(const char* fn, onerf_ctx* ctx, const onerf_render_m
   const onerf_render_multi_ext& x = ext ? *ext : none;
   rc = check_multi_ext(fn, a, &x);
   if (rc != ONERF_OK) return rc;
-  const size_t need = onerf_render_multi_workspace_bytes(a->n_rays, a->n_obj, a->n_samples, a->n_importance);
-  if (!a->workspace || (reinterpret_cast<uintptr_t>(a->workspace) & 255u) != 0) {
-    onerf_set_error("%s: workspace null or not 256-byte aligned", fn);
-    return ONERF_ERR_BAD_ARG;
-  }
-  if (a->workspace_bytes < need) {
-    onerf_set_error("%s: workspace too small (%zu < %zu)", fn, a->workspace_bytes, need);
-    return ONERF_ERR_WORKSPACE;
-  }
+  rc = onerf_check_workspace(fn, a->workspace, a->workspace_bytes,
+                             onerf_render_multi_workspace_bytes(a->n_rays, a->n_obj, a->n_samples, a->n_importance),
+                             ONERF_ERR_WORKSPACE);
+  if (rc != ONERF_OK) return rc;
   return multi_forward(ctx, a, x, stream);
 }
 
@@ -560,35 +540,35 @@ static EditWs edit_ws_layout(char* base, int chunk, int n_obj, int n_samples, in
   const size_t n = chunk, nf = n_importance > 0 ? n : 0, no = n_obj;
   const size_t tc = no * n_samples, tf = no * (n_samples + n_importance);
   EditWs w;
-  size_t off = 0;
-  auto take = [&](size_t floats) { float* p = reinterpret_cast<float*>(base + off); off += align256(floats * sizeof(float)); return p; };
-  w.rays = take(no * n * 8);
-  w.coarse.weights = take(n * tc); w.coarse.opacity = take(n); w.coarse.z_vals = take(n * tc);
-  w.coarse.rgb = take(n * 3); w.coarse.depth = take(n); w.coarse.obj_ids = take(n * tc);
-  w.fine.weights = take(nf * tf); w.fine.opacity = take(nf); w.fine.z_vals = take(nf * tf);
-  w.fine.rgb = take(nf * 3); w.fine.depth = take(nf); w.fine.obj_ids = nullptr;
+  WsCarver c{base};
+  w.rays = c.floats(no * n * 8);
+  w.coarse.weights = c.floats(n * tc); w.coarse.opacity = c.floats(n); w.coarse.z_vals = c.floats(n * tc);
+  w.coarse.rgb = c.floats(n * 3); w.coarse.depth = c.floats(n); w.coarse.obj_ids = c.floats(n * tc);
+  w.fine.weights = c.floats(nf * tf); w.fine.opacity = c.floats(nf); w.fine.z_vals = c.floats(nf * tf);
+  w.fine.rgb = c.floats(nf * 3); w.fine.depth = c.floats(nf); w.fine.obj_ids = nullptr;
   w.multi_bytes = onerf_render_multi_workspace_bytes(chunk, n_obj, n_samples, n_importance);
-  w.multi = base + off;
-  off += align256(w.multi_bytes);
-  w.total = off;
-  w.w_fine = take(no * nf * (n_samples + n_importance));   // past everything onerf_render_edit_frame uses; 0 bytes without
-  w.total_sets = off;                                       // a fine pass
-  w.z_frame = take(no * n * (n_samples + n_importance));
-  w.total_scenes = off;
+  w.multi = c.take(w.multi_bytes);
+  w.total = c.off;
+  w.w_fine = c.floats(no * nf * (n_samples + n_importance));   // past everything onerf_render_edit_frame uses; 0 bytes
+  w.total_sets = c.off;                                         // without a fine pass
+  w.z_frame = c.floats(no * n * (n_samples + n_importance));
+  w.total_scenes = c.off;
   return w;
 }
+
+// rows [r0, ...) of a caller's map of `width` floats per row, or `scratch` where the caller leaves the map NULL
+static float* rows_or(float* out, int64_t r0, int64_t width, float* scratch) { return out ? out + r0 * width : scratch; }
 
 // rows [r0, r0 + chunk) of the tile's maps (T samples per row), or the chunk scratch where a map is NULL
 static onerf_render_multi_maps chunk_maps(const onerf_render_multi_maps& out, const onerf_render_multi_maps& scratch,
                                           int64_t r0, int64_t T) {
-  auto at = [&](float* o, float* s, int64_t width) { return o ? o + r0 * width : s; };
   onerf_render_multi_maps m;
-  m.weights = at(out.weights, scratch.weights, T);
-  m.opacity = at(out.opacity, scratch.opacity, 1);
-  m.z_vals = at(out.z_vals, scratch.z_vals, T);
-  m.rgb = at(out.rgb, scratch.rgb, 3);
-  m.depth = at(out.depth, scratch.depth, 1);
-  m.obj_ids = at(out.obj_ids, scratch.obj_ids, T);
+  m.weights = rows_or(out.weights, r0, T, scratch.weights);
+  m.opacity = rows_or(out.opacity, r0, 1, scratch.opacity);
+  m.z_vals = rows_or(out.z_vals, r0, T, scratch.z_vals);
+  m.rgb = rows_or(out.rgb, r0, 3, scratch.rgb);
+  m.depth = rows_or(out.depth, r0, 1, scratch.depth);
+  m.obj_ids = rows_or(out.obj_ids, r0, T, scratch.obj_ids);
   return m;
 }
 
@@ -609,8 +589,8 @@ extern "C" size_t onerf_render_edit_scenes_workspace_bytes(int chunk_rays, int n
 
 // rows [r0, r0 + chunk) of tile-sized per-set maps (n_obj columns), NULL where the caller's array is NULL
 static onerf_set_maps chunk_set_maps(const onerf_set_maps& out, int64_t r0, int64_t n_obj) {
-  auto at = [&](float* o, int64_t width) { return o ? o + r0 * width : nullptr; };
-  return onerf_set_maps{at(out.opacity, n_obj), at(out.depth, n_obj), at(out.rgb, n_obj * 3)};
+  return onerf_set_maps{rows_or(out.opacity, r0, n_obj, nullptr), rows_or(out.depth, r0, n_obj, nullptr),
+                        rows_or(out.rgb, r0, n_obj * 3, nullptr)};
 }
 
 // onerf_render_edit_frame(_sets, _scenes), refusals reported under the entry `fn`
@@ -628,9 +608,8 @@ static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_
   for (int j = 0; j < n_scenes; ++j) {
     const onerf_edit_scene& sc = scenes[j];
     FN_CHECK_ARG(sc.grid && sc.packed_coarse && sc.code_table, "a source scene needs its grid, packed_coarse and code_table");
-    FN_CHECK_ARG(sc.grid->table && sc.grid->idx_map && sc.grid->voxel_offset && sc.grid->voxel_size &&
-                     sc.grid->voxel_shape && onerf_aligned16(sc.grid->table),
-                 "null / misaligned grid buffer in a source scene");
+    const int rc = onerf_check_grid(fn, sc.grid, " in a source scene");
+    if (rc != ONERF_OK) return rc;
     FN_CHECK_ARG(a->n_importance == 0 || sc.packed_fine, "n_importance > 0 needs a source scene's packed_fine");
     const double k = sc.scale_factor / a->scale_factor;
     FN_CHECK_ARG(sc.scale_factor > 0 && sc.scale_factor <= DBL_MAX && (float)k > 0 && (float)k <= FLT_MAX,
@@ -677,11 +656,8 @@ static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_
   const size_t need = any_source ? onerf_render_edit_scenes_workspace_bytes(chunk, NO, a->n_samples, a->n_importance)
                      : with_sets  ? onerf_render_edit_sets_workspace_bytes(chunk, NO, a->n_samples, a->n_importance)
                                   : onerf_render_edit_workspace_bytes(chunk, NO, a->n_samples, a->n_importance);
-  FN_CHECK_ARG(a->workspace && (reinterpret_cast<uintptr_t>(a->workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
-  if (a->workspace_bytes < need) {
-    onerf_set_error("%s: workspace too small (%zu < %zu)", fn, a->workspace_bytes, need);
-    return ONERF_ERR_WORKSPACE;
-  }
+  rc = onerf_check_workspace(fn, a->workspace, a->workspace_bytes, need, ONERF_ERR_WORKSPACE);
+  if (rc != ONERF_OK) return rc;
   const EditWs w = edit_ws_layout(reinterpret_cast<char*>(a->workspace), chunk, NO, a->n_samples, a->n_importance);
   // sets of source scenes: every set's source (the base scene's for the others), k in float32 of the double ratio
   std::vector<SetSource> src;
@@ -722,8 +698,6 @@ static int render_edit_frame(const char* fn, onerf_ctx* ctx, const onerf_render_
   }
   return ONERF_OK;
 }
-#undef FN_CHECK_ARG
-#undef FN_UNSUPPORTED
 
 extern "C" int onerf_render_edit_frame(onerf_ctx* ctx, const onerf_render_edit_args* a, void* stream) {
   return render_edit_frame(__func__, ctx, a, nullptr, nullptr, nullptr, 0, nullptr, stream);
@@ -756,34 +730,32 @@ struct ValidateWs {
 static ValidateWs validate_ws_layout(char* base, int chunk, int n_samples, int n_importance) {
   const size_t n = chunk, nf = n_importance > 0 ? n : 0;
   ValidateWs w;
-  size_t off = 0;
-  auto take = [&](size_t floats) { float* p = reinterpret_cast<float*>(base + off); off += align256(floats * sizeof(float)); return p; };
+  WsCarver c{base};
   auto maps = [&](size_t rows, size_t S) {
     onerf_render_maps m;
-    m.weights = take(rows * S); m.opacity = take(rows); m.z_vals = take(rows * S); m.rgb = take(rows * 3);
-    m.depth = take(rows); m.rgb_instance = take(rows * 3); m.depth_instance = take(rows); m.opacity_instance = take(rows);
+    m.weights = c.floats(rows * S); m.opacity = c.floats(rows); m.z_vals = c.floats(rows * S); m.rgb = c.floats(rows * 3);
+    m.depth = c.floats(rows); m.rgb_instance = c.floats(rows * 3); m.depth_instance = c.floats(rows);
+    m.opacity_instance = c.floats(rows);
     return m;
   };
-  w.codes = take(n * 64);
+  w.codes = c.floats(n * 64);
   w.coarse = maps(n, n_samples);
   w.fine = maps(nf, (size_t)n_samples + n_importance);
   w.render_bytes = onerf_render_rays_workspace_bytes(chunk, n_samples, n_importance);
-  w.render = base + off;
-  off += align256(w.render_bytes);
-  w.total = off;
+  w.render = c.take(w.render_bytes);
+  w.total = c.off;
   return w;
 }
 
 // rows [r0, ...) of the tile's maps, or the chunk scratch where a map is NULL; per-sample arrays always scratch
 static onerf_render_maps validate_chunk_maps(const onerf_render_maps& out, const onerf_render_maps& scratch, int64_t r0) {
-  auto at = [&](float* o, float* s, int64_t width) { return o ? o + r0 * width : s; };
   onerf_render_maps m = scratch;
-  m.opacity = at(out.opacity, scratch.opacity, 1);
-  m.rgb = at(out.rgb, scratch.rgb, 3);
-  m.depth = at(out.depth, scratch.depth, 1);
-  m.rgb_instance = at(out.rgb_instance, scratch.rgb_instance, 3);
-  m.depth_instance = at(out.depth_instance, scratch.depth_instance, 1);
-  m.opacity_instance = at(out.opacity_instance, scratch.opacity_instance, 1);
+  m.opacity = rows_or(out.opacity, r0, 1, scratch.opacity);
+  m.rgb = rows_or(out.rgb, r0, 3, scratch.rgb);
+  m.depth = rows_or(out.depth, r0, 1, scratch.depth);
+  m.rgb_instance = rows_or(out.rgb_instance, r0, 3, scratch.rgb_instance);
+  m.depth_instance = rows_or(out.depth_instance, r0, 1, scratch.depth_instance);
+  m.opacity_instance = rows_or(out.opacity_instance, r0, 1, scratch.opacity_instance);
   return m;
 }
 
@@ -811,12 +783,9 @@ extern "C" int onerf_validate_frame(onerf_ctx* ctx, const onerf_validate_args* v
   ONERF_CHECK_ARG(v->psnr_mask == ONERF_PSNR_VALID_INSTANCE || v->psnr_mask == ONERF_PSNR_ALL_RAYS, "unknown psnr_mask");
   ONERF_CHECK_ARG(!v->finalize || (la.loss_sum_out && la.terms_out && la.present_out && v->psnr_out), "finalize with a null output");
   const int chunk = v->chunk_rays;
-  const size_t need = onerf_validate_workspace_bytes(chunk, ra.n_samples, ra.n_importance);
-  ONERF_CHECK_ARG(ra.workspace && (reinterpret_cast<uintptr_t>(ra.workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
-  if (ra.workspace_bytes < need) {
-    onerf_set_error("onerf_validate_frame: workspace too small (%zu < %zu)", ra.workspace_bytes, need);
-    return ONERF_ERR_BAD_ARG;
-  }
+  int rc = onerf_check_workspace(__func__, ra.workspace, ra.workspace_bytes,
+                                 onerf_validate_workspace_bytes(chunk, ra.n_samples, ra.n_importance), ONERF_ERR_BAD_ARG);
+  if (rc != ONERF_OK) return rc;
   const ValidateWs w = validate_ws_layout(reinterpret_cast<char*>(ra.workspace), chunk, ra.n_samples, ra.n_importance);
   ONERF_CUDA(cudaMemsetAsync(v->record, 0, ONERF_VALIDATE_RECORD_DOUBLES * sizeof(double), (cudaStream_t)stream));
   // rows [first, first + n) of the image's batch
@@ -826,7 +795,6 @@ extern "C" int onerf_validate_frame(onerf_ctx* ctx, const onerf_validate_args* v
     l.rgbs += first * 3; l.depths += first; l.valid_mask += first; l.instance_mask += first; l.instance_mask_weight += first;
     return l;
   };
-  int rc = ONERF_OK;
   if (n_tile > 0) {
     const onerf_loss_args tile = batch_rows(v->ray_begin, n_tile);
     rc = onerf_launch_batch_stats(ctx, &tile, v->record, (cudaStream_t)stream);
@@ -877,17 +845,16 @@ static InstancesWs instances_ws_layout(char* base, int chunk, int n_codes, int n
   const size_t n = chunk, K = n_codes, S = n_samples, SF = (size_t)n_samples + n_importance;
   const size_t nf = n_importance > 0 ? n : 0;
   InstancesWs w;
-  size_t off = 0;
-  auto take = [&](size_t floats) { float* p = reinterpret_cast<float*>(base + off); off += align256(floats * sizeof(float)); return p; };
+  WsCarver c{base};
   w.rc_stride = (int64_t)(n * ONERF_RAY_CONST_FLOATS);
   w.obj_stride = (int64_t)(n * SF * 4);
-  w.ray_const = take(K * n * ONERF_RAY_CONST_FLOATS);
-  w.scene = take(n * SF * 4);
-  w.obj = take(K * n * SF * 4);
-  w.z_c = take(n * S); w.w_c = take(n * S);
-  w.z_f = take(nf * SF); w.w_f = take(nf * SF);
-  w.scratch = onerf_instance_maps{take(n * 3), take(n), take(n), nullptr, nullptr, nullptr};
-  w.total = off;
+  w.ray_const = c.floats(K * n * ONERF_RAY_CONST_FLOATS);
+  w.scene = c.floats(n * SF * 4);
+  w.obj = c.floats(K * n * SF * 4);
+  w.z_c = c.floats(n * S); w.w_c = c.floats(n * S);
+  w.z_f = c.floats(nf * SF); w.w_f = c.floats(nf * SF);
+  w.scratch = onerf_instance_maps{c.floats(n * 3), c.floats(n), c.floats(n), nullptr, nullptr, nullptr};
+  w.total = c.off;
   return w;
 }
 
@@ -917,13 +884,9 @@ static int instances_pass(onerf_ctx* ctx, const onerf_instances_args* a, const I
   const bool want_obj = m.opacity_instance || m.depth_instance || m.rgb_instance;
   const bool want_scene = feeds_fine || m.rgb || m.depth || m.opacity;
   if (!want_obj && !want_scene) return ONERF_OK;
-  FieldParams base;
-  memset(&base, 0, sizeof(base));
+  FieldParams base = onerf_field_params(ra.grid, packed);
   base.rays = rays; base.z = z; base.z_stride = S;
   base.n_rays = n; base.S = S;
-  if (ra.grid) base.grid = *ra.grid;
-  base.packed = packed;
-  base.L = onerf_make_layout(ra.grid ? 1 : 0);
   base.out_stride = S;
   base.scene_out = w.scene;
   int rc;
@@ -968,15 +931,16 @@ static int instances_pass(onerf_ctx* ctx, const onerf_instances_args* a, const I
     c.n_rays = n; c.n_samples = S;
     c.white_back = ra.white_back; c.is_eval = 1; c.zero_last_delta = ra.zero_last_delta;
     c.weights = w_out;
-    c.opacity = m.opacity ? m.opacity + r0 : w.scratch.opacity;
-    c.rgb = m.rgb ? m.rgb + r0 * 3 : w.scratch.rgb;
-    c.depth = m.depth ? m.depth + r0 : w.scratch.depth;
+    c.opacity = rows_or(m.opacity, r0, 1, w.scratch.opacity);
+    c.rgb = rows_or(m.rgb, r0, 3, w.scratch.rgb);
+    c.depth = rows_or(m.depth, r0, 1, w.scratch.depth);
     rc = onerf_launch_composite(ctx, &c, nullptr, stream);
     if (rc != ONERF_OK) return rc;
   }
-  auto col = [&](float* o, int64_t width) { return o ? o + r0 * K * width : nullptr; };
-  return onerf_launch_composite_instances(ctx, z, w.obj, w.obj_stride, n, S, K, col(m.opacity_instance, 1),
-                                          col(m.depth_instance, 1), col(m.rgb_instance, 3), stream);
+  return onerf_launch_composite_instances(ctx, z, w.obj, w.obj_stride, n, S, K,
+                                          rows_or(m.opacity_instance, r0, K, nullptr),
+                                          rows_or(m.depth_instance, r0, K, nullptr),
+                                          rows_or(m.rgb_instance, r0, K * 3, nullptr), stream);
 }
 
 extern "C" int onerf_render_instances(onerf_ctx* ctx, const onerf_instances_args* a, void* stream_) {
@@ -997,21 +961,16 @@ extern "C" int onerf_render_instances(onerf_ctx* ctx, const onerf_instances_args
   ONERF_CHECK_ARG(a->chunk_rays >= 1, "chunk_rays < 1");
   ONERF_CHECK_ARG(ra.rays && ra.packed_coarse, "null rays / packed_coarse");
   ONERF_CHECK_ARG(ra.n_importance == 0 || ra.packed_fine, "n_importance > 0 needs packed_fine");
-  if (ra.grid)
-    ONERF_CHECK_ARG(ra.grid->table && ra.grid->idx_map && ra.grid->voxel_offset && ra.grid->voxel_size &&
-                        ra.grid->voxel_shape && onerf_aligned16(ra.grid->table),
-                    "null / misaligned grid buffer");
+  int rc = onerf_check_grid(__func__, ra.grid);
+  if (rc != ONERF_OK) return rc;
   ONERF_CHECK_ARG(ra.precision == ONERF_PREC_FP32 || ra.precision == ONERF_PREC_BF16, "unknown precision");
   ONERF_CHECK_ARG(ra.n_importance > 0 || !any_instance_map(a->fine), "fine maps without a fine pass");
   ONERF_CHECK_ARG(instance_maps_aligned(a->coarse) && instance_maps_aligned(a->fine), "maps must be 4-byte aligned");
   const int chunk = a->chunk_rays;
-  const size_t need = onerf_render_instances_workspace_bytes(chunk, a->n_ids, ra.n_samples, ra.n_importance);
-  ONERF_CHECK_ARG(ra.workspace && (reinterpret_cast<uintptr_t>(ra.workspace) & 255u) == 0,
-                  "workspace null or not 256-byte aligned");
-  if (ra.workspace_bytes < need) {
-    onerf_set_error("onerf_render_instances: workspace too small (%zu < %zu)", ra.workspace_bytes, need);
-    return ONERF_ERR_BAD_ARG;
-  }
+  rc = onerf_check_workspace(__func__, ra.workspace, ra.workspace_bytes,
+                             onerf_render_instances_workspace_bytes(chunk, a->n_ids, ra.n_samples, ra.n_importance),
+                             ONERF_ERR_BAD_ARG);
+  if (rc != ONERF_OK) return rc;
   cudaStream_t stream = (cudaStream_t)stream_;
   const InstancesWs w = instances_ws_layout(reinterpret_cast<char*>(ra.workspace), chunk, a->n_ids, ra.n_samples,
                                             ra.n_importance);
@@ -1019,7 +978,7 @@ extern "C" int onerf_render_instances(onerf_ctx* ctx, const onerf_instances_args
   for (int64_t r0 = 0; r0 < n_tile; r0 += chunk) {
     const int n = (int)(n_tile - r0 < chunk ? n_tile - r0 : chunk);
     const float* rays = ra.rays + (a->ray_begin + r0) * 8;
-    int rc = onerf_launch_sample_coarse(ctx, rays, n, S, ra.use_disp, 0.0f, nullptr, 0, nullptr, w.z_c, stream);
+    rc = onerf_launch_sample_coarse(ctx, rays, n, S, ra.use_disp, 0.0f, nullptr, 0, nullptr, w.z_c, stream);
     if (rc != ONERF_OK) return rc;
     rc = instances_pass(ctx, a, w, rays, n, ra.packed_coarse, w.z_c, S, w.w_c, a->coarse, ra.n_importance > 0, r0,
                         stream);

@@ -166,8 +166,6 @@ composite_boxes_kernel(const float* __restrict__ z_all, const float* __restrict_
   }
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 // Per-chunk scratch of n = chunk_rays rows; nothing in it depends on K or the image.  Every per-row array past the
 // first two is indexed by list slot.
 struct BoxesWs {
@@ -183,22 +181,20 @@ BoxesWs boxes_ws_layout(char* base, int chunk, int n_samples, int n_importance) 
   const size_t n = chunk, S = n_samples, SF = (size_t)n_samples + n_importance, nf = n_importance > 0 ? n : 0;
   const size_t n_blocks = (n + kListRows - 1) / kListRows;
   BoxesWs w;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* p = base + off; off += align256(bytes); return p; };
-  auto takef = [&](size_t floats) { return reinterpret_cast<float*>(take(floats * sizeof(float))); };
-  w.rays = takef(n * 8);
-  w.hit = reinterpret_cast<uint8_t*>(take(n));
-  w.block_off = reinterpret_cast<int*>(take(n_blocks * sizeof(int)));
-  w.count = reinterpret_cast<int*>(take(sizeof(int)));
-  w.live = reinterpret_cast<int*>(take(n * sizeof(int)));
-  w.rays_l = takef(n * 8);
-  w.z_c = takef(n * S);
-  w.w_c = takef(n * S);
-  w.z_f = takef(nf * SF);
-  w.codes = takef(n * ONERF_NCODE);
-  w.ray_const = takef(n * ONERF_RAY_CONST_FLOATS);
-  w.field = takef(n * SF * 4);
-  w.total = off;
+  WsCarver c{base};
+  w.rays = c.floats(n * 8);
+  w.hit = static_cast<uint8_t*>(c.take(n));
+  w.block_off = static_cast<int*>(c.take(n_blocks * sizeof(int)));
+  w.count = static_cast<int*>(c.take(sizeof(int)));
+  w.live = static_cast<int*>(c.take(n * sizeof(int)));
+  w.rays_l = c.floats(n * 8);
+  w.z_c = c.floats(n * S);
+  w.w_c = c.floats(n * S);
+  w.z_f = c.floats(nf * SF);
+  w.codes = c.floats(n * ONERF_NCODE);
+  w.ray_const = c.floats(n * ONERF_RAY_CONST_FLOATS);
+  w.field = c.floats(n * SF * 4);
+  w.total = c.off;
   return w;
 }
 
@@ -216,14 +212,10 @@ bool box_maps_aligned(const onerf_box_maps& m) {
 // and object field of the listed rows, compositing (weights to w_out when given, maps to m).
 int boxes_pass(onerf_ctx* ctx, const onerf_render_boxes_args* a, const BoxesWs& w, int n, int64_t g0, const void* packed,
                const float* z, int S, float* w_out, const onerf_box_maps& m, cudaStream_t stream) {
-  FieldParams p;
-  memset(&p, 0, sizeof(p));
+  FieldParams p = onerf_field_params(a->grid, packed);
   p.rays = w.rays_l; p.z = z; p.z_stride = S;
   p.codes = w.codes;
   p.n_rays = n; p.S = S;
-  if (a->grid) p.grid = *a->grid;
-  p.packed = packed;
-  p.L = onerf_make_layout(a->grid ? 1 : 0);
   p.want_object = 1;
   p.obj_out = w.field; p.out_stride = S;
   p.ray_const = w.ray_const;
@@ -290,23 +282,17 @@ extern "C" int onerf_render_boxes(onerf_ctx* ctx, const onerf_render_boxes_args*
   ONERF_UNSUPPORTED(a->n_importance > 0 && (int64_t)a->n_samples + a->n_importance > 2048, "S + K > 2048");
   ONERF_CHECK_ARG(a->packed_coarse, "null packed_coarse");
   ONERF_CHECK_ARG(a->n_importance == 0 || a->packed_fine, "n_importance > 0 needs packed_fine");
-  if (a->grid)
-    ONERF_CHECK_ARG(a->grid->table && a->grid->idx_map && a->grid->voxel_offset && a->grid->voxel_size &&
-                        a->grid->voxel_shape && onerf_aligned16(a->grid->table),
-                    "null / misaligned grid buffer");
+  int rc = onerf_check_grid(__func__, a->grid);
+  if (rc != ONERF_OK) return rc;
   ONERF_CHECK_ARG(a->precision == ONERF_PREC_FP32 || a->precision == ONERF_PREC_BF16, "unknown precision");
   ONERF_CHECK_ARG(a->n_importance > 0 || !(a->fine.opacity || a->fine.depth || a->fine.rgb),
                   "fine maps without a fine pass");
   ONERF_CHECK_ARG(onerf_aligned16(a->code_table), "code_table must be 16-byte aligned");
   ONERF_CHECK_ARG(box_maps_aligned(a->coarse) && box_maps_aligned(a->fine), "maps must be 4-byte aligned");
   const int chunk = a->chunk_rays;
-  const size_t need = onerf_render_boxes_workspace_bytes(chunk, a->n_samples, a->n_importance);
-  ONERF_CHECK_ARG(a->workspace && (reinterpret_cast<uintptr_t>(a->workspace) & 255u) == 0,
-                  "workspace null or not 256-byte aligned");
-  if (a->workspace_bytes < need) {
-    onerf_set_error("onerf_render_boxes: workspace too small (%zu < %zu)", a->workspace_bytes, need);
-    return ONERF_ERR_BAD_ARG;
-  }
+  rc = onerf_check_workspace(__func__, a->workspace, a->workspace_bytes,
+                             onerf_render_boxes_workspace_bytes(chunk, a->n_samples, a->n_importance), ONERF_ERR_BAD_ARG);
+  if (rc != ONERF_OK) return rc;
   cudaStream_t stream = (cudaStream_t)stream_;
   const BoxesWs w = boxes_ws_layout(reinterpret_cast<char*>(a->workspace), chunk, a->n_samples, a->n_importance);
   const int S = a->n_samples, SF = a->n_samples + a->n_importance;
@@ -320,7 +306,7 @@ extern "C" int onerf_render_boxes(onerf_ctx* ctx, const onerf_render_boxes_args*
     }
   for (int64_t g0 = 0; g0 < rows; g0 += chunk) {
     const int n = (int)(rows - g0 < chunk ? rows - g0 : chunk);
-    int rc = onerf_launch_box_rays(ctx, a->H, a->W, a->focal, a->c2w_host, a->boxes_host, K, a->scale_factor,
+    rc = onerf_launch_box_rays(ctx, a->H, a->W, a->focal, a->c2w_host, a->boxes_host, K, a->scale_factor,
                                    a->pixel_begin, T, g0, n, w.rays, w.hit, a->hit, stream);
     if (rc != ONERF_OK) return rc;
     rc = boxes_list(ctx, a, w, n, g0, stream);

@@ -90,9 +90,58 @@ int onerf_launch_rescale_set(onerf_ctx* ctx, const float* z, float* z_out, float
     (ctx)->launches++;                                                            \
   } while (0)
 
+// ONERF_CHECK_ARG / ONERF_UNSUPPORTED reported under the entry `fn` (a local of the caller) instead of __func__, for
+// checks shared by several entry points.
+#define FN_CHECK_ARG(cond, msg)                                                      \
+  do {                                                                               \
+    if (!(cond)) { onerf_set_error("%s: %s", fn, msg); return ONERF_ERR_BAD_ARG; }   \
+  } while (0)
+#define FN_UNSUPPORTED(cond, msg)                                                                 \
+  do {                                                                                            \
+    if (cond) { onerf_set_error("%s: unsupported: %s", fn, msg); return ONERF_ERR_UNSUPPORTED; }  \
+  } while (0)
+
 static inline bool onerf_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 static inline bool onerf_aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
 static inline bool onerf_aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
+
+// The buffers of a voxel grid, refused under the entry `fn` with `where` ending the message.  NULL (the plain-PE model)
+// passes.
+static inline int onerf_check_grid(const char* fn, const onerf_grid* g, const char* where = "") {
+  if (!g || (g->table && g->idx_map && g->voxel_offset && g->voxel_size && g->voxel_shape && onerf_aligned16(g->table)))
+    return ONERF_OK;
+  onerf_set_error("%s: null / misaligned grid buffer%s", fn, where);
+  return ONERF_ERR_BAD_ARG;
+}
+
+// A caller's workspace of `bytes` bytes for an entry `fn` that needs `need`: NULL or misaligned is ONERF_ERR_BAD_ARG, too
+// small is `small_code` (each entry's header names its own).
+static inline int onerf_check_workspace(const char* fn, const void* ws, size_t bytes, size_t need, int small_code) {
+  if (!ws || (reinterpret_cast<uintptr_t>(ws) & 255u) != 0) {
+    onerf_set_error("%s: workspace null or not 256-byte aligned", fn);
+    return ONERF_ERR_BAD_ARG;
+  }
+  if (bytes < need) {
+    onerf_set_error("%s: workspace too small (%zu < %zu)", fn, bytes, need);
+    return small_code;
+  }
+  return ONERF_OK;
+}
+
+static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// Consecutive 256-byte aligned buffers of a workspace, in the order they are taken.  With a NULL base it only sizes the
+// workspace: `off` is then its total size.
+struct WsCarver {
+  char* base;
+  size_t off = 0;
+  void* take(size_t bytes) {
+    void* p = base + off;
+    off += align256(bytes);
+    return p;
+  }
+  float* floats(size_t n) { return static_cast<float*>(take(n * sizeof(float))); }
+};
 
 // ---------------------------------------------------------------------------------------------
 // warp helpers

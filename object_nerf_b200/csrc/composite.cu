@@ -615,11 +615,8 @@ static int composite_multi_ws(onerf_ctx* ctx, int force_merge, const float* z_al
     ONERF_UNSUPPORTED(T > INT32_MAX, "n_obj * n_samples >= 2^31");
     ONERF_UNSUPPORTED(n_samples > kMergeMaxS, "more than 2048 samples per ray set");
     const size_t need = onerf_composite_multi_workspace_bytes(n_rays, n_obj, n_samples);
-    ONERF_CHECK_ARG(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255u) == 0, "workspace null or not 256-byte aligned");
-    if (workspace_bytes < need) {
-      onerf_set_error("%s: workspace too small (%zu < %zu)", __func__, workspace_bytes, need);
-      return ONERF_ERR_WORKSPACE;
-    }
+    const int rc = onerf_check_workspace(__func__, workspace, workspace_bytes, need, ONERF_ERR_WORKSPACE);
+    if (rc != ONERF_OK) return rc;
   }
   return composite_multi_run(ctx, path, z_all, field_all, n_rays, n_obj, n_samples, white_back, nz, z_sorted, weights,
                              obj_ids, weights_unsorted, opacity, rgb, depth, workspace, workspace_bytes, (cudaStream_t)stream);

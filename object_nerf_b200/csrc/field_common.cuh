@@ -1,5 +1,7 @@
 // Parameters shared by the field kernels (FFMA and wgmma) and their launchers.
 #pragma once
+#include <string.h>
+
 #include "common.cuh"
 #include "layout.h"
 
@@ -35,6 +37,16 @@ struct FieldParams {
   // ray sets compacted on the device to the rays that hit the object's box (api.cu: multi_fields).
   const int* n_live;
 };
+
+// Field parameters with the grid (NULL: plain-PE model), the packed weights and their layout set and all else zero.
+static inline FieldParams onerf_field_params(const onerf_grid* grid, const void* packed) {
+  FieldParams p;
+  memset(&p, 0, sizeof(p));
+  if (grid) p.grid = *grid;
+  p.packed = packed;
+  p.L = onerf_make_layout(grid ? 1 : 0);
+  return p;
+}
 
 // rays a field launch evaluates: n_rays, or the device-side count when there is one (read once at kernel start)
 __device__ __forceinline__ int field_rays(const FieldParams& p) {

@@ -1,7 +1,6 @@
 // Voxel pruning entry points (include/onerf_ext.h: onerf_prune_measure, onerf_prune_apply).  The bf16 measure is one
 // launch of the fused tensor-core pass (field_tc.cu: prune_tc_kernel); the fp32 measure stages each chunk of voxels
 // through the FFMA field kernel: points -> scene-only field -> per-voxel maximum of alpha.
-#include <string.h>
 
 #include "prune.cuh"
 #include "../../include/onerf_ext.h"
@@ -11,8 +10,6 @@ namespace {
 constexpr int kChunkVoxels = 32;                                  // voxels per fp32 chunk (the reference's batch)
 constexpr int64_t kChunkPoints = (int64_t)kChunkVoxels * kPruneSamples;
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct PruneWs {
   float *xyz, *z, *rays, *ray_const, *out;
   size_t total;
@@ -20,14 +17,13 @@ struct PruneWs {
 
 PruneWs prune_ws_layout(char* base) {
   PruneWs w;
-  size_t off = 0;
-  auto take = [&](size_t floats) { float* p = reinterpret_cast<float*>(base + off); off += align256(floats * sizeof(float)); return p; };
-  w.xyz = take(kChunkPoints * 3);
-  w.z = take(kChunkPoints);                       // zero depths and one zero ray: the field reads xyz
-  w.rays = take(8);
-  w.ray_const = take(ONERF_RAY_CONST_FLOATS);
-  w.out = take(kChunkPoints * 4);
-  w.total = off;
+  WsCarver c{base};
+  w.xyz = c.floats(kChunkPoints * 3);
+  w.z = c.floats(kChunkPoints);                       // zero depths and one zero ray: the field reads xyz
+  w.rays = c.floats(8);
+  w.ray_const = c.floats(ONERF_RAY_CONST_FLOATS);
+  w.out = c.floats(kChunkPoints * 4);
+  w.total = c.off;
   return w;
 }
 
@@ -88,9 +84,8 @@ extern "C" size_t onerf_prune_workspace_bytes(int precision) {
 extern "C" int onerf_prune_measure(onerf_ctx* ctx, const onerf_prune_args* a, void* stream_) {
   ONERF_CHECK_ARG(ctx && a, "null argument");
   ONERF_CHECK_ARG(a->grid, "the pruning pass needs the voxel model's grid");
-  ONERF_CHECK_ARG(a->grid->table && a->grid->idx_map && a->grid->voxel_offset && a->grid->voxel_size && a->grid->voxel_shape &&
-                      onerf_aligned16(a->grid->table),
-                  "null / misaligned grid buffer");
+  int rc = onerf_check_grid(__func__, a->grid);
+  if (rc != ONERF_OK) return rc;
   ONERF_CHECK_ARG(a->packed, "null packed weights");
   ONERF_CHECK_ARG(a->precision == ONERF_PREC_FP32 || a->precision == ONERF_PREC_BF16, "unknown precision");
   ONERF_CHECK_ARG(a->n_cells >= 0 && a->cell_begin >= 0 && a->cell_begin <= a->cell_end && a->cell_end <= a->n_cells,
@@ -103,21 +98,13 @@ extern "C" int onerf_prune_measure(onerf_ctx* ctx, const onerf_prune_args* a, vo
                   "jitter / max_alpha_out must be 4-byte aligned");
   const size_t need = onerf_prune_workspace_bytes(a->precision);
   if (need > 0) {
-    ONERF_CHECK_ARG(a->workspace && (reinterpret_cast<uintptr_t>(a->workspace) & 255u) == 0,
-                    "workspace null or not 256-byte aligned");
-    if (a->workspace_bytes < need) {
-      onerf_set_error("onerf_prune_measure: workspace too small (%zu < %zu)", a->workspace_bytes, need);
-      return ONERF_ERR_WORKSPACE;
-    }
+    rc = onerf_check_workspace(__func__, a->workspace, a->workspace_bytes, need, ONERF_ERR_WORKSPACE);
+    if (rc != ONERF_OK) return rc;
   }
   if (nk == 0) return ONERF_OK;
   cudaStream_t stream = (cudaStream_t)stream_;
   ONERF_CUDA(cudaMemsetAsync(a->max_alpha_out, 0, (size_t)nk * sizeof(float), stream));
-  FieldParams p;
-  memset(&p, 0, sizeof(p));
-  p.grid = *a->grid;
-  p.packed = a->packed;
-  p.L = onerf_make_layout(1);
+  FieldParams p = onerf_field_params(a->grid, a->packed);
   p.want_scene = 1;
   const PruneSource src{a->cells, a->jitter, a->seed};
   if (a->precision == ONERF_PREC_BF16)
@@ -130,7 +117,7 @@ extern "C" int onerf_prune_measure(onerf_ctx* ctx, const onerf_prune_args* a, vo
   p.n_rays = 1;
   p.ray_const = w.ray_const;
   p.scene_out = w.out;
-  int rc = onerf_launch_ray_const(ctx, p, stream);   // (the direction layers run after sigma; their input is defined)
+  rc = onerf_launch_ray_const(ctx, p, stream);   // (the direction layers run after sigma; their input is defined)
   if (rc != ONERF_OK) return rc;
   for (int64_t k0 = a->cell_begin; k0 < a->cell_end; k0 += kChunkVoxels) {
     const int n = (int)(a->cell_end - k0 < kChunkVoxels ? a->cell_end - k0 : kChunkVoxels);

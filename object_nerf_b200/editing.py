@@ -32,7 +32,6 @@ from typing import Any, Dict, Optional, Sequence
 
 import numpy as np
 import torch
-import torch.distributed as dist
 
 from . import _lib, engine, parallel
 from .multi_rendering import boxes_to_tensor
@@ -41,7 +40,6 @@ from .rendering import _grid_of, _is_voxel
 
 _MAPS = ("weights", "opacity", "z_vals", "rgb", "depth", "obj_ids")
 _SET_MAPS = ("opacity_sets", "depth_sets", "rgb_sets")
-_workspaces: Dict[Any, torch.Tensor] = {}
 
 
 def result_keys(N_importance: int):
@@ -74,15 +72,6 @@ class Scene:
         self.models, self.embeddings, self.code_library, self.scale_factor = models, embeddings, code_library, scale_factor
 
 
-def _workspace(nbytes: int, dev: torch.device) -> torch.Tensor:
-    """One workspace per (device, size), kept across frames (calls on one stream are ordered)."""
-    key = (dev.index, nbytes)
-    ws = _workspaces.get(key)
-    if ws is None:
-        ws = _workspaces[key] = torch.empty(max(nbytes, 256), dtype=torch.uint8, device=dev)
-    return ws
-
-
 def render_frame(models: Dict[str, Any], embeddings: Dict[str, Any], code_library, H: int, W: int, focal: float,
                  sets: Sequence, near: float, far: float, scale_factor: float, background_skip_bbox=None,
                  N_samples: int = 64, N_importance: int = 0, use_disp: bool = False, white_back: bool = False,
@@ -98,15 +87,11 @@ def render_frame(models: Dict[str, Any], embeddings: Dict[str, Any], code_librar
     the code table; `keys` restricts what is kept and returned (the rest goes to scratch).  perturb = 0 and noise_std = 0,
     as EditableRenderer renders."""
     n_pix = int(H) * int(W)
-    begin, end = 0, n_pix
-    if group is not None:
-        begin, end = parallel.shard_bounds(n_pix, dist.get_world_size(group), dist.get_rank(group))
+    begin, end = parallel.tile_bounds(n_pix, group)
     out = render_tile(models, embeddings, code_library, H, W, focal, sets, near, far, scale_factor, begin, end,
                       background_skip_bbox=background_skip_bbox, N_samples=N_samples, N_importance=N_importance,
                       use_disp=use_disp, white_back=white_back, keys=keys, chunk_rays=chunk_rays, precision=precision)
-    if group is not None:
-        out = {k: parallel.gather_tiles(v, n_pix, group) for k, v in out.items()}
-    return out
+    return parallel.gather_tile_maps(out, n_pix, group)
 
 
 def render_tile(models: Dict[str, Any], embeddings: Dict[str, Any], code_library, H: int, W: int, focal: float,
@@ -199,7 +184,7 @@ def render_tile(models: Dict[str, Any], embeddings: Dict[str, Any], code_library
     with_sets = any(k in keys for k in set_keys(N_importance))
     ws_bytes = (lib.onerf_render_edit_scenes_workspace_bytes if scenes else
                 lib.onerf_render_edit_sets_workspace_bytes if with_sets else lib.onerf_render_edit_workspace_bytes)
-    ws = _workspace(ws_bytes(a.chunk_rays, n_obj, a.n_samples, a.n_importance), dev)
+    ws = engine.workspace(ws_bytes(a.chunk_rays, n_obj, a.n_samples, a.n_importance), dev)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
     if scenes:
         _lib.call("onerf_render_edit_frame_scenes", dev, C.byref(a), scenes_c, len(scenes), set_scene,

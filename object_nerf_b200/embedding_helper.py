@@ -160,10 +160,6 @@ class EmbeddingVoxel(nn.Module):
         if n_cells == 0:
             return 0
         dev = occ.device
-        world, rank = 1, 0
-        if group is not None:
-            import torch.distributed as dist
-            world, rank = dist.get_world_size(group), dist.get_rank(group)
         jitter = None
         if _rand is not None:
             # block i holds chunk i's rows: concatenated, row k * 4096 + s is sample s of voxel k
@@ -176,10 +172,11 @@ class EmbeddingVoxel(nn.Module):
         elif seed is None:
             seed = engine.new_seed()
         if group is not None and jitter is None:
+            import torch.distributed as dist
             t = torch.tensor([seed], dtype=torch.int64, device=dev)
             dist.broadcast(t, group_src=0, group=group)
             seed = int(t.item())
-        begin, end = parallel.shard_bounds(n_cells, world, rank)
+        begin, end = parallel.tile_bounds(n_cells, group)
         max_alpha = torch.zeros(end - begin, dtype=torch.float32, device=dev)
         grid = self.grid_buffers()
         packed = engine.packed_for(model, True)

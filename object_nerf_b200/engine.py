@@ -118,6 +118,28 @@ def pack_weights(linears: Sequence, use_voxel: bool, out: Optional[torch.Tensor]
     return out
 
 
+_workspaces = {}   # (device index, bytes) -> workspace
+
+
+def workspace(nbytes: int, dev: torch.device) -> torch.Tensor:
+    """One workspace per (device, size), kept for the life of the process so that a captured call keeps valid addresses
+    (calls on one stream are ordered)."""
+    key = (dev.index, nbytes)
+    ws = _workspaces.get(key)
+    if ws is None:
+        ws = _workspaces[key] = torch.empty(max(nbytes, 256), dtype=torch.uint8, device=dev)
+    return ws
+
+
+def cached_plan(plans, owner, key: tuple, make):
+    """plans[owner][key], made by make() on first use: the buffers of one configuration of a one-call render."""
+    per_owner = plans.setdefault(owner, {})
+    plan = per_owner.get(key)
+    if plan is None:
+        plan = per_owner[key] = make()
+    return plan
+
+
 _pack_cache = {}   # id(model) -> (weakref to the model, content fingerprint, blob)
 
 

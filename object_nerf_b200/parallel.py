@@ -17,6 +17,13 @@ def shard_bounds(n_rays: int, world_size: int, rank: int):
     return start, start + base + (1 if rank < rem else 0)
 
 
+def tile_bounds(n_rays: int, group=None):
+    """The rows this rank renders: all of them without a group, its shard_bounds with one."""
+    if group is None:
+        return 0, n_rays
+    return shard_bounds(n_rays, dist.get_world_size(group), dist.get_rank(group))
+
+
 def gather_tiles(local: torch.Tensor, n_rays: int, group=None) -> torch.Tensor:
     """All-gather ragged row tiles (shard_bounds order) into the full (n_rays, ...) tensor on every rank."""
     world = dist.get_world_size(group)
@@ -29,6 +36,13 @@ def gather_tiles(local: torch.Tensor, n_rays: int, group=None) -> torch.Tensor:
     out = [torch.empty_like(padded) for _ in range(world)]
     dist.all_gather(out, padded.contiguous(), group=group)
     return torch.cat([o[: b - a] for o, (a, b) in zip(out, sizes)], 0)
+
+
+def gather_tile_maps(maps: Dict[str, torch.Tensor], n_rays: int, group=None) -> Dict[str, torch.Tensor]:
+    """gather_tiles of every tensor of `maps`; without a group, `maps` as they are (a new dict)."""
+    if group is None:
+        return dict(maps)
+    return {k: gather_tiles(v, n_rays, group) for k, v in maps.items()}
 
 
 def render_sharded(render_fn: Callable[[torch.Tensor, Dict[str, torch.Tensor]], Dict[str, torch.Tensor]],

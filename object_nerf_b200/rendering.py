@@ -225,6 +225,27 @@ def _result_keys(model_order, forward_instance):
     return [f"{k}_{typ}" for typ in model_order for k in base]
 
 
+def _fit_chunk(chunk: int, ws_bytes, budget: int) -> int:
+    """The largest chunk <= `chunk` whose workspace ws_bytes(chunk) fits `budget` bytes, or 1."""
+    while chunk > 1 and ws_bytes(chunk) > budget:
+        chunk = max(1, min(chunk - 1, chunk * budget // ws_bytes(chunk)))
+    return chunk
+
+
+def _pass_maps(fn: str, keys: Sequence[str], names: Sequence[str], N_importance: int) -> tuple:
+    """The distinct (map, pass) pairs `keys` ask for: a name of `names` for the last pass, or with a "_coarse" / "_fine"
+    suffix for that pass."""
+    last = "fine" if N_importance > 0 else "coarse"
+    maps = []
+    for key in keys:
+        base, _, typ = key.rpartition("_")
+        base, typ = (base, typ) if typ in ("coarse", "fine") else (key, last)
+        if base not in names or (typ == "fine" and N_importance == 0):
+            raise KeyError(f"{fn}: no such map {key!r} (choose from {names}, optionally with _coarse or _fine)")
+        maps.append((base, typ))
+    return tuple(dict.fromkeys(maps))
+
+
 # ------------------------------------------------------------------------------------------------
 # every object's maps in one render
 # ------------------------------------------------------------------------------------------------
@@ -237,9 +258,7 @@ _instance_plans: "weakref.WeakKeyDictionary[Any, Dict[tuple, _InstancesPlan]]" =
 def _instances_chunk(chunk: int, K: int, n_samples: int, n_importance: int) -> int:
     """The largest chunk <= `chunk` whose onerf_render_instances workspace fits INSTANCES_WORKSPACE_BUDGET, or 1."""
     ws = _lib.load().onerf_render_instances_workspace_bytes
-    while chunk > 1 and ws(chunk, K, n_samples, n_importance) > INSTANCES_WORKSPACE_BUDGET:
-        chunk = max(1, min(chunk - 1, chunk * INSTANCES_WORKSPACE_BUDGET // ws(chunk, K, n_samples, n_importance)))
-    return chunk
+    return _fit_chunk(chunk, lambda c: ws(c, K, n_samples, n_importance), INSTANCES_WORKSPACE_BUDGET)
 
 
 class _InstancesPlan:
@@ -291,38 +310,24 @@ def render_instances(models: Dict[str, Any], embeddings: Dict[str, Any], code_li
     INSTANCES_WORKSPACE_BUDGET bytes (1 GiB) of device memory.  Lower the budget (or chunk) to hold less.
     group: a torch.distributed process group; rank r renders parallel.shard_bounds(N, W, r) and the maps are
     all-gathered, so every rank returns the whole of them."""
-    from . import editing, parallel, training
+    from . import parallel, training
     ids = [int(i) for i in ids]
     K = len(ids)
     if not 1 <= K <= _lib.INSTANCES_MAX_CODES:
         raise ValueError(f"render_instances: 1 to {_lib.INSTANCES_MAX_CODES} object ids, got {K}")
     if int(chunk) < 1:
         raise ValueError("render_instances: chunk must be at least 1 ray")
-    last = "fine" if N_importance > 0 else "coarse"
-    maps = []
-    for key in keys:
-        base, _, typ = key.rpartition("_")
-        base, typ = (base, typ) if typ in ("coarse", "fine") else (key, last)
-        if base not in INSTANCE_KEYS or (typ == "fine" and N_importance == 0):
-            raise KeyError(f"render_instances: no such map {key!r} (choose from {INSTANCE_KEYS}, optionally with "
-                           f"_coarse or _fine)")
-        maps.append((base, typ))
-    maps = tuple(dict.fromkeys(maps))
+    maps = _pass_maps("render_instances", keys, INSTANCE_KEYS, N_importance)
     rays = rays.reshape(-1, rays.shape[-1])[:, :8].float().contiguous()
     n, dev = rays.shape[0], rays.device
     emb_xyz = embeddings["xyz"]
     use_voxel = _is_voxel(emb_xyz)
     cfg = dict(N_samples=int(N_samples), N_importance=int(N_importance), use_disp=bool(use_disp),
                white_back=bool(white_back), chunk=int(chunk), precision=engine.train_precision(precision))
-    begin, end = 0, n
-    if group is not None:
-        import torch.distributed as dist
-        begin, end = parallel.shard_bounds(n, dist.get_world_size(group), dist.get_rank(group))
-    plans = _instance_plans.setdefault(models["coarse"], {})
+    begin, end = parallel.tile_bounds(n, group)
     key = (dev, n, begin, end, use_voxel, tuple(sorted(cfg.items())), maps, tuple(ids))
-    plan = plans.get(key)
-    if plan is None:
-        plan = plans[key] = _InstancesPlan(models, n, end - begin, cfg, maps, ids, dev, use_voxel)
+    plan = engine.cached_plan(_instance_plans, models["coarse"], key,
+                              lambda: _InstancesPlan(models, n, end - begin, cfg, maps, ids, dev, use_voxel))
     a = plan.args
     code_table = training._f32_param(code_library.embedding_instance.weight)
     a.render.rays = rays.data_ptr()
@@ -330,16 +335,14 @@ def render_instances(models: Dict[str, Any], embeddings: Dict[str, Any], code_li
     grid = engine.GridBuffers.from_module(emb_xyz) if use_voxel else None
     a.render.grid = C.pointer(grid.c) if use_voxel else None
     a.ray_begin, a.ray_end = begin, end
-    ws = editing._workspace(_lib.load().onerf_render_instances_workspace_bytes(a.chunk_rays, K, cfg["N_samples"],
-                                                                              cfg["N_importance"]), dev)
+    ws = engine.workspace(_lib.load().onerf_render_instances_workspace_bytes(a.chunk_rays, K, cfg["N_samples"],
+                                                                            cfg["N_importance"]), dev)
     a.render.workspace, a.render.workspace_bytes = ws.data_ptr(), ws.numel()
     for typ in plan.model_order:
         training._pack(models, typ, use_voxel, plan.packed)
     if end > begin:                  # an empty tile renders nothing (and its rays may have no storage)
         _lib.call("onerf_render_instances", dev, C.byref(a))
-    if group is None:
-        return dict(plan.maps)
-    return {k: parallel.gather_tiles(v, n, group) for k, v in plan.maps.items()}
+    return parallel.gather_tile_maps(plan.maps, n, group)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -354,9 +357,7 @@ _box_plans: "weakref.WeakKeyDictionary[Any, Dict[tuple, _BoxesPlan]]" = weakref.
 def _boxes_chunk(chunk: int, n_samples: int, n_importance: int) -> int:
     """The largest chunk <= `chunk` whose onerf_render_boxes workspace fits BOXES_WORKSPACE_BUDGET, or 1."""
     ws = _lib.load().onerf_render_boxes_workspace_bytes
-    while chunk > 1 and ws(chunk, n_samples, n_importance) > BOXES_WORKSPACE_BUDGET:
-        chunk = max(1, min(chunk - 1, chunk * BOXES_WORKSPACE_BUDGET // ws(chunk, n_samples, n_importance)))
-    return chunk
+    return _fit_chunk(chunk, lambda c: ws(c, n_samples, n_importance), BOXES_WORKSPACE_BUDGET)
 
 
 class _BoxesPlan:
@@ -413,23 +414,14 @@ def render_boxes(models: Dict[str, Any], embeddings: Dict[str, Any], code_librar
     process, as render_instances' is.
     group: a torch.distributed process group; rank r renders the pixels parallel.shard_bounds(H*W, W, r) and the maps
     are all-gathered, so every rank returns the whole of them."""
-    from . import editing, parallel, ray_utils, training
+    from . import parallel, ray_utils, training
     ids = [int(i) for i in ids]
     K = len(ids)
     if not 1 <= K <= _lib.BOXES_MAX or len(boxes) != K:
         raise ValueError(f"render_boxes: 1 to {_lib.BOXES_MAX} boxes, one id each; got {len(boxes)} boxes, {K} ids")
     if int(chunk) < 1:
         raise ValueError("render_boxes: chunk must be at least 1 row")
-    last = "fine" if N_importance > 0 else "coarse"
-    maps = []
-    for key in keys:
-        base, _, typ = key.rpartition("_")
-        base, typ = (base, typ) if typ in ("coarse", "fine") else (key, last)
-        if base not in BOX_KEYS or (typ == "fine" and N_importance == 0):
-            raise KeyError(f"render_boxes: no such map {key!r} (choose from {BOX_KEYS}, optionally with _coarse or "
-                           f"_fine)")
-        maps.append((base, typ))
-    maps = tuple(dict.fromkeys(maps))
+    maps = _pass_maps("render_boxes", keys, BOX_KEYS, N_importance)
     H, W = int(H), int(W)
     n = H * W
     table = training._f32_param(code_library.embedding_instance.weight)
@@ -438,15 +430,10 @@ def render_boxes(models: Dict[str, Any], embeddings: Dict[str, Any], code_librar
     use_voxel = _is_voxel(emb_xyz)
     cfg = dict(N_samples=int(N_samples), N_importance=int(N_importance), use_disp=bool(use_disp), chunk=int(chunk),
                precision=engine.train_precision(precision))
-    begin, end = 0, n
-    if group is not None:
-        import torch.distributed as dist
-        begin, end = parallel.shard_bounds(n, dist.get_world_size(group), dist.get_rank(group))
-    plans = _box_plans.setdefault(models["coarse"], {})
+    begin, end = parallel.tile_bounds(n, group)
     key = (dev, H, W, begin, end, use_voxel, tuple(sorted(cfg.items())), maps, K)
-    plan = plans.get(key)
-    if plan is None:
-        plan = plans[key] = _BoxesPlan(models, H, W, end - begin, cfg, maps, K, dev, use_voxel)
+    plan = engine.cached_plan(_box_plans, models["coarse"], key,
+                              lambda: _BoxesPlan(models, H, W, end - begin, cfg, maps, K, dev, use_voxel))
     a = plan.args
     for k in range(K):
         plan.ids[k] = ids[k]
@@ -457,15 +444,13 @@ def render_boxes(models: Dict[str, Any], embeddings: Dict[str, Any], code_librar
     grid = engine.GridBuffers.from_module(emb_xyz) if use_voxel else None
     a.grid = C.pointer(grid.c) if use_voxel else None
     a.pixel_begin, a.pixel_end = begin, end
-    ws = editing._workspace(_lib.load().onerf_render_boxes_workspace_bytes(a.chunk_rays, cfg["N_samples"],
-                                                                          cfg["N_importance"]), dev)
+    ws = engine.workspace(_lib.load().onerf_render_boxes_workspace_bytes(a.chunk_rays, cfg["N_samples"],
+                                                                        cfg["N_importance"]), dev)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
     for typ in plan.model_order:
         training._pack(models, typ, use_voxel, plan.packed)
     if end > begin:
         _lib.call("onerf_render_boxes", dev, C.byref(a))
-    out = dict(plan.maps, hit=plan.hit)
-    if group is not None:
-        out = {k: parallel.gather_tiles(v, n, group) for k, v in out.items()}
+    out = parallel.gather_tile_maps(dict(plan.maps, hit=plan.hit), n, group)
     out["hit"] = out["hit"].bool()
     return out

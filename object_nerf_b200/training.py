@@ -72,7 +72,7 @@ from typing import Any, Dict
 
 import torch
 
-from . import _lib, backward, editing, engine, parallel
+from . import _lib, backward, engine, parallel
 from .losses import TERMS, fill_loss_args
 from .rendering import _is_voxel
 
@@ -559,15 +559,10 @@ def validate_frame(models: Dict[str, Any], embeddings: Dict[str, Any], code_libr
                white_back=bool(white_back), rays_in_bbox=bool(rays_in_bbox), chunk=int(chunk),
                precision=engine.train_precision(precision), has_instance_mask=has_mask,
                loss_weights=tuple(float(loss_conf[f"{t}_weight"]) for t in TERMS))
-    begin, end = 0, n
-    if group is not None:
-        import torch.distributed as dist
-        begin, end = parallel.shard_bounds(n, dist.get_world_size(group), dist.get_rank(group))
-    plans = _val_plans.setdefault(models["coarse"], {})
+    begin, end = parallel.tile_bounds(n, group)
     key = (dev, n, begin, end, use_voxel, tuple(sorted(cfg.items())), keys)
-    plan = plans.get(key)
-    if plan is None:
-        plan = plans[key] = _ValPlan(models, n, end - begin, cfg, keys, dev, use_voxel)
+    plan = engine.cached_plan(_val_plans, models["coarse"], key,
+                              lambda: _ValPlan(models, n, end - begin, cfg, keys, dev, use_voxel))
     a = plan.args
     code_table = _f32_param(code_library.embedding_instance.weight)
     # what the call reads, alive until it has been enqueued (a captured call reads the same tensors on every replay)
@@ -582,18 +577,19 @@ def validate_frame(models: Dict[str, Any], embeddings: Dict[str, Any], code_libr
     grid = engine.GridBuffers.from_module(emb_xyz) if use_voxel else None
     a.render.grid = C.pointer(grid.c) if use_voxel else None
     a.ray_begin, a.ray_end, a.finalize = begin, end, int(group is None)
-    ws = editing._workspace(_lib.load().onerf_validate_workspace_bytes(cfg["chunk"], cfg["N_samples"],
-                                                                       cfg["N_importance"]), dev)
+    ws = engine.workspace(_lib.load().onerf_validate_workspace_bytes(cfg["chunk"], cfg["N_samples"], cfg["N_importance"]),
+                          dev)
     a.render.workspace, a.render.workspace_bytes = ws.data_ptr(), ws.numel()
     for typ in plan.model_order:
         _pack(models, typ, use_voxel, plan.packed)
     _lib.call("onerf_validate_frame", dev, C.byref(a))
     maps = dict(plan.maps)
     if group is not None:
+        import torch.distributed as dist
         dist.all_reduce(plan.record, op=dist.ReduceOp.SUM, group=group)
         _lib.call("onerf_validate_finalize", dev, plan.record.data_ptr(), plan.weights, a.loss.has_fine,
                   plan.out.data_ptr(), plan.out[1:].data_ptr(), plan.present.data_ptr(), plan.psnr.data_ptr())
-        maps = {k: parallel.gather_tiles(v, n, group) for k, v in maps.items()}
+        maps = parallel.gather_tile_maps(maps, n, group)
     return {"loss_sum": plan.out[0], "terms": plan.out[1:], "present": plan.present, "psnr": plan.psnr[0], **maps}
 
 
